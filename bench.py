@@ -1,12 +1,13 @@
 #!/usr/bin/env python
 """bench.py -- PartialConv U-Net (ImageFillOrigin) 512x512 images/sec, forward + backward (+ SGD update).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's B200 path (one rank per GPU under torchrun)
+    python bench.py --gpus N --steps K --warmup W            # this repo's GPU path (one rank per GPU under torchrun)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port) on the host cores
+    python bench.py ... --dump-outputs DIR                   # also write what the last timed step computed as DIR/*.npy
 
 Prints ONE JSON line (rank 0).  Workload = BASELINE.json configs[2] ("image_inpainting.py PartialConv UNet
-@512x512 batch=8, 1xB200 fwd+bwd bf16"), the configuration the headline metric is quoted on; weak scaling
-(batch 8 per GPU, gradients all-reduced over NCCL).
+@512x512 batch=8, fwd+bwd bf16"), the configuration the headline metric is quoted on; weak scaling
+(batch 8 per GPU, gradients all-reduced over NCCL).  Weights and inputs are seeded: the same arguments give the same inputs.
 """
 import argparse
 import json
@@ -48,7 +49,15 @@ def parse():
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--profile-layers", action="store_true", help="print a per-layer CUDA-event table to stderr")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the loss of the last timed step and a seeded sample of the parameters it "
+                         "updated to DIR/<name>.npy (float32, rank 0)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs writes what the GPU path computed; it does not apply to --impl reference")
+    return args
 
 
 # --------------------------------------------------------------------------------------------------
@@ -143,14 +152,13 @@ _REF_CACHE = {}
 
 
 def _reference_module():
-    """The UNMODIFIED reference's models.image_inpainting (from /root/reference in the build container, from the staging copy
-    baseline/_ref on the GPU box -- tools/stage_reference.py), or None when neither exists."""
+    """The UNMODIFIED reference's models.image_inpainting from the copy build() staged in oracle/_ref
+    (oracle/stage_reference.py), or None when nothing was staged."""
     if "mod" in _REF_CACHE:
         return _REF_CACHE["mod"]
     _REF_CACHE["mod"] = None
-    sys.path.insert(0, os.path.join(ROOT, "tools"))
     try:
-        from stage_reference import reference_dir
+        from oracle.stage_reference import reference_dir
         ref = reference_dir()
     except Exception:  # noqa: BLE001
         ref = None
@@ -251,7 +259,7 @@ def run_reference(args):
 
 
 # --------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # --------------------------------------------------------------------------------------------------
 WORKLOADS = {
     # BASELINE.json configs[2] (and [4] under torchrun): the headline
@@ -266,7 +274,7 @@ WORKLOADS = {
 }
 KERNEL_OF = {"tc_fwd": "pconv_tc_tma_kernel<MODE=0> (+ conv_k2r 1x1 GEMM + k2r_combine for the RGB tail, s2d_kernel + the same kernel for the space-to-depth stem)",
              "tc_dgrad": "pconv_tc_tma_kernel<MODE=1> / pconv_tc_sp_kernel<MODE=1> (+ k2r_dbuild + 1x1 dgrad for the tail)",
-             "tc_wgrad": "pconv_tc_wgrad_tma_kernel (+ k2r_dbuild + 1x1 wgrad for the tail, s2d_kernel + <64,4,true> for the stem)",
+             "tc_wgrad": "pconv_tc_wgrad_tma_kernel (+ k2r_dbuild + 1x1 wgrad for the tail, s2d_kernel + the same kernel for the stem)",
              "dw_fwd": "dw4_s1_kernel<FLIP=0> (dwconv.cu)", "dw_dgrad": "dw4_s1_kernel<FLIP=1> (dwconv.cu)", "dw_wgrad": "dw4_s1_wgrad_kernel (dwconv.cu)"}
 
 
@@ -310,36 +318,43 @@ def layer_profile(ts, x, mask, peaks, verbose):
             print(f"  {r[0]:14s} {r[1]:36s} {r[2]:8.2f} {unit} {r[3]:8.3f} ms {r[2] / max(r[3], 1e-9):8.1f} T{unit[1]}/s", file=sys.stderr)
         for k, (fl, ms, n) in sorted(fam.items(), key=lambda kv: -kv[1][1]):
             print(f"  == {k:14s} launches={n:3d} {fl / 1e9:9.1f} G {ms:8.3f} ms {fl / 1e9 / max(ms, 1e-9):8.1f} T/s", file=sys.stderr)
-    peak_t = peaks.get("bf16_tflops_sustained") or 1400.0
-    peak_b = peaks.get("hbm_gbs") or 6500.0
+    # fallback: NVIDIA's H100 SXM data sheet (dense BF16, HBM3) -- a ceiling, not a measured rate
+    peak_t = peaks.get("bf16_tflops_sustained") or 989.0
+    peak_b = peaks.get("hbm_gbs") or 3350.0
     roofs = {}
     for k, (work, ms, n) in fam.items():
         if k.startswith("tc_"):
             ach = work / (ms * 1e-3) / 1e12
             roofs[k] = {"bound": "tensor", "kernel": KERNEL_OF.get(k, k), "achieved": ach, "peak": peak_t, "unit": "TFLOP/s", "frac": ach / peak_t,
-                        "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks else "fallback",
+                        "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks else "H100 SXM data sheet",
                         "launches_per_step": n, "flops_per_step": work, "ms_per_step_in_kernel": ms}
         elif k.startswith("dw_"):
             ach = work / (ms * 1e-3) / 1e9
             roofs[k] = {"bound": "hbm", "kernel": KERNEL_OF.get(k, k), "achieved": ach, "peak": peak_b, "unit": "GB/s", "frac": ach / peak_b,
-                        "peak_source": "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback",
+                        "peak_source": "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet",
                         "launches_per_step": n, "bytes_per_step": work, "ms_per_step_in_kernel": ms}
     if not roofs:
         return None, fam, roofs
     dom = max(roofs.items(), key=lambda kv: kv[1]["ms_per_step_in_kernel"])
-    roof = dict(dom[1])
-    # DRAM bytes per launch of that family from the committed `ncu --set full` capture of one step (profiles/README.md)
-    roof["traffic"] = None
-    for name in ("r02_ncu_traffic.json", "r01_ncu_traffic_final.json"):
-        try:
-            t = json.load(open(os.path.join(ROOT, "profiles", name)))[dom[0]]
-            roof["traffic"] = t["dram_bytes"] / max(roof["launches_per_step"], 1)
-            roof["traffic_note"] = (f"dram__bytes_read+write of all kernels of the family in one step (ncu --set full, profiles/{name}) / "
-                                    "launches_per_step: per layer call, like flops_per_step / launches_per_step")
-            break
-        except Exception:  # noqa: BLE001
-            pass
-    return roof, fam, roofs
+    return dict(dom[1]), fam, roofs
+
+
+DUMP_PARAM_SAMPLE = 1 << 22          # 16 MB of float32
+
+
+def dump_outputs(out_dir, loss, net):
+    """What a caller of the timed training step receives after the last timed step: its loss and the parameters it updated.
+    The parameters (in named order, flattened) are written as a fixed, seeded sample of DUMP_PARAM_SAMPLE values when larger."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    flat = torch.cat([p.detach().float().reshape(-1) for _, p in net.named_parameters()])
+    if flat.numel() > DUMP_PARAM_SAMPLE:
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_PARAM_SAMPLE].sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "params.npy"), flat.cpu().numpy())
 
 
 def run_b200(args):
@@ -357,7 +372,7 @@ def run_b200(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device -- the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device -- the GPU path has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     pg = None
@@ -423,11 +438,13 @@ def run_b200(args):
     barrier()
     e0.record()
     for i in range(args.steps):
-        ts.step(dev_x[i % NBUF], dev_m[i % NBUF])
+        last_loss = ts.step(dev_x[i % NBUF], dev_m[i % NBUF])
     e1.record()
     barrier()
     ms_total = maxreduce(e0.elapsed_time(e1))
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss, net)
     value = world * B * args.steps / (ms_total * 1e-3)
     note(f"device-resident done: {ms_total / args.steps:.2f} ms/step; end-to-end timing")
 
@@ -495,7 +512,7 @@ def run_b200(args):
             "config": {"workload": f"{W['label']} 512x512, batch {B} per GPU, fwd+bwd+SGD(nesterov), train-mode BN",
                        "global_batch": B * world, "parallelism": f"dp{world}", "cuda_graph": ts.graph is not None,
                        "allreduce": ("overlapped with backward (captured)" if ts.overlap_active else "after backward") if world > 1 else "none",
-                       "l2": "inputs+activations per step (GBs) exceed the 126 MB L2; no explicit flush",
+                       "l2": "inputs+activations per step (GBs) exceed the 50 MB L2; no explicit flush",
                        "loss": "out.abs().mean()", "algorithmic_tflop_per_step_per_gpu": step_flop / 1e12},
             "step_tflops_per_gpu": step_flop / 1e12 / (ms_total / args.steps * 1e-3),
             "clocks": clk,

@@ -1,10 +1,10 @@
-/* pconv_b200.h -- C ABI of libpconv_b200.so: the B200 (sm_100a) partial-convolution hot path.
+/* pconv_b200.h -- C ABI of libpconv_b200.so: the H100 (sm_90a) partial-convolution hot path.
  *
  * The reference (yu45020/Text_Segmentation_Image_Inpainting) has NO native boundary: its hot
  * path is Python nn.Modules calling ATen (SURVEY 8b).  The drop-in boundary is therefore the
  * nn.Module surface mirrored in text_segmentation_image_inpainting_b200/models/, and THIS
  * header is the C ABI those modules' autograd Functions bind with ctypes.  Each entry point
- * cites the reference statement(s) it replaces (paths relative to /root/reference).
+ * cites the reference statement(s) it replaces (paths relative to the reference checkout).
  *
  * Conventions
  *  - every pointer is a DEVICE pointer unless named h_*; no torch types cross this boundary;
@@ -61,7 +61,7 @@ const char *pcb_last_error(void);
 int pcb_version(void);
 /* Number of kernels this library has launched since load (for bench.py's gpu_launches). */
 unsigned long long pcb_launch_count(void);
-/* 1 if the tcgen05 tensor-core path would be used for this forward problem, else 0. */
+/* 1 if the wgmma tensor-core path would be used for this forward problem, else 0. */
 int pcb_conv_uses_tensor_cores(const pcb_conv *c);
 
 /* ---- partial convolution --------------------------------------------------------------- */
@@ -103,7 +103,7 @@ int pcb_pconv_forward_premasked(const pcb_conv *c, const void *w_fwd, const floa
 /* Forward with the STATISTICS PASS of the BatchNorm that follows the convolution (partial_convolution.py:193-197,
  * BaseModels.py:95-99) fused into the convolution epilogue: bn_sums[co] += sum over pixels of y[.., co], bn_sums[cout + co] +=
  * sum of y^2 (of the values as stored, holes contribute their zeros).  bn_sums = [2][cout] doubles, ZERO on entry; only for
- * problems with pcb_conv_fuses_bn_stats(c) == 1 (the tcgen05 kernels); bn_sums NULL = plain forward.
+ * problems with pcb_conv_fuses_bn_stats(c) == 1 (the tensor-core kernels); bn_sums NULL = plain forward.
  * mask_pass_done != 0: pcb_pconv_mask_pass already ran (see pcb_pconv_forward_premasked).                                    */
 int pcb_conv_fuses_bn_stats(const pcb_conv *c);
 int pcb_pconv_forward_bn(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
@@ -123,7 +123,7 @@ int pcb_pconv_backward_data(const pcb_conv *c, const void *dc, int dc_cstride, c
                             void *const *dx, const int32_t *dx_cstride, pcb_stream_t stream);
 /* 1 when pcb_pconv_backward_data computes the gradient of a 2x-UPSAMPLED source part (x_up == 1) directly at that source's own
  * (half) resolution -- dx[p] is then a [n, h/2, w/2, dx_cstride] buffer and no 2x2 reduction pass follows (sub-pixel path of the
- * tcgen05 kernels and the kernel-to-row path of the RGB tails: image_inpainting.py:183-185 + partial_convolution.py:229-231
+ * tensor-core kernels and the kernel-to-row path of the RGB tails: image_inpainting.py:183-185 + partial_convolution.py:229-231
  * folded into the convolution).  0: dx[p] of
  * every part is a full-resolution [n, h, w, dx_cstride] buffer and the caller reduces 2x2 blocks itself. */
 int pcb_conv_dgrad_at_source_resolution(const pcb_conv *c);

@@ -11,8 +11,7 @@ Parity status: PINNED.  The reference is pure Python over ATen; it imports and
 runs in the build container (torch 2.11 CPU).  `tests/golden/make_golden.py`
 runs the reference's own modules there and commits the outputs as fixtures;
 `tests/test_oracle_golden.py` checks this restatement against those fixtures
-bit-for-bit (same ATen ops, same order), and, when `/root/reference` is
-present, against the live reference modules.
+bit-for-bit (same ATen ops, same order).
 
 Where the arithmetic lives: torch.nn.functional.conv2d / batch_norm /
 interpolate (ATen, third-party, un-vendored; the reference pins no version --

@@ -6,7 +6,7 @@ the reference's own modules by tests/golden/ fixtures.
 Everything is a pure function over tensors plus a reference-format
 ``state_dict`` (same key names as the reference's nn.Modules), so the oracle
 can consume a checkpoint of the reference directly.  Citations are relative to
-/root/reference/.
+the reference checkout.
 """
 from __future__ import annotations
 

@@ -3,7 +3,7 @@ InvertedResidual / scSE / RFB / ASP / DilatedMobileNetV2 / Xception / TextSegame
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).  Pure functions over a reference-format ``state_dict``;
 pinned bit-for-bit against the reference's own modules by tests/golden/seg_*.npz.  Citations relative to
-/root/reference/.
+the reference checkout.
 """
 from __future__ import annotations
 

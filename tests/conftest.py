@@ -8,16 +8,13 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-REFERENCE = os.environ.get("PCB_REFERENCE", "/root/reference")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    config.addinivalue_line("markers", "reference: needs /root/reference (build container only)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
-    have_ref = os.path.isdir(os.path.join(REFERENCE, "models"))
     try:
         import torch
         have_gpu = torch.cuda.is_available()
@@ -29,8 +26,6 @@ def pytest_collection_modifyitems(config, items):
     for it in items:
         if have_timeout and "gpu" in it.keywords and it.get_closest_marker("timeout") is None:
             it.add_marker(pytest.mark.timeout(300, method="thread"))
-        if "reference" in it.keywords and not have_ref:
-            it.add_marker(pytest.mark.skip(reason="/root/reference not present on this box"))
         if "gpu" in it.keywords and not have_gpu:
             it.add_marker(pytest.mark.skip(reason="no CUDA device"))
 

@@ -1,6 +1,6 @@
 """Generate the committed golden fixtures by running the UNMODIFIED reference on CPU.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Needs a checkout of the reference ($PCB_REFERENCE, default /root/reference); the tests only read the fixtures it writes:
 
     python tests/golden/make_golden.py
 
@@ -159,6 +159,7 @@ def gen_network(cls_name, n, hw, grad_keys, step=8, tag=""):
 
 
 if __name__ == "__main__":
+    torch.set_num_threads(8)          # the count the oracle tests replay with (test_oracle_golden.GOLDEN_THREADS)
     gen_l1()
     gen_block_bn()
     gen_upsample()
@@ -168,7 +169,7 @@ if __name__ == "__main__":
                  "decoder.6.0.1.bn_act.0.bias", "encoder.7.0.1.bn_act.0.weight"])
     gen_network("ImageFillOriginV2", 2, 256, ["decoder.7.0.feature_conv.weight"])
     gen_network("ImageFill", 2, 128, ["decoder.3.0.feature_conv.weight"])
-    # the BENCHMARKED resolution (BASELINE.json configs[2]: 512x512): selects the N = 256 tiles, row-halo tiles on every
+    # the BENCHMARKED resolution (BASELINE.json configs[2]: 512x512): selects the widest N tiles, row-halo tiles on every
     # full-resolution decoder layer and the concurrent parity-class data gradients that 256x256 never reaches
     gen_network("ImageFillOrigin", 2, 512,
                 ["encoder.0.0.feature_conv.weight", "decoder.7.0.feature_conv.weight", "decoder.6.0.0.feature_conv.weight",

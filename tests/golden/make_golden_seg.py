@@ -92,6 +92,7 @@ def gen_network(cls_name, n, hw, grad_keys, step=4, tag=""):
 
 
 if __name__ == "__main__":
+    torch.set_num_threads(8)          # the count the oracle tests replay with (test_oracle_golden_seg.GOLDEN_THREADS)
     gen_blocks()
     keys = {}
     keys["TextSegament"] = gen_network("TextSegament", 2, 64, ["out_conv.0.weight", "feature_pooling.rfb_linear_conv.0.weight",

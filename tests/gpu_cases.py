@@ -76,7 +76,7 @@ CONV_CASES = {
     "g_tail_67_3": (67, 3, 3, 1, 1, 1, 1, True, False, 1, 16, 16, F32, "uniform", "pc"),
     "g_bf16_k3": (8, 8, 3, 1, 1, 1, 1, True, False, 2, 12, 12, BF, "uniform", "pc"),
     "g_bf16_dw": (16, 16, 3, 1, 2, 2, 16, False, True, 2, 12, 12, BF, "uniform", "pc"),
-    # ---- tcgen05 path (bf16, channels % 64 == 0)
+    # ---- tensor-core path (bf16, channels % 64 == 0)
     "tc_1x1_k64_n64": (64, 64, 1, 1, 0, 1, 1, False, False, 1, 16, 16, BF, "uniform", "1x1"),
     "tc_1x1_k128_n128": (128, 128, 1, 1, 0, 1, 1, True, False, 1, 16, 16, BF, "uniform", "1x1"),
     "tc_1x1_k256_n64_ragged_m": (256, 64, 1, 1, 0, 1, 1, True, False, 2, 12, 13, BF, "uniform", "1x1"),

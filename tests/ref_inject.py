@@ -1,8 +1,8 @@
 """Import the reference's OWN network files (unmodified) on top of this repo's layer library -- INTEGRATION.md section 1.
 
-`reference_dir()` is /root/reference in the build container and `baseline/_ref` (a verbatim, git-ignored staging copy made by
-tools/stage_reference.py) on the GPU box.  Only the L2 file itself comes from the reference; every `models.*` module it imports
-resolves to `text_segmentation_image_inpainting_b200.models.*`."""
+`reference_dir()` is `oracle/_ref` (a verbatim, git-ignored staging copy made by oracle/stage_reference.py at build time).
+Only the L2 file itself comes from the reference; every `models.*` module it imports resolves to
+`text_segmentation_image_inpainting_b200.models.*`."""
 import contextlib
 import importlib.util
 import os
@@ -10,8 +10,8 @@ import sys
 import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from stage_reference import reference_dir  # noqa: E402
+sys.path.insert(0, ROOT)
+from oracle.stage_reference import reference_dir  # noqa: E402
 
 L1_MODULES = ("BaseModels", "MobileNetV2", "partial_convolution", "Xception", "common")
 
@@ -21,7 +21,7 @@ def reference_l2(filename):
     """`with reference_l2("image_inpainting.py") as mod:` -> the reference's module object, executed with the aliased L1."""
     ref = reference_dir()
     if ref is None:
-        raise FileNotFoundError("the reference is neither at /root/reference nor staged at baseline/_ref")
+        raise FileNotFoundError("the reference is not staged at oracle/_ref (run __graft_entry__.build())")
     import text_segmentation_image_inpainting_b200.models as mine
     saved = {k: v for k, v in sys.modules.items() if k == "models" or k.startswith("models.")}
     for k in saved:

@@ -9,7 +9,7 @@ import sys
 import pytest
 import torch
 
-from conftest import REFERENCE, ROOT
+from conftest import ROOT
 
 from text_segmentation_image_inpainting_b200 import _lib
 from text_segmentation_image_inpainting_b200.masks import HoleMask
@@ -136,7 +136,7 @@ def test_reference_model_files_construct_unchanged_on_top_of_this_layer_library(
     networks must construct and expose the reference's state_dict."""
     from ref_inject import reference_dir, reference_l2
     if reference_dir() is None:
-        pytest.skip("reference neither at /root/reference nor staged at baseline/_ref")
+        pytest.skip("reference not staged in oracle/_ref")
     from text_segmentation_image_inpainting_b200.models import partial_convolution
     want = json.load(open(os.path.join(ROOT, "tests", "golden", "state_dict_keys.json")))
     with reference_l2("image_inpainting.py") as ref_on_mine:

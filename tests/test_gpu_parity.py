@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called through the module surface ->
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the module surface ->
 autograd Functions -> ctypes -> C ABI (include/pconv_b200.h), against the oracle."""
 import pytest
 import torch
@@ -30,18 +30,7 @@ def test_partial_conv_module_fwd_bwd(tag, dev):
     assert _pipeline_clean(), "a tensor-core pipeline wait timed out"
     assert res["mask_equal"], "binary mask update must be bit-exact"
     if tag.startswith("tc_"):
-        assert res["tc"] == 1, "this case must run on the tcgen05 path"
-    for k in ("y", "gx", "gw", "gb"):
-        assert res[k] <= res["tol"], (k, res)
-
-
-@pytest.mark.parametrize("tag", ["tma_halo_k3_192_64_two", "tma_halo_k3_d2_64_128_w256", "tma_k3_64_256_n256", "tma_k5_s2_64_128_box32x4"])
-def test_partial_conv_cta_pair_path(tag, dev, monkeypatch):
-    """The opt-in CTA-pair kernels (cluster of 2, tcgen05 cta_group::2, PCB_CTA_PAIR=1) must stay parity-green."""
-    monkeypatch.setenv("PCB_CTA_PAIR", "1")
-    res = conv_case(tag, dev)
-    assert _pipeline_clean(), "a tensor-core pipeline wait timed out"
-    assert res["mask_equal"] and res["tc"] == 1
+        assert res["tc"] == 1, "this case must run on the tensor-core path"
     for k in ("y", "gx", "gw", "gb"):
         assert res[k] <= res["tol"], (k, res)
 
@@ -71,7 +60,7 @@ def test_network_fp32_matches_reference_golden(cls_name, tag, dev):
 
 @pytest.mark.parametrize("cls_name,tag", NET_GOLDENS)
 def test_network_bf16_tensor_core_mode(cls_name, tag, dev):
-    """bf16 storage + tcgen05: 16+ layers of bf16 rounding -> a few 1e-3 on the output and loss.  Gradients of the
+    """bf16 storage + tensor cores: 16+ layers of bf16 rounding -> a few 1e-3 on the output and loss.  Gradients of the
     BatchNorm scales see LeakyReLU sign flips of pre-activations within one bf16 ulp of zero (a systematic, not a
     random, perturbation): a few percent of max|grad|; convolution weight grads stay at the 1e-3 level."""
     errs = run_net(cls_name, dev, BF, tag)
@@ -130,7 +119,7 @@ def test_bn_act_and_running_stats(c, dev):
 @pytest.mark.parametrize("shape", [(64, 128, 3, 1, 1, (2, 24, 20)), (64, 64, 3, 1, 1, (2, 8, 128)), (128, 256, 3, 2, 1, (2, 32, 32)),
                                    (192, 320, 1, 1, 0, (1, 16, 16))])
 def test_bn_statistics_fused_into_conv_epilogue(shape, dev):
-    """PartialConv -> BatchNorm(train) -> LeakyReLU block: the per-channel sums accumulated in the tcgen05 epilogue
+    """PartialConv -> BatchNorm(train) -> LeakyReLU block: the per-channel sums accumulated in the tensor-core epilogue
     (pcb_pconv_forward_bn) against the separate statistics pass (ops.set_fused_bn_stats(False)) and against the oracle."""
     from gpu_cases import blob
     from oracle.detfill import det_fill_state_dict, det_tensor

@@ -1,8 +1,9 @@
 """Drop-in boundary on the GPU (SURVEY 8b, BASELINE north_star: "the new layers drop into the existing model files unchanged"):
-the reference's OWN models/image_inpainting.py and models/text_segmentation.py -- byte-for-byte, imported from /root/reference or
-its staging copy baseline/_ref -- run forward + backward on cuda:0 on top of this repo's layer library and must reproduce the
-goldens that the same files produced on top of the reference's layer library on CPU (tests/golden/*.npz)."""
-import filecmp
+the reference's OWN models/image_inpainting.py and models/text_segmentation.py -- byte-for-byte, imported from the copy build()
+staged in oracle/_ref -- run forward + backward on cuda:0 on top of this repo's layer library and must reproduce the goldens that
+the same files produced on top of the reference's layer library on CPU (tests/golden/*.npz)."""
+import hashlib
+import json
 import os
 
 import numpy as np
@@ -24,11 +25,14 @@ def dev():
 
 
 def test_staged_reference_is_verbatim():
-    """In the build container both copies exist: the staging copy must be byte-identical to /root/reference."""
-    if not (os.path.isdir("/root/reference/models") and os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "models"))):
-        pytest.skip("needs both /root/reference and baseline/_ref")
-    for f in ("models/image_inpainting.py", "models/text_segmentation.py", "models/partial_convolution.py", "loss.py"):
-        assert filecmp.cmp(os.path.join("/root/reference", f), os.path.join(ROOT, "baseline", "_ref", f), shallow=False), f
+    """The staged copy must be byte-identical to the reference files the goldens were made from (SHA-256 in tests/golden)."""
+    ref = reference_dir()
+    if ref is None:
+        pytest.skip("reference not staged in oracle/_ref")
+    want = json.load(open(os.path.join(ROOT, "tests", "golden", "reference_sha256.json")))
+    for f, digest in want.items():
+        with open(os.path.join(ref, f), "rb") as fh:
+            assert hashlib.sha256(fh.read()).hexdigest() == digest, f
 
 
 def _run_inpainting(mod, cls_name, dev, dtype, tag=""):

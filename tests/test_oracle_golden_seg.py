@@ -19,6 +19,19 @@ from text_segmentation_image_inpainting_b200.models import MobileNetV2 as MM
 from text_segmentation_image_inpainting_b200.models import common as MC
 from text_segmentation_image_inpainting_b200.models import text_segmentation as MT
 
+
+# The goldens were produced with 8 intra-op CPU threads: oneDNN splits its reductions by thread count, so bit-exact comparisons
+# hold only at that count, whatever the machine has.
+GOLDEN_THREADS = 8
+
+
+@pytest.fixture(autouse=True, scope="module")
+def _golden_thread_count():
+    before = torch.get_num_threads()
+    torch.set_num_threads(GOLDEN_THREADS)
+    yield
+    torch.set_num_threads(before)
+
 ACT = ("leaky", 0.3)
 
 

@@ -1,4 +1,4 @@
-"""In-tree nvcc build of libpconv_b200.so (sm_100a only).  No torch headers are involved: the library is
+"""In-tree nvcc build of libpconv_b200.so (sm_90a only).  No torch headers are involved: the library is
 plain CUDA C++ behind a C ABI (include/pconv_b200.h); Python binds it with ctypes."""
 import fcntl
 import hashlib
@@ -13,7 +13,7 @@ LIB = os.path.join(HERE, "libpconv_b200.so")
 STAMP = os.path.join(HERE, "libpconv_b200.stamp")     # fingerprint of the sources the .so was built from (travels with it)
 SOURCES = ["api.cu", "conv_tc.cu", "conv_smallco.cu", "conv_k2r.cu", "conv_stem.cu", "conv_generic.cu", "elementwise.cu", "dwconv.cu", "seg_ops.cu"]
 HEADERS = ["pcb_common.cuh", "pcb_ptx.cuh", os.path.join("..", "..", "include", "pconv_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
               "-cudart", "static"]
 
@@ -48,7 +48,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu for sm_100a and link libpconv_b200.so.  Safe to call from several processes at once (the ranks
+    """Compile every .cu for sm_90a and link libpconv_b200.so.  Safe to call from several processes at once (the ranks
     of a data-parallel job): an exclusive file lock serialises them, objects and the library are written to
     process-private temporaries and renamed into place, and the losers of the race find the stamp up to date."""
     if not force and not needs_build():

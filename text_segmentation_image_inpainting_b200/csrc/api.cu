@@ -1,5 +1,5 @@
 // api.cu -- C-ABI entry points of libpconv_b200.so for the convolution itself (validation + dispatch between
-// the tcgen05 tensor-core kernels and the shape-general kernels), error string, launch counter.
+// the wgmma tensor-core kernels and the shape-general kernels), error string, launch counter.
 #include <stdarg.h>
 #include <string.h>
 
@@ -55,7 +55,7 @@ static bool use_tc(const pcb_conv *c) { return !c->force_generic && !use_dw(c) &
 PCB_API int pcb_conv_uses_tensor_cores(const pcb_conv *c) { return (c && use_tc(c)) ? 1 : 0; }
 
 // 1 when pcb_pconv_backward_data writes the gradient of a 2x-UPSAMPLED source directly at that source's own (half) resolution:
-// dx[p] of such a part is then a [n, h/2, w/2, dx_cstride] buffer and no 2x2 reduction pass follows (the tcgen05 sub-pixel path)
+// dx[p] of such a part is then a [n, h/2, w/2, dx_cstride] buffer and no 2x2 reduction pass follows (the tensor-core sub-pixel path)
 PCB_API int pcb_conv_dgrad_at_source_resolution(const pcb_conv *c) { return (c && use_tc(c) && pcb_tc_subpixel(c)) ? 1 : 0; }
 
 PCB_API size_t pcb_pconv_workspace(const pcb_conv *c) { return (c && use_tc(c)) ? pcb_tc_workspace(c) : 0; }

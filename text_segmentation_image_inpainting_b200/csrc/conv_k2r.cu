@@ -6,14 +6,13 @@
 // the upsampled source to every (tap, cout) column can be computed ONCE PER SOURCE PIXEL:
 //     Z[s][tap, co] = sum_c (u[s][c] * m_u[s]) * W[co][tap][c]              one 1x1 convolution  C_u -> 32  at half resolution
 //     y[p][co]      = ( sum_tap Z[(p + tap - 1) >> 1][tap, co]  +  direct 3x3 over v )  / msum[p] + b[co]   (0 at holes)
-// i.e. 4x fewer pixels and no im2col for the wide part; the 1x1 problem runs on the TMA-fed tcgen05 kernels of conv_tc.cu (its
+// i.e. 4x fewer pixels and no im2col for the wide part; the 1x1 problem runs on the TMA-fed wgmma kernels of conv_tc.cu (its
 // operand stream is the source tensor, read once), the combine pass is a streaming kernel.  The backward pass has the same shape:
 //     D[s][tap, co] = sum over the four children p of s of dc[p - tap + 1][co]     (dc = renormalised output gradient)
 //     du[s][c] = m_u[s] * sum_k D[s][k] W'[k][c]         1x1 data gradient, delivered at SOURCE resolution (no 2x2 reduction pass)
 //     dW'[k][c] = sum_s D[s][k] u[s][c] m_u[s]           1x1 weight gradient, scattered back into the [co][tap][c] master layout
 // and the 81 weight gradients of the image part are reduced on CUDA cores inside the D pass.
-// The mma.sync kernels of conv_smallco.cu stay as the general path (other kernel sizes, wider second parts, PCB_DISABLE_K2R=1);
-// measured at 8 x 512 x 512: forward 0.245 -> see profiles/r02_k2r.txt.
+// The mma.sync kernels of conv_smallco.cu stay as the general path (other kernel sizes, wider second parts, PCB_DISABLE_K2R=1).
 #include <string.h>
 
 #include <algorithm>
@@ -420,7 +419,7 @@ int pcb_k2r_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, 
     K2rParams P;
     base(P, c, K);
     P.dc = static_cast<const bf16 *>(dc); P.dc_cstride = dc_cstride; P.d = d; P.dw = dw;
-    // 170 registers per thread: 128-thread blocks keep three of them resident per SM (256-thread blocks: one, 12 % of the warp slots)
+    // a register-heavy kernel: 128-thread blocks let more of them be resident per SM than 256-thread blocks
     if (K.cs <= 3) k2r_dbuild_kernel<true, 3><<<grid_for(c, 3), 128, 0, st>>>(P);
     else k2r_dbuild_kernel<true, 4><<<grid_for(c, 2), 128, 0, st>>>(P);
     PCB_LAUNCH_CHECK();

@@ -1,9 +1,8 @@
 // conv_smallco.cu -- partial convolution layers with at most 8 OUTPUT channels (the RGB tails of the inpainting U-Nets:
 // cat(up2x(64 ch), image 3 ch) -> 3, 3x3, stride 1;  models/image_inpainting.py:63 / :102 / :126).
 //
-// On the tcgen05 path such a layer pads N = 3 to a 32..64-wide tile and its data gradient pads K = 3 to 64 per tap: >90 % of the
-// tensor work multiplies zeros and the kernels end up bound by operand staging, not by math (0.35-0.86 ms per pass at
-// 8 x 512 x 512).  Here the three GEMMs are shaped around the 8-wide dimension instead, with warp-level mma.sync
+// On the wgmma path such a layer pads N = 3 to a 32..64-wide tile and its data gradient pads K = 3 to 64 per tap: >90 % of the
+// tensor work multiplies zeros and the kernels end up bound by operand staging, not by math.  Here the three GEMMs are shaped around the 8-wide dimension instead, with warp-level mma.sync
 // (m16n8k16, bf16 x bf16 -> fp32) whose N (or K per tap) is exactly 8:
 //   forward   M = 16 pixels, N = 8 cout,          K = tap x packed channels      A: ldmatrix from a haloed, hole-masked x tile
 //   dgrad     M = 16 pixels, N = 8 input chans,   K = (tap, 8 cout) pairs        A: ldmatrix rows gathered from a haloed dc tile

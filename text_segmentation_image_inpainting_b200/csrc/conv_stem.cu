@@ -4,7 +4,7 @@
 //     xs[n][sy][sx][(a, b, ch)] = x[n][2 sy + a][2 sx + b][ch] * mask[...]          32 channels per half-resolution cell
 //     y[o] = sum_t w[t] x[2 o + t - 3]  =  sum_{j=0..3} sum_{a=0,1} w[2 j + a - 1] xs[o + j - 2][a]      (w[-1] = w[7] = 0)
 // i.e. kernel 4, padding 2 in front (the "extra" output row/column a symmetric padding would give is simply not computed).  The
-// stride-2 gather of 7 x 7 x 8-channel windows -- which bound the row-packed cp.async kernel at 16..30 B/clk/SM (DESIGN 4.2) --
+// stride-2 gather of 7 x 7 x 8-channel windows -- which bounds the row-packed cp.async kernel by its 16-byte gathers --
 // becomes the TMA-fed implicit GEMM of conv_tc.cu with row-halo tiles: one 131-cell tile per kernel row serves the four taps, the
 // K steps of the zero half of each 64-channel block are not issued.  x * mask happens in the space-to-depth pass (sub-pixels of a
 // cell have different mask values, so the GEMM itself runs without hole rows); renormalisation, hole zeroing, bias and the

@@ -1,4 +1,4 @@
-// conv_tc.cu -- partial convolution as implicit GEMM on the 5th-gen tensor cores (tcgen05 / TMEM / TMA).
+// conv_tc.cu -- partial convolution as implicit GEMM on the Hopper tensor cores (wgmma / TMA / mbarrier).
 //
 // Replaces (per layer) the reference's pair of dense convolutions + ~9 elementwise passes
 // (models/partial_convolution.py:49-80): `feature_conv(x*mask)`, the all-ones `mask_conv`, `==0`,
@@ -16,10 +16,10 @@
 //                 through row-shifted SWIZZLE_128B descriptors.  2x-upsampled sources are first copied densely into the
 //                 workspace (TMA cannot replicate pixels).
 //     B operand   weights [N][K] bf16 (K padded to the same block structure), TMA 2D tiles (SWIZZLE_128B).
-//     MMA         tcgen05.mma.cta_group::1.kind::f16, M=128 x N in {32,64,128,256} x K=16, fp32 accumulators in TMEM (two
-//                 stages), issued from an elect.sync region of a warp-converged issuer warp; stages recycled through
-//                 tcgen05.commit -> mbarrier.
-//     epilogue    TMEM -> registers (tcgen05.ld 32x32b), fwd: y = hole ? 0 : acc / s + bias (s = mask box sum),
+//     MMA         wgmma.mma_async m64nNk16 bf16 -> fp32, N in {32, 64, 128}: two consumer warpgroups each own 64 rows of the
+//                 128-row tile and hold its accumulators in registers; stages are released through mbarriers once
+//                 wgmma.wait_group reports the MMAs that read them complete.
+//     epilogue    registers -> shared staging tile -> one thread per row, fwd: y = hole ? 0 : acc / s + bias (s = mask box sum),
 //                 dgrad: dx_part = acc * input-mask of that part; bf16 NHWC stores.  Stride-2 dgrad = four stride-1 parity classes.
 //     wgrad       D[k][co] (+)= sum_pixels x[p+tap][k] * dc[p][co]: both operands MN-major "pixel row x 128-byte channel chunk"
 //                 tiles by TMA, split-K over pixels with fp32 red.global.add into the (logical, unpadded) KRSC gradient.
@@ -30,7 +30,7 @@
 //     operand is gathered by 4 producer warps with 16-byte zero-filling cp.async from up to 2 concatenated, optionally
 //     2x-upsampled sources, driven by per-pixel tap-validity words (tapmask_kernel).
 //
-// DESIGN.md section 4 has the anatomy, the measured bounds and the microbenchmarks behind these choices.
+// DESIGN.md section 4 has the anatomy and the reasons behind these choices.
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -46,12 +46,16 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;                 // bf16 elements = 128 bytes = one swizzle row
 constexpr int A_STAGE_BYTES = BLOCK_M * 128;
 constexpr int NUM_PRODUCER_THREADS = 128;
-constexpr int TC_THREADS = 192;             // 4 producer/epilogue warps + TMA warp + MMA warp
 constexpr int TC_MAX_PARTS = 2;             // U-Net inputs are cat([upsampled, skip]) at most
-// cp.async data is published to the MMA thread through the mbarrier the copies arrive on (cp.async.mbarrier.arrive +
-// mbarrier wait = release/acquire), exactly like CUTLASS's sm100 cp.async mainloop; an extra generic->async proxy fence in
-// the single MMA-issuing thread serialised every K block behind it (~1 us each) and is not needed.
-constexpr bool kProxyFence = false;
+// Every tensor-core kernel computes its 128-row tile with TWO consumer warpgroups: warpgroup g issues the m64 wgmmas of rows
+// [64 g, 64 g + 64) into register accumulators and then runs the epilogue of those rows.  wgmma reads shared memory through
+// the async proxy, so data written by cp.async / st.shared is made visible to it with fence.proxy.async after the consumer
+// acquired the stage's mbarrier.
+constexpr int MMA_WARPS = 8;
+constexpr int MMA_THREADS = MMA_WARPS * 32;
+// fp32 staging tile of the forward / dgrad epilogue: [128 rows][BLOCK_N + 4] (the pad spreads the rows over the banks)
+constexpr int acc_pitch(int block_n) { return block_n + 4; }
+constexpr int acc_stage_bytes(int block_n) { return BLOCK_M * acc_pitch(block_n) * 4; }
 
 inline int rup(int v, int m) { return (v + m - 1) / m * m; }
 
@@ -77,7 +81,6 @@ struct TcParams {
     // dgrad gather source
     const bf16 *dc; int dc_cstride, dc_c8, dc_kext;
     int *abort_flag;
-    long long *dbg;           // optional [grid][8] cycle counters written by the MMA thread (PCB_TC_DEBUG_TIMING)
     int l2pf;                 // TMA-fed fwd/dgrad: request the next tile's A boxes into L2 one tile ahead (PCB_TMA_L2_PREFETCH)
     // TMA-fed kernel: the 128 pixels of an M tile form the box {box_w, box_h, box_n} of the (x, y, image) pixel grid
     int box_w, box_h, box_n, stages, use_fix;
@@ -97,8 +100,9 @@ struct TcParams {
     int bn_c;
 };
 
-constexpr int STAT_FLOATS_PER_WARP = 2 * 256;              // [sum | sum of squares] x up to 256 tile columns
-constexpr int STAT_SMEM_BYTES = 4 * STAT_FLOATS_PER_WARP * 4 + 16;
+// fused BatchNorm statistics: eight private slices of [128 sums | 128 squares], one per epilogue warp (row quadrant x column half)
+constexpr int STAT_SLICE = 256;
+constexpr int STAT_SMEM_BYTES = MMA_WARPS * STAT_SLICE * 4 + 16;
 
 // 32 values per lane, 32 lanes: returns in lane l the sum over all lanes of v[l] (a transposing butterfly: 31 shuffles)
 __device__ __forceinline__ float warp_transpose_sum(float (&v)[32], int lane) {
@@ -120,14 +124,22 @@ __device__ __forceinline__ float warp_transpose_sum(float (&v)[32], int lane) {
 __device__ __forceinline__ uint32_t align1024(uint32_t a) { return (a + 1023u) & ~1023u; }
 
 // -------------------------------------------------------------------------------------------------
-// epilogue shared by the forward / dgrad kernels: TMEM -> registers -> renormalise / mask -> bf16 NHWC
+// epilogue shared by the forward / dgrad kernels: staged fp32 accumulators -> renormalise / mask -> bf16 NHWC
 // -------------------------------------------------------------------------------------------------
-// Columns [cb, ce) of the tile (multiples of 32): the kernels with eight epilogue warps give each TMEM lane quadrant to two warps
-// that split the columns.  s_stat: this warp's accumulators [sums of its columns | squares at offset sq_off].
+// `acc_row` is this lane's row of the staging tile (row warp * 32 + lane).  Columns [cb, ce) of the tile (multiples of 32): each
+// row quadrant is drained by two warps that split the columns.  s_stat: this warp's accumulators [sums of its columns | squares
+// at offset sq_off].
+__device__ __forceinline__ void load_acc32(const float *src, uint32_t (&r)[32]) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const uint4 v = reinterpret_cast<const uint4 *>(src)[j];
+        r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
+    }
+}
+
 template <int BLOCK_N, int MODE>
-__device__ __forceinline__ void tc_epilogue(const TcParams &P, uint32_t tmem_base, int warp, int lane, int m0, int n0, float *s_stat,
-                                            int cb = 0, int ce = BLOCK_N, int sq_off = 256) {
-                ptx::tc_fence_after();
+__device__ __forceinline__ void tc_epilogue(const TcParams &P, const float *acc_row, int warp, int lane, int m0, int n0, float *s_stat,
+                                            int cb, int ce, int sq_off) {
                 const int row = warp * 32 + lane;
                 const int m = m0 + row;
                 const bool rvalid = m < P.m_total;
@@ -153,8 +165,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &P, uint32_t tmem_bas
     #pragma unroll 1
                     for (int c0 = cb; c0 < ce; c0 += 32) {
                         uint32_t r[32];
-                        ptx::tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + c0, r);
-                        ptx::tmem_ld_wait();
+                        load_acc32(acc_row + c0, r);
                         if (rvalid) {
                             float *dst = P.partial + static_cast<long long>(m) * P.ncols + n0 + c0;
     #pragma unroll
@@ -166,8 +177,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &P, uint32_t tmem_bas
     #pragma unroll 1
                 for (int c0 = cb; c0 < ce; c0 += 32) {
                     uint32_t r[32];
-                    ptx::tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + c0, r);
-                    ptx::tmem_ld_wait();
+                    load_acc32(acc_row + c0, r);
                     const int col = n0 + c0;
                     bf16 *orow = nullptr;
                     int nstore = 0;                      // channels to store from this 32-column chunk (multiple of 8)
@@ -194,8 +204,8 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &P, uint32_t tmem_bas
                         uint4 o[4];
                         __nv_bfloat162 *ob = reinterpret_cast<__nv_bfloat162 *>(o);
                         // The per-element work is kept to a multiply-add, a select and the conversion: the epilogue of the K <= 512
-                        // problems is ISSUE-bound (it measured 24 instructions per element with per-element bias loads and bounds
-                        // tests), so everything uniform over the chunk is decided here.  Lane l fetches the bias of column col + l
+                        // problems is ISSUE-bound (per-element bias loads and bounds tests would dominate it), so everything uniform
+                        // over the chunk is decided here.  Lane l fetches the bias of column col + l
                         // once; elements get theirs by shuffle.  Columns past cout only exist in the last chunk of a layer.
                         float bl = 0.f;
                         const bool has_bias = (MODE == 0) && (P.bias != nullptr);
@@ -219,21 +229,11 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &P, uint32_t tmem_bas
                             ob[j] = __floats2bfloat162_rn(a, b);
                         }
                         if (nstore > 0) {
-                            // a lane owns one output row: its 64 bytes of this chunk go out as two 32-byte sectors (STG.256) when the
-                            // row is 32-byte aligned -- the 16-byte version issued twice as many half-sector requests, and the
-                            // row-scattered store traffic is what bounds the epilogue (4096 requests per 128 x 256 tile)
+                            // a lane owns one output row: its 64 bytes of this chunk go out as four 16-byte stores
                             uint4 *dst = reinterpret_cast<uint4 *>(orow);
-                            if ((reinterpret_cast<uintptr_t>(orow) & 31) == 0) {
     #pragma unroll
-                                for (int j = 0; j < 4; j += 2) {
-                                    if ((j + 1) * 8 < nstore) ptx::st_global_256(dst + j, o[j], o[j + 1]);
-                                    else if (j * 8 < nstore) dst[j] = o[j];
-                                }
-                            } else {
-    #pragma unroll
-                                for (int j = 0; j < 4; ++j)
-                                    if (j * 8 < nstore) dst[j] = o[j];
-                            }
+                            for (int j = 0; j < 4; ++j)
+                                if (j * 8 < nstore) dst[j] = o[j];
                         }
                         if (stats) {
                             // per-channel sum and sum of squares of what was just stored (rows past the tensor contribute 0)
@@ -255,7 +255,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &P, uint32_t tmem_bas
 
 // flush one warp's per-column statistics of the N tile starting at n0 into the global fp64 sums, and clear them
 template <int BLOCK_N>
-__device__ __forceinline__ void tc_stats_flush(const TcParams &P, float *s_stat, int lane, int n0, int cb = 0, int ce = BLOCK_N, int sq_off = 256) {
+__device__ __forceinline__ void tc_stats_flush(const TcParams &P, float *s_stat, int lane, int n0, int cb, int ce, int sq_off) {
     __syncwarp();
     for (int c0 = cb; c0 < ce; c0 += 32) {
         const int co = n0 + c0 + lane;
@@ -268,27 +268,83 @@ __device__ __forceinline__ void tc_stats_flush(const TcParams &P, float *s_stat,
     __syncwarp();
 }
 
+// The two consumer warpgroups' share of the forward / dgrad epilogue.  Epilogue warp e (0..7) = warp e of the consumer
+// warpgroups: warpgroup g = e / 4 owns rows [64 g, 64 g + 64), i.e. row quadrants 2 g and 2 g + 1, and each quadrant is drained
+// by two warps that split the columns.
+template <int BLOCK_N>
+struct EpiRole {
+    static constexpr int HN = (BLOCK_N >= 64) ? BLOCK_N / 2 : BLOCK_N;
+    int q, half, cb, ce;
+    __device__ __forceinline__ explicit EpiRole(int e) {
+        q = 2 * (e >> 2) + (e & 1);
+        half = (e & 3) >> 1;
+        cb = half * HN;
+        ce = (cb + HN <= BLOCK_N) ? cb + HN : cb;        // a 32-column tile is not split: the second warp only waits
+    }
+    __device__ __forceinline__ int slice() const { return half * 4 + q; }
+};
+
+// register accumulators of warpgroup g (fragment layout: see ptx::wgmma_bf16) -> staging tile -> tc_epilogue of this warp's
+// 32 rows x column half.  Both named barriers span the warpgroup only: the other one keeps its own pace.
+template <int BLOCK_N, int MODE>
+__device__ __forceinline__ void mma_epilogue(const TcParams &P, const float (&acc)[BLOCK_N / 2], float *stage, int e, int lane, int m0, int n0,
+                                             float *s_stat) {
+    constexpr int PITCH = acc_pitch(BLOCK_N);
+    const int g = e >> 2;
+    const int r0 = 64 * g + 16 * (e & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; i += 2) {
+        const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + c0;
+        *reinterpret_cast<float2 *>(stage + row * PITCH + col) = make_float2(acc[i], acc[i + 1]);
+    }
+    ptx::named_sync(1 + g, 128);
+    const EpiRole<BLOCK_N> R(e);
+    tc_epilogue<BLOCK_N, MODE>(P, stage + (R.q * 32 + lane) * PITCH, R.q, lane, m0, n0, s_stat, R.cb, R.ce, 128);
+    ptx::named_sync(1 + g, 128);                          // the staging rows are free for the next tile
+}
+
+// last N tile's BatchNorm statistics: the eight epilogue warps' partials are summed after a CTA-wide barrier, so the global sums
+// receive ONE atomic per channel per CTA.  `stat_base`: slice 0.
+template <int BLOCK_N>
+__device__ __forceinline__ void tc_stats_final(const TcParams &P, const float *stat_base, int e, int lane, int stat_n0) {
+    constexpr int HN = EpiRole<BLOCK_N>::HN;
+    for (int col = e * 32 + lane; col < BLOCK_N; col += MMA_THREADS) {
+        const int co = stat_n0 + col;
+        if (co < P.bn_c) {
+            const int h = col / HN, lc = col - h * HN;
+            float a = 0.f, q = 0.f;
+#pragma unroll
+            for (int w4 = 0; w4 < 4; ++w4) { a += stat_base[(h * 4 + w4) * STAT_SLICE + lc]; q += stat_base[(h * 4 + w4) * STAT_SLICE + 128 + lc]; }
+            atomicAdd(P.bn_sums + co, static_cast<double>(a));
+            atomicAdd(P.bn_sums + P.bn_c + co, static_cast<double>(q));
+        }
+    }
+}
+
+template <int R> __device__ __forceinline__ void zero_acc(float (&a)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) a[i] = 0.f;
+}
+
 // -------------------------------------------------------------------------------------------------
 // forward (MODE 0) / data gradient (MODE 1): PERSISTENT, warp-specialised implicit GEMM.
 //
 // One CTA per SM loops over output tiles (128 pixels x BLOCK_N channels).  Roles:
-//   warps 0-3  A producers  : im2col gather with zero-filling cp.async (padding AND holes), 32-bit offsets
-//   warp  4    B producer   : weight tiles by TMA (SWIZZLE_128B)
-//   warp  5    MMA issuer   : tcgen05.mma into one of TWO TMEM accumulator stages
-//   warps 6-9  epilogue     : tcgen05.ld -> renormalise / mask -> bf16 NHWC stores
-// so the fixed per-tile latencies (mask-word loads, pipeline fill, accumulator drain, stores) of tile i overlap the
-// main loop of tile i+1 -- with one CTA per tile these latencies (~10 us) dominated every layer with a short K loop.
+//   warps 0-3   A producers : im2col gather with zero-filling cp.async (padding AND holes), 32-bit offsets
+//   warps 4-11  consumers   : two warpgroups, wgmma into register accumulators, then the epilogue of their 64 rows
+//   warp  12    B producer  : weight tiles by TMA (SWIZZLE_128B)
+// so the producers' per-tile latencies (mask-word loads, pipeline fill) of tile i+1 overlap the epilogue of tile i.
 //
 // Two A-operand layouts:
 //   HALO = false : per tap, a [128 pixel x 64 channel] tile in the 128B-swizzled K-major layout (any stride / dilation;
 //                  also the row-packed small-Cin mode: K block = kernel row, chunk = tap column).
 //   HALO = true  : stride-1 layers.  Per kernel ROW, each group of 8 consecutive output pixels stages its
 //                  8 + (kw-1)*dil input pixels once in the canonical NO-SWIZZLE K-major layout
-//                  addr(slot, chunk) = chunk*LBO + slot*16; the kw taps of the row are kw UMMA descriptors whose start
+//                  addr(slot, chunk) = chunk*LBO + slot*16; the kw taps of the row are kw wgmma descriptors whose start
 //                  address is shifted by tap*dil slots (SBO = HG*16 between 8-row groups): kw x fewer gathers.
 // -------------------------------------------------------------------------------------------------
 constexpr int HALO_MAX_HG = 12;
-constexpr int PERSIST_THREADS = 320;
+constexpr int PERSIST_THREADS = 4 * 32 + MMA_THREADS + 32;
 constexpr int MAX_RING = 8;
 
 template <int BLOCK_N, int MODE, bool HALO>
@@ -306,9 +362,9 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
     const uint32_t sBar = (sA + SA * A_STAGE + 15u) & ~15u;
     const uint32_t bar_full_a = sBar, bar_empty_a = sBar + 8 * MAX_RING;
     const uint32_t bar_full_b = sBar + 16 * MAX_RING, bar_empty_b = sBar + 24 * MAX_RING;
-    const uint32_t bar_tmem_full = sBar + 32 * MAX_RING, bar_tmem_empty = bar_tmem_full + 16;
-    const uint32_t s_tmem_ptr = bar_tmem_empty + 16;
-    uint32_t *tmem_ptr_generic = reinterpret_cast<uint32_t *>(smem_raw + (s_tmem_ptr - ptx::smem_u32(smem_raw)));
+    const uint32_t s_stat_addr = sBar + 32 * MAX_RING;                                  // BatchNorm statistics slices
+    const uint32_t s_acc = (s_stat_addr + STAT_SMEM_BYTES + 15u) & ~15u;               // epilogue staging tile
+    float *acc_stage = reinterpret_cast<float *>(smem_raw + (s_acc - ptx::smem_u32(smem_raw)));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int taps = P.kh * P.kw;
@@ -326,22 +382,14 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
     };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < MAX_RING; ++s) {
-            ptx::mbar_init(bar_full_a + 8 * s, NUM_PRODUCER_THREADS); ptx::mbar_init(bar_empty_a + 8 * s, 1);
-            ptx::mbar_init(bar_full_b + 8 * s, 1); ptx::mbar_init(bar_empty_b + 8 * s, 1);
+        for (int s = 0; s < MAX_RING; ++s) {      // empty barriers: one arrival per consumer warpgroup
+            ptx::mbar_init(bar_full_a + 8 * s, NUM_PRODUCER_THREADS); ptx::mbar_init(bar_empty_a + 8 * s, 2);
+            ptx::mbar_init(bar_full_b + 8 * s, 1); ptx::mbar_init(bar_empty_b + 8 * s, 2);
         }
-        for (int s = 0; s < 2; ++s) { ptx::mbar_init(bar_tmem_full + 8 * s, 1); ptx::mbar_init(bar_tmem_empty + 8 * s, 128); }
         ptx::fence_mbar_init();
     }
-    if (warp == 4 && lane == 0) ptx::prefetch_tmap(&tmap_w);
-    if (warp == 5) {
-        ptx::tmem_alloc<2 * BLOCK_N>(s_tmem_ptr);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
+    if (warp == 12 && lane == 0) ptx::prefetch_tmap(&tmap_w);
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_generic;
 
     if (warp < 4) {
         // ================================ A producers ================================
@@ -352,7 +400,7 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
         int it = 0;
         bool dead = false;
         // Tap-validity words of the NEXT tile are loaded while the current tile's items stream (software pipelining across
-        // tiles): their ~1 us global-load latency would otherwise stall all gathers at the start of every tile.
+        // tiles): their global-load latency would otherwise stall all gathers at the start of every tile.
         constexpr int NW = HALO ? HALO_MAX_HG : 8;
         uint64_t wnext[TC_MAX_PARTS][NW];
         auto issue_mask_loads = [&](int tl) {
@@ -568,7 +616,7 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
             }
         }
         ptx::cp_async_wait<0>();
-    } else if (warp == 4) {
+    } else if (warp == 12) {
         // ================================ B producer: weight tiles by TMA ================================
         if (lane == 0) {
             int itb = 0;
@@ -602,106 +650,75 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
                 }
             }
         }
-    } else if (warp == 5) {
-        // ================================ MMA issuer ================================
-        if (lane == 0) {
-            constexpr uint32_t idesc = ptx::make_idesc_bf16(BLOCK_M, BLOCK_N, 0, 0);
-            int num_a = 0;
-            if (HALO) {
-                for (int p = 0; p < np; ++p) num_a += ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
-                num_a *= P.kh;
-            } else {
-                num_a = (MODE == 0) ? (P.rowpack ? P.kh : taps * (P.ktap / BLOCK_K)) : taps * (P.dc_kext / BLOCK_K);
-            }
-            int ita = 0, itb = 0, tile_iter = 0;
-            bool dead = false;
-            long long t_acc = 0, t_a = 0, t_b = 0, t_issue = 0;
-            const long long t_begin = clock64();
-            for (int tile = blockIdx.x; tile < num_tiles && !dead; tile += gridDim.x) {
-                const int n0 = (tile % n_tiles) * BLOCK_N;
-                if (!tile_active(n0)) continue;
-                const int acc = tile_iter & 1;
-                long long tq = clock64();
-                // the epilogue must have drained this accumulator stage (two tiles ago)
-                if (!ptx::mbar_wait(bar_tmem_empty + 8 * acc, ((tile_iter >> 1) & 1) ^ 1, P.abort_flag, 106)) { dead = true; break; }
-                t_acc += clock64() - tq;
-                ptx::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-                for (int a = 0; a < num_a && !dead; ++a, ++ita) {
-                    const int sa = ita % SA;
-                    tq = clock64();
-                    if (!ptx::mbar_wait(bar_full_a + 8 * sa, (ita / SA) & 1, P.abort_flag, 104)) { dead = true; break; }
-                    t_a += clock64() - tq;
-                    if (kProxyFence) ptx::fence_proxy_async_smem();
-                    for (int tc = 0; tc < nB; ++tc, ++itb) {
-                        const int sb = itb % SB;
-                        tq = clock64();
-                        if (!ptx::mbar_wait(bar_full_b + 8 * sb, (itb / SB) & 1, P.abort_flag, 105)) { dead = true; break; }
-                        const long long tw = clock64();
-                        t_b += tw - tq;
-                        ptx::tc_fence_after();
-                        const uint64_t db = ptx::make_smem_desc(sB + sb * B_STAGE_BYTES, 16, 1024);
-                        if (HALO) {
-                            const int shift = ((MODE == 0) ? tc : (P.kw - 1 - tc)) * P.dil;    // slots
-                            const uint32_t a0 = sA + sa * A_STAGE + shift * 16;
-#pragma unroll
-                            for (int k = 0; k < BLOCK_K / 16; ++k) {                            // 2 chunks (16 channels) per MMA
-                                const uint64_t da = ptx::make_smem_desc_noswizzle(a0 + k * 2 * LBO, LBO, HG * 16);
-                                ptx::umma_bf16(d_tmem, da, db + 2 * k, idesc, (a | tc | k) != 0);
-                            }
-                        } else {
-                            const uint64_t da = ptx::make_smem_desc(sA + sa * A_STAGE, 16, 1024);
-#pragma unroll
-                            for (int k = 0; k < BLOCK_K / 16; ++k)                              // +32 bytes per K=16 step inside the swizzle row
-                                ptx::umma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (a | k) != 0);
-                        }
-                        ptx::umma_commit(bar_empty_b + 8 * sb);
-                        t_issue += clock64() - tw;
-                    }
-                    ptx::umma_commit(bar_empty_a + 8 * sa);
-                }
-                if (!dead) ptx::umma_commit(bar_tmem_full + 8 * acc);
-                ++tile_iter;
-            }
-            if (P.dbg) {
-                long long *d = P.dbg + 8 * blockIdx.x;
-                d[0] = clock64() - t_begin; d[1] = t_acc; d[2] = t_a; d[3] = t_b; d[4] = t_issue; d[5] = tile_iter; d[6] = ita; d[7] = itb;
-            }
-        }
     } else {
-        // ================================ epilogue warps (6-9) ================================
-        int tile_iter = 0;
-        // fused BatchNorm statistics: this warp's private per-column accumulators in shared memory, flushed to the global fp64
-        // sums whenever the CTA moves to another N tile, and at the end
+        // ================================ consumer warpgroups (warps 4-11) ================================
+        const int e = warp - 4, g = e >> 2;
+        const bool leader = (threadIdx.x & 127) == 0;
+        int num_a = 0;
+        if (HALO) {
+            for (int p = 0; p < np; ++p) num_a += ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
+            num_a *= P.kh;
+        } else {
+            num_a = (MODE == 0) ? (P.rowpack ? P.kh : taps * (P.ktap / BLOCK_K)) : taps * (P.dc_kext / BLOCK_K);
+        }
+        // this warpgroup's 64 rows: 8 groups of 8 rows further into the A stage
+        const uint32_t a_rows = HALO ? 8u * HG * 16u : 64u * 128u;
         float *s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
-                            ? reinterpret_cast<float *>(smem_raw + (((s_tmem_ptr + 32u) & ~15u) - ptx::smem_u32(smem_raw))) + (warp & 3) * STAT_FLOATS_PER_WARP : nullptr;
+                            ? reinterpret_cast<float *>(smem_raw + (s_stat_addr - ptx::smem_u32(smem_raw))) : nullptr;
+        const EpiRole<BLOCK_N> R(e);
+        float *my_stat = s_stat ? s_stat + R.slice() * STAT_SLICE : nullptr;
         int stat_n0 = -1;
-        if (s_stat) {
-            for (int i = lane; i < STAT_FLOATS_PER_WARP; i += 32) s_stat[i] = 0.f;
+        if (my_stat) {
+            for (int i = lane; i < STAT_SLICE; i += 32) my_stat[i] = 0.f;
             __syncwarp();
         }
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int ita = 0, itb = 0;
+        bool dead = false;
+        for (int tile = blockIdx.x; tile < num_tiles && !dead; tile += gridDim.x) {
             const int m0 = (tile / n_tiles) * BLOCK_M, n0 = (tile % n_tiles) * BLOCK_N;
             if (!tile_active(n0)) continue;
-            const int acc = tile_iter & 1;
-            if (s_stat && n0 != stat_n0) {
-                if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0);
+            if (my_stat && n0 != stat_n0) {
+                if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, my_stat, lane, stat_n0, R.cb, R.ce, 128);
                 stat_n0 = n0;
             }
-            if (!ptx::mbar_wait(bar_tmem_full + 8 * acc, (tile_iter >> 1) & 1, P.abort_flag, 102)) { stat_n0 = -1; break; }
-            tc_epilogue<BLOCK_N, MODE>(P, tmem_base + acc * BLOCK_N, warp & 3, lane, m0, n0, s_stat);
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(bar_tmem_empty + 8 * acc);
-            ++tile_iter;
+            float acc[BLOCK_N / 2];
+            zero_acc(acc);
+            for (int a = 0; a < num_a && !dead; ++a, ++ita) {
+                const int sa = ita % SA;
+                if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full_a + 8 * sa, (ita / SA) & 1, P.abort_flag, 104))) { dead = true; break; }
+                ptx::fence_proxy_async_smem();                   // cp.async (generic proxy) data -> wgmma (async proxy)
+                const int sb0 = itb % SB;
+                for (int tc = 0; tc < nB; ++tc, ++itb) {
+                    const int sb = itb % SB;
+                    if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full_b + 8 * sb, (itb / SB) & 1, P.abort_flag, 105))) { dead = true; break; }
+                    const uint64_t db = ptx::make_smem_desc(sB + sb * B_STAGE_BYTES, 16, 1024);
+                    ptx::wgmma_fence();
+                    if (HALO) {
+                        const int shift = ((MODE == 0) ? tc : (P.kw - 1 - tc)) * P.dil;    // slots
+                        const uint32_t a0 = sA + sa * A_STAGE + g * a_rows + shift * 16;
+#pragma unroll
+                        for (int k = 0; k < BLOCK_K / 16; ++k)                              // 2 chunks (16 channels) per MMA
+                            ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, ptx::make_smem_desc_noswizzle(a0 + k * 2 * LBO, LBO, HG * 16), db + 2 * k);
+                    } else {
+                        const uint64_t da = ptx::make_smem_desc(sA + sa * A_STAGE + g * a_rows, 16, 1024);
+#pragma unroll
+                        for (int k = 0; k < BLOCK_K / 16; ++k)                              // +32 bytes per K=16 step inside the swizzle row
+                            ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + 2 * k, db + 2 * k);
+                    }
+                    ptx::wgmma_commit();
+                }
+                // the A item and its weight tiles are released once this warpgroup's MMAs on them completed
+                ptx::wgmma_wait<0>();
+                ptx::wgmma_fence_regs(acc);
+                if (leader) {
+                    for (int tc = 0; tc < nB; ++tc) ptx::mbar_arrive(bar_empty_b + 8 * ((sb0 + tc) % SB));
+                    ptx::mbar_arrive(bar_empty_a + 8 * sa);
+                }
+            }
+            if (dead) { stat_n0 = -1; break; }
+            mma_epilogue<BLOCK_N, MODE>(P, acc, acc_stage, e, lane, m0, n0, my_stat);
         }
-        if (s_stat && stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0);
-    }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 5) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<2 * BLOCK_N>(tmem_base);
+        if (my_stat && stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, my_stat, lane, stat_n0, R.cb, R.ce, 128);
     }
 }
 
@@ -713,39 +730,29 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
 // of two here), so the A operand of tap (tr, tc) / channel block cb is ONE 4-D TMA tile {64 ch, box_w, box_h, box_n} of
 // the NHWC source at coordinates shifted by the tap -- negative / past-the-edge coordinates are zero-filled by the TMA
 // unit (the convolution padding), stride-2 layers use the tensor map's traversal stride, channel padding is the map's
-// channel extent.  TMA writes exactly the 128B-swizzled K-major image UMMA reads.  What TMA cannot know are the HOLES
+// channel extent.  TMA writes exactly the 128B-swizzled K-major image wgmma reads.  What TMA cannot know are the HOLES
 // (x*mask, models/partial_convolution.py:51): four "fixer" warps (one thread per tile row) test the row's tap-validity
 // bit and overwrite hole rows of the landed tile with zeros before handing the stage to the MMA thread
 // (generic-proxy stores -> fence.proxy.async -> mbarrier).  Plain convolutions / dgrad skip the fixers.
 //
-//   warp 0  TMA producer : per K block one A tile (4-D) + one weight tile (2-D) onto the same mbarrier
-//   warp 1  MMA issuer   : 4 x tcgen05.mma (K=16) per K block into one of two TMEM accumulator stages
-//   warps 2-5 fixers     : hole rows -> 0   (MODE 0 with masks only)
-//   warps 6-9 epilogue   : TMEM -> renormalise / mask -> bf16 NHWC
-// Every per-K-block loop is a handful of instructions: a lone thread executes dependent instructions at ~5 cycles each,
-// so index arithmetic in these loops (the old kernels did integer divisions there) directly throttles the tensor pipe.
+//   warps 0-7  consumers  : two warpgroups, 4 x wgmma (K=16) per K block and weight tile, then the epilogue of their 64 rows
+//   warp 8     TMA producer : per K block one A tile (4-D) + the weight tiles (2-D) onto the same mbarrier
+//   warps 9-12 fixers     : hole rows -> 0   (MODE 0 with masks only)
+// Every per-K-block loop of the producer is a handful of instructions: index arithmetic there (the old kernels did integer
+// divisions) directly delays the stages the tensor cores wait for.
 // -------------------------------------------------------------------------------------------------
-constexpr int TMA_THREADS = 320;
+constexpr int TMA_THREADS = MMA_THREADS + 5 * 32;
 
 // HALO = true (stride 1, tiles that are one image-row segment of 128 pixels): per kernel ROW one A tile of
-// 128 + (kw-1)*dil pixel rows is loaded, and the kw taps of that row are kw UMMA descriptors whose start address is
+// 128 + (kw-1)*dil pixel rows is loaded, and the kw taps of that row are kw wgmma descriptors whose start address is
 // shifted by whole 128-byte rows (the 128B swizzle is a function of the absolute smem address, so a row-shifted start
-// reads the same image: probed in tools/ubench/tma_probe.cu) -- kw x less A traffic from L2 and kw x fewer barrier
-// round trips per MMA.  K steps that only cover channel padding (c8 <= 16*k) are skipped.
-// PAIR: two CTAs of a cluster work on two adjacent M tiles with cta_group::2 MMAs (M = 256) issued by the leader (rank 0); each
-// CTA stages its own A tile and HALF of every weight tile.  The peer's MMA warp only relays "my stage is ready" to the leader.
-// EIGHT epilogue warps (6..13): TMEM lane quadrant q = warp & 3 is drained by two warps, each taking half of the tile's columns.
-// With four, a 128 x 256 tile took ~9.6 k cycles to drain (tcgen05.ld, renormalise, bf16, 16-byte stores, statistics butterfly) --
-// longer than the main loop of every K <= 512 problem (the pointwise convolutions of the segmentation nets: the MMA thread waited
-// 500..1700 cycles per K block for a free accumulator, profiles/r02_tc_timing.txt).
-constexpr int TMA_EPI_WARPS = 8;
-constexpr int TMA_THREADS8 = (6 + TMA_EPI_WARPS) * 32;
-template <int BLOCK_N, int MODE, bool HALO, bool PAIR>
-__global__ void __launch_bounds__(TMA_THREADS8, 1)
+// reads the same image) -- kw x less A traffic from L2 and kw x fewer barrier round trips per MMA.  K steps that only cover
+// channel padding (c8 <= 16*k) are skipped.
+template <int BLOCK_N, int MODE, bool HALO>
+__global__ void __launch_bounds__(TMA_THREADS, 1)
 pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1) {
-    constexpr uint32_t B_BYTES = (PAIR ? BLOCK_N / 2 : BLOCK_N) * 128;   // this CTA's share of one weight tile
-    constexpr int TCOLS = (2 * BLOCK_N < 32) ? 32 : 2 * BLOCK_N;
+    constexpr uint32_t B_BYTES = BLOCK_N * 128;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = align1024(ptx::smem_u32(smem_raw));
     const int S = P.stages;
@@ -757,22 +764,18 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
     const uint32_t STAGE_TX = A_BYTES + nB * B_BYTES;
     const uint32_t sBar = smem_base + S * STAGE;
     const uint32_t bar_full = sBar, bar_fixed = sBar + 8 * MAX_RING, bar_empty = sBar + 16 * MAX_RING;
-    const uint32_t bar_peer = sBar + 24 * MAX_RING;                     // PAIR, leader only: the peer's stage s is ready
-    const uint32_t bar_tmem_full = sBar + 32 * MAX_RING, bar_tmem_empty = bar_tmem_full + 16;
-    const uint32_t s_tmem_ptr = bar_tmem_empty + 16;
+    const uint32_t s_stat_addr = sBar + 24 * MAX_RING;
+    const uint32_t s_acc = (s_stat_addr + STAT_SMEM_BYTES + 15u) & ~15u;
     uint8_t *smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
-    uint32_t *tmem_ptr_generic = reinterpret_cast<uint32_t *>(smem_gen + (s_tmem_ptr - smem_base));
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform by construction
     const int np = (MODE == 0) ? P.nparts : 1;
     const int n_tiles = P.ncols / BLOCK_N;
-    const int KS = PAIR ? 1 : P.ksplit;                                 // tile index = (m tile * n_tiles + n tile) * KS + split
-    const uint32_t rank = PAIR ? ptx::cluster_ctarank() : 0u;
+    const int KS = P.ksplit;                                            // tile index = (m tile * n_tiles + n tile) * KS + split
     const int m_tiles = (P.m_total + BLOCK_M - 1) / BLOCK_M;
-    const int num_tiles = (PAIR ? (m_tiles + 1) / 2 : m_tiles) * n_tiles * KS;      // PAIR: a tile is a pair of adjacent M tiles
-    const int tile0 = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-    const int tstep = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-    auto m0_of = [&](int mt) -> int { return (PAIR ? mt * 2 + static_cast<int>(rank) : mt) * BLOCK_M; };
+    const int num_tiles = m_tiles * n_tiles * KS;
+    const int tile0 = static_cast<int>(blockIdx.x), tstep = static_cast<int>(gridDim.x);
+    auto m0_of = [&](int mt) -> int { return mt * BLOCK_M; };
     const bool fix = (MODE == 0) && P.use_fix;
     const int kwi = HALO ? 1 : P.kw;                                   // A items per kernel row
 
@@ -784,36 +787,19 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
     };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < MAX_RING; ++s) {
-            ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, PAIR ? 8 : 4); ptx::mbar_init(bar_empty + 8 * s, 1);
-            ptx::mbar_init(bar_peer + 8 * s, 1);
-        }
-        // PAIR: the leader's accumulator-drained barrier collects the epilogue threads of both CTAs
-        for (int s = 0; s < 2; ++s) {
-            ptx::mbar_init(bar_tmem_full + 8 * s, 1);
-            ptx::mbar_init(bar_tmem_empty + 8 * s, (PAIR ? 2 : 1) * TMA_EPI_WARPS * 32);
+        for (int s = 0; s < MAX_RING; ++s) {      // empty: one arrival per consumer warpgroup
+            ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 2);
         }
         ptx::fence_mbar_init();
     }
-    if (warp == 0 && lane == 0) { ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_a0); if (np > 1) ptx::prefetch_tmap(&tmap_a1); }
-    if (warp == 1) {
-        if (PAIR) { ptx::tmem_alloc_pair<TCOLS>(s_tmem_ptr); ptx::tmem_relinquish_pair(); }
-        else { ptx::tmem_alloc<TCOLS>(s_tmem_ptr); ptx::tmem_relinquish(); }
-    }
-    ptx::tc_fence_before();
+    if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_a0); if (np > 1) ptx::prefetch_tmap(&tmap_a1); }
     __syncthreads();
-    if (PAIR) ptx::cluster_sync();                                     // barriers of both CTAs initialised before any remote arrive
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_generic;
 
-    // The two issuing roles run WARP-CONVERGED (all 32 lanes walk the loops and wait on the barriers; the warp index is a
-    // shuffle broadcast so the compiler knows the role branch is uniform) and only the TMA / MMA / commit instructions sit
-    // inside an elect.sync region.  Written as `if (lane == 0) { whole loop }` the compiler treats every such instruction as
-    // possibly divergent, wraps each in an ELECT/branch loop and keeps its operands in vector registers (R2UR per use):
-    // ~8 dependent uniform-datapath instructions = ~60 cycles per tcgen05.mma, more than the N<=128 MMA itself takes.
-    float *s_stat = nullptr;                                          // epilogue warps: private BatchNorm-statistics accumulators
+    // The producer runs WARP-CONVERGED (all 32 lanes walk the loops and wait on the barriers; the warp index is a shuffle
+    // broadcast so the compiler knows the role branch is uniform) and only the TMA instructions sit inside an elect.sync region.
+    float *s_stat = nullptr;                                          // consumer warps: private BatchNorm-statistics accumulators
     int stat_n0 = -1;                                                  // N tile they currently belong to (-1: none / aborted)
-    if (warp == 0) {
+    if (warp == 8) {
         // ================================ TMA producer ================================
         int s = 0;
         uint32_t ph = 1;                                               // first pass over the ring: stages are free
@@ -823,10 +809,6 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
         const int dstep = (MODE == 0) ? P.dil : -P.dil;
         const int row_k = P.wk_row, col_k = P.wk_col;
         bool dead = false;
-#ifdef PCB_TC_TIMING
-        long long tt_wait = 0, tt_issue = 0;
-        const long long tt0 = clock64();
-#endif
         for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
             const int sp = tile % KS, mn = tile / KS;
             const int m0 = m0_of(mn / n_tiles), n0 = (mn % n_tiles) * BLOCK_N;
@@ -859,43 +841,29 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                         const int gb0 = (p == 0) ? 0 : kext0 / BLOCK_K;          // global K-block index of the part's first block
                         for (int c0 = 0; c0 < kext; c0 += BLOCK_K, kidx += BLOCK_K) {
                             if (KS > 1 && (gb0 + c0 / BLOCK_K) % KS != sp) continue;
-#ifdef PCB_TC_TIMING
-                            const long long tq0 = clock64();
-#endif
                             if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 121))) { dead = true; break; }
-#ifdef PCB_TC_TIMING
-                            const long long tq1 = clock64();
-                            tt_wait += tq1 - tq0;
-#endif
                             if (ptx::elect_one()) {
                                 const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
                                 ptx::mbar_arrive_expect_tx(full, STAGE_TX);
                                 ptx::tma_load_4d(dst, ma, c0, x, y, img, full);
                                 uint32_t bdst = dst + A_ROOM;
                                 for (int tc = 0, kb = kidx; tc < nB; ++tc, kb += col_k, bdst += B_BYTES)
-                                    ptx::tma_load_2d(bdst, &tmap_w, kb, n0 + (PAIR ? static_cast<int>(rank) * (BLOCK_N / 2) : 0), full);
+                                    ptx::tma_load_2d(bdst, &tmap_w, kb, n0, full);
                                 if (nimg >= 0) ptx::tma_prefetch_4d(ma, c0, nx_org + ti * dstep, ny_org + tr * dstep, nimg);
                             }
                             __syncwarp();
-#ifdef PCB_TC_TIMING
-                            tt_issue += clock64() - tq1;
-#endif
                             if (++s == S) { s = 0; ph ^= 1; }
                         }
                         if (dead) break;
                     }
                 }
         }
-#ifdef PCB_TC_TIMING
-        if (P.dbg && lane == 0) { long long *d = P.dbg + 8 * blockIdx.x; d[2] = tt_wait; d[3] = tt_issue; d[4] = clock64() - tt0; }
-#endif
-    } else if (warp == 1) {
-        // ================================ MMA issuer ================================
-        constexpr uint32_t idesc = ptx::make_idesc_bf16(PAIR ? 2 * BLOCK_M : BLOCK_M, BLOCK_N, 0, 0);
-        // PAIR: stage s is ready when the four fixer warps of BOTH CTAs arrived on the leader's bar_fixed (they run as plain
-        // relays when there are no holes to fix), so no extra hop sits between the peer's TMA landing and the leader's MMA
-        const uint32_t ready = (fix || PAIR) ? bar_fixed : bar_full;
-        const uint64_t desc_a0 = ptx::make_smem_desc(smem_base, 16, 1024);
+    } else if (warp < MMA_WARPS) {
+        // ================================ consumer warpgroups ================================
+        const int e = warp, g = warp >> 2;
+        const bool leader = (threadIdx.x & 127) == 0;
+        const uint32_t ready = fix ? bar_fixed : bar_full;
+        const uint64_t desc_a0 = ptx::make_smem_desc(smem_base + g * 64 * 128, 16, 1024);     // this warpgroup's 64 rows
         const uint64_t desc_b0 = ptx::make_smem_desc(smem_base + A_ROOM, 16, 1024);
         const uint32_t stage16 = STAGE >> 4;
         // dgrad walks tap columns right to left inside a halo tile
@@ -909,29 +877,28 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
             nb0 = kext / BLOCK_K; kl0 = min(4, (c8 - (nb0 - 1) * BLOCK_K + 15) >> 4);
             if (MODE == 0 && np > 1) { nb1 = P.parts[1].kext / BLOCK_K; kl1 = min(4, (P.parts[1].c8 - (nb1 - 1) * BLOCK_K + 15) >> 4); }
         }
-        int s = 0, tile_iter = 0;
+        const EpiRole<BLOCK_N> R(e);
+        s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
+                     ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + R.slice() * STAT_SLICE : nullptr;
+        if (s_stat) {
+            for (int i = lane; i < STAT_SLICE; i += 32) s_stat[i] = 0.f;
+            __syncwarp();
+        }
+        float *acc_stage = reinterpret_cast<float *>(smem_gen + (s_acc - smem_base));
+        int s = 0;
         uint32_t ph = 0;
         bool dead = false;
-        long long n_items = 0;
-        long long tm_wait = 0, tm_acc = 0, tm_issue = 0, tm_commit = 0;
-        const long long t_begin = clock64();
-        for (int tile = tile0; tile < num_tiles && !dead && !(PAIR && rank == 1); tile += tstep) {
-            const int sp = tile % KS;
-            const int n0 = ((tile / KS) % n_tiles) * BLOCK_N;
+        for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
+            const int sp = tile % KS, mn = tile / KS;
+            const int m0 = m0_of(mn / n_tiles), n0 = (mn % n_tiles) * BLOCK_N;
             if (!tile_active(n0)) continue;
-            const int acc = tile_iter & 1;
-#ifdef PCB_TC_TIMING
-            const long long ta0 = clock64();
-#endif
-            // the epilogue must have drained this accumulator stage (two tiles ago); PAIR: the peer only relays
-            if (!(PAIR && rank == 1))
-                if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_tmem_empty + 8 * acc, ((tile_iter >> 1) & 1) ^ 1, P.abort_flag, 126))) { dead = true; break; }
-#ifdef PCB_TC_TIMING
-            tm_acc += clock64() - ta0;
-#endif
-            ptx::tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-            uint32_t accum = 0;
+            if (s_stat && n0 != stat_n0) {
+                if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, R.cb, R.ce, 128);
+                stat_n0 = n0;
+            }
+            float acc[BLOCK_N / 2];
+            zero_acc(acc);
+            int held = -1;                                             // stage whose MMAs may still be reading it
             for (int r = 0; r < rows_a && !dead; ++r) {
 #pragma unroll
                 for (int p = 0; p < TC_MAX_PARTS; ++p) {
@@ -939,68 +906,38 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                     const int gb0 = (p == 0) ? 0 : nb0;
                     for (int cb = 0; cb < nbp; ++cb) {
                         if (KS > 1 && (gb0 + cb) % KS != sp) continue;
-#ifdef PCB_TC_TIMING
-                        const long long tq0 = clock64();
-#endif
                         if (!__all_sync(0xffffffffu, ptx::mbar_wait(ready + 8 * s, ph, P.abort_flag, 124))) { dead = true; break; }
-#ifdef PCB_TC_TIMING
-                        const long long tq1 = clock64();
-                        tm_wait += tq1 - tq0;
-#endif
-                        ptx::tc_fence_after();
-                        if (ptx::elect_one()) {
-                            uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16 + shift0), db = desc_b0 + static_cast<uint64_t>(s * stage16);
-                            if (cb + 1 < nbp || klast == 4) {
-                                for (int tc = 0; tc < nB; ++tc, da += dshift, db += B_BYTES >> 4) {
-                                    if (PAIR) {
-                                        ptx::umma_bf16_pair(d_tmem, da, db, idesc, (accum | tc) != 0);
-                                        ptx::umma_bf16_pair_acc(d_tmem, da + 2, db + 2, idesc);
-                                        ptx::umma_bf16_pair_acc(d_tmem, da + 4, db + 4, idesc);
-                                        ptx::umma_bf16_pair_acc(d_tmem, da + 6, db + 6, idesc);
-                                    } else {
-                                        ptx::umma_bf16(d_tmem, da, db, idesc, (accum | tc) != 0);
-                                        ptx::umma_bf16_acc(d_tmem, da + 2, db + 2, idesc);
-                                        ptx::umma_bf16_acc(d_tmem, da + 4, db + 4, idesc);
-                                        ptx::umma_bf16_acc(d_tmem, da + 6, db + 6, idesc);
-                                    }
-                                }
+                        uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16 + shift0), db = desc_b0 + static_cast<uint64_t>(s * stage16);
+                        const int ksteps = (cb + 1 < nbp) ? 4 : klast;
+                        ptx::wgmma_fence();
+                        for (int tc = 0; tc < nB; ++tc, da += dshift, db += B_BYTES >> 4) {
+                            if (ksteps == 4) {
+#pragma unroll
+                                for (int k = 0; k < 4; ++k) ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + 2 * k, db + 2 * k);
                             } else {
-                                for (int tc = 0; tc < nB; ++tc, da += dshift, db += B_BYTES >> 4)
-                                    for (int k = 0; k < klast; ++k) {
-                                        if (PAIR) ptx::umma_bf16_pair(d_tmem, da + 2 * k, db + 2 * k, idesc, (accum | tc | k) != 0);
-                                        else ptx::umma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (accum | tc | k) != 0);
-                                    }
+                                for (int k = 0; k < ksteps; ++k) ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + 2 * k, db + 2 * k);
                             }
-                            if (PAIR) ptx::umma_commit_pair(bar_empty + 8 * s);
-                            else ptx::umma_commit(bar_empty + 8 * s);
                         }
-                        __syncwarp();
-#ifdef PCB_TC_TIMING
-                        tm_issue += clock64() - tq1;
-#endif
-                        accum = 1;
+                        ptx::wgmma_commit();
+                        // keep one K block in flight: the previous stage is released once its MMAs completed
+                        ptx::wgmma_wait<1>();
+                        if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+                        held = s;
                         if (++s == S) { s = 0; ph ^= 1; }
-                        ++n_items;
                     }
                     if (dead) break;
                 }
             }
-            if (!dead && !(PAIR && rank == 1) && ptx::elect_one()) {
-                if (PAIR) ptx::umma_commit_pair(bar_tmem_full + 8 * acc);
-                else ptx::umma_commit(bar_tmem_full + 8 * acc);
-            }
-            __syncwarp();
-            ++tile_iter;
+            ptx::wgmma_wait<0>();
+            ptx::wgmma_fence_regs(acc);
+            if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+            if (dead) { stat_n0 = -1; break; }
+            mma_epilogue<BLOCK_N, MODE>(P, acc, acc_stage, e, lane, m0, n0, s_stat);
         }
-        if (P.dbg && lane == 0) {
-            long long *d = P.dbg + 8 * blockIdx.x;
-            d[0] = clock64() - t_begin; d[1] = tm_wait; d[5] = tile_iter; d[6] = n_items; d[7] = tm_acc; P.dbg[8 * 1024 + 2 * blockIdx.x] = tm_issue; P.dbg[8 * 1024 + 2 * blockIdx.x + 1] = tm_commit;
-        }
-    } else if (warp < 6) {
+    } else if (warp > 8) {
         // ================================ fixers: zero the hole rows of every landed A tile ================================
-        if (fix || PAIR) {
-            const int t = (warp - 2) * 32 + lane;
-            const uint32_t fixed_remote = PAIR ? ptx::mapa(bar_fixed, 0) : 0u;    // the leader's barriers
+        if (fix) {
+            const int t = (warp - 9) * 32 + lane;
             int s = 0;
             uint32_t ph = 0;
             bool dead = false;
@@ -1045,10 +982,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                                     ptx::fence_proxy_async_smem();
                                 }
                                 __syncwarp();
-                                if (lane == 0) {
-                                    if (PAIR && rank == 1) ptx::mbar_arrive_cluster(fixed_remote + 8 * s);
-                                    else ptx::mbar_arrive(bar_fixed + 8 * s);
-                                }
+                                if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
                                 if (++s == S) { s = 0; ph ^= 1; }
                             }
                             if (dead) break;
@@ -1062,7 +996,6 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                     b0 = b1 = 0;
                     if (!fix || tl >= num_tiles) return;
                     const int m0 = m0_of(tl / KS / n_tiles);
-                    if (m0 >= P.m_total) return;                   // PAIR: the peer's half of the last (odd) tile pair is empty
                     const int img = m0 / plane, rem = m0 - img * plane;
                     const int oy = rem / P.wo, ox = rem - oy * P.wo;
 #pragma unroll
@@ -1112,10 +1045,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                                     ptx::fence_proxy_async_smem();
                                 }
                                 __syncwarp();
-                                if (lane == 0) {
-                                    if (PAIR && rank == 1) ptx::mbar_arrive_cluster(fixed_remote + 8 * s);
-                                    else ptx::mbar_arrive(bar_fixed + 8 * s);
-                                }
+                                if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
                                 if (++s == S) { s = 0; ph ^= 1; }
                             }
                             if (dead) break;
@@ -1124,63 +1054,10 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                 }
             }
         }
-    } else {
-        // ================================ epilogue warps (6-13) ================================
-        int tile_iter = 0;
-        // this warp's half of the tile's columns (a 32-column tile is not split: the second warp of the quadrant only arrives)
-        constexpr int HN = (BLOCK_N >= 64) ? BLOCK_N / 2 : BLOCK_N;
-        const int half = (warp - 6) >> 2;
-        const int cb = half * HN, ce = (cb + HN <= BLOCK_N) ? cb + HN : cb;
-        // fused BatchNorm statistics (see pconv_tc_persistent_kernel): eight private slices of [128 sums | 128 squares]
-        s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
-                     ? reinterpret_cast<float *>(smem_gen + (((s_tmem_ptr + 32u) & ~15u) - smem_base)) + (half * 4 + (warp & 3)) * 256 : nullptr;
-        if (s_stat) {
-            for (int i = lane; i < 256; i += 32) s_stat[i] = 0.f;
-            __syncwarp();
-        }
-        for (int tile = tile0; tile < num_tiles; tile += tstep) {
-            const int mn = tile / KS;
-            const int m0 = m0_of(mn / n_tiles), n0 = (mn % n_tiles) * BLOCK_N;
-            if (!tile_active(n0)) continue;
-            const int acc = tile_iter & 1;
-            if (s_stat && n0 != stat_n0) {
-                if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, cb, ce, 128);
-                stat_n0 = n0;
-            }
-            if (!ptx::mbar_wait(bar_tmem_full + 8 * acc, (tile_iter >> 1) & 1, P.abort_flag, 123)) { stat_n0 = -1; break; }
-            tc_epilogue<BLOCK_N, MODE>(P, tmem_base + acc * BLOCK_N, warp & 3, lane, m0, n0, s_stat, cb, ce, 128);
-            ptx::tc_fence_before();
-            if (PAIR && rank == 1) ptx::mbar_arrive_cluster(ptx::mapa(bar_tmem_empty + 8 * acc, 0));   // the leader waits for both epilogues
-            else ptx::mbar_arrive(bar_tmem_empty + 8 * acc);
-            ++tile_iter;
-        }
     }
 
-    ptx::tc_fence_before();
     __syncthreads();
-    // last N tile's BatchNorm statistics: the four epilogue warps' partials are summed here, after the CTA-wide barrier, so the
-    // global sums receive ONE atomic per channel per CTA (148 per address instead of 592)
-    if (s_stat != nullptr && stat_n0 >= 0) {
-        constexpr int HN = (BLOCK_N >= 64) ? BLOCK_N / 2 : BLOCK_N;
-        const float *base = s_stat - (((warp - 6) >> 2) * 4 + (warp & 3)) * 256;
-        for (int col = (warp - 6) * 32 + lane; col < BLOCK_N; col += TMA_EPI_WARPS * 32) {
-            const int co = stat_n0 + col;
-            if (co < P.bn_c) {
-                const int h = col / HN, lc = col - h * HN;
-                float a = 0.f, q = 0.f;
-#pragma unroll
-                for (int w4 = 0; w4 < 4; ++w4) { a += base[(h * 4 + w4) * 256 + lc]; q += base[(h * 4 + w4) * 256 + 128 + lc]; }
-                atomicAdd(P.bn_sums + co, static_cast<double>(a));
-                atomicAdd(P.bn_sums + P.bn_c + co, static_cast<double>(q));
-            }
-        }
-    }
-    if (PAIR) ptx::cluster_sync();                                     // no CTA leaves while its partner may still touch its smem / TMEM
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        if (PAIR) ptx::tmem_dealloc_pair<TCOLS>(tmem_base);
-        else ptx::tmem_dealloc<TCOLS>(tmem_base);
-    }
+    if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - EpiRole<BLOCK_N>(warp).slice() * STAT_SLICE, warp, lane, stat_n0);
 }
 
 
@@ -1199,7 +1076,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
 // The same kernel computes the data gradient w.r.t. x0 directly at SOURCE resolution (MODE 1): its A operand is dc read with a
 // traversal stride of 2 per (class, effective tap) item -- 16/36 of the multiplications of "full-resolution gradient + 2x2 sum",
 // and neither the full-resolution gradient nor the reduction pass exists.
-// Roles / pipeline / epilogue exactly as in pconv_tc_tma_kernel (no CTA pairs, no split-K).
+// Roles / pipeline / epilogue exactly as in pconv_tc_tma_kernel (no split-K).
 // -------------------------------------------------------------------------------------------------
 constexpr int SP_MAX_ITEMS = 40;
 struct SpItem { int part, dx, dy, wk, nb, wk_step, shift0, dshift; };
@@ -1218,7 +1095,6 @@ __global__ void __launch_bounds__(TMA_THREADS, 1)
 pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ SpTable TB, const __grid_constant__ CUtensorMap tmap_w,
                    const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1) {
     constexpr uint32_t B_BYTES = BLOCK_N * 128;
-    constexpr int TCOLS = (2 * BLOCK_N < 32) ? 32 : 2 * BLOCK_N;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = align1024(ptx::smem_u32(smem_raw));
     const int S = P.stages;
@@ -1228,10 +1104,9 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
     const uint32_t STAGE = A_ROOM + nb_max * B_BYTES;
     const uint32_t sBar = smem_base + S * STAGE;
     const uint32_t bar_full = sBar, bar_fixed = sBar + 8 * MAX_RING, bar_empty = sBar + 16 * MAX_RING;
-    const uint32_t bar_tmem_full = sBar + 32 * MAX_RING, bar_tmem_empty = bar_tmem_full + 16;
-    const uint32_t s_tmem_ptr = bar_tmem_empty + 16;
+    const uint32_t s_stat_addr = sBar + 24 * MAX_RING;
+    const uint32_t s_acc = (s_stat_addr + STAT_SMEM_BYTES + 15u) & ~15u;
     uint8_t *smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
-    uint32_t *tmem_ptr_generic = reinterpret_cast<uint32_t *>(smem_gen + (s_tmem_ptr - smem_base));
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     const int n_tiles = P.ncols / BLOCK_N;
@@ -1252,20 +1127,15 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
     }
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 1); }
-        for (int s = 0; s < 2; ++s) { ptx::mbar_init(bar_tmem_full + 8 * s, 1); ptx::mbar_init(bar_tmem_empty + 8 * s, 128); }
+        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 2); }
         ptx::fence_mbar_init();
     }
-    if (warp == 0 && lane == 0) { ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_a0); ptx::prefetch_tmap(&tmap_a1); }
-    if (warp == 1) { ptx::tmem_alloc<TCOLS>(s_tmem_ptr); ptx::tmem_relinquish(); }
-    ptx::tc_fence_before();
+    if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_a0); ptx::prefetch_tmap(&tmap_a1); }
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_generic;
 
     float *s_stat = nullptr;
     int stat_n0 = -1;
-    if (warp == 0) {
+    if (warp == 8) {
         // ================================ TMA producer ================================
         int s = 0;
         uint32_t ph = 1;
@@ -1294,48 +1164,59 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================================ MMA issuer ================================
-        constexpr uint32_t idesc = ptx::make_idesc_bf16(BLOCK_M, BLOCK_N, 0, 0);
+    } else if (warp < MMA_WARPS) {
+        // ================================ consumer warpgroups ================================
+        const int e = warp, g = warp >> 2;
+        const bool leader = (threadIdx.x & 127) == 0;
         const uint32_t ready = fix ? bar_fixed : bar_full;
-        const uint64_t desc_a0 = ptx::make_smem_desc(smem_base, 16, 1024);
+        const uint64_t desc_a0 = ptx::make_smem_desc(smem_base + g * 64 * 128, 16, 1024);     // this warpgroup's 64 rows
         const uint64_t desc_b0 = ptx::make_smem_desc(smem_base + A_ROOM, 16, 1024);
         const uint32_t stage16 = STAGE >> 4;
-        int s = 0, tile_iter = 0;
+        const EpiRole<BLOCK_N> R(e);
+        s_stat = (MODE == 0 && P.bn_sums != nullptr) ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + R.slice() * STAT_SLICE : nullptr;
+        if (s_stat) {
+            for (int i = lane; i < STAT_SLICE; i += 32) s_stat[i] = 0.f;
+            __syncwarp();
+        }
+        float *acc_stage = reinterpret_cast<float *>(smem_gen + (s_acc - smem_base));
+        int s = 0;
         uint32_t ph = 0;
         bool dead = false;
         for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-            const int acc = tile_iter & 1;
-            if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_tmem_empty + 8 * acc, ((tile_iter >> 1) & 1) ^ 1, P.abort_flag, 326))) { dead = true; break; }
-            ptx::tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-            uint32_t accum = 0;
+            const int m0 = (tile / n_tiles) * BLOCK_M, n0 = (tile % n_tiles) * BLOCK_N;
+            if (s_stat && n0 != stat_n0) {
+                if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, R.cb, R.ce, 128);
+                stat_n0 = n0;
+            }
+            float acc[BLOCK_N / 2];
+            zero_acc(acc);
+            int held = -1;
             for (int i = 0; i < TB.n_items && !dead; ++i) {
                 const SpItem it = TB.it[i];
                 for (int cb = 0; cb < nbk[it.part]; ++cb) {
                     if (!__all_sync(0xffffffffu, ptx::mbar_wait(ready + 8 * s, ph, P.abort_flag, 324))) { dead = true; break; }
-                    ptx::tc_fence_after();
-                    if (ptx::elect_one()) {
-                        uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16 + it.shift0), db = desc_b0 + static_cast<uint64_t>(s * stage16);
-                        const int ksteps = (cb + 1 < nbk[it.part]) ? 4 : klast[it.part];
-                        for (int tc = 0; tc < it.nb; ++tc, da += it.dshift, db += B_BYTES >> 4)
-                            for (int k = 0; k < ksteps; ++k)
-                                ptx::umma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (accum | tc | k) != 0);
-                        ptx::umma_commit(bar_empty + 8 * s);
-                    }
-                    __syncwarp();
-                    accum = 1;
+                    uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16 + it.shift0), db = desc_b0 + static_cast<uint64_t>(s * stage16);
+                    const int ksteps = (cb + 1 < nbk[it.part]) ? 4 : klast[it.part];
+                    ptx::wgmma_fence();
+                    for (int tc = 0; tc < it.nb; ++tc, da += it.dshift, db += B_BYTES >> 4)
+                        for (int k = 0; k < ksteps; ++k) ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + 2 * k, db + 2 * k);
+                    ptx::wgmma_commit();
+                    ptx::wgmma_wait<1>();
+                    if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+                    held = s;
                     if (++s == S) { s = 0; ph ^= 1; }
                 }
             }
-            if (!dead && ptx::elect_one()) ptx::umma_commit(bar_tmem_full + 8 * acc);
-            __syncwarp();
-            ++tile_iter;
+            ptx::wgmma_wait<0>();
+            ptx::wgmma_fence_regs(acc);
+            if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+            if (dead) { stat_n0 = -1; break; }
+            mma_epilogue<BLOCK_N, MODE>(P, acc, acc_stage, e, lane, m0, n0, s_stat);
         }
-    } else if (warp < 6) {
+    } else if (warp > 8) {
         // ================================ fixers: zero the hole rows of every landed A tile ================================
         if (fix) {
-            const int t = (warp - 2) * 32 + lane;
+            const int t = (warp - 9) * 32 + lane;
             int s = 0;
             uint32_t ph = 0;
             bool dead = false;
@@ -1397,49 +1278,10 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
                 }
             }
         }
-    } else {
-        // ================================ epilogue warps (6-9) ================================
-        int tile_iter = 0;
-        s_stat = (MODE == 0 && P.bn_sums != nullptr)
-                     ? reinterpret_cast<float *>(smem_gen + (((s_tmem_ptr + 32u) & ~15u) - smem_base)) + (warp & 3) * STAT_FLOATS_PER_WARP : nullptr;
-        if (s_stat) {
-            for (int i = lane; i < STAT_FLOATS_PER_WARP; i += 32) s_stat[i] = 0.f;
-            __syncwarp();
-        }
-        for (int tile = tile0; tile < num_tiles; tile += tstep) {
-            const int m0 = (tile / n_tiles) * BLOCK_M, n0 = (tile % n_tiles) * BLOCK_N;
-            const int acc = tile_iter & 1;
-            if (s_stat && n0 != stat_n0) {
-                if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0);
-                stat_n0 = n0;
-            }
-            if (!ptx::mbar_wait(bar_tmem_full + 8 * acc, (tile_iter >> 1) & 1, P.abort_flag, 323)) { stat_n0 = -1; break; }
-            tc_epilogue<BLOCK_N, MODE>(P, tmem_base + acc * BLOCK_N, warp & 3, lane, m0, n0, s_stat);
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(bar_tmem_empty + 8 * acc);
-            ++tile_iter;
-        }
     }
 
-    ptx::tc_fence_before();
     __syncthreads();
-    if (s_stat != nullptr && stat_n0 >= 0) {
-        const float *base = s_stat - (warp & 3) * STAT_FLOATS_PER_WARP;
-        for (int col = (warp & 3) * 32 + lane; col < BLOCK_N; col += 128) {
-            const int co = stat_n0 + col;
-            if (co < P.bn_c) {
-                float a = 0.f, q = 0.f;
-#pragma unroll
-                for (int w4 = 0; w4 < 4; ++w4) { a += base[w4 * STAT_FLOATS_PER_WARP + col]; q += base[w4 * STAT_FLOATS_PER_WARP + 256 + col]; }
-                atomicAdd(P.bn_sums + co, static_cast<double>(a));
-                atomicAdd(P.bn_sums + P.bn_c + co, static_cast<double>(q));
-            }
-        }
-    }
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<TCOLS>(tmem_base);
-    }
+    if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - EpiRole<BLOCK_N>(warp).slice() * STAT_SLICE, warp, lane, stat_n0);
 }
 
 // nearest 2x upsample of one convolution source into a dense [n, 2hs, 2ws, c8] buffer (TMA cannot replicate pixels)
@@ -1480,23 +1322,41 @@ struct WgParams {
     int box_w, box_h, box_n, stages, use_fix;
 };
 
+// Both weight-gradient kernels: warps 0-7 are two consumer warpgroups; warpgroup g computes rows [64 g, 64 g + 64) of
+// D[k][co] (k = the tile's 128 gathered channels) for every tap of the CTA and adds them into dw from its registers.
+constexpr int WGRAD_THREADS = MMA_THREADS + 5 * 32;
+
+// red.global.add of a consumer thread's accumulators: element i of tap tl is row r0 + 8 ((i / 2) & 1), column 8 (i / 4) +
+// 2 (lane % 4) + (i & 1) of the tile.  ci[h] / tap[h][tl]: input channel (-1: none) and kernel tap of the thread's two rows.
+template <int BLOCK_N, int T>
+__device__ __forceinline__ void wgrad_store(const WgParams &P, const float (&acc)[T][BLOCK_N / 2], int ntap, int lane, int n0,
+                                            const int (&ci)[2], const int (&tap)[2][T]) {
+    const int taps_full = P.kh * P.kw;
+#pragma unroll
+    for (int tl = 0; tl < T; ++tl) {
+        if (tl >= ntap) break;
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) {
+            const int h = (i >> 1) & 1;
+            const int co = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+            if (ci[h] >= 0 && co < P.cout)
+                atomicAdd(P.dw + (static_cast<long long>(co) * taps_full + tap[h][tl]) * P.cin + ci[h], acc[tl][i]);
+        }
+    }
+}
+
 template <int BLOCK_N, int T, int STAGES>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__(WGRAD_THREADS, 1)
 pconv_tc_wgrad_kernel(const __grid_constant__ WgParams P, const __grid_constant__ CUtensorMap tmap_dc) {
     constexpr int B_STAGE_BYTES = BLOCK_N * 128;            // [64 px][BLOCK_N co] as BLOCK_N/64 blocks of 8 KB
     constexpr int A_TAP_BYTES = 16384;                      // [64 px][128 k] as 2 blocks of 8 KB
     constexpr int A_STAGE = T * A_TAP_BYTES;
-    constexpr int TMEM_COLS = (T * BLOCK_N <= 64) ? 64 : (T * BLOCK_N <= 128) ? 128 : (T * BLOCK_N <= 256) ? 256 : 512;
-    static_assert(T * BLOCK_N <= 512, "TMEM overflow");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = align1024(ptx::smem_u32(smem_raw));
     const uint32_t sA = smem_base;
     const uint32_t sB = sA + STAGES * A_STAGE;
     const uint32_t sBar = sB + STAGES * B_STAGE_BYTES;
     const uint32_t bar_full_a = sBar, bar_full_b = sBar + 8 * STAGES, bar_empty = sBar + 16 * STAGES;
-    const uint32_t bar_tmem_full = sBar + 24 * STAGES;
-    const uint32_t s_tmem_ptr = bar_tmem_full + 8;
-    uint32_t *tmem_ptr_generic = reinterpret_cast<uint32_t *>(smem_raw + (s_tmem_ptr - ptx::smem_u32(smem_raw)));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // blockIdx.x = ((co_tile * tap_groups) + tap_group) * ci_tiles + ci_tile ; blockIdx.y = K split
@@ -1517,24 +1377,16 @@ pconv_tc_wgrad_kernel(const __grid_constant__ WgParams P, const __grid_constant_
         for (int s = 0; s < STAGES; ++s) {
             ptx::mbar_init(bar_full_a + 8 * s, NUM_PRODUCER_THREADS);
             ptx::mbar_init(bar_full_b + 8 * s, 1);
-            ptx::mbar_init(bar_empty + 8 * s, 1);
+            ptx::mbar_init(bar_empty + 8 * s, 2);
         }
-        ptx::mbar_init(bar_tmem_full, 1);
         ptx::fence_mbar_init();
     }
-    if (warp == 4 && lane == 0) ptx::prefetch_tmap(&tmap_dc);
-    if (warp == 5) {
-        ptx::tmem_alloc<TMEM_COLS>(s_tmem_ptr);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
+    if (warp == 12 && lane == 0) ptx::prefetch_tmap(&tmap_dc);
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_generic;
 
-    if (warp < 4) {
-        // ============ A producers: gather x rows (K = pixels) for each tap, 2 x 64-element blocks ============
-        const int t = threadIdx.x;
+    if (warp >= MMA_WARPS && warp < MMA_WARPS + 4) {
+        // ============ A producers (warps 8-11): gather x rows (K = pixels) for each tap, 2 x 64-element blocks ============
+        const int t = threadIdx.x - MMA_THREADS;
         const int chunk = t & 7, r0 = t >> 3;
         const uint32_t sw = static_cast<uint32_t>((chunk ^ (r0 & 7)) << 4);
         // the two 64-element blocks of this k tile -> (part, channel offset inside the part, chunk readable?)
@@ -1628,41 +1480,7 @@ pconv_tc_wgrad_kernel(const __grid_constant__ WgParams P, const __grid_constant_
             ptx::mbar_arrive(bar_full_a + 8 * s);
         }
         ptx::cp_async_wait<0>();
-
-        // ============ epilogue: D[k][co] per tap -> red.global.add into dw[co][tap][ci] ============
-        if (!dead && num_kb > 0 && ptx::mbar_wait(bar_tmem_full, 0, P.abort_flag, 202)) {
-            ptx::tc_fence_after();
-            const int row = warp * 32 + lane;
-            const int kpos = ci_tile * 128 + row;
-            for (int tl = 0; tl < ntap; ++tl) {
-                const int tg = tap0 + tl;
-                int ci = -1, tap = tg;
-                if (P.rowpack) {
-                    const int tc = row >> 3, ch = row & 7;
-                    if (row < 64 && ci_tile == 0 && tc < P.kw && ch < P.cin) { ci = ch; tap = tg * P.kw + tc; }
-                } else {
-                    for (int p = 0; p < P.nparts; ++p) {
-                        const int local = kpos - P.parts[p].koff;
-                        if (local >= 0 && local < P.parts[p].c) ci = P.parts[p].choff + local;
-                    }
-                }
-#pragma unroll 1
-                for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-                    uint32_t r[32];
-                    ptx::tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + tl * BLOCK_N + c0, r);
-                    ptx::tmem_ld_wait();
-                    if (ci >= 0) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int co = n0 + c0 + j;
-                            if (co < P.cout)
-                                atomicAdd(P.dw + (static_cast<long long>(co) * taps_full + tap) * P.cin + ci, __uint_as_float(r[j]));
-                        }
-                    }
-                }
-            }
-        }
-    } else if (warp == 4) {
+    } else if (warp == 12) {
         // ============ B producer: dc tiles [64 px][BLOCK_N co] via TMA, BLOCK_N/64 boxes of {64 co, 64 px} ============
         if (lane == 0) {
             for (int it = 0; it < num_kb; ++it) {
@@ -1676,37 +1494,66 @@ pconv_tc_wgrad_kernel(const __grid_constant__ WgParams P, const __grid_constant_
                     ptx::tma_load_2d(sB + s * B_STAGE_BYTES + j * 8192, &tmap_dc, n0 + j * 64, kb * 64, bar_full_b + 8 * s);
             }
         }
-    } else {
-        // ============ MMA issuer: both operands MN-major ============
-        if (lane == 0 && num_kb > 0) {
-            constexpr uint32_t idesc = ptx::make_idesc_bf16(128, BLOCK_N, 1, 1);
-            bool dead = false;
-            for (int it = 0; it < num_kb && !dead; ++it) {
-                const int s = it % STAGES;
-                const uint32_t parity = (it / STAGES) & 1;
-                if (!ptx::mbar_wait(bar_full_a + 8 * s, parity, P.abort_flag, 204) ||
-                    !ptx::mbar_wait(bar_full_b + 8 * s, parity, P.abort_flag, 205)) { dead = true; break; }
-                if (kProxyFence) ptx::fence_proxy_async_smem();
-                ptx::tc_fence_after();
-                for (int tl = 0; tl < ntap; ++tl) {
+    } else if (warp < MMA_WARPS && num_kb > 0) {
+        // ============ consumer warpgroups: both operands MN-major; warpgroup g takes the tile's 64-channel block g ============
+        const int g = warp >> 2;
+        const bool leader = (threadIdx.x & 127) == 0;
+        float acc[T][BLOCK_N / 2];
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {     // 16 pixels (2 atoms of 8 k-rows = 2048 bytes) per step
-                        const uint64_t da = ptx::make_smem_desc(sA + s * A_STAGE + tl * A_TAP_BYTES + k * 2048, 8192, 1024);
-                        const uint64_t db = ptx::make_smem_desc(sB + s * B_STAGE_BYTES + k * 2048, 8192, 1024);
-                        ptx::umma_bf16(tmem_base + tl * BLOCK_N, da, db, idesc, (it | k) != 0);
+        for (int tl = 0; tl < T; ++tl) zero_acc(acc[tl]);
+        bool dead = false;
+        int held = -1;
+        for (int it = 0; it < num_kb && !dead; ++it) {
+            const int s = it % STAGES;
+            const uint32_t parity = (it / STAGES) & 1;
+            if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full_a + 8 * s, parity, P.abort_flag, 204) &&
+                                             ptx::mbar_wait(bar_full_b + 8 * s, parity, P.abort_flag, 205))) { dead = true; break; }
+            ptx::fence_proxy_async_smem();                       // cp.async (generic proxy) data -> wgmma (async proxy)
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int tl = 0; tl < T; ++tl) {
+                if (tl >= ntap) break;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {     // 16 pixels (2 atoms of 8 k-rows = 2048 bytes) per step
+                    const uint64_t da = ptx::make_smem_desc(sA + s * A_STAGE + tl * A_TAP_BYTES + g * 8192 + k * 2048, 8192, 1024);
+                    const uint64_t db = ptx::make_smem_desc(sB + s * B_STAGE_BYTES + k * 2048, 8192, 1024);
+                    ptx::wgmma_bf16<BLOCK_N, 1, 1>(acc[tl], da, db);
+                }
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>();
+            if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+            held = s;
+        }
+        ptx::wgmma_wait<0>();
+#pragma unroll
+        for (int tl = 0; tl < T; ++tl) ptx::wgmma_fence_regs(acc[tl]);
+        if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+        // ============ epilogue: D[k][co] per tap -> red.global.add into dw[co][tap][ci] ============
+        if (!dead) {
+            int ci[2], tap[2][T];
+            for (int h = 0; h < 2; ++h) {
+                const int row = 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+                const int kpos = ci_tile * 128 + row;
+                ci[h] = -1;
+#pragma unroll
+                for (int tl = 0; tl < T; ++tl) tap[h][tl] = tap0 + tl;
+                if (P.rowpack) {
+                    const int tc = row >> 3, ch = row & 7;
+                    if (row < 64 && ci_tile == 0 && tc < P.kw && ch < P.cin) {
+                        ci[h] = ch;
+#pragma unroll
+                        for (int tl = 0; tl < T; ++tl) tap[h][tl] = (tap0 + tl) * P.kw + tc;
+                    }
+                } else {
+                    for (int p = 0; p < P.nparts; ++p) {
+                        const int local = kpos - P.parts[p].koff;
+                        if (local >= 0 && local < P.parts[p].c) ci[h] = P.parts[p].choff + local;
                     }
                 }
-                ptx::umma_commit(bar_empty + 8 * s);
             }
-            if (!dead) ptx::umma_commit(bar_tmem_full);
+            wgrad_store<BLOCK_N, T>(P, acc, ntap, lane, n0, ci, tap);
         }
-    }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 5) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<TMEM_COLS>(tmem_base);
     }
 }
 
@@ -1715,22 +1562,18 @@ pconv_tc_wgrad_kernel(const __grid_constant__ WgParams P, const __grid_constant_
 // weight gradient, TMA-FED.  Same GEMM as pconv_tc_wgrad_kernel (D[ci][co] per tap, K = output pixels, split-K with fp32
 // red.global.add) but the gathered operand is no longer gathered: a K block of 64 consecutive output pixels is a box of the
 // pixel grid, so the x rows of tap (tr, tc) / 64-channel block are one 4-D TMA tile (padding = out-of-range zero fill,
-// stride-2 layers = traversal stride), written as exactly the MN-major 128B-swizzled block UMMA reads.  Holes are zeroed
+// stride-2 layers = traversal stride), written as exactly the MN-major 128B-swizzled block wgmma reads.  Holes are zeroed
 // in the landed tile by four fixer warps (the tap-validity words of the block's pixels), which then run the epilogue.
 //   HALO (stride 1, K block = one image-row segment): a CTA owns one kernel ROW; one tile of 64 + (kw-1)*dil pixel rows per
-//   channel block serves the kw taps of the row through row-shifted descriptors (T = kw accumulators in TMEM).
+//   channel block serves the kw taps of the row through row-shifted descriptors (T = kw register accumulators).
 //   otherwise: a CTA owns T taps, one tile per tap.
-//   warp 0 TMA producer | warp 1 MMA issuer (+ TMEM alloc) | warps 2-5 fixers, then epilogue
+//   warps 0-7 consumer warpgroups (MMA, then epilogue) | warp 8 TMA producer | warps 9-12 fixers
 // -------------------------------------------------------------------------------------------------
-constexpr int WG_THREADS = 192;
-
 template <int BLOCK_N, int T, bool HALO>
-__global__ void __launch_bounds__(WG_THREADS, 1)
+__global__ void __launch_bounds__(WGRAD_THREADS, 1)
 pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_constant__ CUtensorMap tmap_dc,
                           const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1) {
     constexpr uint32_t B_BYTES = BLOCK_N * 128;               // [64 px][BLOCK_N co] as BLOCK_N/64 blocks of 8 KB
-    constexpr int TMEM_COLS = (T * BLOCK_N <= 64) ? 64 : (T * BLOCK_N <= 128) ? 128 : (T * BLOCK_N <= 256) ? 256 : 512;
-    static_assert(T * BLOCK_N <= 512, "TMEM overflow");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = align1024(ptx::smem_u32(smem_raw));
     uint8_t *smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
@@ -1741,9 +1584,7 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
     const uint32_t A_BYTES = (HALO ? 1 : T) * 2 * A_BLK;       // per stage: [tap][channel block]
     const uint32_t STAGE = A_BYTES + B_BYTES;
     const uint32_t sBar = smem_base + S * STAGE;
-    const uint32_t bar_full = sBar, bar_fixed = sBar + 8 * MAX_RING, bar_empty = sBar + 16 * MAX_RING, bar_tmem_full = sBar + 24 * MAX_RING;
-    const uint32_t s_tmem_ptr = bar_tmem_full + 8;
-    uint32_t *tmem_ptr_generic = reinterpret_cast<uint32_t *>(smem_gen + (s_tmem_ptr - smem_base));
+    const uint32_t bar_full = sBar, bar_fixed = sBar + 8 * MAX_RING, bar_empty = sBar + 16 * MAX_RING;
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     // blockIdx.x = ((co_tile * tap_groups) + tap_group) * ci_tiles + ci_tile ; blockIdx.y = K split
@@ -1773,21 +1614,13 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
     const bool fix = P.use_fix != 0;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 1); }
-        ptx::mbar_init(bar_tmem_full, 1);
+        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 2); }
         ptx::fence_mbar_init();
     }
-    if (warp == 0 && lane == 0) { ptx::prefetch_tmap(&tmap_dc); ptx::prefetch_tmap(&tmap_a0); ptx::prefetch_tmap(&tmap_a1); }
-    if (warp == 1) {
-        ptx::tmem_alloc<TMEM_COLS>(s_tmem_ptr);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
+    if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_dc); ptx::prefetch_tmap(&tmap_a0); ptx::prefetch_tmap(&tmap_a1); }
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_generic;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================================ TMA producer ================================
         const int plane = P.ho * P.wo;
         const uint32_t tx_bytes = static_cast<uint32_t>((HALO ? 1 : ntap) * nblk * rows_a * 128) + B_BYTES;
@@ -1817,39 +1650,64 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
             __syncwarp();
             if (++s == S) { s = 0; ph ^= 1; }
         }
-    } else if (warp == 1) {
-        // ================================ MMA issuer: both operands MN-major ================================
-        constexpr uint32_t idesc = ptx::make_idesc_bf16(128, BLOCK_N, 1, 1);
+    } else if (warp < MMA_WARPS) {
+        // ================================ consumer warpgroups: both operands MN-major ================================
+        // warpgroup g takes the tile's 64-channel block g (nothing to compute when that block does not exist)
+        const int g = warp >> 2;
+        const bool leader = (threadIdx.x & 127) == 0, live = blk_part[g] >= 0;
         const uint32_t ready = fix ? bar_fixed : bar_full;
-        const uint64_t desc_a0 = ptx::make_smem_desc(smem_base, A_BLK, 1024);      // LBO = distance between the two 64-channel blocks
+        const uint64_t desc_a0 = ptx::make_smem_desc(smem_base + g * A_BLK, A_BLK, 1024);
         const uint64_t desc_b0 = ptx::make_smem_desc(smem_base + A_BYTES, 8192, 1024);
         const uint32_t stage16 = STAGE >> 4;
         const uint32_t tap16 = HALO ? static_cast<uint32_t>(P.dil * 8) : (2 * A_BLK) >> 4;   // per tap: row shift (halo) or next tile
-        int s = 0;
+        float acc[T][BLOCK_N / 2];
+#pragma unroll
+        for (int tl = 0; tl < T; ++tl) zero_acc(acc[tl]);
+        int s = 0, held = -1;
         uint32_t ph = 0;
         bool dead = false;
         for (int it = 0; it < num_kb; ++it) {
             if (!__all_sync(0xffffffffu, ptx::mbar_wait(ready + 8 * s, ph, P.abort_flag, 224))) { dead = true; break; }
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
+            if (live) {
                 uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16);
                 const uint64_t db = desc_b0 + static_cast<uint64_t>(s * stage16);
-                for (int tl = 0; tl < ntap; ++tl, da += tap16) {
+                ptx::wgmma_fence();
+#pragma unroll
+                for (int tl = 0; tl < T; ++tl, da += tap16) {
+                    if (tl >= ntap) break;
 #pragma unroll
                     for (int k = 0; k < 4; ++k)                  // 16 pixels (two 8-row atoms = 2048 bytes) per step
-                        ptx::umma_bf16(tmem_base + tl * BLOCK_N, da + 128 * k, db + 128 * k, idesc, (it | k) != 0);
+                        ptx::wgmma_bf16<BLOCK_N, 1, 1>(acc[tl], da + 128 * k, db + 128 * k);
                 }
-                ptx::umma_commit(bar_empty + 8 * s);
+                ptx::wgmma_commit();
+                ptx::wgmma_wait<1>();
             }
-            __syncwarp();
+            if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+            held = s;
             if (++s == S) { s = 0; ph ^= 1; }
         }
-        if (!dead && num_kb > 0 && ptx::elect_one()) ptx::umma_commit(bar_tmem_full);
-        __syncwarp();
+        ptx::wgmma_wait<0>();
+#pragma unroll
+        for (int tl = 0; tl < T; ++tl) ptx::wgmma_fence_regs(acc[tl]);
+        if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+        // ---- epilogue: D[ci][co] per tap -> red.global.add into dw[co][tap][ci]
+        if (!dead && live && num_kb > 0) {
+            int ci[2], tap[2][T];
+            for (int h = 0; h < 2; ++h) {
+                const int kpos = ci_tile * 128 + 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+                ci[h] = -1;
+                for (int p = 0; p < P.nparts; ++p) {
+                    const int local = kpos - P.parts[p].koff;
+                    if (local >= 0 && local < P.parts[p].c) ci[h] = P.parts[p].choff + local;
+                }
+#pragma unroll
+                for (int tl = 0; tl < T; ++tl) tap[h][tl] = tap0 + tl;
+            }
+            wgrad_store<BLOCK_N, T>(P, acc, ntap, lane, n0, ci, tap);
+        }
     } else {
-        // ================================ fixers (hole rows -> 0), then epilogue ================================
-        const int f = (warp - 2) * 32 + lane;                   // pixel row of the A blocks owned by this thread
-        bool dead = false;
+        // ================================ fixers (hole rows -> 0) ================================
+        const int f = (warp - 9) * 32 + lane;                   // pixel row of the A blocks owned by this thread
         if (fix) {
             // tap-validity word of the output pixel that looks at this row (halo rows past 63 belong to a later tap column)
             int jpix = f, tcs = 0;
@@ -1868,7 +1726,7 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
             for (int it = 0; it < num_kb; ++it) {
                 const uint64_t w0 = wnext[0], w1 = wnext[1];
                 load_words(kb_begin + it + 1);
-                if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 222))) { dead = true; break; }
+                if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 222))) break;
                 bool wrote = false;
                 if (row_used) {
                     for (int tl = 0; tl < (HALO ? 1 : ntap); ++tl) {
@@ -1892,41 +1750,6 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
                 if (++s == S) { s = 0; ph ^= 1; }
             }
         }
-        // ---- epilogue: D[ci][co] per tap -> red.global.add into dw[co][tap][ci]
-        if (!dead && num_kb > 0 && ptx::mbar_wait(bar_tmem_full, 0, P.abort_flag, 223)) {
-            ptx::tc_fence_after();
-            const int q = warp & 3;                               // TMEM lane quarter this warp may read
-            const int row = q * 32 + lane;
-            const int kpos = ci_tile * 128 + row;
-            int ci = -1;
-            for (int p = 0; p < P.nparts; ++p) {
-                const int local = kpos - P.parts[p].koff;
-                if (local >= 0 && local < P.parts[p].c) ci = P.parts[p].choff + local;
-            }
-            for (int tl = 0; tl < ntap; ++tl) {
-                const int tap = tap0 + tl;
-#pragma unroll 1
-                for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-                    uint32_t r[32];
-                    ptx::tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + tl * BLOCK_N + c0, r);
-                    ptx::tmem_ld_wait();
-                    if (ci >= 0) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int co = n0 + c0 + j;
-                            if (co < P.cout) atomicAdd(P.dw + (static_cast<long long>(co) * taps_full + tap) * P.cin + ci, __uint_as_float(r[j]));
-                        }
-                    }
-                }
-            }
-        }
-    }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<TMEM_COLS>(tmem_base);
     }
 }
 
@@ -2196,41 +2019,27 @@ int halo_hg(const pcb_conv *c, bool rowpack) {
     return hg;
 }
 
-// PCB_TC_DEBUG_TIMING=1: every forward/dgrad launch synchronises and prints where its MMA threads spent their cycles
-long long *debug_buffer() {
-    static long long *buf[PCB_MAX_DEVICES] = {};
-    const int dev = pcb_cur_device();
-    if (!buf[dev] && getenv("PCB_TC_DEBUG_TIMING")) cudaMalloc(&buf[dev], sizeof(long long) * 10 * 1024);
-    return buf[dev];
-}
+// H100: 227 KB of shared memory per block.  The rings get what the epilogue staging tile, the statistics and the barriers leave.
+constexpr size_t MAX_SMEM = 227 * 1024;
+constexpr size_t RING_BUDGET = 208 * 1024;
 
 template <int BLOCK_N, int MODE, bool HALO>
 int launch_persistent(TcParams &P, const CUtensorMap &tm, cudaStream_t st) {
     const size_t a_stage = HALO ? ((8 * 16 * (16 * P.hg + 1) + 127) / 128 * 128) : A_STAGE_BYTES;
     const size_t b_stage = BLOCK_N * 128;
-    const size_t budget = 200 * 1024;
+    const size_t budget = RING_BUDGET - acc_stage_bytes(BLOCK_N);
     P.ring_b = 6;
     P.ring_a = HALO ? 3 : 6;
     while (P.ring_a * a_stage + P.ring_b * b_stage > budget && P.ring_b > 3) --P.ring_b;
     while (P.ring_a * a_stage + P.ring_b * b_stage > budget && P.ring_a > 2) --P.ring_a;
-    const size_t smem = 1024 + P.ring_a * a_stage + P.ring_b * b_stage + 40 * MAX_RING + 64 + STAT_SMEM_BYTES;
+    const size_t smem = 1024 + P.ring_a * a_stage + P.ring_b * b_stage + 32 * MAX_RING + 16 + STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
+    PCB_CHECK(smem <= MAX_SMEM, "tensor-core conv: %zu bytes of shared memory do not fit", smem);
     auto kern = pconv_tc_persistent_kernel<BLOCK_N, MODE, HALO>;
-    PCB_SMEM_OPT_IN(kern, 220 * 1024);
+    PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     const int num_tiles = ((P.m_total + BLOCK_M - 1) / BLOCK_M) * (P.ncols / BLOCK_N);
     const int grid = std::min(num_tiles, pcb_num_sms());
-    P.dbg = debug_buffer();
     kern<<<grid, PERSIST_THREADS, smem, st>>>(P, tm);
     PCB_LAUNCH_CHECK();
-    if (P.dbg) {
-        static long long h[8 * 1024];
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h, P.dbg, sizeof(long long) * 8 * grid, cudaMemcpyDeviceToHost);
-        double tot = 0, acc = 0, a = 0, b = 0, iss = 0, tiles = 0, ia = 0, ib = 0;
-        for (int i = 0; i < grid; ++i) { tot += h[8*i]; acc += h[8*i+1]; a += h[8*i+2]; b += h[8*i+3]; iss += h[8*i+4]; tiles += h[8*i+5]; ia += h[8*i+6]; ib += h[8*i+7]; }
-        fprintf(stderr, "[tc-timing] mode=%d halo=%d N=%d cin=%d cout=%d %dx%d grid=%d tiles/cta=%.1f items/tile=%.1f | per-CTA cycles: total=%.0f wait_acc=%.0f wait_A=%.0f wait_B=%.0f issue=%.0f | per A item: %.0f cyc (wait_A %.0f, wait_B %.0f)\n",
-                MODE, (int)HALO, BLOCK_N, P.cin, P.cout, P.h, P.w, grid, tiles / grid, ia / std::max(1.0, tiles), tot / grid, acc / grid, a / grid, b / grid, iss / grid,
-                tot / std::max(1.0, ia), a / std::max(1.0, ia), b / std::max(1.0, ia));
-    }
     return 0;
 }
 
@@ -2305,8 +2114,8 @@ __global__ void splitk_finish_dgrad_kernel(const float *__restrict__ part, const
 
 // how many CTAs should share the K loop of one output tile
 int pick_ksplit(long long m_total, int ncols, int bn, int blocks_per_tap) {
-    // measured on B200 (8 x 512^2 U-Net, layers at 4x4..16x16): the shorter K loop is paid back by the memset + finish kernels,
-    // so the split is opt-in (PCB_SPLITK=1; the parity tests set it)
+    // the shorter K loop of the low-resolution layers is paid back by the memset + finish kernels, so the split is opt-in
+    // (PCB_SPLITK=1; the parity tests set it)
     if (!getenv("PCB_SPLITK")) return 1;
     const long long tiles = ((m_total + BLOCK_M - 1) / BLOCK_M) * (ncols / bn);
     const int sms = pcb_num_sms();
@@ -2361,104 +2170,57 @@ size_t tapmask_bytes(const pcb_conv *c) {
     return (static_cast<size_t>(c->nparts) * c->n * c->ho * c->wo * sizeof(uint64_t) + 255) / 256 * 256;
 }
 
-template <int BLOCK_N, int MODE, bool HALO, bool PAIR>
+template <int BLOCK_N, int MODE, bool HALO>
 int launch_tma_n(TcParams &P, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, cudaStream_t st) {
     const int nb = HALO ? P.kw : 1;
     const size_t a_room = (static_cast<size_t>(BLOCK_M + (HALO ? (P.kw - 1) * P.dil : 0)) * 128 + 1023) / 1024 * 1024;
-    const size_t stage = a_room + static_cast<size_t>(nb) * (PAIR ? BLOCK_N / 2 : BLOCK_N) * 128;
-    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (208 * 1024) / stage));
+    const size_t stage = a_room + static_cast<size_t>(nb) * BLOCK_N * 128;
+    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (RING_BUDGET - acc_stage_bytes(BLOCK_N)) / stage));
     PCB_CHECK(P.stages >= 2, "TMA-fed conv: stage of %zu bytes does not fit twice", stage);
-    const size_t smem = 1024 + P.stages * stage + 32 * MAX_RING + 64 + STAT_SMEM_BYTES;
-    auto kern = pconv_tc_tma_kernel<BLOCK_N, MODE, HALO, PAIR>;
-    PCB_SMEM_OPT_IN(kern, 224 * 1024);
+    const size_t smem = 1024 + P.stages * stage + 24 * MAX_RING + 16 + STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
+    auto kern = pconv_tc_tma_kernel<BLOCK_N, MODE, HALO>;
+    PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     if (P.ksplit < 1) P.ksplit = 1;
     const int m_tiles = (P.m_total + BLOCK_M - 1) / BLOCK_M;
-    P.dbg = debug_buffer();
-    int grid;
-    if (PAIR) {
-        // clusters of two CTAs (same TPC): the pair shares every weight tile, the leader issues M = 256 MMAs for both
-        const int pair_tiles = ((m_tiles + 1) / 2) * (P.ncols / BLOCK_N);
-        grid = 2 * std::min(pair_tiles, pcb_num_sms() / 2);
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TMA_THREADS8); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        PCB_CUDA(cudaLaunchKernelEx(&cfg, kern, P, tw, ta0, ta1));
-        pcb_count_launch();
-    } else {
-        const int num_tiles = m_tiles * (P.ncols / BLOCK_N) * P.ksplit;
-        grid = std::min(num_tiles, pcb_num_sms());
-        kern<<<grid, TMA_THREADS8, smem, st>>>(P, tw, ta0, ta1);
-        PCB_LAUNCH_CHECK();
-    }
-    if (P.dbg) {
-        static long long h[8 * 1024];
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h, P.dbg, sizeof(long long) * 8 * grid, cudaMemcpyDeviceToHost);
-        double tot = 0, tiles = 0, items = 0, mw = 0, tw = 0, ti = 0, ma = 0, mi = 0, mc = 0;
-        for (int i = 0; i < grid; ++i) { tot += h[8*i]; tiles += h[8*i+5]; items += h[8*i+6]; mw += h[8*i+1]; tw += h[8*i+2]; ti += h[8*i+3]; ma += h[8*i+7]; }
-#ifdef PCB_TC_TIMING
-        {
-            static long long h2[2 * 1024];
-            cudaMemcpy(h2, P.dbg + 8 * 1024, sizeof(long long) * 2 * grid, cudaMemcpyDeviceToHost);
-            for (int i = 0; i < grid; ++i) { mi += h2[2*i]; mc += h2[2*i+1]; }
-        }
-        fprintf(stderr, "[tc-timing]   per item: MMA thread: wait data %.0f, wait accumulator %.0f, issue MMAs %.0f, commit %.0f | TMA thread: wait free stage %.0f, issue %.0f\n",
-                mw / std::max(1.0, items), ma / std::max(1.0, items), mi / std::max(1.0, items), mc / std::max(1.0, items), tw / std::max(1.0, items), ti / std::max(1.0, items));
-#endif
-        fprintf(stderr, "[tc-timing] TMA mode=%d halo=%d N=%d cin=%d cout=%d %dx%d s%d grid=%d stages=%d(%zu B) fix=%d tiles/cta=%.1f items/tile=%.1f | per-CTA cycles %.0f | per item %.0f cyc = %.0f per tap\n",
-                MODE, (int)HALO, BLOCK_N, P.cin, P.cout, P.h, P.w, P.stride, grid, P.stages, stage, P.use_fix, tiles / grid, items / std::max(1.0, tiles), tot / grid,
-                tot / std::max(1.0, items), tot / std::max(1.0, items) / nb);
-    }
+    const int num_tiles = m_tiles * (P.ncols / BLOCK_N) * P.ksplit;
+    const int grid = std::min(num_tiles, pcb_num_sms());
+    kern<<<grid, TMA_THREADS, smem, st>>>(P, tw, ta0, ta1);
+    PCB_LAUNCH_CHECK();
     return 0;
 }
 
 template <int MODE>
-int launch_tma(TcParams &P, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, int bn, bool halo, cudaStream_t st, bool pair = false) {
-    if (pair) {
-        if (halo) {
-            if (bn == 128) return launch_tma_n<128, MODE, true, true>(P, tw, ta0, ta1, st);
-            return launch_tma_n<64, MODE, true, true>(P, tw, ta0, ta1, st);
-        }
-        if (bn == 256) return launch_tma_n<256, MODE, false, true>(P, tw, ta0, ta1, st);
-        if (bn == 128) return launch_tma_n<128, MODE, false, true>(P, tw, ta0, ta1, st);
-        return launch_tma_n<64, MODE, false, true>(P, tw, ta0, ta1, st);
-    }
+int launch_tma(TcParams &P, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, int bn, bool halo, cudaStream_t st) {
     if (halo) {
-        if (bn == 256) return launch_tma_n<256, MODE, true, false>(P, tw, ta0, ta1, st);
-        if (bn == 128) return launch_tma_n<128, MODE, true, false>(P, tw, ta0, ta1, st);
-        if (bn == 64) return launch_tma_n<64, MODE, true, false>(P, tw, ta0, ta1, st);
-        return launch_tma_n<32, MODE, true, false>(P, tw, ta0, ta1, st);
+        if (bn == 128) return launch_tma_n<128, MODE, true>(P, tw, ta0, ta1, st);
+        if (bn == 64) return launch_tma_n<64, MODE, true>(P, tw, ta0, ta1, st);
+        return launch_tma_n<32, MODE, true>(P, tw, ta0, ta1, st);
     }
-    if (bn == 256) return launch_tma_n<256, MODE, false, false>(P, tw, ta0, ta1, st);
-    if (bn == 128) return launch_tma_n<128, MODE, false, false>(P, tw, ta0, ta1, st);
-    if (bn == 64) return launch_tma_n<64, MODE, false, false>(P, tw, ta0, ta1, st);
-    return launch_tma_n<32, MODE, false, false>(P, tw, ta0, ta1, st);
+    if (bn == 128) return launch_tma_n<128, MODE, false>(P, tw, ta0, ta1, st);
+    if (bn == 64) return launch_tma_n<64, MODE, false>(P, tw, ta0, ta1, st);
+    return launch_tma_n<32, MODE, false>(P, tw, ta0, ta1, st);
 }
 
-// CTA pairs (opt-in, PCB_CTA_PAIR=1): N tiles of at least 64 columns, at least two M tiles, no split-K
-bool use_pair(int bn, long long m_total, int ksplit) {
-    return getenv("PCB_CTA_PAIR") != nullptr && bn >= 64 && bn <= 256 && m_total > BLOCK_M && ksplit <= 1;
+// at least three stages of (halo tile of 128 + (kw-1)*dil pixel rows + kw weight tiles) fit in shared memory next to the
+// epilogue staging tile of an N tile of block_n columns
+bool halo_stages_fit(int kw, int dil, int block_n) {
+    const size_t stage = (static_cast<size_t>(128 + (kw - 1) * dil) * 128 + 1023) / 1024 * 1024 + static_cast<size_t>(kw) * block_n * 128;
+    return 3 * stage + acc_stage_bytes(block_n) <= RING_BUDGET;
 }
 
-// halo tiles: stride 1, the M tile is one image-row segment, a kernel row's halo fits the 256-pixel TMA box, and at
-// least three stages of (halo tile + kw weight tiles) fit in shared memory for the chosen N tile
+// halo tiles: stride 1, the M tile is one image-row segment, a kernel row's halo fits the 256-pixel TMA box, and the stages fit
 bool tma_halo_ok(const pcb_conv *c, int bw, int bh, int bn, int block_n) {
     if (getenv("PCB_DISABLE_TMA_HALO")) return false;
     if (!(c->stride == 1 && bw == 128 && bh == 1 && bn == 1 && c->kw >= 2 && 128 + (c->kw - 1) * c->dil <= 256 && c->kh <= 8)) return false;
-    const size_t stage = (static_cast<size_t>(128 + (c->kw - 1) * c->dil) * 128 + 1023) / 1024 * 1024 + static_cast<size_t>(c->kw) * block_n * 128;
-    return 3 * stage <= 208 * 1024;
+    return halo_stages_fit(c->kw, c->dil, block_n);
 }
 
 // widest N tile that divides `cols` and still leaves at least one tile per SM; low-resolution layers (a handful of M tiles
-// against a multi-megabyte weight matrix) get NARROWER N tiles: each CTA's operand stream is latency-bound (~100 GB/s through a
-// 4..8-stage ring), so the time of such a layer is (bytes per CTA) / that rate -- more, smaller CTAs stream the weights in parallel
+// against a multi-megabyte weight matrix) get NARROWER N tiles: each CTA's operand stream is latency-bound (a ring of a few
+// stages), so the time of such a layer is (bytes per CTA) / that rate -- more, smaller CTAs stream the weights in parallel
+// (at most 128 columns: a consumer warpgroup holds 64 rows x N fp32 accumulators in registers)
 int pick_bn(int cols, long long m_total) {
     const long long m_tiles = (m_total + BLOCK_M - 1) / BLOCK_M;
-    if (cols % 256 == 0 && m_tiles * (cols / 256) >= pcb_num_sms()) return 256;
     if (cols <= 32) return 32;
     int bn = (cols % 128 == 0) ? 128 : 64;
     if (!getenv("PCB_NO_NARROW_N"))
@@ -2549,16 +2311,13 @@ SpPlan sp_plan(const pcb_conv *c) {
     if (S.net_total > SP_MAX_ITEMS) return S;
     S.kd_sp = static_cast<long long>(S.net_total) * L.cout64;
     S.ok = true;
-    // Measured on B200 (8 x 512^2 U-Net, profiles/r02_subpixel.txt): these kernels are bound by the TMA unit's request rate
-    // (about one 128-byte tile row per 4 cycles and SM), not by the tensor pipe.
     //  * DATA GRADIENT: one launch over the source grid replaces the full-resolution gradient of the upsampled part AND its 2x2
-    //    reduction pass -- a clear win wherever the source grid has at least a wave of tiles (192->64 @256^2: 0.28 -> 0.15 ms);
-    //    low-resolution layers keep the regular kernel (their launches are latency-bound either way).
+    //    reduction pass; it is used wherever the source grid has at least a third of a wave of tiles -- low-resolution layers keep
+    //    the regular kernel (their launches are latency-bound either way).
     //  * FORWARD: 37 % fewer MMAs but MORE tile rows per output pixel (the skip part is read with a traversal stride of 2, which
-    //    costs the TMA unit two rows per delivered row, and row-halo re-use is lost where the class grid is narrower than 128):
-    //    192->64 @256^2 0.26 -> 0.34 ms.  Off by default (PCB_SUBPIXEL_FWD=1 enables it; parity-tested either way).
+    //    costs the TMA unit two rows per delivered row, and row-halo re-use is lost where the class grid is narrower than 128).
+    //    Off by default (PCB_SUBPIXEL_FWD=1 enables it; parity-tested either way).
     const long long src_tiles = (static_cast<long long>(c->n) * (c->h / 2) * (c->w / 2) + BLOCK_M - 1) / BLOCK_M;
-    // (768->256 @64^2, 64 source tiles: 0.091 ms against 0.096 + 0.025 ms of reduction pass; @32^2, 16 tiles: 0.101 against 0.067)
     S.dgrad = src_tiles >= pcb_num_sms() / 3 || getenv("PCB_SUBPIXEL_ALL") != nullptr;
     S.fwd = getenv("PCB_SUBPIXEL_FWD") != nullptr || getenv("PCB_SUBPIXEL_ALL") != nullptr;
     S.sp_fwd_elems = S.fwd ? off : 0;
@@ -2654,17 +2413,20 @@ int sp_weight_prepare(const pcb_conv *c, const SpPlan &S, const Layout &L, const
     return 0;
 }
 
+// sub-pixel tiles are at most 64 columns wide: two stages of (A tile + up to four weight tiles) must fit next to the staging tile
+int sp_bn(int cols, long long m_total) { return std::min(pick_bn(cols, m_total), 64); }
+
 template <int BLOCK_N, int MODE>
 int launch_sp_n(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, cudaStream_t st) {
     int nb_max = 1;
     for (int i = 0; i < TB.n_items; ++i) nb_max = std::max(nb_max, TB.it[i].nb);
     const size_t a_room = (static_cast<size_t>(TB.rows_max) * 128 + 1023) / 1024 * 1024;
     const size_t stage = a_room + static_cast<size_t>(nb_max) * BLOCK_N * 128;
-    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (208 * 1024) / stage));
+    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (RING_BUDGET - acc_stage_bytes(BLOCK_N)) / stage));
     PCB_CHECK(P.stages >= 2, "sub-pixel conv: stage of %zu bytes does not fit twice", stage);
-    const size_t smem = 1024 + P.stages * stage + 32 * MAX_RING + 64 + STAT_SMEM_BYTES;
+    const size_t smem = 1024 + P.stages * stage + 24 * MAX_RING + 16 + STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
     auto kern = pconv_tc_sp_kernel<BLOCK_N, MODE>;
-    PCB_SMEM_OPT_IN(kern, 224 * 1024);
+    PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     const int num_tiles = ((P.m_total + BLOCK_M - 1) / BLOCK_M) * (P.ncols / BLOCK_N);
     const int grid = std::min(num_tiles, pcb_num_sms());
     kern<<<grid, TMA_THREADS, smem, st>>>(P, TB, tw, ta0, ta1);
@@ -2674,8 +2436,6 @@ int launch_sp_n(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUt
 
 template <int MODE>
 int launch_sp(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, int bn, cudaStream_t st) {
-    if (bn == 256) return launch_sp_n<256, MODE>(P, TB, tw, ta0, ta1, st);
-    if (bn == 128) return launch_sp_n<128, MODE>(P, TB, tw, ta0, ta1, st);
     if (bn == 64) return launch_sp_n<64, MODE>(P, TB, tw, ta0, ta1, st);
     return launch_sp_n<32, MODE>(P, TB, tw, ta0, ta1, st);
 }
@@ -2711,7 +2471,7 @@ int sp_forward(const pcb_conv *c, const SpPlan &S, const Layout &L, const bf16 *
     P.bn_sums = bn_sums; P.bn_c = c->cout;
     P.box_w = S.bw; P.box_h = S.bh; P.box_n = S.bn;
     const int cols = (c->cout <= 32) ? 32 : L.rows_f;
-    const int bn = pick_bn(cols, m_class);
+    const int bn = sp_bn(cols, m_class);
     P.ncols = cols;
     for (int p = 0; p < c->nparts; ++p)
         if (c->parts[p].mask) P.use_fix = 1;
@@ -2798,7 +2558,7 @@ int sp_dgrad_up(const pcb_conv *c, const SpPlan &S, const Layout &L, const void 
     P.abort_flag = flag;
     P.ncols = S.kext_u;
     P.box_w = S.bw; P.box_h = S.bh; P.box_n = S.bn;
-    const int bn = pick_bn(S.kext_u, m_src);
+    const int bn = sp_bn(S.kext_u, m_src);
     SpTable TB;
     memset(&TB, 0, sizeof(TB));
     TB.step[0] = 2; TB.es[0] = 2; TB.ph[0] = c->ho; TB.pw[0] = c->wo; TB.arows[0] = BLOCK_M; TB.rows_max = BLOCK_M;
@@ -2942,7 +2702,7 @@ int pcb_tc_forward_mask_pass(const pcb_conv *c, uint64_t *tapmask, cudaStream_t 
     return launch_tapmask(c, tapmask, st);
 }
 
-// true when pcb_tc_forward_ws accumulates the BatchNorm statistics of its output itself (tcgen05 kernels, no split-K)
+// true when pcb_tc_forward_ws accumulates the BatchNorm statistics of its output itself (tensor-core kernels, no split-K)
 bool pcb_tc_fuses_bn_stats(const pcb_conv *c) {
     return pcb_tc_eligible(c) && !smallco_ok(c) && !getenv("PCB_SPLITK") && !getenv("PCB_DISABLE_FUSED_BN_STATS");
 }
@@ -3027,10 +2787,6 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
             PCB_LAUNCH_CHECK();
             return 0;
         }
-        if (use_pair(bn, m_total, P.ksplit)) {            // each CTA of a pair loads half of every weight tile
-            if (int rc = make_tmap_2d(&tm, w_fwd, L.rows_f, L.kf, L.kf, bn / 2)) return rc;
-            return launch_tma<0>(P, tm, ta[0], ta[1], bn, halo, st, true);
-        }
         return launch_tma<0>(P, tm, ta[0], ta[1], bn, halo, st);
     }
     if (int rc = make_tmap_2d(&tm, w_fwd, L.rows_f, L.kf, L.kf, L.bn_f)) return rc;
@@ -3104,10 +2860,6 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
             PCB_LAUNCH_CHECK();
             return 0;
         }
-        if (use_pair(bn, m_total, P.ksplit)) {
-            if (int rc = make_tmap_2d(&tm, w_dgrad, rup(L.ktap, 128), L.kd, L.kd, bn / 2)) return rc;
-            return launch_tma<1>(P, tm, ta, ta, bn, halo, st, true);
-        }
         return launch_tma<1>(P, tm, ta, ta, bn, halo, st);
     }
     if (tma_dgrad_s2_ok(c)) {
@@ -3151,8 +2903,8 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
             Q.m_total = static_cast<int>(m_class);
             Q.sub = 2; Q.py = py; Q.px = px; Q.fh = c->h; Q.fw = c->w;
             Q.wk_base = (tr0 * c->kw + tc0) * L.cout64; Q.wk_row = 2 * c->kw * L.cout64; Q.wk_col = 2 * L.cout64;
-            const size_t stage = (static_cast<size_t>(128 + (Q.kw - 1)) * 128 + 1023) / 1024 * 1024 + static_cast<size_t>(Q.kw) * bn * 128;
-            const bool halo = !getenv("PCB_DISABLE_TMA_HALO") && Q.box_w == 128 && Q.box_h == 1 && Q.box_n == 1 && Q.kw >= 2 && 3 * stage <= 208 * 1024;
+            const bool halo = !getenv("PCB_DISABLE_TMA_HALO") && Q.box_w == 128 && Q.box_h == 1 && Q.box_n == 1 && Q.kw >= 2 &&
+                              halo_stages_fit(Q.kw, 1, bn);
             CUtensorMap ta;
             if (int rc = make_tmap_nhwc(&ta, dc, P.dc_c8, c->wo, c->ho, c->n, dc_cstride, Q.box_w + (halo ? Q.kw - 1 : 0), Q.box_h, Q.box_n, 1)) return rc;
             cudaStream_t cs = (fork && cls > 0) ? aux[cls - 1] : st;
@@ -3198,11 +2950,11 @@ template <int BLOCK_N, int T, bool HALO>
 int launch_wgrad_tma(WgParams &P, const CUtensorMap &tdc, const CUtensorMap &ta0, const CUtensorMap &ta1, cudaStream_t st) {
     const size_t a_blk = (static_cast<size_t>(64 + (HALO ? (P.kw - 1) * P.dil : 0)) * 128 + 1023) / 1024 * 1024;
     const size_t stage = (HALO ? 1 : T) * 2 * a_blk + static_cast<size_t>(BLOCK_N) * 128;
-    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (200 * 1024) / stage));
+    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, RING_BUDGET / stage));
     PCB_CHECK(P.stages >= 2, "TMA-fed wgrad: stage of %zu bytes does not fit twice", stage);
-    const size_t smem = 1024 + P.stages * stage + 24 * MAX_RING + 64;
+    const size_t smem = 1024 + P.stages * stage + 24 * MAX_RING;
     auto kern = pconv_tc_wgrad_tma_kernel<BLOCK_N, T, HALO>;
-    PCB_SMEM_OPT_IN(kern, 220 * 1024);
+    PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     P.tap_groups = HALO ? P.kh : (P.kh * P.kw + T - 1) / T;
     P.ci_tiles = (P.ktap + 127) / 128;
     const int co_tiles = (P.cout + BLOCK_N - 1) / BLOCK_N;
@@ -3214,14 +2966,14 @@ int launch_wgrad_tma(WgParams &P, const CUtensorMap &tdc, const CUtensorMap &ta0
     P.kb_per_split = (total_kb + splits - 1) / splits;
     splits = (total_kb + P.kb_per_split - 1) / P.kb_per_split;
     dim3 grid(base_ctas, splits);
-    kern<<<grid, WG_THREADS, smem, st>>>(P, tdc, ta0, ta1);
+    kern<<<grid, WGRAD_THREADS, smem, st>>>(P, tdc, ta0, ta1);
     PCB_LAUNCH_CHECK();
     return 0;
 }
 
 template <int BLOCK_N, int T, int STAGES>
 static int launch_wgrad(WgParams &P, const CUtensorMap &tm, int cout, cudaStream_t st) {
-    constexpr size_t smem = 1024 + STAGES * (T * 16384 + BLOCK_N * 128) + 24 * STAGES + 16 + 16;
+    constexpr size_t smem = 1024 + STAGES * (T * 16384 + BLOCK_N * 128) + 24 * STAGES;
     auto kern = pconv_tc_wgrad_kernel<BLOCK_N, T, STAGES>;
     PCB_SMEM_OPT_IN(kern, (int)smem);
     P.tap_groups = (P.ntaps + T - 1) / T;
@@ -3235,7 +2987,7 @@ static int launch_wgrad(WgParams &P, const CUtensorMap &tm, int cout, cudaStream
     P.kb_per_split = (total_kb + splits - 1) / splits;
     splits = (total_kb + P.kb_per_split - 1) / P.kb_per_split;
     dim3 grid(base_ctas, splits);
-    kern<<<grid, TC_THREADS, smem, st>>>(P, tm);
+    kern<<<grid, WGRAD_THREADS, smem, st>>>(P, tm);
     PCB_LAUNCH_CHECK();
     return 0;
 }
@@ -3271,8 +3023,8 @@ int pcb_tc_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, v
     if (int rc = make_tmap_2d(&tm, dc, m_total, c->cout, dc_cstride, 64)) return rc;
     if (tma_wgrad_ok(c)) {
         kblock_box(c->wo, c->ho, &P.box_w, &P.box_h, &P.box_n);
-        // row-halo tiles: kw == 3, or the 4x4 space-to-depth stem problem (kw == 4, N = 64: four accumulators = 256 TMEM columns)
-        const bool halo = !getenv("PCB_DISABLE_TMA_HALO") && c->stride == 1 && (c->kw == 3 || (c->kw == 4 && c->cout <= 64)) && P.box_w == 64 &&
+        // row-halo tiles for kw == 3: the three taps of a kernel row are three 64 x 64 register accumulators per consumer thread
+        const bool halo = !getenv("PCB_DISABLE_TMA_HALO") && c->stride == 1 && c->kw == 3 && P.box_w == 64 &&
                           P.box_h == 1 && P.box_n == 1 && 64 + (c->kw - 1) * c->dil <= 256;
         const int hx = halo ? (c->kw - 1) * c->dil : 0;
         CUtensorMap ta[TC_MAX_PARTS];
@@ -3296,17 +3048,9 @@ int pcb_tc_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, v
             if (int rc = make_tmap_nhwc(&ta[p], src, c8, c->w, c->h, c->n, cs, P.box_w + hx, P.box_h, P.box_n, c->stride)) return rc;
         }
         if (c->nparts < 2) ta[1] = ta[0];
-        if (halo) {
-            if (c->kw == 4) return launch_wgrad_tma<64, 4, true>(P, tm, ta[0], ta[1], st);
-            if (c->cout % 128 == 0) return launch_wgrad_tma<128, 3, true>(P, tm, ta[0], ta[1], st);
-            return launch_wgrad_tma<64, 3, true>(P, tm, ta[0], ta[1], st);
-        }
-        if (c->cout % 256 == 0) return launch_wgrad_tma<256, 2, false>(P, tm, ta[0], ta[1], st);
-        if (c->cout % 128 == 0) return launch_wgrad_tma<128, 3, false>(P, tm, ta[0], ta[1], st);
+        if (halo) return launch_wgrad_tma<64, 3, true>(P, tm, ta[0], ta[1], st);
         return launch_wgrad_tma<64, 3, false>(P, tm, ta[0], ta[1], st);
     }
-    if (c->cout % 256 == 0) return launch_wgrad<256, 2, 3>(P, tm, c->cout, st);
-    if (c->cout % 128 == 0) return launch_wgrad<128, 3, 3>(P, tm, c->cout, st);
     return launch_wgrad<64, 3, 3>(P, tm, c->cout, st);
 }
 

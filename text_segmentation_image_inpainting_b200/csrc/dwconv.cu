@@ -171,8 +171,8 @@ __global__ void __launch_bounds__(256) dw_wgrad_kernel(const DwParams P, const T
 
 // =================================================================================================================
 // 3x3 depthwise kernels, second generation (any stride / dilation).  The first-generation kernels above spend most of their
-// instructions on 64-bit index divisions per element and reload the nine weight vectors for every output; at 8 x 512^2 they
-// reach ~13 % of the HBM roofline (ncu: issue-bound, not bandwidth-bound).  Here
+// instructions on 64-bit index divisions per element and reload the nine weight vectors for every output: they are
+// issue-bound, not bandwidth-bound.  Here
 //   * a block owns a chunk of `cvb` channel vectors (8 channels each) x PL pixel lanes; a thread keeps ONE channel vector for
 //     its whole life, so the nine weight vectors (fwd / dgrad) or the nine gradient accumulators (wgrad) live in registers,
 //   * rows are walked by blockIdx.y in groups, pixels of a row by the PL lanes: all index math is 32-bit adds,
@@ -392,9 +392,8 @@ __global__ void __launch_bounds__(256) dw3_wgrad_kernel(const DwParams P, const 
 
 // =================================================================================================================
 // 3x3 depthwise, stride 1, padding == dilation (every depthwise layer of the reference's segmentation networks), ordinary
-// (mask-free) convolution: third generation.  Measured on the second generation (ncu, 1152 channels @ 64x64, dilation 8): nine
-// 16-byte loads per output vector whose vertical re-use distance (dilation x row x channels) exceeds L1, i.e. 9x the
-// algorithmic bytes out of L2 and ~13 % of the HBM roofline.  Here
+// (mask-free) convolution: third generation.  The second generation issues nine 16-byte loads per output vector whose vertical
+// re-use distance (dilation x row x channels) exceeds L1 at large dilations, i.e. up to 9x the algorithmic bytes out of L2.  Here
 //   * a thread owns one output COLUMN x one channel QUAD (4 channels, 8-byte accesses) and walks down the rows of ONE
 //     dilation phase (rows a, a+d, a+2d, ...): a dilated 3x3 convolution is a plain 3x3 convolution inside each phase, so
 //     every input row is loaded once per thread (its three horizontal taps x-d, x, x+d) and scattered into the three output
@@ -468,14 +467,22 @@ inline Dw4Geom dw4_geom(int c, int w, int h, int dil) {
 }
 
 // y[oy][ox][c] = b[c] + sum_{tr,tc} w[tr][tc][c] * x[oy + (tr-1) d][ox + (tc-1) d][c]      (FLIP: w[2-tr][2-tc], no bias: data gradient)
-// The arithmetic is packed fp32 (FFMA2: two fp32 FMAs per instruction on sm_100): these kernels are ISSUE-bound, not
-// bandwidth-bound (ncu: 42 % issue-active at 24 % occupancy, ~100 instructions per 16 bytes moved in the scalar version), so
-// halving the FMA count and walking pointers instead of re-deriving 64-bit addresses is what moves them towards the roofline.
+// The arithmetic works on four channels at a time through pointers that are walked, not re-derived: these kernels are
+// ISSUE-bound, not bandwidth-bound (~100 instructions per 16 bytes moved in a scalar version with 64-bit address arithmetic).
 struct F4 { float2 lo, hi; };
 __device__ __forceinline__ F4 f4_zero() { F4 r; r.lo = make_float2(0.f, 0.f); r.hi = make_float2(0.f, 0.f); return r; }
-__device__ __forceinline__ F4 f4_fma(const F4 &a, const F4 &b, const F4 &c) { F4 r; r.lo = __ffma2_rn(a.lo, b.lo, c.lo); r.hi = __ffma2_rn(a.hi, b.hi, c.hi); return r; }
-__device__ __forceinline__ F4 f4_mul(const F4 &a, const F4 &b) { F4 r; r.lo = __fmul2_rn(a.lo, b.lo); r.hi = __fmul2_rn(a.hi, b.hi); return r; }
-__device__ __forceinline__ F4 f4_add(const F4 &a, const F4 &b) { F4 r; r.lo = __fadd2_rn(a.lo, b.lo); r.hi = __fadd2_rn(a.hi, b.hi); return r; }
+__device__ __forceinline__ F4 f4_fma(const F4 &a, const F4 &b, const F4 &c) {
+    F4 r;
+    r.lo = make_float2(fmaf(a.lo.x, b.lo.x, c.lo.x), fmaf(a.lo.y, b.lo.y, c.lo.y));
+    r.hi = make_float2(fmaf(a.hi.x, b.hi.x, c.hi.x), fmaf(a.hi.y, b.hi.y, c.hi.y));
+    return r;
+}
+__device__ __forceinline__ F4 f4_mul(const F4 &a, const F4 &b) {
+    F4 r; r.lo = make_float2(__fmul_rn(a.lo.x, b.lo.x), __fmul_rn(a.lo.y, b.lo.y)); r.hi = make_float2(__fmul_rn(a.hi.x, b.hi.x), __fmul_rn(a.hi.y, b.hi.y)); return r;
+}
+__device__ __forceinline__ F4 f4_add(const F4 &a, const F4 &b) {
+    F4 r; r.lo = make_float2(__fadd_rn(a.lo.x, b.lo.x), __fadd_rn(a.lo.y, b.lo.y)); r.hi = make_float2(__fadd_rn(a.hi.x, b.hi.x), __fadd_rn(a.hi.y, b.hi.y)); return r;
+}
 template <typename T> __device__ __forceinline__ F4 f4_of(const Raw4<T> &q) {
     float v[4];
     q.unpack(v);
@@ -510,7 +517,7 @@ __global__ void __launch_bounds__(256, 2) dw4_s1_kernel(const T *__restrict__ x,
     const int pgroups = dil / ppb;
     const int pg = z % pgroups, nn = z / pgroups;
     // weights stay PACKED (bf16: 2 registers per tap instead of 4) and are unpacked at use: the 18 registers this frees pay for a
-    // six-row load queue -- these kernels are bound by bytes in flight per SM, not by issue slots (profiles/r02_ncu_dw.txt)
+    // six-row load queue -- these kernels are bound by bytes in flight per SM, not by issue slots
     constexpr int QF = sizeof(T) == 2 ? DW4_QF : DW4_Q;          // fp32 storage (exact mode): raw rows are twice as wide
     Raw4<T> wt[3][3];
     F4 bs = f4_zero(), st_s = f4_zero(), st_q = f4_zero();

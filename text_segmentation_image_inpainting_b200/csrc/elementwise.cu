@@ -38,8 +38,8 @@ inline int ew_grid_red(long long work_items, int per_block) {
 // shared memory and flushed with fp64 atomics.
 // ---------------------------------------------------------------------------------------------
 // All NRED partial sets are staged in shared memory at once and the cv*8 channel columns are summed by cv*8 threads in
-// parallel (the first version let only the cv threads of row 0 walk all rows serially, twice: ~4 us of tail per block -- as
-// long as the block's whole streaming phase).
+// parallel (letting only the cv threads of row 0 walk all rows serially, twice, makes the tail of a block as long as its
+// whole streaming phase).
 template <int NRED>
 __device__ __forceinline__ void block_flush(float (&acc)[NRED][8], int cv, int rpb, int r, int v, double *const (&out)[NRED]) {
     __shared__ float s_red[NRED][EW_THREADS][8];
@@ -166,9 +166,8 @@ __global__ void __launch_bounds__(EW_THREADS) bn_act_fwd_kernel(const T *__restr
 // 8 channels from the complete fp64 sums (produced by the convolution epilogue or pcb_bn_stats_acc), block 0 additionally
 // updates the running statistics and writes the per-channel coefficients the backward needs.
 //   coef: [4][c] floats = scale (gamma * invstd) | shift (beta - mean * scale) | mean | invstd
-// (fp64 arithmetic runs at 1/64 of the fp32 rate on this GPU: the coefficient prologue is done ONCE per channel and block,
-// cooperatively, and handed to the threads through shared memory -- with every thread finalising its own 8 channels the
-// prologue alone cost ~1 us per block and put a 10 us floor under every launch.)
+// (fp64 arithmetic is much slower than fp32: the coefficient prologue is done ONCE per channel and block, cooperatively, and
+// handed to the threads through shared memory instead of every thread finalising its own 8 channels in fp64.)
 template <typename T, int ACT>
 __global__ void __launch_bounds__(EW_THREADS) bn_fwd_fused_kernel(const T *__restrict__ x, long long count, int c, const double *__restrict__ sums,
                                                                   const float *__restrict__ gamma, const float *__restrict__ beta,
@@ -542,7 +541,7 @@ __global__ void __launch_bounds__(EW_THREADS) renorm_bwd_vec_kernel(const T *__r
         for (long long row = static_cast<long long>(blockIdx.x) * rpb + r; row < count; row += static_cast<long long>(gridDim.x) * rpb) {
             const float s = msum ? __ldg(msum + row) : 1.f;
             const bool hole = (s == 0.f);
-            const float inv = 1.0f / s;         // one reciprocal per row (ncu: 53 instructions per element with g / s, 57 % issue-bound)
+            const float inv = 1.0f / s;         // one reciprocal per row instead of a division per element
             float g[8], d[8];
             Vec8<T>::load(dy + row * dys + v * 8, g);
 #pragma unroll
@@ -893,8 +892,8 @@ extern "C" __attribute__((visibility("default"))) int pcb_pconv_renorm_backward(
     if (dbias) PCB_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float) * c->cout, ST));
     if (mg == 1 && c->cout % 8 == 0 && c->cout <= 2048 && dc_cstride == c->cout && dy_cstride % 8 == 0) {
         const int rpb = EW_THREADS / (c->cout / 8);
-        // with a bias gradient the kernel ends in cout atomics per block on the same cout addresses: one resident wave
-        // (2048 blocks x 64 atomics measured 116 us for the 134 MB of the U-Net stem, 4.6x the streaming time)
+        // with a bias gradient the kernel ends in cout atomics per block on the same cout addresses: one resident wave keeps
+        // the number of atomics per address small next to the streaming work
         const int vgrid = dbias ? ew_grid_red(count, rpb * 8) : ew_grid(count, rpb * 8);
         if (c->dtype == PCB_BF16) renorm_bwd_vec_kernel<bf16><<<vgrid, EW_THREADS, 0, ST>>>(static_cast<const bf16 *>(dy), dy_cstride, msum, count, c->cout, c->no_guard, static_cast<bf16 *>(dc), dc_cstride, dbias);
         else renorm_bwd_vec_kernel<float><<<vgrid, EW_THREADS, 0, ST>>>(static_cast<const float *>(dy), dy_cstride, msum, count, c->cout, c->no_guard, static_cast<float *>(dc), dc_cstride, dbias);

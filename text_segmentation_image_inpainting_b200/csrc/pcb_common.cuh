@@ -1,4 +1,4 @@
-// pcb_common.cuh -- shared host/device helpers for libpconv_b200 (sm_100a only).
+// pcb_common.cuh -- shared host/device helpers for libpconv_b200 (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -50,7 +50,7 @@ static inline int pcb_num_sms() {
     if (!sms[dev]) {
         int v = 0;
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-        sms[dev] = v > 0 ? v : 148;
+        sms[dev] = v > 0 ? v : 132;
     }
     return sms[dev];
 }

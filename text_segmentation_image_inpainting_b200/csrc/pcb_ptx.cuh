@@ -1,6 +1,6 @@
-// pcb_ptx.cuh -- inline-PTX wrappers for the Blackwell (sm_100a) async machinery used by the
-// tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), cp.async (LDGSTS), tcgen05 (UMMA /
-// TMEM).  No CUTLASS dependency: these are the raw instructions.
+// pcb_ptx.cuh -- inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the
+// tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), cp.async (LDGSTS), wgmma.
+// No CUTLASS dependency: these are the raw instructions.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -67,7 +67,7 @@ __device__ __forceinline__ void cp_async_16(uint32_t dst, const void *src, bool 
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// generic-proxy writes (st.shared / cp.async) -> async-proxy readers (TMA store, tcgen05.mma)
+// generic-proxy writes (st.shared / cp.async) -> async-proxy readers (TMA store, wgmma)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------- TMA
@@ -81,12 +81,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *m, 
         : "memory");
 }
 // 4-D tile (channels, x, y, image): out-of-range coordinates (negative included) are zero-filled -- the conv padding
-// 256-bit global store (STG.256, sm_100): one full 32-byte sector per lane and instruction.  `p` must be 32-byte aligned.
-__device__ __forceinline__ void st_global_256(void *p, const uint4 &a, const uint4 &b) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-                 : "memory");
-}
 // L2 prefetch of a tile (no shared-memory destination, no barrier): turns the later load of the same box into an L2 hit
 __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap *m, int c0, int c1, int c2, int c3) {
     asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
@@ -100,107 +94,57 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap *m, 
         : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <int NCOLS> __device__ __forceinline__ void tmem_alloc(uint32_t smem_dst) {   // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "n"(NCOLS) : "memory");
+// ---------------------------------------------------------------- wgmma (Hopper warpgroup MMA)
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 x bf16 -> fp32 register accumulators, issued by all 128 threads of one
+// warpgroup.  TA / TB: 0 = K-major operand, 1 = MN-major operand.  Accumulator fragment of thread t (warp w = t / 32 of the
+// warpgroup, lane l): d[i] is row 16 w + l / 4 + 8 ((i / 2) & 1), column 8 (i / 4) + 2 (l % 4) + (i & 1).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers must not be touched by the compiler while MMAs are in flight
+template <int R> __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {    // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-    const uint32_t acc = accumulate ? 1u : 0u;
+template <int TA, int TB> __device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-        : "memory");
+        "{\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, 1, 1, 1, %18, %19;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "n"(TA), "n"(TB));
 }
-// same with the accumulate flag known at compile time (no predicate plumbing in the issuing thread's instruction stream)
-__device__ __forceinline__ void umma_bf16_acc(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc) {
+template <int TA, int TB> __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc)
-        : "memory");
+        "{\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, %34, %35;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "n"(TA), "n"(TB));
 }
-// ---------------------------------------------------------------- CTA pairs (cluster of 2, tcgen05 cta_group::2)
-// Mechanics verified on B200 by tools/ubench/cta_pair_probe.cu.
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// address of the same shared-memory location in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) {
-    uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-template <int NCOLS> __device__ __forceinline__ void tmem_alloc_pair(uint32_t smem_dst) {   // whole warp, in both CTAs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() { asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory"); }
-template <int NCOLS> __device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-// D[256 x N] (+)= [A0; A1] * [B0; B1]^T : each CTA of the pair holds its 128 A rows and its N/2 B rows at the same smem offsets;
-// issued by ONE thread of the leader CTA (rank 0)
-__device__ __forceinline__ void umma_bf16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-    const uint32_t acc = accumulate ? 1u : 0u;
+template <int TA, int TB> __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-        : "memory");
+        "{\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1, %66, %67;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void umma_bf16_pair_acc(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc)
-        : "memory");
+template <int N, int TA, int TB> __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc) {
+    if constexpr (N == 32) wgmma_m64n32<TA, TB>(d, a_desc, b_desc);
+    else if constexpr (N == 64) wgmma_m64n64<TA, TB>(d, a_desc, b_desc);
+    else { static_assert(N == 128, "wgmma tile width"); wgmma_m64n128<TA, TB>(d, a_desc, b_desc); }
 }
-// all previously issued pair MMAs complete -> one arrival on `bar` (same offset) in both CTAs
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-
-// keep a value in a register: the compiler may not rematerialise it from constant memory (a lone thread pays the full
-// ~50-cycle LDC latency for every such reload inside its per-K-block loop)
-#define PCB_PIN(x) asm volatile("" : "+r"(x))
-// all previously issued MMAs of this thread complete -> one arrival on `bar`
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (lane i <- TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// named barrier over the `threads` threads of one role (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (64-bit), sm_100 format:
+// Shared-memory matrix descriptor (64-bit), sm_90 wgmma format:
 //   [ 0,14) start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1   [49,52) base offset
-//   [61,64) layout: 0 none, 1 128B(base 32B), 2 SWIZZLE_128B, 4 SWIZZLE_64B, 6 SWIZZLE_32B
+//   [32,46) stride-dim byte offset >> 4   [49,52) base offset   [62,64) layout: 0 none, 1 SWIZZLE_128B, 2 64B, 3 32B
 // Tiles here are "row = 128 bytes, 8 rows = one 1024-byte swizzle atom" (what TMA SWIZZLE_128B and the
 // software gather both produce):
 //   K-major  operand: rows are M/N, the 128 B are 64 bf16 of K  -> SBO = 1024 (next 8 rows), LBO unused (1).
@@ -211,28 +155,17 @@ __host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, 
     d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= 1ull << 46;     // descriptor version (Blackwell)
-    d |= 2ull << 61;     // SWIZZLE_128B
+    d |= 1ull << 62;     // SWIZZLE_128B
     return d;
 }
-// Same, layout type 0 (no swizzle, "interleave"): core matrices are 8 rows x 16 bytes stored contiguously (128 B).
+// Same, no swizzle ("interleave"): core matrices are 8 rows x 16 bytes stored contiguously (128 B).
 //   K-major : LBO = byte distance between the two 8-element K chunks of one MMA, SBO = distance between 8-row groups.
-//   MN-major: SBO = byte distance between 8-element M/N chunks,                 LBO = distance between 8-row K groups.
 __host__ __device__ __forceinline__ uint64_t make_smem_desc_noswizzle(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= 1ull << 46;     // descriptor version (Blackwell)
     return d;
-}
-// Instruction descriptor (32-bit) for kind::f16: bf16 A/B, fp32 accumulate.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (1 = bf16)  [10,13) B fmt (1 = bf16)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-           (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-           (static_cast<uint32_t>(m >> 4) << 24);
 }
 
 }  // namespace ptx

@@ -89,7 +89,7 @@ class BaseModule(nn.Module):
 # -------------------------------------
 class B200Conv2d(nn.Conv2d):
     """An ``nn.Conv2d`` (isinstance / out_channels / state_dict identical -- SURVEY 8b "attribute conventions")
-    whose forward runs on libpconv_b200: dense and 1x1 convolutions on the tcgen05 implicit-GEMM kernel,
+    whose forward runs on libpconv_b200: dense and 1x1 convolutions on the wgmma implicit-GEMM kernel,
     depthwise ones on the vectorised HBM-bound kernel, anything else on the shape-general kernel."""
 
     def __init__(self, *args, **kwargs):

@@ -141,7 +141,7 @@ class DoubleUpSample(nn.Module):
     def __init__(self, scale_factor, mode="nearest"):
         super().__init__()
         if scale_factor != 2 or mode != "nearest":
-            raise NotImplementedError("only nearest x2 has a B200 kernel (the only use in the reference networks)")
+            raise NotImplementedError("only nearest x2 has a GPU kernel (the only use in the reference networks)")
         self.upsample = nn.Upsample(scale_factor=scale_factor, mode=mode)   # kept for attribute compatibility
 
     def forward(self, args):

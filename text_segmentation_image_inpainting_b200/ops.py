@@ -24,7 +24,7 @@ def _dtype_code(t: torch.Tensor) -> int:
         return PCB_F32
     if t.dtype == torch.bfloat16:
         return PCB_BF16
-    raise _lib.PcbError(f"unsupported dtype {t.dtype}: the B200 path computes in float32 or bfloat16")
+    raise _lib.PcbError(f"unsupported dtype {t.dtype}: the GPU path computes in float32 or bfloat16")
 
 
 def as_feature(x: torch.Tensor) -> torch.Tensor:
@@ -52,7 +52,7 @@ def act_code(act) -> Tuple[int, float]:
         return ACT_RELU6, 0.0
     if isinstance(act, nn.ReLU):
         return ACT_RELU, 0.0
-    raise NotImplementedError(f"activation {type(act).__name__} has no fused B200 kernel (supported: ReLU, ReLU6, LeakyReLU)")
+    raise NotImplementedError(f"activation {type(act).__name__} has no fused GPU kernel (supported: ReLU, ReLU6, LeakyReLU)")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -414,7 +414,7 @@ class PartialConvFn(torch.autograd.Function):
             dcs = nhwc_layout(dc)
         elif geom.plain and not ctx.has_bias and geom.cout % 8 == 0 and nhwc_layout(gy) == geom.cout and gy.data_ptr() % 16 == 0:
             # ordinary convolution without bias: the renormaliser is 1 and there is no bias gradient -- the "renormalisation
-            # backward" would be a copy of gy (it was 15 % of a segmentation step)
+            # backward" would be a copy of gy
             dc = gy
             dcs = geom.cout
         else:

@@ -1,5 +1,4 @@
-"""Time single partial-conv layers of the bench network (forward + backward) with CUDA events; with
-PCB_TC_DEBUG_TIMING=1 the library also prints where the MMA threads wait.  Development tool."""
+"""Time single partial-conv layers of the bench network (forward + backward) with CUDA events.  Development tool."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
 import torch
@@ -44,7 +43,6 @@ for name in names:
     y.backward(gy); torch.cuda.synchronize()
     if ONCE:
         continue
-    quiet = os.environ.pop("PCB_TC_DEBUG_TIMING", None)
     for tag, fn in (("fwd", lambda: fwd()), ("fwd+bwd", lambda: fwd().backward(gy))):
         for _ in range(3): fn()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -52,5 +50,3 @@ for name in names:
         for _ in range(10): fn()
         e1.record(); torch.cuda.synchronize()
         print(f"{name:16s} {tag:8s} {e0.elapsed_time(e1) / 10:8.3f} ms", flush=True)
-    if quiet is not None:
-        os.environ["PCB_TC_DEBUG_TIMING"] = quiet

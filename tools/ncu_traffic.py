@@ -1,6 +1,6 @@
 """Reduce `ncu -i step.ncu-rep --page raw --csv` (an `ncu --set full --profile-from-start off ... python tools/profile_step.py`
 capture of ONE eager training step) to
-  * profiles/<prefix>_ncu_traffic.json : per conv family {launches, dram_bytes, time_us_under_ncu} -- bench.py's roofline.traffic
+  * <out.json> : per conv family {launches, dram_bytes, time_us_under_ncu}
   * a per-launch table on stdout       : time, DRAM read/write, SM / tensor-pipe / L2 throughput %, grid
 Usage: python tools/ncu_traffic.py raw.csv out.json > table.txt
 Family = the role of the kernel in the step (what bench.py's CUDA-event families time as tc_fwd / tc_dgrad / tc_wgrad / dw_*).
