@@ -48,7 +48,8 @@ constexpr int A_STAGE_BYTES = BLOCK_M * 128;
 constexpr int NUM_PRODUCER_THREADS = 128;
 constexpr int TC_MAX_PARTS = 2;             // U-Net inputs are cat([upsampled, skip]) at most
 // Every tensor-core kernel computes its 128-row tile with TWO consumer warpgroups: warpgroup g issues the m64 wgmmas of rows
-// [64 g, 64 g + 64) into register accumulators and then runs the epilogue of those rows.  wgmma reads shared memory through
+// [64 g, 64 g + 64) into register accumulators and then stages them for the epilogue (run by the same warps in the cp.async-gather
+// kernel, by dedicated epilogue warps in the TMA-fed kernels).  wgmma reads shared memory through
 // the async proxy, so data written by cp.async / st.shared is made visible to it with fence.proxy.async after the consumer
 // acquired the stage's mbarrier.
 constexpr int MMA_WARPS = 8;
@@ -100,9 +101,13 @@ struct TcParams {
     int bn_c;
 };
 
-// fused BatchNorm statistics: eight private slices of [128 sums | 128 squares], one per epilogue warp (row quadrant x column half)
+// fused BatchNorm statistics: private slices of [128 sums | 128 squares], one per epilogue warp -- eight in the cp.async-gather
+// kernel (row quadrant x column half), four in the TMA-fed kernels (row quadrant, all BLOCK_N <= 128 columns)
 constexpr int STAT_SLICE = 256;
 constexpr int STAT_SMEM_BYTES = MMA_WARPS * STAT_SLICE * 4 + 16;
+// TMA-fed kernels: four dedicated epilogue warps; warp w drains rows [32 w, 32 w + 32) of the staging tile
+constexpr int EPI_WARPS = 4;
+constexpr int EPI_STAT_SMEM_BYTES = EPI_WARPS * STAT_SLICE * 4;
 
 // 32 values per lane, 32 lanes: returns in lane l the sum over all lanes of v[l] (a transposing butterfly: 31 shuffles)
 __device__ __forceinline__ float warp_transpose_sum(float (&v)[32], int lane) {
@@ -126,9 +131,8 @@ __device__ __forceinline__ uint32_t align1024(uint32_t a) { return (a + 1023u) &
 // -------------------------------------------------------------------------------------------------
 // epilogue shared by the forward / dgrad kernels: staged fp32 accumulators -> renormalise / mask -> bf16 NHWC
 // -------------------------------------------------------------------------------------------------
-// `acc_row` is this lane's row of the staging tile (row warp * 32 + lane).  Columns [cb, ce) of the tile (multiples of 32): each
-// row quadrant is drained by two warps that split the columns.  s_stat: this warp's accumulators [sums of its columns | squares
-// at offset sq_off].
+// `acc_row` is the row of the staging tile that holds GEMM row `er.m`.  Columns [cb, ce) of the tile (multiples of 32).  s_stat:
+// this warp's accumulators [sums of its columns | squares at offset sq_off].
 __device__ __forceinline__ void load_acc32(const float *src, uint32_t (&r)[32]) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -137,30 +141,57 @@ __device__ __forceinline__ void load_acc32(const float *src, uint32_t (&r)[32]) 
     }
 }
 
+// What the epilogue of one row needs from global memory and the pixel arithmetic.  The dedicated epilogue warps fetch it
+// before they wait for the tile's accumulators, so the load latency is hidden behind the MMAs.
+struct EpiRow {
+    long long mo;                 // pixel index in the full-resolution output (fwd) / gradient (dgrad)
+    int m;
+    bool rvalid, hole;
+    float inv;                    // fwd: 1 / mask box sum
+    float dscale[TC_MAX_PARTS];   // dgrad: input mask of part p at this pixel (1 / 0; 1 without a mask)
+};
+
+template <int MODE>
+__device__ __forceinline__ EpiRow tc_epi_row(const TcParams &P, int m) {
+    EpiRow er;
+    er.m = m;
+    er.rvalid = m < P.m_total;
+    er.inv = 0.f;
+    er.hole = false;
+    er.mo = m;
+    int en = 0, eh = 0, ew = 0;
+    if (MODE == 1 && er.rvalid) {
+        en = m / (P.h * P.w); const int rem = m - en * P.h * P.w; eh = rem / P.w; ew = rem - eh * P.w;
+        eh = eh * P.sub + P.py; ew = ew * P.sub + P.px;
+        er.mo = (static_cast<long long>(en) * P.fh + eh) * P.fw + ew;
+    }
+    if (MODE == 0 && er.rvalid && P.sub != 1) {  // sub-pixel class launch: the tile grid is every `sub`-th output pixel
+        en = m / (P.ho * P.wo); const int rem = m - en * P.ho * P.wo; eh = rem / P.wo; ew = rem - eh * P.wo;
+        er.mo = (static_cast<long long>(en) * P.fh + eh * P.sub + P.py) * P.fw + ew * P.sub + P.px;
+    }
+    if (MODE == 0 && er.rvalid) {
+        const float s = P.msum ? P.msum[er.mo] : 1.f;               // null: plain convolution (renormaliser 1)
+        er.hole = (s == 0.f) && !P.no_guard;
+        er.inv = er.hole ? 0.f : 1.0f / s;        // no_guard: 1/0 = inf -> 0*inf = NaN like the reference
+    }
+#pragma unroll
+    for (int p = 0; p < TC_MAX_PARTS; ++p) {
+        er.dscale[p] = 1.f;
+        if (MODE == 1 && p < P.nparts) {
+            const TcPart &pt = P.parts[p];
+            if (er.rvalid && pt.dx != nullptr && pt.mask != nullptr)      // dx = acc * input mask of this part
+                er.dscale[p] = pt.mask[(static_cast<long long>(en) * (P.fh >> pt.mup) + (eh >> pt.mup)) * (P.fw >> pt.mup) + (ew >> pt.mup)] ? 1.f : 0.f;
+        }
+    }
+    return er;
+}
+
 template <int BLOCK_N, int MODE>
-__device__ __forceinline__ void tc_epilogue(const TcParams &P, const float *acc_row, int warp, int lane, int m0, int n0, float *s_stat,
+__device__ __forceinline__ void tc_epilogue(const TcParams &P, const EpiRow &er, const float *acc_row, int lane, int n0, float *s_stat,
                                             int cb, int ce, int sq_off) {
-                const int row = warp * 32 + lane;
-                const int m = m0 + row;
-                const bool rvalid = m < P.m_total;
-                float inv = 0.f;
-                bool hole = false;
-                int en = 0, eh = 0, ew = 0;
-                long long mo = m;                         // pixel index in the full-resolution output (fwd) / gradient (dgrad)
-                if (MODE == 1 && rvalid) {
-                    en = m / (P.h * P.w); const int rem = m - en * P.h * P.w; eh = rem / P.w; ew = rem - eh * P.w;
-                    eh = eh * P.sub + P.py; ew = ew * P.sub + P.px;
-                    mo = (static_cast<long long>(en) * P.fh + eh) * P.fw + ew;
-                }
-                if (MODE == 0 && rvalid && P.sub != 1) {  // sub-pixel class launch: the tile grid is every `sub`-th output pixel
-                    en = m / (P.ho * P.wo); const int rem = m - en * P.ho * P.wo; eh = rem / P.wo; ew = rem - eh * P.wo;
-                    mo = (static_cast<long long>(en) * P.fh + eh * P.sub + P.py) * P.fw + ew * P.sub + P.px;
-                }
-                if (MODE == 0 && rvalid) {
-                    const float s = P.msum ? P.msum[mo] : 1.f;               // null: plain convolution (renormaliser 1)
-                    hole = (s == 0.f) && !P.no_guard;
-                    inv = hole ? 0.f : 1.0f / s;         // no_guard: 1/0 = inf -> 0*inf = NaN like the reference
-                }
+                const int m = er.m;
+                const bool rvalid = er.rvalid, hole = er.hole;
+                const long long mo = er.mo;
                 if (P.partial != nullptr) {                // split-K: raw accumulators, reduced across CTAs with fp32 adds
     #pragma unroll 1
                     for (int c0 = cb; c0 < ce; c0 += 32) {
@@ -181,19 +212,20 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &P, const float *acc_
                     const int col = n0 + c0;
                     bf16 *orow = nullptr;
                     int nstore = 0;                      // channels to store from this 32-column chunk (multiple of 8)
-                    float scale = inv;
+                    float scale = er.inv;
                     if (MODE == 0) {
                         if (rvalid && col < P.y_cstride) { orow = P.y + mo * P.y_cstride + col; nstore = min(32, P.y_cstride - col); }
                     } else {
                         scale = 1.f;
-                        for (int p = 0; p < P.nparts; ++p) {
+#pragma unroll
+                        for (int p = 0; p < TC_MAX_PARTS; ++p) {
+                            if (p >= P.nparts) break;
                             const TcPart &pt = P.parts[p];
                             const int local = col - pt.koff;
                             if (local >= 0 && local < pt.kext && pt.dx != nullptr && local < pt.c8 && rvalid) {
                                 orow = pt.dx + mo * pt.dx_cstride + local;
                                 nstore = min(32, pt.c8 - local);
-                                if (pt.mask != nullptr)          // dx = acc * input mask of this part
-                                    scale = pt.mask[(static_cast<long long>(en) * (P.fh >> pt.mup) + (eh >> pt.mup)) * (P.fw >> pt.mup) + (ew >> pt.mup)] ? 1.f : 0.f;
+                                scale = er.dscale[p];
                             }
                         }
                     }
@@ -284,37 +316,44 @@ struct EpiRole {
     __device__ __forceinline__ int slice() const { return half * 4 + q; }
 };
 
-// register accumulators of warpgroup g (fragment layout: see ptx::wgmma_bf16) -> staging tile -> tc_epilogue of this warp's
-// 32 rows x column half.  Both named barriers span the warpgroup only: the other one keeps its own pace.
-template <int BLOCK_N, int MODE>
-__device__ __forceinline__ void mma_epilogue(const TcParams &P, const float (&acc)[BLOCK_N / 2], float *stage, int e, int lane, int m0, int n0,
-                                             float *s_stat) {
+// register accumulators of consumer warp e (fragment layout: see ptx::wgmma_bf16) -> its 16 rows of the staging tile
+template <int BLOCK_N>
+__device__ __forceinline__ void stage_acc(const float (&acc)[BLOCK_N / 2], float *stage, int e, int lane) {
     constexpr int PITCH = acc_pitch(BLOCK_N);
-    const int g = e >> 2;
-    const int r0 = 64 * g + 16 * (e & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+    const int r0 = 64 * (e >> 2) + 16 * (e & 3) + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; i += 2) {
         const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + c0;
         *reinterpret_cast<float2 *>(stage + row * PITCH + col) = make_float2(acc[i], acc[i + 1]);
     }
+}
+
+// register accumulators of warpgroup g -> staging tile -> tc_epilogue of this warp's 32 rows x column half.  Both named barriers
+// span the warpgroup only: the other one keeps its own pace.
+template <int BLOCK_N, int MODE>
+__device__ __forceinline__ void mma_epilogue(const TcParams &P, const float (&acc)[BLOCK_N / 2], float *stage, int e, int lane, int m0, int n0,
+                                             float *s_stat) {
+    constexpr int PITCH = acc_pitch(BLOCK_N);
+    const int g = e >> 2;
+    stage_acc<BLOCK_N>(acc, stage, e, lane);
     ptx::named_sync(1 + g, 128);
     const EpiRole<BLOCK_N> R(e);
-    tc_epilogue<BLOCK_N, MODE>(P, stage + (R.q * 32 + lane) * PITCH, R.q, lane, m0, n0, s_stat, R.cb, R.ce, 128);
+    const EpiRow er = tc_epi_row<MODE>(P, m0 + R.q * 32 + lane);
+    tc_epilogue<BLOCK_N, MODE>(P, er, stage + (R.q * 32 + lane) * PITCH, lane, n0, s_stat, R.cb, R.ce, 128);
     ptx::named_sync(1 + g, 128);                          // the staging rows are free for the next tile
 }
 
-// last N tile's BatchNorm statistics: the eight epilogue warps' partials are summed after a CTA-wide barrier, so the global sums
-// receive ONE atomic per channel per CTA.  `stat_base`: slice 0.
+// TMA-fed kernels: last N tile's BatchNorm statistics.  The EPI_WARPS epilogue warps' partials (slice w = [sums of the tile's
+// columns | squares at offset 128]) are summed after a CTA-wide barrier, so the global sums receive ONE atomic per channel per
+// CTA.  `stat_base`: slice 0.
 template <int BLOCK_N>
-__device__ __forceinline__ void tc_stats_final(const TcParams &P, const float *stat_base, int e, int lane, int stat_n0) {
-    constexpr int HN = EpiRole<BLOCK_N>::HN;
-    for (int col = e * 32 + lane; col < BLOCK_N; col += MMA_THREADS) {
+__device__ __forceinline__ void tc_stats_final(const TcParams &P, const float *stat_base, int w, int lane, int stat_n0) {
+    for (int col = w * 32 + lane; col < BLOCK_N; col += EPI_WARPS * 32) {
         const int co = stat_n0 + col;
         if (co < P.bn_c) {
-            const int h = col / HN, lc = col - h * HN;
             float a = 0.f, q = 0.f;
 #pragma unroll
-            for (int w4 = 0; w4 < 4; ++w4) { a += stat_base[(h * 4 + w4) * STAT_SLICE + lc]; q += stat_base[(h * 4 + w4) * STAT_SLICE + 128 + lc]; }
+            for (int w4 = 0; w4 < EPI_WARPS; ++w4) { a += stat_base[w4 * STAT_SLICE + col]; q += stat_base[w4 * STAT_SLICE + 128 + col]; }
             atomicAdd(P.bn_sums + co, static_cast<double>(a));
             atomicAdd(P.bn_sums + P.bn_c + co, static_cast<double>(q));
         }
@@ -735,13 +774,65 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
 // bit and overwrite hole rows of the landed tile with zeros before handing the stage to the MMA thread
 // (generic-proxy stores -> fence.proxy.async -> mbarrier).  Plain convolutions / dgrad skip the fixers.
 //
-//   warps 0-7  consumers  : two warpgroups, 4 x wgmma (K=16) per K block and weight tile, then the epilogue of their 64 rows
-//   warp 8     TMA producer : per K block one A tile (4-D) + the weight tiles (2-D) onto the same mbarrier
-//   warps 9-12 fixers     : hole rows -> 0   (MODE 0 with masks only)
+//   warps 0-7   consumers  : two warpgroups, 4 x wgmma (K=16) per K block and weight tile, then their accumulators -> staging tile
+//   warp 8      TMA producer : per K block one A tile (4-D) + the weight tiles (2-D) onto the same mbarrier
+//   warps 9-12  fixers     : hole rows -> 0   (MODE 0 with masks only)
+//   warps 13-16 epilogue   : staging tile -> renormalise / mask -> bf16 NHWC stores (+ BatchNorm statistics)
 // Every per-K-block loop of the producer is a handful of instructions: index arithmetic there (the old kernels did integer
 // divisions) directly delays the stages the tensor cores wait for.
+// The epilogue of tile i overlaps the MMAs of tile i+1 through ONE staging tile and two mbarriers: the consumers wait on
+// acc_empty before they write it and arrive on acc_full after; the epilogue warps wait on acc_full and arrive on acc_empty once
+// they have read it.  The epilogue warps fetch a tile's per-row data (mask sums, dgrad mask bytes) before they wait.
 // -------------------------------------------------------------------------------------------------
-constexpr int TMA_THREADS = MMA_THREADS + 5 * 32;
+constexpr int EPI_WARP0 = MMA_WARPS + 5;
+constexpr int TMA_THREADS = (EPI_WARP0 + EPI_WARPS) * 32;
+
+// shared memory behind the TMA-fed kernels' rings: full / fixed / empty barriers, acc_full / acc_empty, the statistics slices
+constexpr size_t TMA_BAR_BYTES = 24 * MAX_RING + 16;
+
+// epilogue warp w of the TMA-fed kernels: drains rows [32 w, 32 w + 32) x all columns of every tile the consumers stage (same
+// tile walk), one row per thread.  `tile_origin(tile, m0, n0)` gives a tile's origin, n0 < 0 for a tile the consumers skip.
+// stat_n0: N tile the statistics slice s_stat currently belongs to (-1: none / aborted).
+template <int BLOCK_N, int MODE, typename TileFn>
+__device__ __forceinline__ void tma_epilogue_warps(const TcParams &P, int tile0, int tstep, int num_tiles, TileFn tile_origin,
+                                                   const float *acc_stage, uint32_t acc_full, uint32_t acc_empty, float *s_stat,
+                                                   int &stat_n0, int w, int lane, int code) {
+    constexpr int PITCH = acc_pitch(BLOCK_N);
+    const float *acc_row = acc_stage + (w * 32 + lane) * PITCH;
+    if (s_stat) {
+        for (int i = lane; i < STAT_SLICE; i += 32) s_stat[i] = 0.f;
+        __syncwarp();
+    }
+    uint32_t ph = 0;
+    for (int tile = tile0; tile < num_tiles; tile += tstep) {
+        int m0, n0;
+        tile_origin(tile, m0, n0);
+        if (n0 < 0) continue;
+        if (s_stat && n0 != stat_n0) {
+            if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, 0, BLOCK_N, 128);
+            stat_n0 = n0;
+        }
+        const EpiRow er = tc_epi_row<MODE>(P, m0 + w * 32 + lane);
+        if (!__all_sync(0xffffffffu, ptx::mbar_wait(acc_full, ph, P.abort_flag, code))) { stat_n0 = -1; return; }
+        ph ^= 1;
+        tc_epilogue<BLOCK_N, MODE>(P, er, acc_row, lane, n0, s_stat, 0, BLOCK_N, 128);
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(acc_empty);
+    }
+}
+
+// consumer warp e after a tile's K loop: wait until the epilogue warps have read the staging tile, write this warp's accumulator
+// rows into it, hand it over.  false: aborted.
+template <int BLOCK_N>
+__device__ __forceinline__ bool tma_stage_tile(const TcParams &P, const float (&acc)[BLOCK_N / 2], float *acc_stage, uint32_t acc_full,
+                                               uint32_t acc_empty, uint32_t &ph, int e, int lane, int code) {
+    if (!__all_sync(0xffffffffu, ptx::mbar_wait(acc_empty, ph, P.abort_flag, code))) return false;
+    ph ^= 1;
+    stage_acc<BLOCK_N>(acc, acc_stage, e, lane);
+    __syncwarp();
+    if (lane == 0) ptx::mbar_arrive(acc_full);
+    return true;
+}
 
 // HALO = true (stride 1, tiles that are one image-row segment of 128 pixels): per kernel ROW one A tile of
 // 128 + (kw-1)*dil pixel rows is loaded, and the kw taps of that row are kw wgmma descriptors whose start address is
@@ -764,8 +855,9 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
     const uint32_t STAGE_TX = A_BYTES + nB * B_BYTES;
     const uint32_t sBar = smem_base + S * STAGE;
     const uint32_t bar_full = sBar, bar_fixed = sBar + 8 * MAX_RING, bar_empty = sBar + 16 * MAX_RING;
-    const uint32_t s_stat_addr = sBar + 24 * MAX_RING;
-    const uint32_t s_acc = (s_stat_addr + STAT_SMEM_BYTES + 15u) & ~15u;
+    const uint32_t acc_full = sBar + 24 * MAX_RING, acc_empty = acc_full + 8;
+    const uint32_t s_stat_addr = sBar + TMA_BAR_BYTES;
+    const uint32_t s_acc = s_stat_addr + EPI_STAT_SMEM_BYTES;
     uint8_t *smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform by construction
@@ -790,6 +882,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
         for (int s = 0; s < MAX_RING; ++s) {      // empty: one arrival per consumer warpgroup
             ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 2);
         }
+        ptx::mbar_init(acc_full, MMA_WARPS); ptx::mbar_init(acc_empty, EPI_WARPS);     // one arrival per warp
         ptx::fence_mbar_init();
     }
     if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_a0); if (np > 1) ptx::prefetch_tmap(&tmap_a1); }
@@ -797,9 +890,21 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
 
     // The producer runs WARP-CONVERGED (all 32 lanes walk the loops and wait on the barriers; the warp index is a shuffle
     // broadcast so the compiler knows the role branch is uniform) and only the TMA instructions sit inside an elect.sync region.
-    float *s_stat = nullptr;                                          // consumer warps: private BatchNorm-statistics accumulators
+    float *s_stat = nullptr;                                          // epilogue warps: private BatchNorm-statistics accumulators
     int stat_n0 = -1;                                                  // N tile they currently belong to (-1: none / aborted)
-    if (warp == 8) {
+    float *acc_stage = reinterpret_cast<float *>(smem_gen + (s_acc - smem_base));
+    if (warp >= EPI_WARP0) {
+        // ================================ epilogue warps ================================
+        const int w = warp - EPI_WARP0;
+        s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
+                     ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + w * STAT_SLICE : nullptr;
+        auto origin = [&](int tile, int &m0, int &n0) {
+            const int mn = tile / KS;
+            m0 = m0_of(mn / n_tiles); n0 = (mn % n_tiles) * BLOCK_N;
+            if (!tile_active(n0)) n0 = -1;
+        };
+        tma_epilogue_warps<BLOCK_N, MODE>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, s_stat, stat_n0, w, lane, 126);
+    } else if (warp == 8) {
         // ================================ TMA producer ================================
         int s = 0;
         uint32_t ph = 1;                                               // first pass over the ring: stages are free
@@ -877,25 +982,13 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
             nb0 = kext / BLOCK_K; kl0 = min(4, (c8 - (nb0 - 1) * BLOCK_K + 15) >> 4);
             if (MODE == 0 && np > 1) { nb1 = P.parts[1].kext / BLOCK_K; kl1 = min(4, (P.parts[1].c8 - (nb1 - 1) * BLOCK_K + 15) >> 4); }
         }
-        const EpiRole<BLOCK_N> R(e);
-        s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
-                     ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + R.slice() * STAT_SLICE : nullptr;
-        if (s_stat) {
-            for (int i = lane; i < STAT_SLICE; i += 32) s_stat[i] = 0.f;
-            __syncwarp();
-        }
-        float *acc_stage = reinterpret_cast<float *>(smem_gen + (s_acc - smem_base));
         int s = 0;
-        uint32_t ph = 0;
+        uint32_t ph = 0, aph = 1;                                      // aph: first pass, the staging tile is free
         bool dead = false;
         for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
             const int sp = tile % KS, mn = tile / KS;
-            const int m0 = m0_of(mn / n_tiles), n0 = (mn % n_tiles) * BLOCK_N;
+            const int n0 = (mn % n_tiles) * BLOCK_N;
             if (!tile_active(n0)) continue;
-            if (s_stat && n0 != stat_n0) {
-                if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, R.cb, R.ce, 128);
-                stat_n0 = n0;
-            }
             float acc[BLOCK_N / 2];
             zero_acc(acc);
             int held = -1;                                             // stage whose MMAs may still be reading it
@@ -931,8 +1024,8 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
             ptx::wgmma_wait<0>();
             ptx::wgmma_fence_regs(acc);
             if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
-            if (dead) { stat_n0 = -1; break; }
-            mma_epilogue<BLOCK_N, MODE>(P, acc, acc_stage, e, lane, m0, n0, s_stat);
+            if (dead) break;
+            if (!tma_stage_tile<BLOCK_N>(P, acc, acc_stage, acc_full, acc_empty, aph, e, lane, 125)) break;
         }
     } else if (warp > 8) {
         // ================================ fixers: zero the hole rows of every landed A tile ================================
@@ -1057,7 +1150,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
     }
 
     __syncthreads();
-    if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - EpiRole<BLOCK_N>(warp).slice() * STAT_SLICE, warp, lane, stat_n0);
+    if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - (warp - EPI_WARP0) * STAT_SLICE, warp - EPI_WARP0, lane, stat_n0);
 }
 
 
@@ -1104,8 +1197,9 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
     const uint32_t STAGE = A_ROOM + nb_max * B_BYTES;
     const uint32_t sBar = smem_base + S * STAGE;
     const uint32_t bar_full = sBar, bar_fixed = sBar + 8 * MAX_RING, bar_empty = sBar + 16 * MAX_RING;
-    const uint32_t s_stat_addr = sBar + 24 * MAX_RING;
-    const uint32_t s_acc = (s_stat_addr + STAT_SMEM_BYTES + 15u) & ~15u;
+    const uint32_t acc_full = sBar + 24 * MAX_RING, acc_empty = acc_full + 8;
+    const uint32_t s_stat_addr = sBar + TMA_BAR_BYTES;
+    const uint32_t s_acc = s_stat_addr + EPI_STAT_SMEM_BYTES;
     uint8_t *smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
@@ -1128,6 +1222,7 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 2); }
+        ptx::mbar_init(acc_full, MMA_WARPS); ptx::mbar_init(acc_empty, EPI_WARPS);     // one arrival per warp
         ptx::fence_mbar_init();
     }
     if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_a0); ptx::prefetch_tmap(&tmap_a1); }
@@ -1135,7 +1230,14 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
 
     float *s_stat = nullptr;
     int stat_n0 = -1;
-    if (warp == 8) {
+    float *acc_stage = reinterpret_cast<float *>(smem_gen + (s_acc - smem_base));
+    if (warp >= EPI_WARP0) {
+        // ================================ epilogue warps ================================
+        const int w = warp - EPI_WARP0;
+        s_stat = (MODE == 0 && P.bn_sums != nullptr) ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + w * STAT_SLICE : nullptr;
+        auto origin = [&](int tile, int &m0, int &n0) { m0 = (tile / n_tiles) * BLOCK_M; n0 = (tile % n_tiles) * BLOCK_N; };
+        tma_epilogue_warps<BLOCK_N, MODE>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, s_stat, stat_n0, w, lane, 326);
+    } else if (warp == 8) {
         // ================================ TMA producer ================================
         int s = 0;
         uint32_t ph = 1;
@@ -1172,22 +1274,10 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
         const uint64_t desc_a0 = ptx::make_smem_desc(smem_base + g * 64 * 128, 16, 1024);     // this warpgroup's 64 rows
         const uint64_t desc_b0 = ptx::make_smem_desc(smem_base + A_ROOM, 16, 1024);
         const uint32_t stage16 = STAGE >> 4;
-        const EpiRole<BLOCK_N> R(e);
-        s_stat = (MODE == 0 && P.bn_sums != nullptr) ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + R.slice() * STAT_SLICE : nullptr;
-        if (s_stat) {
-            for (int i = lane; i < STAT_SLICE; i += 32) s_stat[i] = 0.f;
-            __syncwarp();
-        }
-        float *acc_stage = reinterpret_cast<float *>(smem_gen + (s_acc - smem_base));
         int s = 0;
-        uint32_t ph = 0;
+        uint32_t ph = 0, aph = 1;                                      // aph: first pass, the staging tile is free
         bool dead = false;
         for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-            const int m0 = (tile / n_tiles) * BLOCK_M, n0 = (tile % n_tiles) * BLOCK_N;
-            if (s_stat && n0 != stat_n0) {
-                if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, R.cb, R.ce, 128);
-                stat_n0 = n0;
-            }
             float acc[BLOCK_N / 2];
             zero_acc(acc);
             int held = -1;
@@ -1210,8 +1300,8 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
             ptx::wgmma_wait<0>();
             ptx::wgmma_fence_regs(acc);
             if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
-            if (dead) { stat_n0 = -1; break; }
-            mma_epilogue<BLOCK_N, MODE>(P, acc, acc_stage, e, lane, m0, n0, s_stat);
+            if (dead) break;
+            if (!tma_stage_tile<BLOCK_N>(P, acc, acc_stage, acc_full, acc_empty, aph, e, lane, 325)) break;
         }
     } else if (warp > 8) {
         // ================================ fixers: zero the hole rows of every landed A tile ================================
@@ -1281,7 +1371,7 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
     }
 
     __syncthreads();
-    if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - EpiRole<BLOCK_N>(warp).slice() * STAT_SLICE, warp, lane, stat_n0);
+    if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - (warp - EPI_WARP0) * STAT_SLICE, warp - EPI_WARP0, lane, stat_n0);
 }
 
 // nearest 2x upsample of one convolution source into a dense [n, 2hs, 2ws, c8] buffer (TMA cannot replicate pixels)
@@ -2177,7 +2267,7 @@ int launch_tma_n(TcParams &P, const CUtensorMap &tw, const CUtensorMap &ta0, con
     const size_t stage = a_room + static_cast<size_t>(nb) * BLOCK_N * 128;
     P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (RING_BUDGET - acc_stage_bytes(BLOCK_N)) / stage));
     PCB_CHECK(P.stages >= 2, "TMA-fed conv: stage of %zu bytes does not fit twice", stage);
-    const size_t smem = 1024 + P.stages * stage + 24 * MAX_RING + 16 + STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
+    const size_t smem = 1024 + P.stages * stage + TMA_BAR_BYTES + EPI_STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
     auto kern = pconv_tc_tma_kernel<BLOCK_N, MODE, HALO>;
     PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     if (P.ksplit < 1) P.ksplit = 1;
@@ -2424,7 +2514,7 @@ int launch_sp_n(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUt
     const size_t stage = a_room + static_cast<size_t>(nb_max) * BLOCK_N * 128;
     P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (RING_BUDGET - acc_stage_bytes(BLOCK_N)) / stage));
     PCB_CHECK(P.stages >= 2, "sub-pixel conv: stage of %zu bytes does not fit twice", stage);
-    const size_t smem = 1024 + P.stages * stage + 24 * MAX_RING + 16 + STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
+    const size_t smem = 1024 + P.stages * stage + TMA_BAR_BYTES + EPI_STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
     auto kern = pconv_tc_sp_kernel<BLOCK_N, MODE>;
     PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     const int num_tiles = ((P.m_total + BLOCK_M - 1) / BLOCK_M) * (P.ncols / BLOCK_N);
