@@ -108,6 +108,20 @@ int pcb_pconv_forward_premasked(const pcb_conv *c, const void *w_fwd, const floa
 int pcb_conv_fuses_bn_stats(const pcb_conv *c);
 int pcb_pconv_forward_bn(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
                          uint8_t *newmask, void *workspace, int mask_pass_done, double *bn_sums, pcb_stream_t stream);
+/* Inference forward with the EVAL-MODE BatchNorm and the activation that follow the convolution applied in its epilogue
+ * (partial_convolution.py:193-201 and BaseModels.py:95-99 with the BatchNorm in eval mode): with v = the value
+ * pcb_pconv_forward would store (0 at holes),
+ *   y = act(v * scale[co] + shift[co])      rounded to the storage type once,
+ * so hole pixels hold act(shift[co]) -- the reference's BatchNorm runs over the zeros the partial convolution wrote.
+ * Channels [cout, y_cstride) are zeros.  scale / shift: fp32 [cout] from pcb_bn_finalize(training = 0), or both NULL for an
+ * activation alone ([PartialConv, PartialActivation] blocks).  act: PCB_ACT_*, slope: LeakyReLU's negative slope.
+ * Only for problems with pcb_conv_fuses_affine_act(c) == 1 (the tensor-core kernels without split-K and the depthwise 3x3
+ * kernels -- the problems pcb_conv_fuses_bn_stats accepts, whether or not PCB_DISABLE_FUSED_BN_STATS is set); others are
+ * rejected.  mask_pass_done: see pcb_pconv_forward_premasked.                                                                */
+int pcb_conv_fuses_affine_act(const pcb_conv *c);
+int pcb_pconv_forward_affine_act(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
+                                 uint8_t *newmask, void *workspace, int mask_pass_done, const float *scale, const float *shift,
+                                 int act, float slope, pcb_stream_t stream);
 
 /* Backward of the renormalisation (autograd of partial_convolution.py:71-72):
  *   dc = dy * [s>0] / s          (NHWC [n,ho,wo,dc_cstride]; channels [cout, dc_cstride) zeroed)
@@ -231,6 +245,14 @@ int pcb_scse_forward(const void *x, const float *cse, const float *ws, void *y, 
                      pcb_stream_t stream);
 int pcb_scse_backward(const void *gy, const void *x, const float *cse, const float *ws, const float *sse, void *dx, float *dcse,
                       float *dws, int dtype, int n, long long hw, int c, pcb_stream_t stream);
+/* Post-processing of the text-segmentation logits in one launch (Examples/demo_segmentation.py:33-36, Dataloader.py:308-316):
+ *   b   = MaxPool2d(3, stride 1, pad 1)(sigmoid(x) > 0.5)            over the whole [h, w] map (x: channel 0 of an NHWC tensor
+ *                                                                      with pixel stride `cstride`, PCB_F32 or PCB_BF16),
+ *   out = upsample_bilinear2d(b[:h_valid, :w_valid], (oh, ow), align_corners=False) > 0     (the unpad, then the resize).
+ * out: uint8 [n, oh, ow], 1 / 0.  Exact: the resize sums {0, 1} values with non-negative weights, so the kernel tests the taps
+ * with positive weight; the threshold is 1 / (1 + expf(-x)) > 0.5 in fp32.                                                     */
+int pcb_seg_mask_postprocess(const void *logits, int dtype, int n, int h, int w, int cstride, int h_valid, int w_valid, int oh,
+                             int ow, uint8_t *out, pcb_stream_t stream);
 
 /* ---- loss / optimiser used by the benchmark step (SURVEY 8d: loss = out.abs().mean()) ------ */
 int pcb_l1_mean_forward(const void *x, int dtype, long long numel, float *loss /* device scalar, overwritten */,

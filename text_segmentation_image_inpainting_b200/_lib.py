@@ -40,7 +40,11 @@ _SIGS = {
     "pcb_pconv_forward_premasked": (c_int, [ctypes.POINTER(Conv), c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcb_conv_fuses_bn_stats": (c_int, [ctypes.POINTER(Conv)]),
     "pcb_pconv_forward_bn": (c_int, [ctypes.POINTER(Conv), c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
-    "pcb_pconv_mask_pass": (c_int, [ctypes.POINTER(Conv), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcb_conv_fuses_affine_act": (c_int, [ctypes.POINTER(Conv)]),
+    "pcb_pconv_forward_affine_act": (c_int, [ctypes.POINTER(Conv), c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                             c_void_p, c_void_p, c_int, c_float, c_void_p]),
+    "pcb_seg_mask_postprocess": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pcb_pconv_mask_pass":(c_int, [ctypes.POINTER(Conv), c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcb_pconv_renorm_backward": (c_int, [ctypes.POINTER(Conv), c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "pcb_pconv_backward_data": (c_int, [ctypes.POINTER(Conv), c_void_p, c_int, c_void_p, c_void_p, ctypes.POINTER(c_void_p),
                                         ctypes.POINTER(ctypes.c_int32), c_void_p]),

@@ -92,8 +92,17 @@ PCB_API int pcb_conv_fuses_bn_stats(const pcb_conv *c) {
     return (use_tc(c) && pcb_tc_fuses_bn_stats(c)) ? 1 : 0;
 }
 
+// 1 when the forward kernel this problem dispatches to can apply an eval-mode BatchNorm + activation in its epilogue: the same
+// problems as pcb_conv_fuses_bn_stats, independent of PCB_DISABLE_FUSED_BN_STATS (which only concerns the training statistics)
+PCB_API int pcb_conv_fuses_affine_act(const pcb_conv *c) {
+    if (!c || c->force_generic) return 0;
+    if (use_dw(c)) return pcb_dw_fuses_affine_act(c) ? 1 : 0;
+    return (use_tc(c) && pcb_tc_fuses_affine_act(c)) ? 1 : 0;
+}
+
 static int pconv_forward_impl(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
-                              uint8_t *newmask, void *workspace, bool mask_pass_done, double *bn_sums, pcb_stream_t stream) {
+                              uint8_t *newmask, void *workspace, bool mask_pass_done, double *bn_sums, const pcb_ep *ep,
+                              pcb_stream_t stream) {
     if (int rc = validate(c, true)) return rc;
     PCB_CHECK(w_fwd && y && msum && newmask && y_cstride >= c->cout, "pcb_pconv_forward: bad arguments");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -101,21 +110,22 @@ static int pconv_forward_impl(const pcb_conv *c, const void *w_fwd, const float 
     else if (!mask_pass_done)
         if (int rc = pcb_mask_sums(c, msum, newmask, st)) return rc;
     PCB_CHECK(bn_sums == nullptr || pcb_conv_fuses_bn_stats(c), "pcb_pconv_forward_bn: this problem's kernel does not fuse the BatchNorm statistics (ask pcb_conv_fuses_bn_stats first)");
+    PCB_CHECK(ep == nullptr || pcb_conv_fuses_affine_act(c), "pcb_pconv_forward_affine_act: this problem's kernel does not apply a fused BatchNorm + activation (ask pcb_conv_fuses_affine_act first)");
     if (use_dw(c)) {
         PCB_CHECK(y_cstride % 8 == 0, "depthwise forward: y channel stride must be a multiple of 8");
-        return pcb_dw_forward(c, w_fwd, bias, y, y_cstride, msum, bn_sums, st);
+        return pcb_dw_forward(c, w_fwd, bias, y, y_cstride, msum, bn_sums, ep, st);
     }
     if (use_tc(c)) {
         PCB_CHECK(workspace != nullptr, "pcb_pconv_forward: workspace required for the tensor-core path");
         PCB_CHECK((reinterpret_cast<uintptr_t>(w_fwd) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0, "w / y must be 16-byte aligned");
-        return pcb_tc_forward_ws(c, w_fwd, bias, y, y_cstride, msum, static_cast<uint64_t *>(workspace), mask_pass_done, bn_sums, st);
+        return pcb_tc_forward_ws(c, w_fwd, bias, y, y_cstride, msum, static_cast<uint64_t *>(workspace), mask_pass_done, bn_sums, ep, st);
     }
     return pcb_generic_forward(c, w_fwd, bias, y, y_cstride, msum, st);
 }
 
 PCB_API int pcb_pconv_forward(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
                               uint8_t *newmask, void *workspace, pcb_stream_t stream) {
-    return pconv_forward_impl(c, w_fwd, bias, y, y_cstride, msum, newmask, workspace, false, nullptr, stream);
+    return pconv_forward_impl(c, w_fwd, bias, y, y_cstride, msum, newmask, workspace, false, nullptr, nullptr, stream);
 }
 
 // Forward with the statistics pass of the BatchNorm that follows (partial_convolution.py:193-197, BaseModels.py:95-99) fused into
@@ -123,7 +133,17 @@ PCB_API int pcb_pconv_forward(const pcb_conv *c, const void *w_fwd, const float 
 // `bn_sums` must be zero on entry and the problem must satisfy pcb_conv_fuses_bn_stats.  mask_pass_done: see pcb_pconv_forward_premasked.
 PCB_API int pcb_pconv_forward_bn(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
                                  uint8_t *newmask, void *workspace, int mask_pass_done, double *bn_sums, pcb_stream_t stream) {
-    return pconv_forward_impl(c, w_fwd, bias, y, y_cstride, msum, newmask, workspace, mask_pass_done != 0, bn_sums, stream);
+    return pconv_forward_impl(c, w_fwd, bias, y, y_cstride, msum, newmask, workspace, mask_pass_done != 0, bn_sums, nullptr, stream);
+}
+
+// Inference forward with the eval-mode BatchNorm + activation behind the convolution applied in its epilogue (see the header)
+PCB_API int pcb_pconv_forward_affine_act(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
+                                         uint8_t *newmask, void *workspace, int mask_pass_done, const float *scale, const float *shift,
+                                         int act, float slope, pcb_stream_t stream) {
+    PCB_CHECK(act >= PCB_ACT_NONE && act <= PCB_ACT_RELU6, "pcb_pconv_forward_affine_act: bad activation %d", act);
+    PCB_CHECK((scale == nullptr) == (shift == nullptr), "pcb_pconv_forward_affine_act: scale and shift must both be given or both be NULL");
+    const pcb_ep ep{scale, shift, act, slope};
+    return pconv_forward_impl(c, w_fwd, bias, y, y_cstride, msum, newmask, workspace, mask_pass_done != 0, nullptr, &ep, stream);
 }
 
 // The forward in two calls, for callers that run the mask chain of a network ahead of the feature path on another stream:
@@ -143,7 +163,7 @@ PCB_API int pcb_pconv_mask_pass(const pcb_conv *c, float *msum, uint8_t *newmask
 
 PCB_API int pcb_pconv_forward_premasked(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
                                         uint8_t *newmask, void *workspace, pcb_stream_t stream) {
-    return pconv_forward_impl(c, w_fwd, bias, y, y_cstride, msum, newmask, workspace, true, nullptr, stream);
+    return pconv_forward_impl(c, w_fwd, bias, y, y_cstride, msum, newmask, workspace, true, nullptr, nullptr, stream);
 }
 
 PCB_API int pcb_pconv_backward_data(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_fwd, const void *w_dgrad,

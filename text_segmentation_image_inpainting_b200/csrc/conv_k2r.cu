@@ -370,7 +370,7 @@ int pcb_k2r_forward(const pcb_conv *c, const pcb_smallco_layout &L, const void *
     bf16 *z = reinterpret_cast<bf16 *>(ws);
     uint64_t *sub_ws = reinterpret_cast<uint64_t *>(ws + zbytes(c) + rup256(sizeof(float) * K2R_N * K.cu));
     // Z = (u * m_u) W'^T : raw accumulators (no renormaliser, no bias) of the 1x1 problem
-    if (int rc = pcb_tc_forward_ws(&K.sub, w_fwd_extra, nullptr, z, K2R_N, nullptr, sub_ws, false, nullptr, st)) return rc;
+    if (int rc = pcb_tc_forward_ws(&K.sub, w_fwd_extra, nullptr, z, K2R_N, nullptr, sub_ws, false, nullptr, nullptr, st)) return rc;
     K2rParams P;
     base(P, c, K);
     P.z = z; P.w_fwd = static_cast<const bf16 *>(w_fwd); P.kf = L.kf; P.ktap = L.ktap; P.koff_s = L.koff[K.ps];

@@ -131,7 +131,7 @@ int pcb_stem_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fw
 }
 
 int pcb_stem_forward(const pcb_conv *c, const void *w_fwd_extra, const float *bias, void *y, int y_cstride, const float *msum, void *workspace,
-                     double *bn_sums, cudaStream_t st) {
+                     double *bn_sums, const pcb_ep *ep, cudaStream_t st) {
     StemPlan K = plan_of(c);
     PCB_CHECK(K.ok && workspace, "space-to-depth stem forward: wrong layer / no workspace");
     uint8_t *ws = static_cast<uint8_t *>(workspace);
@@ -142,8 +142,9 @@ int pcb_stem_forward(const pcb_conv *c, const void *w_fwd_extra, const float *bi
     // tap-validity words of the 4x4 problem (in-bounds bits only: no holes) where its kernel wants them (the gather kernels of
     // non-power-of-two grids; the TMA-fed kernels zero-fill out-of-range coordinates themselves)
     if (int rc = pcb_tc_forward_mask_pass(&K.sub, sub_ws, st)) return rc;
-    // the layer's own mask sums drive the epilogue (renormalise, zero at holes, bias, BatchNorm statistics); no hole rows in the GEMM
-    return pcb_tc_forward_ws(&K.sub, w_fwd_extra, bias, y, y_cstride, msum, sub_ws, true, bn_sums, st);
+    // the layer's own mask sums drive the epilogue (renormalise, zero at holes, bias, BatchNorm statistics or the eval-mode
+    // BatchNorm + activation); no hole rows in the GEMM
+    return pcb_tc_forward_ws(&K.sub, w_fwd_extra, bias, y, y_cstride, msum, sub_ws, true, bn_sums, ep, st);
 }
 
 int pcb_stem_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st) {

@@ -99,6 +99,12 @@ struct TcParams {
     // pass over y (nn.BatchNorm2d in training mode, partial_convolution.py:193-197) disappears.  null: off.
     double *bn_sums;
     int bn_c;
+    // fused eval-mode BatchNorm + activation (forward, MODE 0, inference): the stored value is
+    // apply_act(v * ep_scale[co] + ep_shift[co]) with v = the renormalised output (0 at holes), rounded to bf16 once.
+    // ep_scale == null: activation only (scale 1, shift 0).  ep_on == 0: off (the training path).
+    const float *ep_scale, *ep_shift;
+    int ep_on, ep_act;
+    float ep_slope;
 };
 
 // fused BatchNorm statistics: private slices of [128 sums | 128 squares], one per epilogue warp -- eight in the cp.async-gather
@@ -243,6 +249,10 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &P, const EpiRow &er,
                         const bool has_bias = (MODE == 0) && (P.bias != nullptr);
                         if (has_bias && col + lane < P.cout) bl = P.bias[col + lane];
                         const bool edge = (MODE == 0) && (col + 32 > P.cout);
+                        // eval-mode BatchNorm + activation: scale / shift fetched like the bias (one load per lane, then shuffles)
+                        const bool ep = (MODE == 0) && (P.ep_on != 0);
+                        float el = 1.f, eh = 0.f;
+                        if (ep && P.ep_scale != nullptr && col + lane < P.cout) { el = P.ep_scale[col + lane]; eh = P.ep_shift[col + lane]; }
     #pragma unroll
                         for (int j = 0; j < 16; ++j) {
                             float a = __uint_as_float(r[2 * j]), b = __uint_as_float(r[2 * j + 1]);
@@ -251,6 +261,10 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &P, const EpiRow &er,
                                 const float b1 = has_bias ? __shfl_sync(0xffffffffu, bl, 2 * j + 1) : 0.f;
                                 a = hole ? 0.f : fmaf(a, scale, b0);
                                 b = hole ? 0.f : fmaf(b, scale, b1);
+                                if (ep) {                  // holes become apply_act(shift): the BatchNorm sees the zeros written above
+                                    a = apply_act(fmaf(a, __shfl_sync(0xffffffffu, el, 2 * j), __shfl_sync(0xffffffffu, eh, 2 * j)), P.ep_act, P.ep_slope);
+                                    b = apply_act(fmaf(b, __shfl_sync(0xffffffffu, el, 2 * j + 1), __shfl_sync(0xffffffffu, eh, 2 * j + 1)), P.ep_act, P.ep_slope);
+                                }
                                 if (edge) {
                                     if (col + 2 * j >= P.cout) a = 0.f;
                                     if (col + 2 * j + 1 >= P.cout) b = 0.f;
@@ -2091,6 +2105,11 @@ int launch_tapmask(const pcb_conv *c, uint64_t *out, cudaStream_t st) {
     return 0;
 }
 
+void set_ep(TcParams &P, const pcb_ep *ep) {
+    if (ep == nullptr) return;
+    P.ep_on = 1; P.ep_scale = ep->scale; P.ep_shift = ep->shift; P.ep_act = ep->act; P.ep_slope = ep->slope;
+}
+
 void base_params(TcParams &P, const pcb_conv *c, const Layout &L) {
     memset(&P, 0, sizeof(P));
     P.n = c->n; P.h = c->h; P.w = c->w; P.cin = c->cin; P.cout = c->cout; P.kh = c->kh; P.kw = c->kw; P.stride = c->stride;
@@ -2549,7 +2568,7 @@ int class_streams(ClassStreams4 **out) {
 
 // forward over cat([up2x(x_u), x_s]): four class launches (see pconv_tc_sp_kernel)
 int sp_forward(const pcb_conv *c, const SpPlan &S, const Layout &L, const bf16 *w_sp, const float *bias, void *y, int y_cstride, const float *msum,
-               double *bn_sums, int *flag, cudaStream_t st) {
+               double *bn_sums, const pcb_ep *ep, int *flag, cudaStream_t st) {
     const int hc = c->h / 2, wc = c->w / 2;
     const long long m_class = static_cast<long long>(c->n) * hc * wc;
     TcParams P;
@@ -2559,6 +2578,7 @@ int sp_forward(const pcb_conv *c, const SpPlan &S, const Layout &L, const bf16 *
     P.sub = 2; P.fh = c->ho; P.fw = c->wo;
     P.bias = bias; P.msum = msum; P.y = static_cast<bf16 *>(y); P.y_cstride = y_cstride; P.abort_flag = flag;
     P.bn_sums = bn_sums; P.bn_c = c->cout;
+    set_ep(P, ep);
     P.box_w = S.bw; P.box_h = S.bh; P.box_n = S.bn;
     const int cols = (c->cout <= 32) ? 32 : L.rows_f;
     const int bn = sp_bn(cols, m_class);
@@ -2794,11 +2814,17 @@ int pcb_tc_forward_mask_pass(const pcb_conv *c, uint64_t *tapmask, cudaStream_t 
 
 // true when pcb_tc_forward_ws accumulates the BatchNorm statistics of its output itself (tensor-core kernels, no split-K)
 bool pcb_tc_fuses_bn_stats(const pcb_conv *c) {
-    return pcb_tc_eligible(c) && !smallco_ok(c) && !getenv("PCB_SPLITK") && !getenv("PCB_DISABLE_FUSED_BN_STATS");
+    return pcb_tc_fuses_affine_act(c) && !getenv("PCB_DISABLE_FUSED_BN_STATS");
+}
+
+// true when pcb_tc_forward_ws can apply an eval-mode BatchNorm + activation in its epilogue (the same kernels as above: the
+// small-Cout / RGB-tail kernels have no such epilogue, split-K applies its epilogue in a separate finish kernel)
+bool pcb_tc_fuses_affine_act(const pcb_conv *c) {
+    return pcb_tc_eligible(c) && !smallco_ok(c) && !getenv("PCB_SPLITK");
 }
 
 int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, const float *msum,
-                      uint64_t *tapmask, bool mask_pass_done, double *bn_sums, cudaStream_t st) {
+                      uint64_t *tapmask, bool mask_pass_done, double *bn_sums, const pcb_ep *ep, cudaStream_t st) {
     int *flag = abort_flag_ptr();
     PCB_CHECK(flag != nullptr, "cudaMalloc(abort flag) failed");
     const long long m_total = static_cast<long long>(c->n) * c->ho * c->wo;
@@ -2809,9 +2835,11 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
         if (int rc = pcb_tc_forward_mask_pass(c, tapmask, st)) return rc;
     if (stem_ok(c)) {
         PCB_CHECK(bn_sums == nullptr || pcb_tc_fuses_bn_stats(c), "fused BatchNorm statistics requested from a kernel that does not produce them");
-        return pcb_stem_forward(c, static_cast<const bf16 *>(w_fwd) + stem_base(L), bias, y, y_cstride, msum, tapmask, bn_sums, st);
+        PCB_CHECK(ep == nullptr || pcb_tc_fuses_affine_act(c), "fused BatchNorm + activation requested from a kernel that does not apply it");
+        return pcb_stem_forward(c, static_cast<const bf16 *>(w_fwd) + stem_base(L), bias, y, y_cstride, msum, tapmask, bn_sums, ep, st);
     }
     if (smallco_ok(c)) {
+        PCB_CHECK(ep == nullptr, "fused BatchNorm + activation requested from a small-Cout kernel that does not apply it");
         if (pcb_k2r_ok(c)) {
             size_t fb, db;
             k2r_bases(L, &fb, &db);
@@ -2823,7 +2851,7 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
         const SpPlan S = sp_plan(c);
         if (S.ok && S.fwd) {
             PCB_CHECK(bn_sums == nullptr || pcb_tc_fuses_bn_stats(c), "fused BatchNorm statistics requested from a kernel that does not produce them");
-            return sp_forward(c, S, L, static_cast<const bf16 *>(w_fwd) + static_cast<size_t>(L.rows_f) * L.kf, bias, y, y_cstride, msum, bn_sums, flag, st);
+            return sp_forward(c, S, L, static_cast<const bf16 *>(w_fwd) + static_cast<size_t>(L.rows_f) * L.kf, bias, y, y_cstride, msum, bn_sums, ep, flag, st);
         }
     }
     TcParams P;
@@ -2833,6 +2861,8 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
     P.bias = bias; P.msum = msum; P.y = static_cast<bf16 *>(y); P.y_cstride = y_cstride; P.abort_flag = flag;
     PCB_CHECK(bn_sums == nullptr || pcb_tc_fuses_bn_stats(c), "fused BatchNorm statistics requested from a kernel that does not produce them");
     P.bn_sums = bn_sums; P.bn_c = c->cout;
+    PCB_CHECK(ep == nullptr || pcb_tc_fuses_affine_act(c), "fused BatchNorm + activation requested from a kernel that does not apply it");
+    set_ep(P, ep);
     P.ncols = L.rows_f;
     CUtensorMap tm;
     if (tma_fwd_ok(c)) {
@@ -2866,6 +2896,7 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
         if (int rc = make_tmap_2d(&tm, w_fwd, L.rows_f, L.kf, L.kf, bn)) return rc;
         P.ksplit = pick_ksplit(m_total, P.ncols, bn, L.ktap / BLOCK_K);
         if (P.ksplit > 1) {
+            PCB_CHECK(!P.ep_on, "split-K forward: the finish kernel does not apply a fused BatchNorm + activation");
             const size_t bytes = static_cast<size_t>(m_total) * P.ncols * sizeof(float);
             P.partial = splitk_scratch(bytes);
             PCB_CHECK(P.partial != nullptr, "split-K scratch allocation failed");

@@ -14,6 +14,16 @@
 
 namespace {
 
+// eval-mode BatchNorm + activation in the forward epilogue of the 3x3 kernels (see pcb_ep); on == 0: off
+struct DwEp { const float *scale, *shift; int on, act; float slope; };
+
+inline DwEp dw_ep(const pcb_ep *e) {
+    DwEp d;
+    memset(&d, 0, sizeof(d));
+    if (e != nullptr) { d.on = 1; d.scale = e->scale; d.shift = e->shift; d.act = e->act; d.slope = e->slope; }
+    return d;
+}
+
 struct DwParams {
     int n, h, w, c, kh, kw, stride, pad_h, pad_w, dil, ho, wo;
     int x_cstride, y_cstride;
@@ -22,6 +32,7 @@ struct DwParams {
     const float *msum;       // [mg][n*ho*wo] or null (plain): renormaliser
     int mg;                  // 1, or c (per-channel sums: groups > 1 && !same_holes)
     int no_guard;
+    DwEp ep;
 };
 
 __device__ __forceinline__ bool dw_mask(const DwParams &P, int nn, int hi, int wi) {
@@ -202,7 +213,8 @@ template <typename T> __device__ __forceinline__ void dw3_load_weights(const T *
 
 constexpr int DW3_ROWS = 8;                         // output rows per block (forward / dgrad)
 
-template <typename T, bool PLAIN>
+// EP: eval-mode BatchNorm + activation before the store (inference: never together with the statistics)
+template <typename T, bool PLAIN, bool EP>
 __global__ void __launch_bounds__(256) dw3_fwd_kernel(const DwParams P, const T *__restrict__ x, const T *__restrict__ w_t,
                                                       const float *__restrict__ bias, T *__restrict__ y, int cvb, int pl,
                                                       double *__restrict__ bn_sums) {
@@ -210,12 +222,13 @@ __global__ void __launch_bounds__(256) dw3_fwd_kernel(const DwParams P, const T 
     const int vl = static_cast<int>(threadIdx.x) % cvb;
     const int v = blockIdx.x * cvb + vl, lane_px = static_cast<int>(threadIdx.x) / cvb;
     const bool active = lane_px < pl && v < (P.c >> 3);
-    if (!active && bn_sums == nullptr) return;
+    if (!active && (EP || bn_sums == nullptr)) return;
     const int ch = v * 8;
-    float wt[9][8], bs[8], st_s[8], st_q[8];
+    float wt[9][8], bs[8], st_s[8], st_q[8], es[8], eh[8];
     if (active) dw3_load_weights(w_t, P.c, ch, wt);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { bs[j] = (active && bias) ? bias[ch + j] : 0.f; st_s[j] = 0.f; st_q[j] = 0.f; }
+    for (int j = 0; j < 8; ++j) { bs[j] = (active && bias) ? bias[ch + j] : 0.f; st_s[j] = 0.f; st_q[j] = 0.f; es[j] = 1.f; eh[j] = 0.f; }
+    if (EP && active && P.ep.scale) { Vec8<float>::load(P.ep.scale + ch, es); Vec8<float>::load(P.ep.shift + ch, eh); }
     const int rows_total = P.n * P.ho;
     const long long total = static_cast<long long>(rows_total) * P.wo;
     for (int rr = 0; rr < DW3_ROWS; ++rr) {
@@ -253,14 +266,18 @@ __global__ void __launch_bounds__(256) dw3_fwd_kernel(const DwParams P, const T 
                 if (P.no_guard) o[j] = acc[j] / s + bs[j];
                 else o[j] = (s == 0.f) ? 0.f : acc[j] / s + bs[j];
             }
+            if (EP) {                                   // eval-mode BatchNorm + activation: holes become apply_act(shift)
+#pragma unroll
+                for (int j = 0; j < 8; ++j) o[j] = apply_act(fmaf(o[j], es[j], eh[j]), P.ep.act, P.ep.slope);
+            }
             Vec8<T>::store(y + m * P.y_cstride + ch, o);
-            if (bn_sums != nullptr) {                   // BatchNorm statistics of what was stored (bf16-rounded in bf16 mode)
+            if (!EP && bn_sums != nullptr) {            // BatchNorm statistics of what was stored (bf16-rounded in bf16 mode)
 #pragma unroll
                 for (int j = 0; j < 8; ++j) { const float r = to_f32(from_f32<T>(o[j])); st_s[j] += r; st_q[j] = fmaf(r, r, st_q[j]); }
             }
         }
     }
-    if (bn_sums != nullptr) {
+    if (!EP && bn_sums != nullptr) {
         // fused statistics pass of the BatchNorm that follows the depthwise convolution (BaseModels.py:95-99): per channel,
         // the PL pixel lanes' partial sums are added through shared memory; one fp64 atomic per channel and block
 #pragma unroll
@@ -504,9 +521,10 @@ template <typename T> __device__ __forceinline__ F4 f4_as_stored(const F4 &v) {
 
 constexpr int DW4_QF = 6;                           // forward / data gradient: rows of loads in flight per thread (a multiple of 3)
 constexpr int DW4_Q = 3;                            // rows of loads in flight per thread = the period of the accumulator rotation
-template <typename T, bool FLIP>
+// EP: eval-mode BatchNorm + activation before the store (forward only; never together with the statistics)
+template <typename T, bool FLIP, bool EP>
 __global__ void __launch_bounds__(256, 2) dw4_s1_kernel(const T *__restrict__ x, int x_cstride, const T *__restrict__ w_t, const float *__restrict__ bias,
-                                                        T *__restrict__ y, int y_cstride, double *__restrict__ bn_sums,
+                                                        T *__restrict__ y, int y_cstride, double *__restrict__ bn_sums, const DwEp ep,
                                                         int n, int h, int w, int c, int dil, int cq, int xt, int nseg, int rseg, int ppb) {
     __shared__ float s_stat[256][2];
     const int ql = static_cast<int>(threadIdx.x) % cq, xl = static_cast<int>(threadIdx.x) / cq;
@@ -520,7 +538,12 @@ __global__ void __launch_bounds__(256, 2) dw4_s1_kernel(const T *__restrict__ x,
     // six-row load queue -- these kernels are bound by bytes in flight per SM, not by issue slots
     constexpr int QF = sizeof(T) == 2 ? DW4_QF : DW4_Q;          // fp32 storage (exact mode): raw rows are twice as wide
     Raw4<T> wt[3][3];
-    F4 bs = f4_zero(), st_s = f4_zero(), st_q = f4_zero();
+    F4 bs = f4_zero(), st_s = f4_zero(), st_q = f4_zero(), es, eh = f4_zero();
+    es.lo = es.hi = make_float2(1.f, 1.f);
+    if (EP && ep.scale) {
+        const float4 a = *reinterpret_cast<const float4 *>(ep.scale + ch), b = *reinterpret_cast<const float4 *>(ep.shift + ch);
+        es.lo = make_float2(a.x, a.y); es.hi = make_float2(a.z, a.w); eh.lo = make_float2(b.x, b.y); eh.hi = make_float2(b.z, b.w);
+    }
 #pragma unroll
     for (int tr = 0; tr < 3; ++tr)
 #pragma unroll
@@ -555,10 +578,15 @@ __global__ void __launch_bounds__(256, 2) dw4_s1_kernel(const T *__restrict__ x,
 #pragma unroll
             for (int k = 0; k < QF; ++k) fetch(q[k]);
             auto emit = [&](const F4 &accv) {
-                const F4 o = f4_add(accv, bs);
+                F4 o = f4_add(accv, bs);
+                if (EP) {                                      // eval-mode BatchNorm + activation
+                    o = f4_fma(o, es, eh);
+                    o.lo = make_float2(apply_act(o.lo.x, ep.act, ep.slope), apply_act(o.lo.y, ep.act, ep.slope));
+                    o.hi = make_float2(apply_act(o.hi.x, ep.act, ep.slope), apply_act(o.hi.y, ep.act, ep.slope));
+                }
                 f4_store<T>(ps, o);
                 ps += yrow;
-                if (bn_sums != nullptr) { const F4 r = f4_as_stored<T>(o); st_s = f4_add(st_s, r); st_q = f4_fma(r, r, st_q); }
+                if (!EP && bn_sums != nullptr) { const F4 r = f4_as_stored<T>(o); st_s = f4_add(st_s, r); st_q = f4_fma(r, r, st_q); }
             };
             // three accumulators in rotating roles (period 3; QF is a multiple of it): while input sub-row i is processed, `top` belongs to
             // output row i-1 (receives tap row 2 and is complete), `mid` to output i (tap row 1), `bot` to output i+1 (tap row 0)
@@ -586,7 +614,7 @@ __global__ void __launch_bounds__(256, 2) dw4_s1_kernel(const T *__restrict__ x,
             }
         }
     }
-    if (bn_sums != nullptr) {
+    if (!EP && bn_sums != nullptr) {
         const float ss[4] = {st_s.lo.x, st_s.lo.y, st_s.hi.x, st_s.hi.y}, sq[4] = {st_q.lo.x, st_q.lo.y, st_q.hi.x, st_q.hi.y};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -750,21 +778,30 @@ int pcb_dw_weight_prepare(const pcb_conv *c, const float *w_master, void *w_t, c
 }
 
 bool pcb_dw_fuses_bn_stats(const pcb_conv *c) {
-    return pcb_dw_eligible(c) && c->kh == 3 && c->kw == 3 && !getenv("PCB_DW_GEN1") && !getenv("PCB_DISABLE_FUSED_BN_STATS");
+    return pcb_dw_fuses_affine_act(c) && !getenv("PCB_DISABLE_FUSED_BN_STATS");
+}
+
+// the 3x3 kernels (dw3_fwd_kernel, dw4_s1_kernel) can apply an eval-mode BatchNorm + activation before they store
+bool pcb_dw_fuses_affine_act(const pcb_conv *c) {
+    return pcb_dw_eligible(c) && c->kh == 3 && c->kw == 3 && !getenv("PCB_DW_GEN1");
 }
 
 int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *y, int y_cstride, const float *msum, double *bn_sums,
-                   cudaStream_t st) {
+                   const pcb_ep *ep, cudaStream_t st) {
     PCB_CHECK(bn_sums == nullptr || pcb_dw_fuses_bn_stats(c), "depthwise forward: fused BatchNorm statistics need the 3x3 kernels");
+    PCB_CHECK(ep == nullptr || pcb_dw_fuses_affine_act(c), "depthwise forward: fused BatchNorm + activation needs the 3x3 kernels");
     DwParams P;
     fill(P, c);
+    P.ep = dw_ep(ep);
     P.y_cstride = y_cstride;
     P.msum = msum;       // plain mode: mask_sums wrote 1.0 everywhere, so the same epilogue applies
     if (dw4_ok(c)) {
         const Dw4Geom g = dw4_geom(c->cin, c->w, c->h, c->dil);
         const dim3 grid(g.chunks, g.xtiles, c->n * g.pgroups * g.nseg);
-        if (c->dtype == PCB_BF16) dw4_s1_kernel<bf16, false><<<grid, 256, 0, st>>>(static_cast<const bf16 *>(c->parts[0].x), c->parts[0].x_cstride, static_cast<const bf16 *>(w_t), bias, static_cast<bf16 *>(y), y_cstride, bn_sums, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
-        else dw4_s1_kernel<float, false><<<grid, 256, 0, st>>>(static_cast<const float *>(c->parts[0].x), c->parts[0].x_cstride, static_cast<const float *>(w_t), bias, static_cast<float *>(y), y_cstride, bn_sums, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
+#define PCB_DW4_FWD(TT, EP_) dw4_s1_kernel<TT, false, EP_><<<grid, 256, 0, st>>>(static_cast<const TT *>(c->parts[0].x), c->parts[0].x_cstride, static_cast<const TT *>(w_t), bias, static_cast<TT *>(y), y_cstride, bn_sums, P.ep, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb)
+        if (c->dtype == PCB_BF16) { if (ep) PCB_DW4_FWD(bf16, true); else PCB_DW4_FWD(bf16, false); }
+        else { if (ep) PCB_DW4_FWD(float, true); else PCB_DW4_FWD(float, false); }
+#undef PCB_DW4_FWD
         PCB_LAUNCH_CHECK();
         return 0;
     }
@@ -772,9 +809,14 @@ int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *
         const Dw3Geom g = dw3_geom(c->cin);
         const dim3 grid(g.chunks, (c->n * c->ho + DW3_ROWS - 1) / DW3_ROWS);
         const bool plain = c->plain && c->parts[0].mask == nullptr;
-#define PCB_DW3_FWD(TT, PL_) dw3_fwd_kernel<TT, PL_><<<grid, 256, 0, st>>>(P, static_cast<const TT *>(c->parts[0].x), static_cast<const TT *>(w_t), bias, static_cast<TT *>(y), g.cvb, g.pl, bn_sums)
-        if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_FWD(bf16, true); else PCB_DW3_FWD(bf16, false); }
-        else { if (plain) PCB_DW3_FWD(float, true); else PCB_DW3_FWD(float, false); }
+#define PCB_DW3_FWD(TT, PL_, EP_) dw3_fwd_kernel<TT, PL_, EP_><<<grid, 256, 0, st>>>(P, static_cast<const TT *>(c->parts[0].x), static_cast<const TT *>(w_t), bias, static_cast<TT *>(y), g.cvb, g.pl, bn_sums)
+        if (ep) {
+            if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_FWD(bf16, true, true); else PCB_DW3_FWD(bf16, false, true); }
+            else { if (plain) PCB_DW3_FWD(float, true, true); else PCB_DW3_FWD(float, false, true); }
+        } else {
+            if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_FWD(bf16, true, false); else PCB_DW3_FWD(bf16, false, false); }
+            else { if (plain) PCB_DW3_FWD(float, true, false); else PCB_DW3_FWD(float, false, false); }
+        }
 #undef PCB_DW3_FWD
         PCB_LAUNCH_CHECK();
         return 0;
@@ -792,8 +834,8 @@ int pcb_dw_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
     if (dw4_ok(c)) {                                      // stride 1, pad == dil: the data gradient is the same convolution with flipped taps
         const Dw4Geom g = dw4_geom(c->cin, c->w, c->h, c->dil);
         const dim3 grid(g.chunks, g.xtiles, c->n * g.pgroups * g.nseg);
-        if (c->dtype == PCB_BF16) dw4_s1_kernel<bf16, true><<<grid, 256, 0, st>>>(static_cast<const bf16 *>(dc), dc_cstride, static_cast<const bf16 *>(w_t), nullptr, static_cast<bf16 *>(dx), dx_cstride, nullptr, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
-        else dw4_s1_kernel<float, true><<<grid, 256, 0, st>>>(static_cast<const float *>(dc), dc_cstride, static_cast<const float *>(w_t), nullptr, static_cast<float *>(dx), dx_cstride, nullptr, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
+        if (c->dtype == PCB_BF16) dw4_s1_kernel<bf16, true, false><<<grid, 256, 0, st>>>(static_cast<const bf16 *>(dc), dc_cstride, static_cast<const bf16 *>(w_t), nullptr, static_cast<bf16 *>(dx), dx_cstride, nullptr, P.ep, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
+        else dw4_s1_kernel<float, true, false><<<grid, 256, 0, st>>>(static_cast<const float *>(dc), dc_cstride, static_cast<const float *>(w_t), nullptr, static_cast<float *>(dx), dx_cstride, nullptr, P.ep, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
         PCB_LAUNCH_CHECK();
         return 0;
     }

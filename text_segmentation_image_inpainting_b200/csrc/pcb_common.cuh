@@ -135,6 +135,10 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+// eval-mode BatchNorm + activation applied in a forward epilogue: y = apply_act(v * scale[co] + shift[co]); scale == null means
+// activation only.  A null `const pcb_ep *` means off.
+struct pcb_ep { const float *scale, *shift; int act; float slope; };
+
 // internal cross-file entry points -------------------------------------------------------------
 int pcb_generic_forward(const pcb_conv *c, const void *w, const float *bias, void *y, int y_cstride, const float *msum, cudaStream_t st);
 int pcb_generic_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_krsc, void *const *dx, const int *dx_cstride,
@@ -149,8 +153,9 @@ void pcb_tc_weight_layout(const pcb_conv *c, size_t *fwd_elems, size_t *dgrad_el
 int pcb_tc_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd, void *w_dgrad, bool zero_padding, cudaStream_t st);
 int pcb_tc_forward_mask_pass(const pcb_conv *c, uint64_t *tapmask, cudaStream_t st);
 int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, const float *msum,
-                      uint64_t *tapmask, bool mask_pass_done, double *bn_sums, cudaStream_t st);
+                      uint64_t *tapmask, bool mask_pass_done, double *bn_sums, const pcb_ep *ep, cudaStream_t st);
 bool pcb_tc_fuses_bn_stats(const pcb_conv *c);
+bool pcb_tc_fuses_affine_act(const pcb_conv *c);
 bool pcb_tc_subpixel(const pcb_conv *c);
 int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_dgrad, void *const *dx, const int *dx_cstride,
                  cudaStream_t st);
@@ -180,13 +185,14 @@ size_t pcb_stem_weight_extra(const pcb_conv *c);
 size_t pcb_stem_workspace(const pcb_conv *c);
 int pcb_stem_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd_extra, bool zero_padding, cudaStream_t st);
 int pcb_stem_forward(const pcb_conv *c, const void *w_fwd_extra, const float *bias, void *y, int y_cstride, const float *msum, void *workspace,
-                     double *bn_sums, cudaStream_t st);
+                     double *bn_sums, const pcb_ep *ep, cudaStream_t st);
 int pcb_stem_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st);
 // depthwise fast path (dwconv.cu)
 bool pcb_dw_eligible(const pcb_conv *c);
 int pcb_dw_weight_prepare(const pcb_conv *c, const float *w_master, void *w_t, cudaStream_t st);
 int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *y, int y_cstride, const float *msum, double *bn_sums,
-                   cudaStream_t st);
+                   const pcb_ep *ep, cudaStream_t st);
 bool pcb_dw_fuses_bn_stats(const pcb_conv *c);
+bool pcb_dw_fuses_affine_act(const pcb_conv *c);
 int pcb_dw_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_t, void *dx, int dx_cstride, cudaStream_t st);
 int pcb_dw_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, bool zero_dw, cudaStream_t st);

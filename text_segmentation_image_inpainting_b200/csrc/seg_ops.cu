@@ -311,6 +311,57 @@ __global__ void gap_bwd_kernel(const float *__restrict__ g, T *__restrict__ dx, 
     }
 }
 
+// ------------------------------------------------------------------------------------------------ text-mask post-processing
+// The demo's post-processing of the segmentation logits (Examples/demo_segmentation.py:33-36, Dataloader.py:308-316):
+//   b = maxpool3x3(sigmoid(x) > 0.5) over the full padded map,  crop to [h_valid, w_valid],
+//   out = upsample_bilinear2d(crop, (oh, ow), align_corners=False) > 0.
+// The inputs of the resize are {0, 1} and its weights are non-negative, so "sum > 0" is "some tap with a positive weight is 1":
+// each output pixel tests the (at most four) taps with positive weight, which makes the result exact.  Source indices and
+// lambdas follow ATen's UpSample.h (area_pixel_compute_scale / compute_source_index_and_lambda) in fp32.
+__device__ __forceinline__ void post_taps(int d, int in_size, int out_size, int &i0, int &i1, bool &w0, bool &w1) {
+    if (in_size == out_size) { i0 = i1 = d; w0 = true; w1 = false; return; }
+    const float scale = static_cast<float>(in_size) / static_cast<float>(out_size);
+    float src = scale * (static_cast<float>(d) + 0.5f) - 0.5f;
+    if (src < 0.f) src = 0.f;
+    i0 = min(static_cast<int>(floorf(src)), in_size - 1);
+    const float l1 = fminf(fmaxf(src - static_cast<float>(i0), 0.f), 1.f);
+    i1 = i0 + (i0 < in_size - 1 ? 1 : 0);
+    w0 = (1.f - l1) > 0.f; w1 = l1 > 0.f;
+}
+
+template <typename T>
+__device__ __forceinline__ bool post_pooled(const T *__restrict__ x, int cstride, int nn, int h, int w, int iy, int ix) {
+    for (int dy = -1; dy <= 1; ++dy) {
+        const int yy = iy + dy;
+        if (yy < 0 || yy >= h) continue;
+        for (int dx = -1; dx <= 1; ++dx) {
+            const int xx = ix + dx;
+            if (xx < 0 || xx >= w) continue;
+            const float v = to_f32(x[(static_cast<long long>(nn * h + yy) * w + xx) * cstride]);
+            if (1.0f / (1.0f + expf(-v)) > 0.5f) return true;      // the demo's sigmoid threshold, accurate expf
+        }
+    }
+    return false;
+}
+
+template <typename T>
+__global__ void seg_mask_post_kernel(const T *__restrict__ x, int cstride, int n, int h, int w, int hv, int wv, int oh, int ow,
+                                     uint8_t *__restrict__ out) {
+    const long long total = static_cast<long long>(n) * oh * ow;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const int ox = static_cast<int>(i % ow);
+        const long long t = i / ow;
+        const int oy = static_cast<int>(t % oh), nn = static_cast<int>(t / oh);
+        int y0, y1, x0, x1;
+        bool wy0, wy1, wx0, wx1;
+        post_taps(oy, hv, oh, y0, y1, wy0, wy1);
+        post_taps(ox, wv, ow, x0, x1, wx0, wx1);
+        const bool v = (wy0 && wx0 && post_pooled(x, cstride, nn, h, w, y0, x0)) || (wy0 && wx1 && post_pooled(x, cstride, nn, h, w, y0, x1)) ||
+                       (wy1 && wx0 && post_pooled(x, cstride, nn, h, w, y1, x0)) || (wy1 && wx1 && post_pooled(x, cstride, nn, h, w, y1, x1));
+        out[i] = v ? 1 : 0;
+    }
+}
+
 }  // namespace
 
 #define ST static_cast<cudaStream_t>(stream)
@@ -406,6 +457,19 @@ PCB_API int pcb_scse_backward(const void *gy, const void *x, const float *cse, c
         if (c <= 256) PCB_SCSE_BWD(float, 1); else if (c <= 512) PCB_SCSE_BWD(float, 2); else PCB_SCSE_BWD(float, 4);
     }
 #undef PCB_SCSE_BWD
+    PCB_LAUNCH_CHECK();
+    return 0;
+}
+
+PCB_API int pcb_seg_mask_postprocess(const void *logits, int dtype, int n, int h, int w, int cstride, int h_valid, int w_valid, int oh,
+                                     int ow, uint8_t *out, pcb_stream_t stream) {
+    PCB_CHECK(logits && out && (dtype == PCB_F32 || dtype == PCB_BF16), "pcb_seg_mask_postprocess: bad arguments");
+    PCB_CHECK(n > 0 && h > 0 && w > 0 && cstride > 0 && oh > 0 && ow > 0, "pcb_seg_mask_postprocess: non-positive size");
+    PCB_CHECK(h_valid > 0 && h_valid <= h && w_valid > 0 && w_valid <= w, "pcb_seg_mask_postprocess: crop %dx%d outside the %dx%d map",
+              h_valid, w_valid, h, w);
+    const int grid = sg_grid(static_cast<long long>(n) * oh * ow);
+    if (dtype == PCB_BF16) seg_mask_post_kernel<bf16><<<grid, 256, 0, ST>>>(static_cast<const bf16 *>(logits), cstride, n, h, w, h_valid, w_valid, oh, ow, out);
+    else seg_mask_post_kernel<float><<<grid, 256, 0, ST>>>(static_cast<const float *>(logits), cstride, n, h, w, h_valid, w_valid, oh, ow, out);
     PCB_LAUNCH_CHECK();
     return 0;
 }

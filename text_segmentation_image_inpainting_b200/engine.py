@@ -1,5 +1,7 @@
 """Training-step engine for the partial-conv U-Nets: flat fp32 parameter / gradient arenas, one fused SGD
 launch, optional data-parallel gradient all-reduce (NCCL over NVLink) and whole-step CUDA-graph capture.
+Inference engines (InferStep, SegInferStep): graph-captured eval-mode forward with the BatchNorm + activation passes fused
+into the convolution epilogues.
 
 The reference has no train script (SURVEY 3): its recipe is prose -- SGD + Nesterov momentum, weight decay,
 cyclic LR (checkpoints/ReadME.md:4).  One step here = forward + loss + backward (+ all-reduce) + SGD update,
@@ -7,6 +9,7 @@ the unit BASELINE.json's images/sec is quoted on.
 """
 from __future__ import annotations
 
+import ctypes
 import os
 from typing import List, Optional
 
@@ -344,3 +347,146 @@ class SegTrainStep(TrainStep):
         xin = buf[:, :c]
         xin.copy_(x)
         return ops.l1_mean(self.net(xin))
+
+
+class InferStep:
+    """Graph-captured inference of the partial-conv U-Nets: ``run(x, mask)`` with the reference's inputs (fp32 NCHW image and
+    {0, 1} hole mask, prepared like TrainStep._prepare) returns the output as a static fp32 NCHW buffer that the next call
+    overwrites.  The net runs in eval mode under no_grad, with the mask chain on its own stream and every eval-mode BatchNorm +
+    activation that directly follows a convolution applied in that convolution's epilogue (ops.set_fused_eval_epilogue).  The
+    first call for an input shape runs the forward eagerly (operand caches, BatchNorm coefficients, counters), then captures it
+    in one CUDA graph; later calls copy the inputs in and replay.
+
+    Counters (from the eager warm-up): `launches_per_run` (this library's kernels per forward), `fused_sites` / `unfused_sites`
+    (BatchNorm/activation passes applied in a convolution epilogue / still run on their own).
+
+    Weights: a change of the weight epoch since capture (``load_state_dict`` and the initialisers bump it) makes the next run()
+    rewrite the captured operand buffers in place (pcb_conv_weight_refresh) and the BatchNorm coefficients before it replays;
+    call refresh() after a mutation that does not bump the epoch."""
+
+    def __init__(self, net: torch.nn.Module, compute_dtype=torch.bfloat16):
+        self.net = net.eval()
+        self.dtype = compute_dtype
+        self._bns = [m for m in net.modules() if isinstance(m, torch.nn.BatchNorm2d)]
+        self._graphs = {}
+        self._captured_operands = []          # (cache, operand buffers, geometry, weight) of every captured convolution
+        self._epoch = None
+        self.launches_per_run = 0
+        self.fused_sites = self.unfused_sites = 0
+
+    _prepare = TrainStep._prepare
+
+    def _forward(self, x, mask):
+        xin, hm = self._prepare(x, mask)
+        return self.net((xin, hm))
+
+    def _key(self, x, mask):
+        return tuple(x.shape), x.dtype, (tuple(mask.shape), mask.dtype) if mask is not None else None
+
+    def _inputs(self, x, mask):
+        return (x, mask)
+
+    def _run_forward(self, *inputs):
+        ops.set_fused_eval_epilogue(True)
+        ops.set_mask_chain_stream(True)
+        try:
+            with torch.no_grad():
+                out = self._forward(*inputs)
+        finally:
+            ops.set_mask_chain_stream(False)
+            ops.set_fused_eval_epilogue(False)
+            ops.join_mask_streams()
+        return out
+
+    def _check_markers(self):
+        from .models.BaseModels import B200BNAct
+        stale = [name for name, m in self.net.named_modules() if isinstance(m, B200BNAct) and "_pcb_fused_out" in m.__dict__]
+        if stale:
+            raise _lib.PcbError(f"fused convolution outputs were never consumed by their BatchNorm: {stale}")
+
+    def _refresh_coefficients(self):
+        for bn in self._bns:
+            if not bn.training and bn.running_mean is not None and bn.weight is not None and bn.bias is not None:
+                ops.bn_eval_coefficients(bn)
+
+    def _capture(self, inputs):
+        for _ in range(2):                    # eager warm-up: operand caches, coefficients, counters
+            ops.EPILOGUE_SITES.update(fused=0, unfused=0)
+            before = _lib.launch_count()
+            out = self._run_forward(*inputs)
+            self.launches_per_run = _lib.launch_count() - before
+            self.fused_sites, self.unfused_sites = ops.EPILOGUE_SITES["fused"], ops.EPILOGUE_SITES["unfused"]
+            self._check_markers()
+        torch.cuda.synchronize()
+        static_in = tuple(t.clone() if t is not None else None for t in inputs)
+        static_out = torch.empty(tuple(out.shape), dtype=torch.float32, device=out.device)
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            static_out.copy_(self._run_forward(*static_in))
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            static_out.copy_(self._run_forward(*static_in))
+        self._check_markers()
+        # the captured kernels hold raw pointers to the operand buffers current at capture: keep them (and what rewrites them)
+        for m in self.net.modules():
+            cache = getattr(m, "_wcache", None)
+            if isinstance(cache, dict) and cache.get("val") is not None:
+                self._captured_operands.append((cache, cache["val"], cache["geom"], cache["weight"]))
+        torch.cuda.synchronize()
+        return graph, static_in, static_out
+
+    def refresh(self):
+        """Rewrite the captured operand buffers and BatchNorm coefficients from the current parameters and buffers."""
+        ops.bump_weight_epoch()
+        self._refresh()
+
+    def _refresh(self):
+        lib = _lib.load()
+        for cache, val, geom, weight in self._captured_operands:
+            w_fwd, w_dg = val
+            wm = weight.detach().float().contiguous(memory_format=CL)
+            _lib.check(lib.pcb_conv_weight_refresh(ctypes.byref(geom.struct(None)), wm.data_ptr(), w_fwd.data_ptr(), ops._ptr(w_dg),
+                                                   ops._stream()))
+            if cache.get("val") is val:       # eager calls find the refreshed buffers current
+                cache["key"] = (weight.data_ptr(), weight._version, str(weight.device), ops._WEIGHT_EPOCH, geom.signature)
+                cache["ready"] = None
+        self._refresh_coefficients()
+        self._epoch = ops._WEIGHT_EPOCH
+
+    def run(self, *inputs) -> torch.Tensor:
+        key = self._key(*inputs)
+        entry = self._graphs.get(key)
+        if entry is None:
+            if self._epoch is not None and self._epoch != ops._WEIGHT_EPOCH:
+                self._refresh()
+            entry = self._graphs[key] = self._capture(self._inputs(*inputs))
+            self._epoch = ops._WEIGHT_EPOCH
+        elif self._epoch != ops._WEIGHT_EPOCH:
+            self._refresh()
+        graph, static_in, static_out = entry
+        for dst, src in zip(static_in, self._inputs(*inputs)):
+            if dst is not None and src.data_ptr() != dst.data_ptr():
+                dst.copy_(src, non_blocking=True)
+        graph.replay()
+        return static_out
+
+
+class SegInferStep(InferStep):
+    """InferStep for the segmentation networks (models/text_segmentation.py): ``run(x)``, fp32 NCHW image; returns the logits
+    [n, 1, h, w] as a static fp32 NCHW buffer.  The demo's mask is ``ops.text_mask_postprocess(out, border_pad, out_hw)``."""
+
+    def _forward(self, x):
+        n, c, h, w = x.shape
+        buf = torch.empty((n, (c + 7) // 8 * 8, h, w), dtype=self.dtype, device=x.device, memory_format=CL).zero_()
+        xin = buf[:, :c]
+        xin.copy_(x)
+        return self.net(xin)
+
+    def _key(self, x):
+        return tuple(x.shape), x.dtype
+
+    def _inputs(self, x):
+        return (x,)

@@ -105,6 +105,17 @@ class B200Conv2d(nn.Conv2d):
         # convolution accumulates the per-channel sum / sum of squares of its output in its own epilogue and parks them on the
         # BatchNorm, which then skips its statistics pass over y (keyed by y's address and shape: any other input is ignored).
         hint = self.__dict__.get("_bn_hint")
+        # Inference (ops.set_fused_eval_epilogue): the eval-mode BatchNorm + activation behind this convolution is applied in its
+        # epilogue and the output is marked for that BatchNorm, which then passes it through.  Not where the BatchNorm adds a
+        # residual (InvertedResidual marks its last BatchNorm `_pcb_residual_site`): the add must follow the BatchNorm, not the activation.
+        if hint is not None and x.is_cuda and not hint.__dict__.get("_pcb_residual_site"):
+            epi = ops.eval_epilogue(hint[0], hint[1] if len(hint) > 1 else None)
+            if epi is not None:
+                y = ops.conv2d(x, self.weight, self.bias, self.stride, self.padding, self.dilation, self.groups, cache=self._wcache,
+                               epilogue=epi)
+                if epi.fused:
+                    hint.__dict__["_pcb_fused_out"] = (y.data_ptr(), tuple(y.shape))
+                return y
         handoff = None
         if hint is not None and hint[0].training and hint[0].weight is not None and x.is_cuda:
             handoff = ops.RenormHandoff(want_stats=True)
@@ -121,6 +132,12 @@ class B200BNAct(nn.Sequential):
 
     def forward(self, x, residual=None):
         from .. import ops
+        fused = self.__dict__.pop("_pcb_fused_out", None)
+        if fused is not None and fused == (x.data_ptr(), tuple(x.shape)):
+            if residual is not None:
+                raise ops._lib.PcbError("a convolution output that already went through this BatchNorm + activation reached it "
+                                        "again with a residual: mark the BatchNorm `_pcb_residual_site`")
+            return x                                        # applied in the producing convolution's epilogue
         act = self[1] if len(self) > 1 else None
         pend = self.__dict__.pop("_pending_stats", None)
         pre = pend[2] if (pend is not None and self[0].training and pend[0] == x.data_ptr() and pend[1] == tuple(x.shape)) else None

@@ -29,6 +29,9 @@ class InvertedResidual(BaseModule):
         if add_sece:
             m += [SpatialChannelSqueezeExcitation(out_channel, reduction=16, activation=activation)]
         self.conv = nn.Sequential(*m)
+        if self.res_connect and isinstance(self.conv[-1], B200BNAct):
+            # forward() folds the shortcut into this BatchNorm pass: its convolution must not apply it in the epilogue
+            self.conv[-1].__dict__["_pcb_residual_site"] = True
 
     def forward(self, x):
         if not self.res_connect:

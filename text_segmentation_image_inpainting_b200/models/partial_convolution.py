@@ -42,14 +42,14 @@ class PartialConv(BaseModule):
             p.requires_grad = False
         self._wcache = {}
 
-    def _conv(self, x, mask, no_guard=False, handoff=None):
+    def _conv(self, x, mask, no_guard=False, handoff=None, epilogue=None):
         fc = self.feature_conv
         return ops.partial_conv(x, mask, fc.weight, fc.bias, fc.stride, fc.padding, fc.dilation, fc.groups,
-                                same_holes=self.same_holes, no_guard=no_guard, cache=self._wcache, handoff=handoff)
+                                same_holes=self.same_holes, no_guard=no_guard, cache=self._wcache, handoff=handoff, epilogue=epilogue)
 
-    def forward(self, args, handoff=None):
+    def forward(self, args, handoff=None, epilogue=None):
         x, mask = args
-        return self._conv(x, mask, handoff=handoff)
+        return self._conv(x, mask, handoff=handoff, epilogue=epilogue)
 
 
 class PartialConv1x1(BaseModule):
@@ -78,9 +78,9 @@ class PartialConvNoHoles(PartialConv):
         super().__init__(in_channels, out_channels, kernel_size, stride, padding, dilation, groups, bias)
         assert self.feature_conv.groups == 1
 
-    def forward(self, args):
+    def forward(self, args, epilogue=None):
         x, mask = args
-        return self._conv(x, mask, no_guard=True)
+        return self._conv(x, mask, no_guard=True, epilogue=epilogue)
 
 
 def partial_convolution_block(in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, groups=1, bias=False,
@@ -102,14 +102,32 @@ def partial_convolution_block(in_channels, out_channels, kernel_size, stride=1, 
 class PartialBlock(nn.Sequential):
     """The nn.Sequential of the reference's factory (same children, same state_dict keys).  When it is exactly
     [PartialConv, PartialActivatedBN] the convolution output has a single consumer by construction, so the BatchNorm
-    backward may absorb the convolution's renormalisation backward (ops.RenormHandoff)."""
+    backward may absorb the convolution's renormalisation backward (ops.RenormHandoff).  For the same reason, under the
+    inference engines' switch (ops.set_fused_eval_epilogue), an eval-mode [PartialConv | PartialConvNoHoles, PartialActivatedBN |
+    PartialActivation] block applies its BatchNorm + activation in the convolution epilogue.  Residual sites never come through
+    here: DoublePartialResidual and PartialInvertedResidual call their last convolution and BatchNorm separately."""
 
     def forward(self, args):
+        epi = self._eval_epilogue()
+        if epi is not None:
+            y, m = self[0](args, epilogue=epi)
+            return (y, m) if epi.fused else self[1]((y, m))        # refused by the kernel: the two-pass path
         if len(self) == 2 and type(self[0]) is PartialConv and isinstance(self[1], PartialActivatedBN):
             bn = self[1].bn_act[0]
             h = ops.RenormHandoff(want_stats=bn.training and bn.weight is not None)
             return self[1](self[0](args, handoff=h), handoff=h)
         return super().forward(args)
+
+
+    def _eval_epilogue(self):
+        if len(self) != 2 or type(self[0]) not in (PartialConv, PartialConvNoHoles) or not ops.fused_eval_epilogue_enabled():
+            return None
+        tail = self[1]
+        if isinstance(tail, PartialActivatedBN):
+            return ops.eval_epilogue(tail.bn_act[0], tail.bn_act[1] if len(tail.bn_act) > 1 else None)
+        if isinstance(tail, PartialActivation):
+            return ops.eval_epilogue(None, tail.act_fn)
+        return None
 
 
 class PartialActivatedBN(BaseModule):

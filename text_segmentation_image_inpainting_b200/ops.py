@@ -329,6 +329,144 @@ def _workspace(lib, c, device):
     return torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=device)
 
 
+def _pconv_launch(lib, geom: ConvGeom, c: Conv, w_fwd, b32, y, bn_sums, epi: Optional["EvalEpilogue"]):
+    """Mask pass + forward of one partial convolution into `y`; returns (msum, newmask).  `bn_sums`: training statistics
+    target (pcb_pconv_forward_bn); `epi`: eval-mode BatchNorm + activation applied in the epilogue (pcb_pconv_forward_affine_act)."""
+    global _LAST_MASK_EVENT
+    _LAST_MASK_EVENT = None
+    dev = y.device
+
+    def forward(mask_pass_done, msum, newmask, ws):
+        if epi is None:
+            return lib.pcb_pconv_forward_bn(ctypes.byref(c), w_fwd.data_ptr(), _ptr(b32), y.data_ptr(), nhwc_layout(y), msum.data_ptr(),
+                                            newmask.data_ptr(), ws.data_ptr(), mask_pass_done, _ptr(bn_sums), _stream())
+        scale, shift = epi.coefficients()
+        return lib.pcb_pconv_forward_affine_act(ctypes.byref(c), w_fwd.data_ptr(), _ptr(b32), y.data_ptr(), nhwc_layout(y), msum.data_ptr(),
+                                                newmask.data_ptr(), ws.data_ptr(), mask_pass_done, _ptr(scale), _ptr(shift), epi.code,
+                                                epi.slope, _stream())
+
+    if _MASK_CHAIN_STREAM and _PROFILE is None and not geom.plain:
+        # Mask updates never depend on features (partial_convolution.py:59-77): the mask pass of this layer runs on the
+        # mask stream, ordered only after the passes that produced its input planes, i.e. ahead of the feature path.
+        # Its buffers are allocated on that stream and kept alive until join_side_streams() (engine, once per step).
+        main, ms = torch.cuda.current_stream(), _mask_stream(dev)
+        for (_, _, _, pl, _) in geom.parts:
+            if pl is None:
+                continue
+            ev_in = getattr(pl, "_pcb_ev", None)
+            if ev_in is None:                        # a plane written on the main stream (the network's input mask): mark it
+                ev_in = torch.cuda.Event()           # ready from here on, so later consumers (the tail) need not wait for main
+                ev_in.record(main)
+                pl._pcb_ev = ev_in
+            ms.wait_event(ev_in)
+        with torch.cuda.stream(ms):
+            msum = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.float32, device=dev)
+            newmask = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.uint8, device=dev)
+            ws = _workspace(lib, c, dev)
+            _lib.check(lib.pcb_pconv_mask_pass(ctypes.byref(c), msum.data_ptr(), newmask.data_ptr(), ws.data_ptr(), _stream()))
+            ev = torch.cuda.Event()
+            ev.record()
+        main.wait_event(ev)
+        _DEFERRED.append((msum, newmask, ws))
+        _LAST_MASK_EVENT = ev
+        _lib.check(forward(1, msum, newmask, ws))
+    else:
+        msum = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.float32, device=dev)
+        newmask = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.uint8, device=dev)
+        ws = _workspace(lib, c, dev)
+        with _Timed("fwd", geom):
+            _lib.check(forward(0, msum, newmask, ws))
+    return msum, newmask
+
+
+# ------------------------------------------------------------------------------------------------
+# inference: eval-mode BatchNorm + activation fused into the convolution epilogue
+# ------------------------------------------------------------------------------------------------
+_FUSED_EVAL_EPILOGUE = False
+# sites seen while the switch is on: "fused" = BatchNorm/activation passes applied in a convolution epilogue, "unfused" =
+# BatchNorm/activation passes that still ran on their own (bn_act / activation_only)
+EPILOGUE_SITES = {"fused": 0, "unfused": 0}
+
+
+def set_fused_eval_epilogue(enabled: bool):
+    """Let the convolution blocks apply their eval-mode BatchNorm + activation in the convolution epilogue (the inference
+    engines set this for the duration of their forward).  Off by default: a plain ``net.eval(); net(x)`` runs the two-pass path."""
+    global _FUSED_EVAL_EPILOGUE
+    _FUSED_EVAL_EPILOGUE = bool(enabled)
+
+
+def fused_eval_epilogue_enabled() -> bool:
+    return _FUSED_EVAL_EPILOGUE
+
+
+def bn_eval_coefficients(bn) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(scale, shift) fp32 [c] of an eval-mode nn.BatchNorm2d, from pcb_bn_finalize(training=0) -- the same coefficients the
+    two-pass path computes.  Cached on the module; rewritten IN PLACE when the weight epoch or a parameter / buffer version
+    changes, so a captured graph that reads them sees the new values.  Not recomputed during a graph capture."""
+    key = (_WEIGHT_EPOCH, bn.weight._version, bn.bias._version, bn.running_mean._version, bn.running_var._version,
+           bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr())
+    cache = bn.__dict__.setdefault("_pcb_eval_coef", {})
+    if cache.get("key") != key:
+        if torch.cuda.is_current_stream_capturing():
+            raise _lib.PcbError("BatchNorm eval coefficients are stale inside a graph capture: refresh them before capturing")
+        c = bn.num_features
+        buf = cache.get("buf")
+        if buf is None or buf.device != bn.weight.device:
+            buf = torch.empty((2, c), dtype=torch.float32, device=bn.weight.device)
+        momentum = 0.1 if bn.momentum is None else bn.momentum
+        lib = _lib.load()
+        _lib.check(lib.pcb_bn_finalize(None, None, 1, c, bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(),
+                                       bn.running_var.data_ptr(), None, float(momentum), float(bn.eps), 0,
+                                       buf[0].data_ptr(), buf[1].data_ptr(), None, None, _stream()))
+        cache["key"], cache["buf"] = key, buf
+    return cache["buf"][0], cache["buf"][1]
+
+
+class EvalEpilogue:
+    """An eval-mode BatchNorm (or none) + activation that a convolution may apply in its epilogue.  `fused` tells the caller
+    whether it did (pcb_conv_fuses_affine_act refused the problem otherwise: the caller then runs the BatchNorm pass itself)."""
+
+    def __init__(self, bn, act):
+        self.bn, self.act = bn, act
+        self.code, self.slope = act_code(act)
+        self.fused = False
+
+    def coefficients(self):
+        return bn_eval_coefficients(self.bn) if self.bn is not None else (None, None)
+
+
+def eval_epilogue(bn, act) -> Optional[EvalEpilogue]:
+    """The epilogue for a convolution whose ONLY consumer is `act(bn(.))`, or None when the switch is off, the BatchNorm is in
+    training mode / has no running statistics or affine parameters, or the activation has no kernel."""
+    if not _FUSED_EVAL_EPILOGUE:
+        return None
+    if bn is not None and (bn.training or bn.running_mean is None or bn.weight is None or bn.bias is None):
+        return None
+    try:
+        return EvalEpilogue(bn, act)
+    except NotImplementedError:
+        return None
+
+
+def _partial_conv_fused_eval(geom: ConvGeom, wprep, bias, xs, epi: EvalEpilogue):
+    """Forward of a partial convolution with `epi` applied in its epilogue (inference only: no autograd), or None when the
+    kernel this problem dispatches to cannot apply it."""
+    lib = _lib.load()
+    c = geom.struct(xs)
+    if torch.is_grad_enabled() or not lib.pcb_conv_fuses_affine_act(ctypes.byref(c)):
+        return None
+    dev = xs[0].device
+    if geom.dtype == PCB_BF16:
+        y = padded_empty(geom.n, geom.cout, geom.ho, geom.wo, xs[0].dtype, dev)
+    else:
+        y = torch.empty((geom.n, geom.cout, geom.ho, geom.wo), dtype=xs[0].dtype, device=dev, memory_format=CL)
+    b32 = bias.detach().float().contiguous() if bias is not None else None
+    msum, newmask = _pconv_launch(lib, geom, c, wprep[0], b32, y, None, epi)
+    epi.fused = True
+    EPILOGUE_SITES["fused"] += 1
+    return y, msum, newmask
+
+
 class PartialConvFn(torch.autograd.Function):
     """y, msum, newmask = pconv(cat(up?(x_i)), W, b | mask)   (models/partial_convolution.py:49-80 / :121-137)."""
 
@@ -349,41 +487,7 @@ class PartialConvFn(torch.autograd.Function):
                 and nhwc_layout(y) == geom.cout:
             bn_sums = zeros_f64(2 * geom.cout, dev)
             handoff.bn_sums = bn_sums
-        global _LAST_MASK_EVENT
-        _LAST_MASK_EVENT = None
-        if _MASK_CHAIN_STREAM and _PROFILE is None and not geom.plain:
-            # Mask updates never depend on features (partial_convolution.py:59-77): the mask pass of this layer runs on the
-            # mask stream, ordered only after the passes that produced its input planes, i.e. ahead of the feature path.
-            # Its buffers are allocated on that stream and kept alive until join_side_streams() (engine, once per step).
-            main, ms = torch.cuda.current_stream(), _mask_stream(dev)
-            for (_, _, _, pl, _) in geom.parts:
-                if pl is None:
-                    continue
-                ev_in = getattr(pl, "_pcb_ev", None)
-                if ev_in is None:                        # a plane written on the main stream (the network's input mask): mark it
-                    ev_in = torch.cuda.Event()           # ready from here on, so later consumers (the tail) need not wait for main
-                    ev_in.record(main)
-                    pl._pcb_ev = ev_in
-                ms.wait_event(ev_in)
-            with torch.cuda.stream(ms):
-                msum = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.float32, device=dev)
-                newmask = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.uint8, device=dev)
-                ws = _workspace(lib, c, dev)
-                _lib.check(lib.pcb_pconv_mask_pass(ctypes.byref(c), msum.data_ptr(), newmask.data_ptr(), ws.data_ptr(), _stream()))
-                ev = torch.cuda.Event()
-                ev.record()
-            main.wait_event(ev)
-            _DEFERRED.append((msum, newmask, ws))
-            _LAST_MASK_EVENT = ev
-            _lib.check(lib.pcb_pconv_forward_bn(ctypes.byref(c), w_fwd.data_ptr(), _ptr(b32), y.data_ptr(), nhwc_layout(y),
-                                                msum.data_ptr(), newmask.data_ptr(), ws.data_ptr(), 1, _ptr(bn_sums), _stream()))
-        else:
-            msum = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.float32, device=dev)
-            newmask = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.uint8, device=dev)
-            ws = _workspace(lib, c, dev)
-            with _Timed("fwd", geom):
-                _lib.check(lib.pcb_pconv_forward_bn(ctypes.byref(c), w_fwd.data_ptr(), _ptr(b32), y.data_ptr(), nhwc_layout(y), msum.data_ptr(),
-                                                    newmask.data_ptr(), ws.data_ptr(), 0, _ptr(bn_sums), _stream()))
+        msum, newmask = _pconv_launch(lib, geom, c, w_fwd, b32, y, bn_sums, None)
         ctx.geom, ctx.wprep, ctx.has_bias, ctx.weight_ref, ctx.bias_ref = geom, wprep, bias is not None, weight, bias
         ctx.handoff = handoff
         if handoff is not None:
@@ -650,6 +754,15 @@ def join_side_streams():
     _DEFERRED.clear()
 
 
+def join_mask_streams():
+    """Make the current stream wait for the mask passes issued on the mask stream since the last join (inference: a forward
+    without side streams).  Waits only when there were any, so a graph capture never depends on a stream it did not use."""
+    if _DEFERRED:
+        for st in _MASK_STREAMS.values():
+            torch.cuda.current_stream().wait_stream(st)
+    _DEFERRED.clear()
+
+
 def set_overlap_wgrad(enabled: bool):
     global _OVERLAP_WGRAD
     _OVERLAP_WGRAD = bool(enabled)
@@ -683,9 +796,11 @@ def set_fused_bn_stats(enabled: bool):
 
 
 def partial_conv(x, mask, weight, bias, stride, padding, dilation, groups, same_holes=False, no_guard=False, cache=None,
-                 plain=False, handoff=None):
+                 plain=False, handoff=None, epilogue: Optional[EvalEpilogue] = None):
     """Returns (y, new_mask: HoleMask).  `x` is a tensor or a LazyCat; `mask` a HoleMask or a dense tensor; with
-    ``plain=True`` the mask is ignored and an ordinary convolution is computed (same kernels, renormaliser 1)."""
+    ``plain=True`` the mask is ignored and an ordinary convolution is computed (same kernels, renormaliser 1).
+    `epilogue` (inference, no autograd): the eval-mode BatchNorm + activation that is y's only consumer, applied in the
+    convolution epilogue when the kernel can (``epilogue.fused`` tells; otherwise y is the plain convolution output)."""
     if isinstance(x, LazyCat):
         xs, ups = x.xs, x.ups
     else:
@@ -712,7 +827,8 @@ def partial_conv(x, mask, weight, bias, stride, padding, dilation, groups, same_
     except TooManyParts:
         return _partial_conv_dense_masks(x, hm, weight, bias, stride, padding, dilation, groups, same_holes, no_guard, cache)
     wprep = prepare_weight(weight, geom, cache if cache is not None else {})
-    y, msum, newmask = PartialConvFn.apply(geom, wprep, weight, bias, handoff, *xs)
+    out = _partial_conv_fused_eval(geom, wprep, bias, xs, epilogue) if epilogue is not None else None
+    y, msum, newmask = out if out is not None else PartialConvFn.apply(geom, wprep, weight, bias, handoff, *xs)
     planes = [newmask[g] for g in range(geom.mg)]
     if _LAST_MASK_EVENT is not None:                      # written on the mask stream: consumers there wait on this event
         for pl in planes:
@@ -918,6 +1034,8 @@ def bn_act(x, bn, act, residual=None, handoff=None, pre_sums=None):
     convolution whose output `x` is, when this call is that output's only consumer."""
     x = as_feature(x)
     code, slope = act_code(act)
+    if _FUSED_EVAL_EPILOGUE:
+        EPILOGUE_SITES["unfused"] += 1
     if residual is not None:
         residual = as_feature(residual)
     if bn is None:
@@ -938,6 +1056,8 @@ def bn_act(x, bn, act, residual=None, handoff=None, pre_sums=None):
 def activation_only(x, act, residual=None):
     x = as_feature(x)
     code, slope = act_code(act)
+    if _FUSED_EVAL_EPILOGUE:
+        EPILOGUE_SITES["unfused"] += 1
     return BNActFn.apply(x, None, None, residual, None, None, None, False, 0.0, 0.0, code, slope)
 
 
@@ -1061,14 +1181,15 @@ def _dense8(x: torch.Tensor):
     return buf.as_strided((n, c8, h, w), (h * w * c8, 1, w * c8, c8)), c
 
 
-def conv2d(x, weight, bias, stride, padding, dilation, groups, cache=None, handoff=None):
+def conv2d(x, weight, bias, stride, padding, dilation, groups, cache=None, handoff=None, epilogue=None):
     """nn.Conv2d on the same kernels as the partial convolution (`plain`: mask ignored, renormaliser 1)."""
     x = as_feature_padded(x)
     if x.dtype == torch.bfloat16 and x.shape[1] < 8 and nhwc_layout(x) % 8 != 0 and groups == 1:
         buf = padded_empty(*x.shape, x.dtype, x.device)          # 16-byte pixels -> row-packed tensor-core path
         buf.copy_(x)
         x = buf
-    y, _ = partial_conv(x, None, weight, bias, stride, padding, dilation, groups, cache=cache, plain=True, handoff=handoff)
+    y, _ = partial_conv(x, None, weight, bias, stride, padding, dilation, groups, cache=cache, plain=True, handoff=handoff,
+                        epilogue=epilogue)
     return y
 
 
@@ -1188,3 +1309,26 @@ def global_avg_pool(x):
 
 def scse_gate(x, cse, ws):
     return _ScseFn.apply(as_feature(x), cse, ws)
+
+
+# ------------------------------------------------------------------------------------------------
+# post-processing of the text-segmentation output
+# ------------------------------------------------------------------------------------------------
+def text_mask_postprocess(logits: torch.Tensor, border_pad, out_hw) -> torch.Tensor:
+    """The demo's mask from the segmentation logits in one launch (Examples/demo_segmentation.py:33-36 with the resizer of
+    Dataloader.py:308-316): ``upsample_bilinear(unpad(maxpool3x3(sigmoid(logits) > 0.5)), out_hw) > 0`` of channel 0.
+    `border_pad`: the (left, right, top, bottom) padding EvaluateSet added (``boarder_pad``; it pads right or bottom only);
+    `out_hw`: (height, width) of the original image.  Returns uint8 [n, 1, oh, ow] (1 = text); the reference's 3-channel
+    boolean is ``out.expand(-1, 3, -1, -1).bool()``."""
+    if logits.dim() != 4 or not logits.is_cuda:
+        raise _lib.PcbError("text_mask_postprocess: expected 4-D CUDA logits [n, c, h, w]")
+    left, right, top, bottom = (int(v) for v in border_pad)
+    if left != 0 or top != 0 or right < 0 or bottom < 0:
+        raise NotImplementedError("text_mask_postprocess: only non-negative right / bottom padding (the EvaluateSet layout)")
+    x = logits if nhwc_layout(logits) is not None else as_feature(logits)
+    n, _, h, w = x.shape
+    oh, ow = (int(v) for v in out_hw)
+    out = torch.empty((n, 1, oh, ow), dtype=torch.uint8, device=x.device)
+    _lib.check(_lib.load().pcb_seg_mask_postprocess(x.data_ptr(), _dtype_code(x), n, h, w, nhwc_layout(x), h - bottom, w - right, oh, ow,
+                                                    out.data_ptr(), _stream()))
+    return out
