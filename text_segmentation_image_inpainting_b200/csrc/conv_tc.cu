@@ -1432,15 +1432,17 @@ constexpr int WGRAD_THREADS = MMA_THREADS + 5 * 32;
 
 // red.global.add of a consumer thread's accumulators: element i of tap tl is row r0 + 8 ((i / 2) & 1), column 8 (i / 4) +
 // 2 (lane % 4) + (i & 1) of the tile.  ci[h] / tap[h][tl]: input channel (-1: none) and kernel tap of the thread's two rows.
+// Only the first `ncols` (64 or BLOCK_N) columns were computed.
 template <int BLOCK_N, int T>
 __device__ __forceinline__ void wgrad_store(const WgParams &P, const float (&acc)[T][BLOCK_N / 2], int ntap, int lane, int n0,
-                                            const int (&ci)[2], const int (&tap)[2][T]) {
+                                            int ncols, const int (&ci)[2], const int (&tap)[2][T]) {
     const int taps_full = P.kh * P.kw;
 #pragma unroll
     for (int tl = 0; tl < T; ++tl) {
         if (tl >= ntap) break;
 #pragma unroll
         for (int i = 0; i < BLOCK_N / 2; ++i) {
+            if (2 * i >= ncols) break;
             const int h = (i >> 1) & 1;
             const int co = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
             if (ci[h] >= 0 && co < P.cout)
@@ -1656,7 +1658,7 @@ pconv_tc_wgrad_kernel(const __grid_constant__ WgParams P, const __grid_constant_
                     }
                 }
             }
-            wgrad_store<BLOCK_N, T>(P, acc, ntap, lane, n0, ci, tap);
+            wgrad_store<BLOCK_N, T>(P, acc, ntap, lane, n0, BLOCK_N, ci, tap);
         }
     }
 }
@@ -1667,17 +1669,30 @@ pconv_tc_wgrad_kernel(const __grid_constant__ WgParams P, const __grid_constant_
 // red.global.add) but the gathered operand is no longer gathered: a K block of 64 consecutive output pixels is a box of the
 // pixel grid, so the x rows of tap (tr, tc) / 64-channel block are one 4-D TMA tile (padding = out-of-range zero fill,
 // stride-2 layers = traversal stride), written as exactly the MN-major 128B-swizzled block wgmma reads.  Holes are zeroed
-// in the landed tile by four fixer warps (the tap-validity words of the block's pixels), which then run the epilogue.
+// in the landed tile by three fixer warps (the tap-validity words of the block's pixels).
 //   HALO (stride 1, K block = one image-row segment): a CTA owns one kernel ROW; one tile of 64 + (kw-1)*dil pixel rows per
 //   channel block serves the kw taps of the row through row-shifted descriptors (T = kw register accumulators).
 //   otherwise: a CTA owns T taps, one tile per tap.
-//   warps 0-7 consumer warpgroups (MMA, then epilogue) | warp 8 TMA producer | warps 9-12 fixers
+//   warpgroups 0-1 consumers (MMA, then the red.global.add epilogue) | warpgroup 2: warp 8 TMA producer, warps 9-11 fixers
+// BLOCK_N = 128 needs T x 64 fp32 accumulators per consumer thread: setmaxnreg moves registers from warpgroup 2 to the
+// consumers (2 x 128 x 224 + 128 x 56 = 64,512 of the SM's 65,536; the kernel launches at 168 = 64,512 / 384).
+// Who computes what: with both 64-channel blocks of the M tile present, warpgroup g takes block g for all BLOCK_N output
+// channels.  With one block, a 128-wide tile gives warpgroup g output channels [64 g, 64 g + 64) of it; a 64-wide tile
+// (cout <= 64) leaves warpgroup 1 idle.  Both warpgroups release every stage.
 // -------------------------------------------------------------------------------------------------
+constexpr int WGRAD_TMA_THREADS = 384;
+constexpr int WGRAD_FIX_THREADS = 96;
+constexpr int WGRAD_TMA_REGS = 168;                           // per thread at launch: setmaxnreg needs a fixed count
+constexpr int WGRAD_CONSUMER_REGS = 224, WGRAD_SUPPORT_REGS = 56;
+static_assert(2 * 128 * WGRAD_CONSUMER_REGS + 128 * WGRAD_SUPPORT_REGS == WGRAD_TMA_THREADS * WGRAD_TMA_REGS &&
+              WGRAD_TMA_THREADS * WGRAD_TMA_REGS <= 65536, "wgrad register budget");
+
 template <int BLOCK_N, int T, bool HALO>
-__global__ void __launch_bounds__(WGRAD_THREADS, 1)
+__global__ void __maxnreg__(WGRAD_TMA_REGS)
 pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_constant__ CUtensorMap tmap_dc,
                           const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1) {
     constexpr uint32_t B_BYTES = BLOCK_N * 128;               // [64 px][BLOCK_N co] as BLOCK_N/64 blocks of 8 KB
+    constexpr int FIX_ROWS = HALO ? 3 : 1;                    // A-block rows per fixer thread: rows_a <= 256 (launch_wgrad_tma)
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = align1024(ptx::smem_u32(smem_raw));
     uint8_t *smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
@@ -1715,53 +1730,33 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
             }
     }
     const int nblk = (blk_part[0] >= 0 ? 1 : 0) + (blk_part[1] >= 0 ? 1 : 0);
+    const int solo = nblk == 1 ? (blk_part[0] >= 0 ? 0 : 1) : -1;      // the only channel block, or -1
     const bool fix = P.use_fix != 0;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 2); }
+        for (int s = 0; s < MAX_RING; ++s) {
+            ptx::mbar_init(bar_full + 8 * s, 1);
+            ptx::mbar_init(bar_fixed + 8 * s, WGRAD_FIX_THREADS / 32);
+            ptx::mbar_init(bar_empty + 8 * s, 2);                     // one arrival per consumer warpgroup
+        }
         ptx::fence_mbar_init();
     }
     if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_dc); ptx::prefetch_tmap(&tmap_a0); ptx::prefetch_tmap(&tmap_a1); }
     __syncthreads();
-
-    if (warp == 8) {
-        // ================================ TMA producer ================================
-        const int plane = P.ho * P.wo;
-        const uint32_t tx_bytes = static_cast<uint32_t>((HALO ? 1 : ntap) * nblk * rows_a * 128) + B_BYTES;
-        int s = 0;
-        uint32_t ph = 1;
-        for (int it = 0; it < num_kb; ++it) {
-            const int m0 = (kb_begin + it) * 64;
-            const int img = m0 / plane, rem = m0 - img * plane;
-            const int oy = rem / P.wo, ox = rem - oy * P.wo;
-            if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 221))) break;
-            if (ptx::elect_one()) {
-                const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
-                ptx::mbar_arrive_expect_tx(full, tx_bytes);
-                for (int tl = 0; tl < (HALO ? 1 : ntap); ++tl) {
-                    const int tap = tap0 + tl;
-                    const int tr = HALO ? tap_group : tap / P.kw, tc = HALO ? 0 : tap - tr * P.kw;
-                    const int y = oy * P.stride - P.pad_h + tr * P.dil, x = ox * P.stride - P.pad_w + tc * P.dil;
-#pragma unroll
-                    for (int hb = 0; hb < 2; ++hb)
-                        if (blk_part[hb] >= 0)
-                            ptx::tma_load_4d(dst + (tl * 2 + hb) * A_BLK, blk_part[hb] == 0 ? &tmap_a0 : &tmap_a1, blk_c0[hb], x, y, img, full);
-                }
-#pragma unroll
-                for (int j = 0; j < BLOCK_N / 64; ++j)
-                    ptx::tma_load_2d(dst + A_BYTES + j * 8192, &tmap_dc, n0 + j * 64, m0, full);
-            }
-            __syncwarp();
-            if (++s == S) { s = 0; ph ^= 1; }
-        }
-    } else if (warp < MMA_WARPS) {
+    if (warp < MMA_WARPS) {
+        ptx::setmaxnreg_inc<WGRAD_CONSUMER_REGS>();
         // ================================ consumer warpgroups: both operands MN-major ================================
-        // warpgroup g takes the tile's 64-channel block g (nothing to compute when that block does not exist)
+        // warpgroup g multiplies channel block ablk of the A tile by output channels [nc0, nc0 + ncols) of the B tile; a
+        // 64-wide tile with one channel block leaves warpgroup 1 idle (it still releases every stage)
         const int g = warp >> 2;
-        const bool leader = (threadIdx.x & 127) == 0, live = blk_part[g] >= 0;
+        const int ablk = solo >= 0 ? solo : g;
+        const bool split_n = solo >= 0 && BLOCK_N == 128;
+        const bool live = !(solo >= 0 && BLOCK_N == 64) || g == 0;
+        const int nc0 = split_n ? 64 * g : 0, ncols = split_n ? 64 : BLOCK_N;
+        const bool leader = (threadIdx.x & 127) == 0;
         const uint32_t ready = fix ? bar_fixed : bar_full;
-        const uint64_t desc_a0 = ptx::make_smem_desc(smem_base + g * A_BLK, A_BLK, 1024);
-        const uint64_t desc_b0 = ptx::make_smem_desc(smem_base + A_BYTES, 8192, 1024);
+        const uint64_t desc_a0 = ptx::make_smem_desc(smem_base + ablk * A_BLK, A_BLK, 1024);
+        const uint64_t desc_b0 = ptx::make_smem_desc(smem_base + A_BYTES + nc0 * 128, 8192, 1024);
         const uint32_t stage16 = STAGE >> 4;
         const uint32_t tap16 = HALO ? static_cast<uint32_t>(P.dil * 8) : (2 * A_BLK) >> 4;   // per tap: row shift (halo) or next tile
         float acc[T][BLOCK_N / 2];
@@ -1772,10 +1767,24 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
         bool dead = false;
         for (int it = 0; it < num_kb; ++it) {
             if (!__all_sync(0xffffffffu, ptx::mbar_wait(ready + 8 * s, ph, P.abort_flag, 224))) { dead = true; break; }
-            if (live) {
-                uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16);
-                const uint64_t db = desc_b0 + static_cast<uint64_t>(s * stage16);
-                ptx::wgmma_fence();
+            if (!live) {
+                if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
+                held = s;
+                if (++s == S) { s = 0; ph ^= 1; }
+                continue;
+            }
+            uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16);
+            const uint64_t db = desc_b0 + static_cast<uint64_t>(s * stage16);
+            ptx::wgmma_fence();
+            if (BLOCK_N == 128 && split_n) {
+#pragma unroll
+                for (int tl = 0; tl < T; ++tl, da += tap16) {
+                    if (tl >= ntap) break;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        ptx::wgmma_m64n64<1, 1>(acc[tl], da + 128 * k, db + 128 * k);     // columns 0-63 of acc
+                }
+            } else {
 #pragma unroll
                 for (int tl = 0; tl < T; ++tl, da += tap16) {
                     if (tl >= ntap) break;
@@ -1783,9 +1792,9 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
                     for (int k = 0; k < 4; ++k)                  // 16 pixels (two 8-row atoms = 2048 bytes) per step
                         ptx::wgmma_bf16<BLOCK_N, 1, 1>(acc[tl], da + 128 * k, db + 128 * k);
                 }
-                ptx::wgmma_commit();
-                ptx::wgmma_wait<1>();
             }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>();
             if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
             held = s;
             if (++s == S) { s = 0; ph ^= 1; }
@@ -1798,7 +1807,7 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
         if (!dead && live && num_kb > 0) {
             int ci[2], tap[2][T];
             for (int h = 0; h < 2; ++h) {
-                const int kpos = ci_tile * 128 + 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+                const int kpos = ci_tile * 128 + 64 * ablk + 16 * (warp & 3) + (lane >> 2) + 8 * h;
                 ci[h] = -1;
                 for (int p = 0; p < P.nparts; ++p) {
                     const int local = kpos - P.parts[p].koff;
@@ -1807,48 +1816,93 @@ pconv_tc_wgrad_tma_kernel(const __grid_constant__ WgParams P, const __grid_const
 #pragma unroll
                 for (int tl = 0; tl < T; ++tl) tap[h][tl] = tap0 + tl;
             }
-            wgrad_store<BLOCK_N, T>(P, acc, ntap, lane, n0, ci, tap);
+            wgrad_store<BLOCK_N, T>(P, acc, ntap, lane, n0 + nc0, ncols, ci, tap);
         }
     } else {
-        // ================================ fixers (hole rows -> 0) ================================
-        const int f = (warp - 9) * 32 + lane;                   // pixel row of the A blocks owned by this thread
-        if (fix) {
-            // tap-validity word of the output pixel that looks at this row (halo rows past 63 belong to a later tap column)
-            int jpix = f, tcs = 0;
-            if (HALO && f > 63) { tcs = (f - 63 + P.dil - 1) / P.dil; jpix = f - tcs * P.dil; }
-            const bool row_used = f < rows_a;
-            uint64_t wnext[2];
-            auto load_words = [&](int kb) {
-                const int m = kb * 64 + jpix;
+        ptx::setmaxnreg_dec<WGRAD_SUPPORT_REGS>();      // the whole of warpgroup 2, fixers included when there are no holes
+        if (warp == 8) {
+            // ================================ TMA producer ================================
+            const int plane = P.ho * P.wo;
+            const uint32_t tx_bytes = static_cast<uint32_t>((HALO ? 1 : ntap) * nblk * rows_a * 128) + B_BYTES;
+            int s = 0;
+            uint32_t ph = 1;
+            for (int it = 0; it < num_kb; ++it) {
+                const int m0 = (kb_begin + it) * 64;
+                const int img = m0 / plane, rem = m0 - img * plane;
+                const int oy = rem / P.wo, ox = rem - oy * P.wo;
+                if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 221))) break;
+                if (ptx::elect_one()) {
+                    const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
+                    ptx::mbar_arrive_expect_tx(full, tx_bytes);
+                    for (int tl = 0; tl < (HALO ? 1 : ntap); ++tl) {
+                        const int tap = tap0 + tl;
+                        const int tr = HALO ? tap_group : tap / P.kw, tc = HALO ? 0 : tap - tr * P.kw;
+                        const int y = oy * P.stride - P.pad_h + tr * P.dil, x = ox * P.stride - P.pad_w + tc * P.dil;
 #pragma unroll
-                for (int hb = 0; hb < 2; ++hb)
-                    wnext[hb] = (row_used && blk_part[hb] >= 0 && m < P.m_total && kb < kb_begin + num_kb) ? __ldg(P.parts[blk_part[hb]].tapmask + m) : 0ull;
+                        for (int hb = 0; hb < 2; ++hb)
+                            if (blk_part[hb] >= 0)
+                                ptx::tma_load_4d(dst + (tl * 2 + hb) * A_BLK, blk_part[hb] == 0 ? &tmap_a0 : &tmap_a1, blk_c0[hb], x, y, img, full);
+                    }
+#pragma unroll
+                    for (int j = 0; j < BLOCK_N / 64; ++j)
+                        ptx::tma_load_2d(dst + A_BYTES + j * 8192, &tmap_dc, n0 + j * 64, m0, full);
+                }
+                __syncwarp();
+                if (++s == S) { s = 0; ph ^= 1; }
+            }
+        } else if (fix) {
+            // ================================ fixers (hole rows -> 0) ================================
+            // thread fi owns pixel rows fi + 96 j of the A blocks.  A row takes the tap-validity word of the output pixel that
+            // reads it (halo rows past 63 belong to a later tap column).
+            const int fi = (warp - 9) * 32 + lane;
+            int jpix[FIX_ROWS], bit[FIX_ROWS];
+#pragma unroll
+            for (int j = 0; j < FIX_ROWS; ++j) {
+                const int f = fi + WGRAD_FIX_THREADS * j;
+                const int tcs = (HALO && f > 63) ? (f - 63 + P.dil - 1) / P.dil : 0;
+                jpix[j] = f < rows_a ? f - tcs * P.dil : -1;
+                bit[j] = HALO ? tap_group * P.kw + tcs : tap0;
+            }
+            uint64_t wnext[FIX_ROWS][2];
+            auto load_words = [&](int kb) {
+#pragma unroll
+                for (int j = 0; j < FIX_ROWS; ++j) {
+                    const int m = kb * 64 + jpix[j];
+#pragma unroll
+                    for (int hb = 0; hb < 2; ++hb)
+                        wnext[j][hb] = (jpix[j] >= 0 && blk_part[hb] >= 0 && m < P.m_total && kb < kb_begin + num_kb) ? __ldg(P.parts[blk_part[hb]].tapmask + m) : 0ull;
+                }
             };
             load_words(kb_begin);
             int s = 0;
             uint32_t ph = 0;
             for (int it = 0; it < num_kb; ++it) {
-                const uint64_t w0 = wnext[0], w1 = wnext[1];
+                uint32_t hole = 0;                                   // bit (j * 2 + hb) * T + tl: row j of tile (tl, hb) -> 0
+#pragma unroll
+                for (int j = 0; j < FIX_ROWS; ++j)
+#pragma unroll
+                    for (int hb = 0; hb < 2; ++hb)
+#pragma unroll
+                        for (int tl = 0; tl < (HALO ? 1 : T); ++tl)
+                            if (tl < ntap && jpix[j] >= 0 && blk_part[hb] >= 0 && ((wnext[j][hb] >> (bit[j] + tl)) & 1ull) == 0ull)
+                                hole |= 1u << ((j * 2 + hb) * T + tl);
                 load_words(kb_begin + it + 1);
                 if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 222))) break;
-                bool wrote = false;
-                if (row_used) {
-                    for (int tl = 0; tl < (HALO ? 1 : ntap); ++tl) {
-                        const int bit = HALO ? tap_group * P.kw + tcs : tap0 + tl;
+                if (hole) {
 #pragma unroll
-                        for (int hb = 0; hb < 2; ++hb) {
-                            if (blk_part[hb] < 0) continue;
-                            if ((((hb ? w1 : w0) >> bit) & 1ull) == 0ull) {
-                                uint4 *r = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + (tl * 2 + hb) * A_BLK + f * 128);
-                                const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+                    for (int j = 0; j < FIX_ROWS; ++j)
 #pragma unroll
-                                for (int k = 0; k < 8; ++k) r[k] = z;
-                                wrote = true;
-                            }
-                        }
-                    }
+                        for (int hb = 0; hb < 2; ++hb)
+#pragma unroll
+                            for (int tl = 0; tl < (HALO ? 1 : T); ++tl)
+                                if ((hole >> ((j * 2 + hb) * T + tl)) & 1u) {
+                                    uint4 *r = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + (tl * 2 + hb) * A_BLK + (fi + WGRAD_FIX_THREADS * j) * 128);
+                                    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+                                    for (int k = 0; k < 8; ++k) r[k] = z;
+                                }
                 }
-                if (__any_sync(0xffffffffu, wrote)) ptx::fence_proxy_async_smem();
+                if (__any_sync(0xffffffffu, hole != 0)) ptx::fence_proxy_async_smem();
                 __syncwarp();
                 if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
                 if (++s == S) { s = 0; ph ^= 1; }
@@ -3069,7 +3123,9 @@ static bool tma_wgrad_ok(const pcb_conv *c) {
 
 template <int BLOCK_N, int T, bool HALO>
 int launch_wgrad_tma(WgParams &P, const CUtensorMap &tdc, const CUtensorMap &ta0, const CUtensorMap &ta1, cudaStream_t st) {
-    const size_t a_blk = (static_cast<size_t>(64 + (HALO ? (P.kw - 1) * P.dil : 0)) * 128 + 1023) / 1024 * 1024;
+    const int rows_a = 64 + (HALO ? (P.kw - 1) * P.dil : 0);
+    PCB_CHECK(rows_a <= (HALO ? 3 : 1) * WGRAD_FIX_THREADS, "TMA-fed wgrad: %d-row A blocks exceed the fixer warps", rows_a);
+    const size_t a_blk = (static_cast<size_t>(rows_a) * 128 + 1023) / 1024 * 1024;
     const size_t stage = (HALO ? 1 : T) * 2 * a_blk + static_cast<size_t>(BLOCK_N) * 128;
     P.stages = static_cast<int>(std::min<size_t>(MAX_RING, RING_BUDGET / stage));
     PCB_CHECK(P.stages >= 2, "TMA-fed wgrad: stage of %zu bytes does not fit twice", stage);
@@ -3081,13 +3137,14 @@ int launch_wgrad_tma(WgParams &P, const CUtensorMap &tdc, const CUtensorMap &ta0
     const int co_tiles = (P.cout + BLOCK_N - 1) / BLOCK_N;
     const int base_ctas = co_tiles * P.tap_groups * P.ci_tiles;
     const int total_kb = (P.m_total + 63) / 64;
-    int splits = (2 * pcb_num_sms() + base_ctas - 1) / base_ctas;      // one CTA per SM at a time: ~2 waves
+    // one CTA per SM at a time: ~2 waves (measured faster than one wave for the large layers at 128-wide tiles)
+    int splits = (2 * pcb_num_sms() + base_ctas - 1) / base_ctas;
     splits = std::max(1, std::min(splits, total_kb));
     splits = std::min(splits, 65535);
     P.kb_per_split = (total_kb + splits - 1) / splits;
     splits = (total_kb + P.kb_per_split - 1) / P.kb_per_split;
     dim3 grid(base_ctas, splits);
-    kern<<<grid, WGRAD_THREADS, smem, st>>>(P, tdc, ta0, ta1);
+    kern<<<grid, WGRAD_TMA_THREADS, smem, st>>>(P, tdc, ta0, ta1);
     PCB_LAUNCH_CHECK();
     return 0;
 }
@@ -3169,6 +3226,12 @@ int pcb_tc_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, v
             if (int rc = make_tmap_nhwc(&ta[p], src, c8, c->w, c->h, c->n, cs, P.box_w + hx, P.box_h, P.box_n, c->stride)) return rc;
         }
         if (c->nparts < 2) ta[1] = ta[0];
+        // 128 output channels per tile, except for layers with at most 64 and for short reductions (< 128 K blocks of 64
+        // pixels): there each CTA has few K blocks and its red.global.add epilogue, twice as long at 128 columns, dominates
+        if (c->cout > 64 && m_total >= 128 * 64) {
+            if (halo) return launch_wgrad_tma<128, 3, true>(P, tm, ta[0], ta[1], st);
+            return launch_wgrad_tma<128, 3, false>(P, tm, ta[0], ta[1], st);
+        }
         if (halo) return launch_wgrad_tma<64, 3, true>(P, tm, ta[0], ta[1], st);
         return launch_wgrad_tma<64, 3, false>(P, tm, ta[0], ta[1], st);
     }

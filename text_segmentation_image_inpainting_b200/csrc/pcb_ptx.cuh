@@ -115,7 +115,9 @@ template <int TA, int TB> __device__ __forceinline__ void wgmma_m64n32(float (&d
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
         : "l"(a_desc), "l"(b_desc), "n"(TA), "n"(TB));
 }
-template <int TA, int TB> __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+// d may be a wider accumulator array: its first 32 registers are the 64 columns
+template <int TA, int TB, int R> __device__ __forceinline__ void wgmma_m64n64(float (&d)[R], uint64_t a_desc, uint64_t b_desc) {
+    static_assert(R >= 32, "m64n64 accumulator");
     asm volatile(
         "{\n\t"
         "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
@@ -138,6 +140,11 @@ template <int N, int TA, int TB> __device__ __forceinline__ void wgmma_bf16(floa
     else if constexpr (N == 64) wgmma_m64n64<TA, TB>(d, a_desc, b_desc);
     else { static_assert(N == 128, "wgmma tile width"); wgmma_m64n128<TA, TB>(d, a_desc, b_desc); }
 }
+// ---------------------------------------------------------------- register reallocation (per warpgroup)
+// setmaxnreg: all four warps of a warpgroup execute it (.sync.aligned).  dec returns registers to the CTA's pool, inc blocks
+// until the pool holds enough; N is a multiple of 8 in [24, 256].
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 // named barrier over the `threads` threads of one role (id 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
