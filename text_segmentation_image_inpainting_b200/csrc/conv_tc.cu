@@ -16,11 +16,12 @@
 //                 through row-shifted SWIZZLE_128B descriptors.  2x-upsampled sources are first copied densely into the
 //                 workspace (TMA cannot replicate pixels).
 //     B operand   weights [N][K] bf16 (K padded to the same block structure), TMA 2D tiles (SWIZZLE_128B).
-//     MMA         wgmma.mma_async m64nNk16 bf16 -> fp32, N in {32, 64, 128}: two consumer warpgroups each own 64 rows of the
-//                 128-row tile and hold its accumulators in registers; stages are released through mbarriers once
+//     MMA         wgmma.mma_async m64nNk16 bf16 -> fp32, N in {32, 64, 128, 256}: two consumer warpgroups each own 64 rows of
+//                 the 128-row tile and hold its accumulators in registers; stages are released through mbarriers once
 //                 wgmma.wait_group reports the MMAs that read them complete.
-//     epilogue    registers -> shared staging tile -> one thread per row, fwd: y = hole ? 0 : acc / s + bias (s = mask box sum),
-//                 dgrad: dx_part = acc * input-mask of that part; bf16 NHWC stores.  Stride-2 dgrad = four stride-1 parity classes.
+//     epilogue    registers -> fwd: y = hole ? 0 : acc / s + bias (s = mask box sum) in the consumers -> bf16 staging tile ->
+//                 one thread per row, dgrad: dx_part = staged value * input-mask of that part; bf16 NHWC stores.
+//                 Stride-2 dgrad = four stride-1 parity classes.
 //     wgrad       D[k][co] (+)= sum_pixels x[p+tap][k] * dc[p][co]: both operands MN-major "pixel row x 128-byte channel chunk"
 //                 tiles by TMA, split-K over pixels with fp32 red.global.add into the (logical, unpadded) KRSC gradient.
 //
@@ -111,9 +112,37 @@ struct TcParams {
 // kernel (row quadrant x column half), four in the TMA-fed kernels (row quadrant, all BLOCK_N <= 128 columns)
 constexpr int STAT_SLICE = 256;
 constexpr int STAT_SMEM_BYTES = MMA_WARPS * STAT_SLICE * 4 + 16;
-// TMA-fed kernels: four dedicated epilogue warps; warp w drains rows [32 w, 32 w + 32) of the staging tile
+// TMA-fed kernels: four dedicated epilogue warps; warp w drains rows [32 w, 32 w + 32) of the staging tile.  Their statistics
+// slices are [256 sums | 256 squares] (all BLOCK_N <= 256 columns).
 constexpr int EPI_WARPS = 4;
-constexpr int EPI_STAT_SMEM_BYTES = EPI_WARPS * STAT_SLICE * 4;
+constexpr int EPI_STAT_SLICE = 512;
+constexpr int EPI_STAT_SQ = EPI_STAT_SLICE / 2;
+constexpr int EPI_STAT_SMEM_BYTES = EPI_WARPS * EPI_STAT_SLICE * 4;
+// TMA-fed kernels: the consumers finish the element math and stage bf16 [128 rows][BLOCK_N + 8] (a row is an odd number of
+// 16-byte units, so the epilogue warps' one-row-per-lane 16-byte loads are conflict-free); split-K stages raw fp32 partials
+constexpr int bf16_pitch(int block_n) { return block_n + 8; }
+constexpr int bf16_stage_bytes(int block_n) { return BLOCK_M * bf16_pitch(block_n) * 2; }
+
+// 16 values per lane, 32 lanes: returns in lane l the sum over all lanes of v[l & 15].  The reduction tree is the one
+// warp_transpose_sum builds for the same column (lanes paired across bit 4 first, then bits 3 .. 0), so the sums are bitwise
+// equal to it; the first level keeps all 16 values (both partners hold the same sums).
+__device__ __forceinline__ float warp_transpose_sum16(float (&v)[16], int lane) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], 16);
+#pragma unroll
+    for (int off = 8, n = 16; off >= 1; off >>= 1, n >>= 1) {
+        const bool upper = (lane & off) != 0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            if (i < (n >> 1)) {
+                const float send = upper ? v[i] : v[i + (n >> 1)];
+                const float keep = upper ? v[i + (n >> 1)] : v[i];
+                v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+            }
+        }
+    }
+    return v[0];
+}
 
 // 32 values per lane, 32 lanes: returns in lane l the sum over all lanes of v[l] (a transposing butterfly: 31 shuffles)
 __device__ __forceinline__ float warp_transpose_sum(float (&v)[32], int lane) {
@@ -157,8 +186,9 @@ struct EpiRow {
     float dscale[TC_MAX_PARTS];   // dgrad: input mask of part p at this pixel (1 / 0; 1 without a mask)
 };
 
+// renorm = false: leave inv / hole unset (the TMA-fed kernels' consumers apply the renormalisation themselves)
 template <int MODE>
-__device__ __forceinline__ EpiRow tc_epi_row(const TcParams &P, int m) {
+__device__ __forceinline__ EpiRow tc_epi_row(const TcParams &P, int m, bool renorm = true) {
     EpiRow er;
     er.m = m;
     er.rvalid = m < P.m_total;
@@ -175,7 +205,7 @@ __device__ __forceinline__ EpiRow tc_epi_row(const TcParams &P, int m) {
         en = m / (P.ho * P.wo); const int rem = m - en * P.ho * P.wo; eh = rem / P.wo; ew = rem - eh * P.wo;
         er.mo = (static_cast<long long>(en) * P.fh + eh * P.sub + P.py) * P.fw + ew * P.sub + P.px;
     }
-    if (MODE == 0 && er.rvalid) {
+    if (MODE == 0 && er.rvalid && renorm) {
         const float s = P.msum ? P.msum[er.mo] : 1.f;               // null: plain convolution (renormaliser 1)
         er.hole = (s == 0.f) && !P.no_guard;
         er.inv = er.hole ? 0.f : 1.0f / s;        // no_guard: 1/0 = inf -> 0*inf = NaN like the reference
@@ -367,7 +397,7 @@ __device__ __forceinline__ void tc_stats_final(const TcParams &P, const float *s
         if (co < P.bn_c) {
             float a = 0.f, q = 0.f;
 #pragma unroll
-            for (int w4 = 0; w4 < EPI_WARPS; ++w4) { a += stat_base[w4 * STAT_SLICE + col]; q += stat_base[w4 * STAT_SLICE + 128 + col]; }
+            for (int w4 = 0; w4 < EPI_WARPS; ++w4) { a += stat_base[w4 * EPI_STAT_SLICE + col]; q += stat_base[w4 * EPI_STAT_SLICE + EPI_STAT_SQ + col]; }
             atomicAdd(P.bn_sums + co, static_cast<double>(a));
             atomicAdd(P.bn_sums + P.bn_c + co, static_cast<double>(q));
         }
@@ -784,37 +814,123 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
 // the NHWC source at coordinates shifted by the tap -- negative / past-the-edge coordinates are zero-filled by the TMA
 // unit (the convolution padding), stride-2 layers use the tensor map's traversal stride, channel padding is the map's
 // channel extent.  TMA writes exactly the 128B-swizzled K-major image wgmma reads.  What TMA cannot know are the HOLES
-// (x*mask, models/partial_convolution.py:51): four "fixer" warps (one thread per tile row) test the row's tap-validity
-// bit and overwrite hole rows of the landed tile with zeros before handing the stage to the MMA thread
+// (x*mask, models/partial_convolution.py:51): three "fixer" warps (each thread loops over tile rows) test the rows'
+// tap-validity bits and overwrite hole rows of the landed tile with zeros before handing the stage to the MMA thread
 // (generic-proxy stores -> fence.proxy.async -> mbarrier).  Plain convolutions / dgrad skip the fixers.
 //
-//   warps 0-7   consumers  : two warpgroups, 4 x wgmma (K=16) per K block and weight tile, then their accumulators -> staging tile
-//   warp 8      TMA producer : per K block one A tile (4-D) + the weight tiles (2-D) onto the same mbarrier
-//   warps 9-12  fixers     : hole rows -> 0   (MODE 0 with masks only)
-//   warps 13-16 epilogue   : staging tile -> renormalise / mask -> bf16 NHWC stores (+ BatchNorm statistics)
+//   warpgroups 0-1 consumers  : 4 x wgmma (K=16) per K block and weight tile, then the element math of their 64 rows -> staging
+//   warpgroup 2    warp 8      TMA producer : per K block one A tile (4-D) + the weight tiles (2-D) onto the same mbarrier
+//                  warps 9-11  fixers       : hole rows -> 0   (MODE 0 with masks only)
+//   warpgroup 3    epilogue   : staging tile -> dgrad input mask -> bf16 NHWC stores (+ BatchNorm statistics)
+// The roles are whole warpgroups so that setmaxnreg can move registers to the consumers: a 128 x 256 tile is 64 x 256 fp32
+// accumulators = 128 registers per consumer thread (2 x 128 x TMA_CONSUMER_REGS + 2 x 128 x TMA_SUPPORT_REGS = 65,536).
 // Every per-K-block loop of the producer is a handful of instructions: index arithmetic there (the old kernels did integer
 // divisions) directly delays the stages the tensor cores wait for.
 // The epilogue of tile i overlaps the MMAs of tile i+1 through ONE staging tile and two mbarriers: the consumers wait on
 // acc_empty before they write it and arrive on acc_full after; the epilogue warps wait on acc_full and arrive on acc_empty once
-// they have read it.  The epilogue warps fetch a tile's per-row data (mask sums, dgrad mask bytes) before they wait.
+// they have read it.  The consumers fetch their rows' mask sums, the epilogue warps the dgrad mask bytes, before the K loop /
+// the wait.
 // -------------------------------------------------------------------------------------------------
-constexpr int EPI_WARP0 = MMA_WARPS + 5;
+constexpr int EPI_WARP0 = MMA_WARPS + 4;
 constexpr int TMA_THREADS = (EPI_WARP0 + EPI_WARPS) * 32;
+constexpr int TMA_FIX_THREADS = 96;
+constexpr int TMA_REGS = 128;                                  // per thread at launch: setmaxnreg needs a fixed count
+constexpr int TMA_CONSUMER_REGS = 192, TMA_SUPPORT_REGS = 64;
+static_assert(TMA_THREADS == 512 && 2 * 128 * TMA_CONSUMER_REGS + 2 * 128 * TMA_SUPPORT_REGS == TMA_THREADS * TMA_REGS &&
+              TMA_THREADS * TMA_REGS <= 65536, "TMA-fed fwd / dgrad register budget");
 
 // shared memory behind the TMA-fed kernels' rings: full / fixed / empty barriers, acc_full / acc_empty, the statistics slices
 constexpr size_t TMA_BAR_BYTES = 24 * MAX_RING + 16;
 
+// bf16-staged epilogue of one row (TMA-fed kernels): the consumers already applied the forward's renormalisation, bias, eval
+// BatchNorm + activation and the zeroing of columns >= cout, and rounded once; what is left is the dgrad input mask, the
+// 16-byte stores and the BatchNorm statistics of the stored values (same values, same reduction order as tc_epilogue).
+// dgrad: the staged value is bf16(acc), multiplied here by the 0 / 1 mask -- equal to rounding acc * mask except where |acc|
+// is finite but rounds to bf16 infinity (inf * 0 = NaN instead of 0).
+template <int BLOCK_N, int MODE>
+__device__ __forceinline__ void tc_epilogue_bf16(const TcParams &P, const EpiRow &er, const bf16 *srow, int lane, int n0, float *s_stat) {
+    const bool stats = (MODE == 0) && (s_stat != nullptr);
+#pragma unroll 1
+    for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
+        const int col = n0 + c0;
+        bf16 *orow = nullptr;
+        int nstore = 0;                                  // channels to store from this 32-column chunk (multiple of 8)
+        float scale = 1.f;
+        if (MODE == 0) {
+            if (er.rvalid && col < P.y_cstride) { orow = P.y + er.mo * P.y_cstride + col; nstore = min(32, P.y_cstride - col); }
+        } else {
+#pragma unroll
+            for (int p = 0; p < TC_MAX_PARTS; ++p) {
+                if (p >= P.nparts) break;
+                const TcPart &pt = P.parts[p];
+                const int local = col - pt.koff;
+                if (local >= 0 && local < pt.kext && pt.dx != nullptr && local < pt.c8 && er.rvalid) {
+                    orow = pt.dx + er.mo * pt.dx_cstride + local;
+                    nstore = min(32, pt.c8 - local);
+                    scale = er.dscale[p];
+                }
+            }
+        }
+        if (nstore == 0 && !stats) continue;
+        uint4 o[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) o[j] = reinterpret_cast<const uint4 *>(srow + c0)[j];
+        if (MODE == 1 && scale != 1.f) {
+            __nv_bfloat162 *ob = reinterpret_cast<__nv_bfloat162 *>(o);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const float2 f = __bfloat1622float2(ob[j]);
+                ob[j] = __floats2bfloat162_rn(f.x * scale, f.y * scale);
+            }
+        }
+        if (nstore > 0) {
+            uint4 *dst = reinterpret_cast<uint4 *>(orow);
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (j * 8 < nstore) dst[j] = o[j];
+        }
+        if (stats) {
+            // per-channel sum and sum of squares of what was just stored (rows past the tensor contribute 0), 16 columns at a
+            // time: lane l ends up with column c0 + l
+            const float live = er.rvalid ? 1.f : 0.f;
+            const __nv_bfloat162 *ob = reinterpret_cast<const __nv_bfloat162 *>(o);
+            float cs = 0.f, cq = 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float v[16];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float2 f = __bfloat1622float2(ob[8 * h + j]);
+                    v[2 * j] = f.x * live; v[2 * j + 1] = f.y * live;
+                }
+                const float s = warp_transpose_sum16(v, lane);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float2 f = __bfloat1622float2(ob[8 * h + j]);
+                    const float a = f.x * live, b = f.y * live;
+                    v[2 * j] = a * a; v[2 * j + 1] = b * b;
+                }
+                const float q = warp_transpose_sum16(v, lane);
+                if ((lane >> 4) == h) { cs = s; cq = q; }
+            }
+            s_stat[c0 + lane] += cs;                     // this warp's private accumulators: no atomics needed
+            s_stat[EPI_STAT_SQ + c0 + lane] += cq;
+        }
+    }
+}
+
 // epilogue warp w of the TMA-fed kernels: drains rows [32 w, 32 w + 32) x all columns of every tile the consumers stage (same
 // tile walk), one row per thread.  `tile_origin(tile, m0, n0)` gives a tile's origin, n0 < 0 for a tile the consumers skip.
-// stat_n0: N tile the statistics slice s_stat currently belongs to (-1: none / aborted).
+// stat_n0: N tile the statistics slice s_stat currently belongs to (-1: none / aborted).  `stage`: bf16 staging tile, or the
+// fp32 one of a split-K launch (P.partial).
 template <int BLOCK_N, int MODE, typename TileFn>
 __device__ __forceinline__ void tma_epilogue_warps(const TcParams &P, int tile0, int tstep, int num_tiles, TileFn tile_origin,
-                                                   const float *acc_stage, uint32_t acc_full, uint32_t acc_empty, float *s_stat,
+                                                   const uint8_t *stage, uint32_t acc_full, uint32_t acc_empty, float *s_stat,
                                                    int &stat_n0, int w, int lane, int code) {
-    constexpr int PITCH = acc_pitch(BLOCK_N);
-    const float *acc_row = acc_stage + (w * 32 + lane) * PITCH;
+    const int row = w * 32 + lane;
+    const bool f32 = P.partial != nullptr;
     if (s_stat) {
-        for (int i = lane; i < STAT_SLICE; i += 32) s_stat[i] = 0.f;
+        for (int i = lane; i < EPI_STAT_SLICE; i += 32) s_stat[i] = 0.f;
         __syncwarp();
     }
     uint32_t ph = 0;
@@ -823,26 +939,94 @@ __device__ __forceinline__ void tma_epilogue_warps(const TcParams &P, int tile0,
         tile_origin(tile, m0, n0);
         if (n0 < 0) continue;
         if (s_stat && n0 != stat_n0) {
-            if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, 0, BLOCK_N, 128);
+            if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, 0, BLOCK_N, EPI_STAT_SQ);
             stat_n0 = n0;
         }
-        const EpiRow er = tc_epi_row<MODE>(P, m0 + w * 32 + lane);
+        const EpiRow er = tc_epi_row<MODE>(P, m0 + row, false);     // split-K stores raw partials, bf16 was renormalised
         if (!__all_sync(0xffffffffu, ptx::mbar_wait(acc_full, ph, P.abort_flag, code))) { stat_n0 = -1; return; }
         ph ^= 1;
-        tc_epilogue<BLOCK_N, MODE>(P, er, acc_row, lane, n0, s_stat, 0, BLOCK_N, 128);
+        if constexpr (BLOCK_N <= 128) {
+            if (f32) tc_epilogue<BLOCK_N, MODE>(P, er, reinterpret_cast<const float *>(stage) + row * acc_pitch(BLOCK_N), lane, n0, s_stat, 0, BLOCK_N, EPI_STAT_SQ);
+        }
+        if (!f32) tc_epilogue_bf16<BLOCK_N, MODE>(P, er, reinterpret_cast<const bf16 *>(stage) + row * bf16_pitch(BLOCK_N), lane, n0, s_stat);
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(acc_empty);
     }
 }
 
-// consumer warp e after a tile's K loop: wait until the epilogue warps have read the staging tile, write this warp's accumulator
-// rows into it, hand it over.  false: aborted.
-template <int BLOCK_N>
-__device__ __forceinline__ bool tma_stage_tile(const TcParams &P, const float (&acc)[BLOCK_N / 2], float *acc_stage, uint32_t acc_full,
-                                               uint32_t acc_empty, uint32_t &ph, int e, int lane, int code) {
+// What a consumer thread needs for the forward element math of its two rows per m64 block (rows r0 and r0 + 8 of the
+// accumulator fragment): fetched when the tile starts, so the loads hide behind the K loop.
+struct ConsRows {
+    float inv[2];
+    bool hole[2];
+};
+template <int MODE>
+__device__ __forceinline__ ConsRows cons_rows(const TcParams &P, int m0, int e, int lane) {
+    ConsRows cr;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        cr.inv[h] = 0.f; cr.hole[h] = false;
+        if (MODE == 0 && P.partial == nullptr) {
+            const EpiRow er = tc_epi_row<0>(P, m0 + 64 * (e >> 2) + 16 * (e & 3) + (lane >> 2) + 8 * h);
+            cr.inv[h] = er.inv; cr.hole[h] = er.hole;
+        }
+    }
+    return cr;
+}
+
+// register accumulators of consumer warp e -> its 16 rows of the bf16 staging tile, with the fp32 element math of the forward
+// epilogue (the expression tc_epilogue evaluates, in the same order) done here, rounded to bf16 once:
+//   y = hole ? 0 : acc * (1 / mask sum) + bias;  eval: y = act(y * scale + shift);  columns >= cout: 0
+// dgrad stages bf16(acc).  Bias / scale / shift: one pair of columns per fragment column block, from L1.
+template <int BLOCK_N, int MODE>
+__device__ __forceinline__ void stage_acc_bf16(const TcParams &P, const float (&acc)[BLOCK_N / 2], bf16 *stage, int e, int lane, int n0,
+                                               const ConsRows &cr) {
+    constexpr int PITCH = bf16_pitch(BLOCK_N);
+    const int r0 = 64 * (e >> 2) + 16 * (e & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+    const bool has_bias = (MODE == 0) && (P.bias != nullptr);
+    const bool ep = (MODE == 0) && (P.ep_on != 0);
+    const bool ep_aff = ep && (P.ep_scale != nullptr);
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int col = n0 + 8 * j + c0;
+        float b0 = 0.f, b1 = 0.f, s0 = 1.f, s1 = 1.f, t0 = 0.f, t1 = 0.f;
+        if (MODE == 0) {
+            const bool in0 = col < P.cout, in1 = col + 1 < P.cout;
+            if (has_bias) { if (in0) b0 = __ldg(P.bias + col); if (in1) b1 = __ldg(P.bias + col + 1); }
+            if (ep_aff) {
+                if (in0) { s0 = __ldg(P.ep_scale + col); t0 = __ldg(P.ep_shift + col); }
+                if (in1) { s1 = __ldg(P.ep_scale + col + 1); t1 = __ldg(P.ep_shift + col + 1); }
+            }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float a = acc[4 * j + 2 * h], b = acc[4 * j + 2 * h + 1];
+            if (MODE == 0) {
+                a = cr.hole[h] ? 0.f : fmaf(a, cr.inv[h], b0);
+                b = cr.hole[h] ? 0.f : fmaf(b, cr.inv[h], b1);
+                if (ep) {                          // holes become apply_act(shift): the BatchNorm sees the zeros written above
+                    a = apply_act(fmaf(a, s0, t0), P.ep_act, P.ep_slope);
+                    b = apply_act(fmaf(b, s1, t1), P.ep_act, P.ep_slope);
+                }
+                if (col >= P.cout) a = 0.f;
+                if (col + 1 >= P.cout) b = 0.f;
+            }
+            *reinterpret_cast<__nv_bfloat162 *>(stage + (r0 + 8 * h) * PITCH + 8 * j + c0) = __floats2bfloat162_rn(a, b);
+        }
+    }
+}
+
+// consumer warp e after a tile's K loop: wait until the epilogue warps have read the staging tile, write this warp's rows into
+// it (bf16 with the element math, or raw fp32 for split-K), hand it over.  false: aborted.
+template <int BLOCK_N, int MODE>
+__device__ __forceinline__ bool tma_stage_tile(const TcParams &P, const float (&acc)[BLOCK_N / 2], uint8_t *stage, uint32_t acc_full,
+                                               uint32_t acc_empty, uint32_t &ph, int e, int lane, int n0, const ConsRows &cr, int code) {
     if (!__all_sync(0xffffffffu, ptx::mbar_wait(acc_empty, ph, P.abort_flag, code))) return false;
     ph ^= 1;
-    stage_acc<BLOCK_N>(acc, acc_stage, e, lane);
+    if constexpr (BLOCK_N <= 128) {
+        if (P.partial != nullptr) stage_acc<BLOCK_N>(acc, reinterpret_cast<float *>(stage), e, lane);
+    }
+    if (P.partial == nullptr) stage_acc_bf16<BLOCK_N, MODE>(P, acc, reinterpret_cast<bf16 *>(stage), e, lane, n0, cr);
     __syncwarp();
     if (lane == 0) ptx::mbar_arrive(acc_full);
     return true;
@@ -854,7 +1038,7 @@ __device__ __forceinline__ bool tma_stage_tile(const TcParams &P, const float (&
 // reads the same image) -- kw x less A traffic from L2 and kw x fewer barrier round trips per MMA.  K steps that only cover
 // channel padding (c8 <= 16*k) are skipped.
 template <int BLOCK_N, int MODE, bool HALO>
-__global__ void __launch_bounds__(TMA_THREADS, 1)
+__global__ void __maxnreg__(TMA_REGS)
 pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1) {
     constexpr uint32_t B_BYTES = BLOCK_N * 128;
@@ -894,7 +1078,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < MAX_RING; ++s) {      // empty: one arrival per consumer warpgroup
-            ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 2);
+            ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, TMA_FIX_THREADS / 32); ptx::mbar_init(bar_empty + 8 * s, 2);
         }
         ptx::mbar_init(acc_full, MMA_WARPS); ptx::mbar_init(acc_empty, EPI_WARPS);     // one arrival per warp
         ptx::fence_mbar_init();
@@ -906,78 +1090,9 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
     // broadcast so the compiler knows the role branch is uniform) and only the TMA instructions sit inside an elect.sync region.
     float *s_stat = nullptr;                                          // epilogue warps: private BatchNorm-statistics accumulators
     int stat_n0 = -1;                                                  // N tile they currently belong to (-1: none / aborted)
-    float *acc_stage = reinterpret_cast<float *>(smem_gen + (s_acc - smem_base));
-    if (warp >= EPI_WARP0) {
-        // ================================ epilogue warps ================================
-        const int w = warp - EPI_WARP0;
-        s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
-                     ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + w * STAT_SLICE : nullptr;
-        auto origin = [&](int tile, int &m0, int &n0) {
-            const int mn = tile / KS;
-            m0 = m0_of(mn / n_tiles); n0 = (mn % n_tiles) * BLOCK_N;
-            if (!tile_active(n0)) n0 = -1;
-        };
-        tma_epilogue_warps<BLOCK_N, MODE>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, s_stat, stat_n0, w, lane, 126);
-    } else if (warp == 8) {
-        // ================================ TMA producer ================================
-        int s = 0;
-        uint32_t ph = 1;                                               // first pass over the ring: stages are free
-        const int plane = (MODE == 0) ? P.ho * P.wo : P.h * P.w;
-        const int pwid = (MODE == 0) ? P.wo : P.w;
-        const int kext0 = (MODE == 0) ? P.parts[0].kext : P.dc_kext, kext1 = (MODE == 0 && np > 1) ? P.parts[1].kext : 0;
-        const int dstep = (MODE == 0) ? P.dil : -P.dil;
-        const int row_k = P.wk_row, col_k = P.wk_col;
-        bool dead = false;
-        for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-            const int sp = tile % KS, mn = tile / KS;
-            const int m0 = m0_of(mn / n_tiles), n0 = (mn % n_tiles) * BLOCK_N;
-            if (!tile_active(n0)) continue;
-            const int img = m0 / plane, rem = m0 - img * plane;
-            const int oy = rem / pwid, ox = rem - oy * pwid;
-            // leftmost / topmost source coordinate of tap column 0 (fwd) -- dgrad walks its taps right to left
-            const int x_org = (MODE == 0) ? ox * P.stride - P.pad_w : (HALO ? ox + P.pad_w - hx : ox + P.pad_w);
-            const int y_org = (MODE == 0) ? oy * P.stride - P.pad_h : oy + P.pad_h;
-            // optional L2 prefetch (P.l2pf): while tile t is loaded, the A boxes of this CTA's NEXT tile are requested into L2, one
-            // tile's worth of stages ahead, so that their loads find L2 instead of DRAM (the ring is round-trip-latency bound)
-            int nx_org = 0, ny_org = 0, nimg = -1;
-            if (P.l2pf && tile + tstep < num_tiles) {
-                const int nmn = (tile + tstep) / KS;
-                const int nm0 = m0_of(nmn / n_tiles);
-                if (nm0 != m0) {
-                    nimg = nm0 / plane;
-                    const int nrem = nm0 - nimg * plane, noy = nrem / pwid, nox = nrem - noy * pwid;
-                    nx_org = (MODE == 0) ? nox * P.stride - P.pad_w : (HALO ? nox + P.pad_w - hx : nox + P.pad_w);
-                    ny_org = (MODE == 0) ? noy * P.stride - P.pad_h : noy + P.pad_h;
-                }
-            }
-            int krow = P.wk_base;                                      // weight K index of (tr, tap column 0, part 0, block 0)
-            for (int tr = 0, y = y_org; tr < P.kh && !dead; ++tr, y += dstep, krow += row_k)
-                for (int ti = 0, x = x_org, kidx = krow; ti < kwi && !dead; ++ti, x += dstep, kidx = krow + ti * col_k) {
-#pragma unroll
-                    for (int p = 0; p < TC_MAX_PARTS; ++p) {
-                        const int kext = (p == 0) ? kext0 : kext1;
-                        const CUtensorMap *ma = (p == 0) ? &tmap_a0 : &tmap_a1;
-                        const int gb0 = (p == 0) ? 0 : kext0 / BLOCK_K;          // global K-block index of the part's first block
-                        for (int c0 = 0; c0 < kext; c0 += BLOCK_K, kidx += BLOCK_K) {
-                            if (KS > 1 && (gb0 + c0 / BLOCK_K) % KS != sp) continue;
-                            if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 121))) { dead = true; break; }
-                            if (ptx::elect_one()) {
-                                const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
-                                ptx::mbar_arrive_expect_tx(full, STAGE_TX);
-                                ptx::tma_load_4d(dst, ma, c0, x, y, img, full);
-                                uint32_t bdst = dst + A_ROOM;
-                                for (int tc = 0, kb = kidx; tc < nB; ++tc, kb += col_k, bdst += B_BYTES)
-                                    ptx::tma_load_2d(bdst, &tmap_w, kb, n0, full);
-                                if (nimg >= 0) ptx::tma_prefetch_4d(ma, c0, nx_org + ti * dstep, ny_org + tr * dstep, nimg);
-                            }
-                            __syncwarp();
-                            if (++s == S) { s = 0; ph ^= 1; }
-                        }
-                        if (dead) break;
-                    }
-                }
-        }
-    } else if (warp < MMA_WARPS) {
+    uint8_t *acc_stage = smem_gen + (s_acc - smem_base);
+    if (warp < MMA_WARPS) {
+        ptx::setmaxnreg_inc<TMA_CONSUMER_REGS>();
         // ================================ consumer warpgroups ================================
         const int e = warp, g = warp >> 2;
         const bool leader = (threadIdx.x & 127) == 0;
@@ -1003,6 +1118,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
             const int sp = tile % KS, mn = tile / KS;
             const int n0 = (mn % n_tiles) * BLOCK_N;
             if (!tile_active(n0)) continue;
+            const ConsRows cr = cons_rows<MODE>(P, m0_of(mn / n_tiles), e, lane);
             float acc[BLOCK_N / 2];
             zero_acc(acc);
             int held = -1;                                             // stage whose MMAs may still be reading it
@@ -1039,123 +1155,215 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
             ptx::wgmma_fence_regs(acc);
             if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
             if (dead) break;
-            if (!tma_stage_tile<BLOCK_N>(P, acc, acc_stage, acc_full, acc_empty, aph, e, lane, 125)) break;
+            if (!tma_stage_tile<BLOCK_N, MODE>(P, acc, acc_stage, acc_full, acc_empty, aph, e, lane, n0, cr, 125)) break;
         }
-    } else if (warp > 8) {
-        // ================================ fixers: zero the hole rows of every landed A tile ================================
-        if (fix) {
-            const int t = (warp - 9) * 32 + lane;
+    } else {
+        ptx::setmaxnreg_dec<TMA_SUPPORT_REGS>();       // warpgroups 2 and 3, fixers included when there are no holes
+        if (warp >= EPI_WARP0) {
+            // ================================ epilogue warps ================================
+            const int w = warp - EPI_WARP0;
+            s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
+                         ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + w * EPI_STAT_SLICE : nullptr;
+            auto origin = [&](int tile, int &m0, int &n0) {
+                const int mn = tile / KS;
+                m0 = m0_of(mn / n_tiles); n0 = (mn % n_tiles) * BLOCK_N;
+                if (!tile_active(n0)) n0 = -1;
+            };
+            tma_epilogue_warps<BLOCK_N, MODE>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, s_stat, stat_n0, w, lane, 126);
+            // last N tile's statistics: all four slices are complete once the epilogue warpgroup passed this barrier (no CTA-wide
+            // barrier: the warpgroups run under different register limits, setmaxnreg regions must not meet again)
+            ptx::named_sync(1, EPI_WARPS * 32);
+            if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - w * EPI_STAT_SLICE, w, lane, stat_n0);
+        } else if (warp == 8) {
+            // ================================ TMA producer ================================
             int s = 0;
-            uint32_t ph = 0;
+            uint32_t ph = 1;                                               // first pass over the ring: stages are free
+            const int plane = (MODE == 0) ? P.ho * P.wo : P.h * P.w;
+            const int pwid = (MODE == 0) ? P.wo : P.w;
+            const int kext0 = (MODE == 0) ? P.parts[0].kext : P.dc_kext, kext1 = (MODE == 0 && np > 1) ? P.parts[1].kext : 0;
+            const int dstep = (MODE == 0) ? P.dil : -P.dil;
+            const int row_k = P.wk_row, col_k = P.wk_col;
             bool dead = false;
-            if (!HALO) {
-                // one thread per tile row; validity = the row's tap bit (bounds + hole)
-                uint64_t wnext[TC_MAX_PARTS];
-                auto load_words = [&](int tl) {
-#pragma unroll
-                    for (int p = 0; p < TC_MAX_PARTS; ++p) {
-                        wnext[p] = 0ull;
-                        const int m = m0_of(tl / KS / n_tiles) + t;
-                        if (fix && p < P.nparts && tl < num_tiles && m < P.m_total) wnext[p] = __ldg(P.parts[p].tapmask + m);
-                    }
-                };
-                load_words(tile0);
-                for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-                    const int sp = tile % KS;
-                    uint64_t wcur[TC_MAX_PARTS];
-#pragma unroll
-                    for (int p = 0; p < TC_MAX_PARTS; ++p) wcur[p] = wnext[p];
-                    load_words(tile + tstep);                      // next tile's words travel while this tile streams
-                    if (MODE == 1 && !tile_active(((tile / KS) % n_tiles) * BLOCK_N)) continue;
-                    const int taps = P.kh * P.kw;
-                    for (int tap = 0; tap < taps && !dead; ++tap) {
-#pragma unroll
-                        for (int p = 0; p < TC_MAX_PARTS; ++p) {
-                            if (p >= np) break;
-                            const bool hole = fix && ((wcur[p] >> tap) & 1ull) == 0ull;
-                            const bool any_hole = __any_sync(0xffffffffu, hole);
-                            const int nb = ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
-                            const int gb0 = (p == 0) ? 0 : P.parts[0].kext / BLOCK_K;
-                            for (int cb = 0; cb < nb; ++cb) {
-                                if (KS > 1 && (gb0 + cb) % KS != sp) continue;
-                                if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 122)) { dead = true; break; }
-                                if (any_hole) {
-                                    if (hole) {
-                                        uint4 *r = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + t * 128);
-                                        const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-#pragma unroll
-                                        for (int k = 0; k < 8; ++k) r[k] = z;
-                                    }
-                                    ptx::fence_proxy_async_smem();
-                                }
-                                __syncwarp();
-                                if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
-                                if (++s == S) { s = 0; ph ^= 1; }
-                            }
-                            if (dead) break;
-                        }
+            for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
+                const int sp = tile % KS, mn = tile / KS;
+                const int m0 = m0_of(mn / n_tiles), n0 = (mn % n_tiles) * BLOCK_N;
+                if (!tile_active(n0)) continue;
+                const int img = m0 / plane, rem = m0 - img * plane;
+                const int oy = rem / pwid, ox = rem - oy * pwid;
+                // leftmost / topmost source coordinate of tap column 0 (fwd) -- dgrad walks its taps right to left
+                const int x_org = (MODE == 0) ? ox * P.stride - P.pad_w : (HALO ? ox + P.pad_w - hx : ox + P.pad_w);
+                const int y_org = (MODE == 0) ? oy * P.stride - P.pad_h : oy + P.pad_h;
+                // optional L2 prefetch (P.l2pf): while tile t is loaded, the A boxes of this CTA's NEXT tile are requested into L2, one
+                // tile's worth of stages ahead, so that their loads find L2 instead of DRAM (the ring is round-trip-latency bound)
+                int nx_org = 0, ny_org = 0, nimg = -1;
+                if (P.l2pf && tile + tstep < num_tiles) {
+                    const int nmn = (tile + tstep) / KS;
+                    const int nm0 = m0_of(nmn / n_tiles);
+                    if (nm0 != m0) {
+                        nimg = nm0 / plane;
+                        const int nrem = nm0 - nimg * plane, noy = nrem / pwid, nox = nrem - noy * pwid;
+                        nx_org = (MODE == 0) ? nox * P.stride - P.pad_w : (HALO ? nox + P.pad_w - hx : nox + P.pad_w);
+                        ny_org = (MODE == 0) ? noy * P.stride - P.pad_h : noy + P.pad_h;
                     }
                 }
-            } else {
-                // one thread per halo pixel row (threads < hx own a second one); validity = the source mask at that pixel
-                const int plane = P.ho * P.wo;
-                auto load_bits = [&](int tl, uint32_t &b0, uint32_t &b1) {       // bit (p*8 + tr): pixel row is a hole
-                    b0 = b1 = 0;
-                    if (!fix || tl >= num_tiles) return;
-                    const int m0 = m0_of(tl / KS / n_tiles);
-                    const int img = m0 / plane, rem = m0 - img * plane;
-                    const int oy = rem / P.wo, ox = rem - oy * P.wo;
-#pragma unroll
-                    for (int p = 0; p < TC_MAX_PARTS; ++p) {
-                        if (p >= P.nparts || P.parts[p].mask == nullptr) continue;
-                        const int mup = P.parts[p].mup;
-                        const uint8_t *mk = P.parts[p].mask + static_cast<long long>(img) * (P.h >> mup) * (P.w >> mup);
-                        for (int tr = 0; tr < P.kh; ++tr) {
-                            const int y = oy - P.pad_h + tr * P.dil;
-                            if (y < 0 || y >= P.h) continue;            // rows outside the image were zero-filled by TMA
-                            const int x0 = ox - P.pad_w + t, x1 = x0 + 128;
-                            if (x0 >= 0 && x0 < P.w && __ldg(mk + (y >> mup) * (P.w >> mup) + (x0 >> mup)) == 0) b0 |= 1u << (p * 8 + tr);
-                            if (t < hx && x1 < P.w && __ldg(mk + (y >> mup) * (P.w >> mup) + (x1 >> mup)) == 0) b1 |= 1u << (p * 8 + tr);
-                        }
-                    }
-                };
-                uint32_t n0b, n1b;
-                load_bits(tile0, n0b, n1b);
-                for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-                    const int sp = tile % KS;
-                    const uint32_t c0b = n0b, c1b = n1b;
-                    load_bits(tile + tstep, n0b, n1b);
-                    if (MODE == 1 && !tile_active(((tile / KS) % n_tiles) * BLOCK_N)) continue;
-                    for (int tr = 0; tr < P.kh && !dead; ++tr) {
+                int krow = P.wk_base;                                      // weight K index of (tr, tap column 0, part 0, block 0)
+                for (int tr = 0, y = y_org; tr < P.kh && !dead; ++tr, y += dstep, krow += row_k)
+                    for (int ti = 0, x = x_org, kidx = krow; ti < kwi && !dead; ++ti, x += dstep, kidx = krow + ti * col_k) {
 #pragma unroll
                         for (int p = 0; p < TC_MAX_PARTS; ++p) {
-                            if (p >= np) break;
-                            const bool h0 = (c0b >> (p * 8 + tr)) & 1u, h1 = (c1b >> (p * 8 + tr)) & 1u;
-                            const bool any_hole = __any_sync(0xffffffffu, h0 || h1);
-                            const int nb = ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
-                            const int gb0 = (p == 0) ? 0 : P.parts[0].kext / BLOCK_K;
-                            for (int cb = 0; cb < nb; ++cb) {
-                                if (KS > 1 && (gb0 + cb) % KS != sp) continue;
-                                if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 122)) { dead = true; break; }
-                                if (any_hole) {
-                                    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-                                    if (h0) {
-                                        uint4 *r = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + t * 128);
-#pragma unroll
-                                        for (int k = 0; k < 8; ++k) r[k] = z;
-                                    }
-                                    if (h1) {
-                                        uint4 *r = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + (t + 128) * 128);
-#pragma unroll
-                                        for (int k = 0; k < 8; ++k) r[k] = z;
-                                    }
-                                    ptx::fence_proxy_async_smem();
+                            const int kext = (p == 0) ? kext0 : kext1;
+                            const CUtensorMap *ma = (p == 0) ? &tmap_a0 : &tmap_a1;
+                            const int gb0 = (p == 0) ? 0 : kext0 / BLOCK_K;          // global K-block index of the part's first block
+                            for (int c0 = 0; c0 < kext; c0 += BLOCK_K, kidx += BLOCK_K) {
+                                if (KS > 1 && (gb0 + c0 / BLOCK_K) % KS != sp) continue;
+                                if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 121))) { dead = true; break; }
+                                if (ptx::elect_one()) {
+                                    const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
+                                    ptx::mbar_arrive_expect_tx(full, STAGE_TX);
+                                    ptx::tma_load_4d(dst, ma, c0, x, y, img, full);
+                                    uint32_t bdst = dst + A_ROOM;
+                                    for (int tc = 0, kb = kidx; tc < nB; ++tc, kb += col_k, bdst += B_BYTES)
+                                        ptx::tma_load_2d(bdst, &tmap_w, kb, n0, full);
+                                    if (nimg >= 0) ptx::tma_prefetch_4d(ma, c0, nx_org + ti * dstep, ny_org + tr * dstep, nimg);
                                 }
                                 __syncwarp();
-                                if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
                                 if (++s == S) { s = 0; ph ^= 1; }
                             }
                             if (dead) break;
+                        }
+                    }
+            }
+        } else {
+            // ================================ fixers: zero the hole rows of every landed A tile ================================
+            // thread t owns tile rows t, t + 96 (and t + 192: halo rows up to 256)
+            if (fix) {
+                constexpr int FR = HALO ? 3 : 2;
+                const int t = (warp - 9) * 32 + lane;
+                int s = 0;
+                uint32_t ph = 0;
+                bool dead = false;
+                auto zero_row = [&](int row) {
+                    uint4 *r = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + row * 128);
+                    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) r[k] = z;
+                };
+                if (!HALO) {
+                    // validity = the row's tap bit (bounds + hole)
+                    uint64_t wnext[FR][TC_MAX_PARTS];
+                    auto load_words = [&](int tl) {
+#pragma unroll
+                        for (int r = 0; r < FR; ++r)
+#pragma unroll
+                            for (int p = 0; p < TC_MAX_PARTS; ++p) {
+                                wnext[r][p] = 0ull;
+                                const int m = m0_of(tl / KS / n_tiles) + t + TMA_FIX_THREADS * r;
+                                if (p < P.nparts && tl < num_tiles && t + TMA_FIX_THREADS * r < BLOCK_M && m < P.m_total)
+                                    wnext[r][p] = __ldg(P.parts[p].tapmask + m);
+                            }
+                    };
+                    load_words(tile0);
+                    for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
+                        const int sp = tile % KS;
+                        uint64_t wcur[FR][TC_MAX_PARTS];
+#pragma unroll
+                        for (int r = 0; r < FR; ++r)
+#pragma unroll
+                            for (int p = 0; p < TC_MAX_PARTS; ++p) wcur[r][p] = wnext[r][p];
+                        load_words(tile + tstep);                      // next tile's words travel while this tile streams
+                        if (MODE == 1 && !tile_active(((tile / KS) % n_tiles) * BLOCK_N)) continue;
+                        const int taps = P.kh * P.kw;
+                        for (int tap = 0; tap < taps && !dead; ++tap) {
+#pragma unroll
+                            for (int p = 0; p < TC_MAX_PARTS; ++p) {
+                                if (p >= np) break;
+                                bool hole[FR], mine = false;
+#pragma unroll
+                                for (int r = 0; r < FR; ++r) {      // rows past the tile (t + 96 >= 128) are not rows
+                                    hole[r] = t + TMA_FIX_THREADS * r < BLOCK_M && ((wcur[r][p] >> tap) & 1ull) == 0ull;
+                                    mine = mine || hole[r];
+                                }
+                                const bool any_hole = __any_sync(0xffffffffu, mine);
+                                const int nb = ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
+                                const int gb0 = (p == 0) ? 0 : P.parts[0].kext / BLOCK_K;
+                                for (int cb = 0; cb < nb; ++cb) {
+                                    if (KS > 1 && (gb0 + cb) % KS != sp) continue;
+                                    if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 122)) { dead = true; break; }
+                                    if (any_hole) {
+#pragma unroll
+                                        for (int r = 0; r < FR; ++r)
+                                            if (hole[r]) zero_row(t + TMA_FIX_THREADS * r);
+                                        ptx::fence_proxy_async_smem();
+                                    }
+                                    __syncwarp();
+                                    if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
+                                    if (++s == S) { s = 0; ph ^= 1; }
+                                }
+                                if (dead) break;
+                            }
+                        }
+                    }
+                } else {
+                    // validity = the source mask at the halo pixel row (rows < 128 + hx)
+                    const int plane = P.ho * P.wo;
+                    auto load_bits = [&](int tl, uint32_t (&b)[FR]) {       // bit (p*8 + tr) of b[r]: pixel row t + 96 r is a hole
+#pragma unroll
+                        for (int r = 0; r < FR; ++r) b[r] = 0;
+                        if (tl >= num_tiles) return;
+                        const int m0 = m0_of(tl / KS / n_tiles);
+                        const int img = m0 / plane, rem = m0 - img * plane;
+                        const int oy = rem / P.wo, ox = rem - oy * P.wo;
+#pragma unroll
+                        for (int p = 0; p < TC_MAX_PARTS; ++p) {
+                            if (p >= P.nparts || P.parts[p].mask == nullptr) continue;
+                            const int mup = P.parts[p].mup;
+                            const uint8_t *mk = P.parts[p].mask + static_cast<long long>(img) * (P.h >> mup) * (P.w >> mup);
+                            for (int tr = 0; tr < P.kh; ++tr) {
+                                const int y = oy - P.pad_h + tr * P.dil;
+                                if (y < 0 || y >= P.h) continue;            // rows outside the image were zero-filled by TMA
+#pragma unroll
+                                for (int r = 0; r < FR; ++r) {
+                                    const int row = t + TMA_FIX_THREADS * r, x = ox - P.pad_w + row;
+                                    if (row < BLOCK_M + hx && x >= 0 && x < P.w && __ldg(mk + (y >> mup) * (P.w >> mup) + (x >> mup)) == 0)
+                                        b[r] |= 1u << (p * 8 + tr);
+                                }
+                            }
+                        }
+                    };
+                    uint32_t nb_bits[FR];
+                    load_bits(tile0, nb_bits);
+                    for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
+                        const int sp = tile % KS;
+                        uint32_t cb_bits[FR];
+#pragma unroll
+                        for (int r = 0; r < FR; ++r) cb_bits[r] = nb_bits[r];
+                        load_bits(tile + tstep, nb_bits);
+                        if (MODE == 1 && !tile_active(((tile / KS) % n_tiles) * BLOCK_N)) continue;
+                        for (int tr = 0; tr < P.kh && !dead; ++tr) {
+#pragma unroll
+                            for (int p = 0; p < TC_MAX_PARTS; ++p) {
+                                if (p >= np) break;
+                                bool hole[FR], mine = false;
+#pragma unroll
+                                for (int r = 0; r < FR; ++r) { hole[r] = (cb_bits[r] >> (p * 8 + tr)) & 1u; mine = mine || hole[r]; }
+                                const bool any_hole = __any_sync(0xffffffffu, mine);
+                                const int nb = ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
+                                const int gb0 = (p == 0) ? 0 : P.parts[0].kext / BLOCK_K;
+                                for (int cb = 0; cb < nb; ++cb) {
+                                    if (KS > 1 && (gb0 + cb) % KS != sp) continue;
+                                    if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 122)) { dead = true; break; }
+                                    if (any_hole) {
+#pragma unroll
+                                        for (int r = 0; r < FR; ++r)
+                                            if (hole[r]) zero_row(t + TMA_FIX_THREADS * r);
+                                        ptx::fence_proxy_async_smem();
+                                    }
+                                    __syncwarp();
+                                    if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
+                                    if (++s == S) { s = 0; ph ^= 1; }
+                                }
+                                if (dead) break;
+                            }
                         }
                     }
                 }
@@ -1163,8 +1371,6 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
         }
     }
 
-    __syncthreads();
-    if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - (warp - EPI_WARP0) * STAT_SLICE, warp - EPI_WARP0, lane, stat_n0);
 }
 
 
@@ -1198,7 +1404,7 @@ struct SpTable {
 };
 
 template <int BLOCK_N, int MODE>
-__global__ void __launch_bounds__(TMA_THREADS, 1)
+__global__ void __maxnreg__(TMA_REGS)
 pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ SpTable TB, const __grid_constant__ CUtensorMap tmap_w,
                    const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1) {
     constexpr uint32_t B_BYTES = BLOCK_N * 128;
@@ -1235,7 +1441,7 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
     }
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, 4); ptx::mbar_init(bar_empty + 8 * s, 2); }
+        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, TMA_FIX_THREADS / 32); ptx::mbar_init(bar_empty + 8 * s, 2); }
         ptx::mbar_init(acc_full, MMA_WARPS); ptx::mbar_init(acc_empty, EPI_WARPS);     // one arrival per warp
         ptx::fence_mbar_init();
     }
@@ -1244,43 +1450,9 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
 
     float *s_stat = nullptr;
     int stat_n0 = -1;
-    float *acc_stage = reinterpret_cast<float *>(smem_gen + (s_acc - smem_base));
-    if (warp >= EPI_WARP0) {
-        // ================================ epilogue warps ================================
-        const int w = warp - EPI_WARP0;
-        s_stat = (MODE == 0 && P.bn_sums != nullptr) ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + w * STAT_SLICE : nullptr;
-        auto origin = [&](int tile, int &m0, int &n0) { m0 = (tile / n_tiles) * BLOCK_M; n0 = (tile % n_tiles) * BLOCK_N; };
-        tma_epilogue_warps<BLOCK_N, MODE>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, s_stat, stat_n0, w, lane, 326);
-    } else if (warp == 8) {
-        // ================================ TMA producer ================================
-        int s = 0;
-        uint32_t ph = 1;
-        bool dead = false;
-        for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-            const int m0 = (tile / n_tiles) * BLOCK_M, n0 = (tile % n_tiles) * BLOCK_N;
-            const int img = m0 / plane, rem = m0 - img * plane;
-            const int oy = rem / gw, ox = rem - oy * gw;
-            for (int i = 0; i < TB.n_items && !dead; ++i) {
-                const SpItem it = TB.it[i];
-                const CUtensorMap *ma = (it.part == 0) ? &tmap_a0 : &tmap_a1;
-                const int x = ox * TB.step[it.part] + it.dx, y = oy * TB.step[it.part] + it.dy;
-                const uint32_t a_bytes = static_cast<uint32_t>(TB.arows[it.part]) * 128u;      // what the part's box delivers
-                for (int cb = 0; cb < nbk[it.part]; ++cb) {
-                    if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 321))) { dead = true; break; }
-                    if (ptx::elect_one()) {
-                        const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
-                        ptx::mbar_arrive_expect_tx(full, a_bytes + it.nb * B_BYTES);
-                        ptx::tma_load_4d(dst, ma, cb * BLOCK_K, x, y, img, full);
-                        uint32_t bdst = dst + A_ROOM;
-                        for (int tc = 0, kb = it.wk + cb * BLOCK_K; tc < it.nb; ++tc, kb += it.wk_step, bdst += B_BYTES)
-                            ptx::tma_load_2d(bdst, &tmap_w, kb, n0, full);
-                    }
-                    __syncwarp();
-                    if (++s == S) { s = 0; ph ^= 1; }
-                }
-            }
-        }
-    } else if (warp < MMA_WARPS) {
+    uint8_t *acc_stage = smem_gen + (s_acc - smem_base);
+    if (warp < MMA_WARPS) {
+        ptx::setmaxnreg_inc<TMA_CONSUMER_REGS>();
         // ================================ consumer warpgroups ================================
         const int e = warp, g = warp >> 2;
         const bool leader = (threadIdx.x & 127) == 0;
@@ -1292,6 +1464,7 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
         uint32_t ph = 0, aph = 1;                                      // aph: first pass, the staging tile is free
         bool dead = false;
         for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
+            const ConsRows cr = cons_rows<MODE>(P, (tile / n_tiles) * BLOCK_M, e, lane);
             float acc[BLOCK_N / 2];
             zero_acc(acc);
             int held = -1;
@@ -1315,77 +1488,122 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
             ptx::wgmma_fence_regs(acc);
             if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
             if (dead) break;
-            if (!tma_stage_tile<BLOCK_N>(P, acc, acc_stage, acc_full, acc_empty, aph, e, lane, 325)) break;
+            if (!tma_stage_tile<BLOCK_N, MODE>(P, acc, acc_stage, acc_full, acc_empty, aph, e, lane, (tile % n_tiles) * BLOCK_N, cr, 325)) break;
         }
-    } else if (warp > 8) {
-        // ================================ fixers: zero the hole rows of every landed A tile ================================
-        if (fix) {
-            const int t = (warp - 9) * 32 + lane;
+    } else {
+        ptx::setmaxnreg_dec<TMA_SUPPORT_REGS>();       // warpgroups 2 and 3, fixers included when there are no holes
+        if (warp >= EPI_WARP0) {
+            // ================================ epilogue warps ================================
+            const int w = warp - EPI_WARP0;
+            s_stat = (MODE == 0 && P.bn_sums != nullptr) ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + w * EPI_STAT_SLICE : nullptr;
+            auto origin = [&](int tile, int &m0, int &n0) { m0 = (tile / n_tiles) * BLOCK_M; n0 = (tile % n_tiles) * BLOCK_N; };
+            tma_epilogue_warps<BLOCK_N, MODE>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, s_stat, stat_n0, w, lane, 326);
+            // last N tile's statistics: all four slices are complete once the epilogue warpgroup passed this barrier (no CTA-wide
+            // barrier: the warpgroups run under different register limits, setmaxnreg regions must not meet again)
+            ptx::named_sync(1, EPI_WARPS * 32);
+            if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - w * EPI_STAT_SLICE, w, lane, stat_n0);
+        } else if (warp == 8) {
+            // ================================ TMA producer ================================
             int s = 0;
-            uint32_t ph = 0;
+            uint32_t ph = 1;
             bool dead = false;
-            // bit i of b0 / b1: row t / row t + 128 of item i's A tile is a hole (rows outside the image were zero-filled by TMA)
-            auto load_bits = [&](int tl, uint64_t &b0, uint64_t &b1) {
-                b0 = b1 = 0ull;
-                if (tl >= num_tiles) return;
-                const int m0 = (tl / n_tiles) * BLOCK_M;
+            for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
+                const int m0 = (tile / n_tiles) * BLOCK_M, n0 = (tile % n_tiles) * BLOCK_N;
                 const int img = m0 / plane, rem = m0 - img * plane;
                 const int oy = rem / gw, ox = rem - oy * gw;
-                for (int i = 0; i < TB.n_items; ++i) {
-                    const SpItem it = TB.it[i];
-                    const uint8_t *mk = P.parts[it.part].mask;
-                    if (mk == nullptr) continue;
-                    const int pwid = TB.pw[it.part], phei = TB.ph[it.part], es = TB.es[it.part];
-                    const int hrows = TB.arows[it.part] - BLOCK_M;
-                    const int x0 = ox * TB.step[it.part] + it.dx, y0 = oy * TB.step[it.part] + it.dy;
-                    int tx, ty, tn;
-                    if (hrows > 0 || (P.box_h == 1 && P.box_n == 1)) { tx = t; ty = 0; tn = 0; }
-                    else { tx = t % P.box_w; ty = (t / P.box_w) % P.box_h; tn = t / (P.box_w * P.box_h); }
-                    const int X = x0 + tx * es, Y = y0 + ty * es, IM = img + tn;
-                    if (X >= 0 && X < pwid && Y >= 0 && Y < phei && IM < P.n &&
-                        __ldg(mk + (static_cast<long long>(IM) * phei + Y) * pwid + X) == 0) b0 |= 1ull << i;
-                    if (t < hrows) {
-                        const int X1 = x0 + (t + 128) * es;
-                        if (X1 >= 0 && X1 < pwid && Y >= 0 && Y < phei && __ldg(mk + (static_cast<long long>(IM) * phei + Y) * pwid + X1) == 0) b1 |= 1ull << i;
-                    }
-                }
-            };
-            uint64_t n0b, n1b;
-            load_bits(tile0, n0b, n1b);
-            for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-                const uint64_t c0b = n0b, c1b = n1b;
-                load_bits(tile + tstep, n0b, n1b);
                 for (int i = 0; i < TB.n_items && !dead; ++i) {
-                    const bool h0 = (c0b >> i) & 1ull, h1 = (c1b >> i) & 1ull;
-                    const bool any_hole = __any_sync(0xffffffffu, h0 || h1);
-                    const int nb_i = nbk[TB.it[i].part];
-                    for (int cb = 0; cb < nb_i; ++cb) {
-                        if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 322)) { dead = true; break; }
-                        if (any_hole) {
-                            const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-                            if (h0) {
-                                uint4 *r = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + t * 128);
-#pragma unroll
-                                for (int k = 0; k < 8; ++k) r[k] = z;
-                            }
-                            if (h1) {
-                                uint4 *r = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + (t + 128) * 128);
-#pragma unroll
-                                for (int k = 0; k < 8; ++k) r[k] = z;
-                            }
-                            ptx::fence_proxy_async_smem();
+                    const SpItem it = TB.it[i];
+                    const CUtensorMap *ma = (it.part == 0) ? &tmap_a0 : &tmap_a1;
+                    const int x = ox * TB.step[it.part] + it.dx, y = oy * TB.step[it.part] + it.dy;
+                    const uint32_t a_bytes = static_cast<uint32_t>(TB.arows[it.part]) * 128u;      // what the part's box delivers
+                    for (int cb = 0; cb < nbk[it.part]; ++cb) {
+                        if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 321))) { dead = true; break; }
+                        if (ptx::elect_one()) {
+                            const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
+                            ptx::mbar_arrive_expect_tx(full, a_bytes + it.nb * B_BYTES);
+                            ptx::tma_load_4d(dst, ma, cb * BLOCK_K, x, y, img, full);
+                            uint32_t bdst = dst + A_ROOM;
+                            for (int tc = 0, kb = it.wk + cb * BLOCK_K; tc < it.nb; ++tc, kb += it.wk_step, bdst += B_BYTES)
+                                ptx::tma_load_2d(bdst, &tmap_w, kb, n0, full);
                         }
                         __syncwarp();
-                        if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
                         if (++s == S) { s = 0; ph ^= 1; }
+                    }
+                }
+            }
+        } else {
+            // ================================ fixers: zero the hole rows of every landed A tile ================================
+            // thread t owns A-tile rows t, t + 96 and t + 192 (a part's box delivers at most 256 rows)
+            if (fix) {
+                constexpr int FR = 3;
+                const int t = (warp - 9) * 32 + lane;
+                int s = 0;
+                uint32_t ph = 0;
+                bool dead = false;
+                // bit i of b[r]: row t + 96 r of item i's A tile is a hole (rows outside the image were zero-filled by TMA)
+                auto load_bits = [&](int tl, uint64_t (&b)[FR]) {
+#pragma unroll
+                    for (int r = 0; r < FR; ++r) b[r] = 0ull;
+                    if (tl >= num_tiles) return;
+                    const int m0 = (tl / n_tiles) * BLOCK_M;
+                    const int img = m0 / plane, rem = m0 - img * plane;
+                    const int oy = rem / gw, ox = rem - oy * gw;
+                    for (int i = 0; i < TB.n_items; ++i) {
+                        const SpItem it = TB.it[i];
+                        const uint8_t *mk = P.parts[it.part].mask;
+                        if (mk == nullptr) continue;
+                        const int pwid = TB.pw[it.part], phei = TB.ph[it.part], es = TB.es[it.part];
+                        const int hrows = TB.arows[it.part] - BLOCK_M;
+                        const int x0 = ox * TB.step[it.part] + it.dx, y0 = oy * TB.step[it.part] + it.dy;
+#pragma unroll
+                        for (int r = 0; r < FR; ++r) {
+                            const int row = t + TMA_FIX_THREADS * r;
+                            if (row >= BLOCK_M + hrows) continue;
+                            int tx, ty, tn;           // rows past 128 only exist in one-row halo boxes
+                            if (hrows > 0 || (P.box_h == 1 && P.box_n == 1)) { tx = row; ty = 0; tn = 0; }
+                            else { tx = row % P.box_w; ty = (row / P.box_w) % P.box_h; tn = row / (P.box_w * P.box_h); }
+                            const int X = x0 + tx * es, Y = y0 + ty * es, IM = img + tn;
+                            if (X >= 0 && X < pwid && Y >= 0 && Y < phei && IM < P.n &&
+                                __ldg(mk + (static_cast<long long>(IM) * phei + Y) * pwid + X) == 0) b[r] |= 1ull << i;
+                        }
+                    }
+                };
+                uint64_t nb_bits[FR];
+                load_bits(tile0, nb_bits);
+                for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
+                    uint64_t cb_bits[FR];
+#pragma unroll
+                    for (int r = 0; r < FR; ++r) cb_bits[r] = nb_bits[r];
+                    load_bits(tile + tstep, nb_bits);
+                    for (int i = 0; i < TB.n_items && !dead; ++i) {
+                        bool hole[FR], mine = false;
+#pragma unroll
+                        for (int r = 0; r < FR; ++r) { hole[r] = (cb_bits[r] >> i) & 1ull; mine = mine || hole[r]; }
+                        const bool any_hole = __any_sync(0xffffffffu, mine);
+                        const int nb_i = nbk[TB.it[i].part];
+                        for (int cb = 0; cb < nb_i; ++cb) {
+                            if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 322)) { dead = true; break; }
+                            if (any_hole) {
+                                const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+                                for (int r = 0; r < FR; ++r)
+                                    if (hole[r]) {
+                                        uint4 *rw = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + (t + TMA_FIX_THREADS * r) * 128);
+#pragma unroll
+                                        for (int k = 0; k < 8; ++k) rw[k] = z;
+                                    }
+                                ptx::fence_proxy_async_smem();
+                            }
+                            __syncwarp();
+                            if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
+                            if (++s == S) { s = 0; ph ^= 1; }
+                        }
                     }
                 }
             }
         }
     }
 
-    __syncthreads();
-    if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - (warp - EPI_WARP0) * STAT_SLICE, warp - EPI_WARP0, lane, stat_n0);
 }
 
 // nearest 2x upsample of one convolution source into a dense [n, 2hs, 2ws, c8] buffer (TMA cannot replicate pixels)
@@ -2333,14 +2551,22 @@ size_t tapmask_bytes(const pcb_conv *c) {
     return (static_cast<size_t>(c->nparts) * c->n * c->ho * c->wo * sizeof(uint64_t) + 255) / 256 * 256;
 }
 
+// shared memory of a TMA-fed fwd / dgrad / sub-pixel launch outside its ring: alignment slack, barriers, statistics slices and
+// the staging tile (bf16, or fp32 for the raw partials of a split-K launch); the ring gets the rest of the opt-in maximum
+size_t tma_fixed_smem(int block_n, bool splitk) {
+    return 1024 + TMA_BAR_BYTES + EPI_STAT_SMEM_BYTES + (splitk ? acc_stage_bytes(block_n) : bf16_stage_bytes(block_n));
+}
+
 template <int BLOCK_N, int MODE, bool HALO>
 int launch_tma_n(TcParams &P, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, cudaStream_t st) {
     const int nb = HALO ? P.kw : 1;
     const size_t a_room = (static_cast<size_t>(BLOCK_M + (HALO ? (P.kw - 1) * P.dil : 0)) * 128 + 1023) / 1024 * 1024;
     const size_t stage = a_room + static_cast<size_t>(nb) * BLOCK_N * 128;
-    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (RING_BUDGET - acc_stage_bytes(BLOCK_N)) / stage));
+    PCB_CHECK(BLOCK_N <= 128 || P.partial == nullptr, "TMA-fed conv: split-K stages fp32 partials, at most 128 columns wide");
+    const size_t fixed = tma_fixed_smem(BLOCK_N, P.partial != nullptr);
+    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (MAX_SMEM - fixed) / stage));
     PCB_CHECK(P.stages >= 2, "TMA-fed conv: stage of %zu bytes does not fit twice", stage);
-    const size_t smem = 1024 + P.stages * stage + TMA_BAR_BYTES + EPI_STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
+    const size_t smem = fixed + P.stages * stage;
     auto kern = pconv_tc_tma_kernel<BLOCK_N, MODE, HALO>;
     PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     if (P.ksplit < 1) P.ksplit = 1;
@@ -2354,18 +2580,22 @@ int launch_tma_n(TcParams &P, const CUtensorMap &tw, const CUtensorMap &ta0, con
 
 template <int MODE>
 int launch_tma(TcParams &P, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, int bn, bool halo, cudaStream_t st) {
+    PCB_CHECK(!(halo && bn == 256), "TMA-fed conv: no 256-wide row-halo tiles");
     if (halo) {
         if (bn == 128) return launch_tma_n<128, MODE, true>(P, tw, ta0, ta1, st);
         if (bn == 64) return launch_tma_n<64, MODE, true>(P, tw, ta0, ta1, st);
         return launch_tma_n<32, MODE, true>(P, tw, ta0, ta1, st);
     }
+    if (bn == 256) return launch_tma_n<256, MODE, false>(P, tw, ta0, ta1, st);
     if (bn == 128) return launch_tma_n<128, MODE, false>(P, tw, ta0, ta1, st);
     if (bn == 64) return launch_tma_n<64, MODE, false>(P, tw, ta0, ta1, st);
     return launch_tma_n<32, MODE, false>(P, tw, ta0, ta1, st);
 }
 
 // at least three stages of (halo tile of 128 + (kw-1)*dil pixel rows + kw weight tiles) fit in shared memory next to the
-// epilogue staging tile of an N tile of block_n columns
+// epilogue staging tile of an N tile of block_n columns.  The test keeps the fp32 staging size and ring budget it was
+// introduced with although the tiles now stage bf16: halo tiles sum a layer's K blocks in another order, so moving this
+// boundary would change which layers' outputs round differently.
 bool halo_stages_fit(int kw, int dil, int block_n) {
     const size_t stage = (static_cast<size_t>(128 + (kw - 1) * dil) * 128 + 1023) / 1024 * 1024 + static_cast<size_t>(kw) * block_n * 128;
     return 3 * stage + acc_stage_bytes(block_n) <= RING_BUDGET;
@@ -2381,10 +2611,20 @@ bool tma_halo_ok(const pcb_conv *c, int bw, int bh, int bn, int block_n) {
 // widest N tile that divides `cols` and still leaves at least one tile per SM; low-resolution layers (a handful of M tiles
 // against a multi-megabyte weight matrix) get NARROWER N tiles: each CTA's operand stream is latency-bound (a ring of a few
 // stages), so the time of such a layer is (bytes per CTA) / that rate -- more, smaller CTAs stream the weights in parallel
-// (at most 128 columns: a consumer warpgroup holds 64 rows x N fp32 accumulators in registers)
-int pick_bn(int cols, long long m_total) {
+// (a consumer warpgroup holds 64 rows x N fp32 accumulators in registers).
+// 256-wide tiles pull a quarter fewer operand bytes from L2 per FLOP and give every ring stage twice the MMA work.  The
+// persistent CTAs walk the tiles in waves of one tile per SM, so 256 columns can only win when their (twice as long) waves are
+// at most half as many as those of 128-wide tiles.  Measured per layer on ImageFillOrigin 512^2, batch 8 (tools/tc_layers.py,
+// H100 at 700 W, 128 forced vs this rule): the data gradients win wherever that holds (dec1 1024 columns, 256 tiles: 0.137 ->
+// 0.133 ms; dec5 768 columns, 768 tiles: 0.262 -> 0.252 ms), the forward only where 256 columns take ONE wave instead of two
+// (dec1, 128 tiles: 0.199 -> 0.191 ms).  With more waves the forward lost (enc2 and dec5, 256 tiles: 0.164 -> 0.172 and
+// 0.271 -> 0.295 ms; enc3: 0.082 -> 0.089 ms): its consumers also do the epilogue's element math, twice as much per tile.
+int pick_bn(int cols, long long m_total, bool fwd) {
     const long long m_tiles = (m_total + BLOCK_M - 1) / BLOCK_M;
     if (cols <= 32) return 32;
+    const long long sms = pcb_num_sms();
+    auto waves = [&](int b) { return (m_tiles * (cols / b) + sms - 1) / sms; };
+    if (cols % 256 == 0 && 2 * waves(256) <= waves(128) && (!fwd || waves(256) == 1)) return 256;
     int bn = (cols % 128 == 0) ? 128 : 64;
     if (!getenv("PCB_NO_NARROW_N"))
         while (bn > 32 && cols % (bn / 2) == 0 && m_tiles * (cols / bn) < pcb_num_sms() / 2) bn /= 2;
@@ -2577,7 +2817,7 @@ int sp_weight_prepare(const pcb_conv *c, const SpPlan &S, const Layout &L, const
 }
 
 // sub-pixel tiles are at most 64 columns wide: two stages of (A tile + up to four weight tiles) must fit next to the staging tile
-int sp_bn(int cols, long long m_total) { return std::min(pick_bn(cols, m_total), 64); }
+int sp_bn(int cols, long long m_total) { return std::min(pick_bn(cols, m_total, true), 64); }
 
 template <int BLOCK_N, int MODE>
 int launch_sp_n(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, cudaStream_t st) {
@@ -2585,9 +2825,10 @@ int launch_sp_n(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUt
     for (int i = 0; i < TB.n_items; ++i) nb_max = std::max(nb_max, TB.it[i].nb);
     const size_t a_room = (static_cast<size_t>(TB.rows_max) * 128 + 1023) / 1024 * 1024;
     const size_t stage = a_room + static_cast<size_t>(nb_max) * BLOCK_N * 128;
-    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (RING_BUDGET - acc_stage_bytes(BLOCK_N)) / stage));
+    const size_t fixed = tma_fixed_smem(BLOCK_N, false);
+    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (MAX_SMEM - fixed) / stage));
     PCB_CHECK(P.stages >= 2, "sub-pixel conv: stage of %zu bytes does not fit twice", stage);
-    const size_t smem = 1024 + P.stages * stage + TMA_BAR_BYTES + EPI_STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
+    const size_t smem = fixed + P.stages * stage;
     auto kern = pconv_tc_sp_kernel<BLOCK_N, MODE>;
     PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     const int num_tiles = ((P.m_total + BLOCK_M - 1) / BLOCK_M) * (P.ncols / BLOCK_N);
@@ -2861,7 +3102,7 @@ int pcb_tc_forward_mask_pass(const pcb_conv *c, uint64_t *tapmask, cudaStream_t 
     if (tma_fwd_ok(c)) {                                  // row-halo tiles: the fixers read the mask planes themselves
         int bw, bh, bn;
         tile_box(c->wo, c->ho, &bw, &bh, &bn);
-        if (tma_halo_ok(c, bw, bh, bn, pick_bn(c->cout <= 32 ? 32 : L.rows_f, m_total))) return 0;
+        if (tma_halo_ok(c, bw, bh, bn, pick_bn(c->cout <= 32 ? 32 : L.rows_f, m_total, true))) return 0;
     }
     return launch_tapmask(c, tapmask, st);
 }
@@ -2921,7 +3162,7 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
     CUtensorMap tm;
     if (tma_fwd_ok(c)) {
         tile_box(c->wo, c->ho, &P.box_w, &P.box_h, &P.box_n);
-        const int bn = pick_bn(c->cout <= 32 ? 32 : L.rows_f, m_total);
+        const int bn = pick_bn(c->cout <= 32 ? 32 : L.rows_f, m_total, true);
         const bool halo = tma_halo_ok(c, P.box_w, P.box_h, P.box_n, bn);
         const int hx = halo ? (c->kw - 1) * c->dil : 0;
         CUtensorMap ta[TC_MAX_PARTS];
@@ -3017,7 +3258,7 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
     CUtensorMap tm;
     if (tma_dgrad_ok(c)) {
         tile_box(c->w, c->h, &P.box_w, &P.box_h, &P.box_n);
-        bn = pick_bn(L.ktap, m_total);
+        bn = pick_bn(L.ktap, m_total, false);
         const bool halo = tma_halo_ok(c, P.box_w, P.box_h, P.box_n, bn);
         P.wk_base = 0; P.wk_col = L.cout64; P.wk_row = c->kw * L.cout64;
         CUtensorMap ta;
@@ -3044,7 +3285,7 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
         const int hh = c->h / 2, hw = c->w / 2;
         const long long m_class = static_cast<long long>(c->n) * hh * hw;
         tile_box(hw, hh, &P.box_w, &P.box_h, &P.box_n);
-        bn = pick_bn(L.ktap, m_class);
+        bn = pick_bn(L.ktap, m_class, false);
         if (int rc = make_tmap_2d(&tm, w_dgrad, rup(L.ktap, 128), L.kd, L.kd, bn)) return rc;
         // The classes write disjoint pixels.  When one class does not fill the GPU (low-resolution layers) the four launches
         // run concurrently: fork onto three internal streams after an event on `st`, join before returning (also valid

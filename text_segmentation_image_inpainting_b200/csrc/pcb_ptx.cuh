@@ -135,10 +135,19 @@ template <int TA, int TB> __device__ __forceinline__ void wgmma_m64n128(float (&
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(a_desc), "l"(b_desc), "n"(TA), "n"(TB));
 }
+// N = 256 is issued as two m64n128 halves (columns [0, 128) into d[0..63], [128, 256) into d[64..127]) over a K-major B tile
+// whose rows are 128 bytes apart, so the second half starts 128 rows = 16 KB further.  One m64n256 instruction would need
+// ~154 registers at once, and ptxas checks an instruction against the kernel's launch register limit (128 at 512 threads)
+// even inside a setmaxnreg region; the accumulators themselves may exceed it there.
 template <int N, int TA, int TB> __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc) {
     if constexpr (N == 32) wgmma_m64n32<TA, TB>(d, a_desc, b_desc);
     else if constexpr (N == 64) wgmma_m64n64<TA, TB>(d, a_desc, b_desc);
-    else { static_assert(N == 128, "wgmma tile width"); wgmma_m64n128<TA, TB>(d, a_desc, b_desc); }
+    else if constexpr (N == 128) wgmma_m64n128<TA, TB>(d, a_desc, b_desc);
+    else {
+        static_assert(N == 256 && TB == 0, "wgmma tile width");
+        wgmma_m64n128<TA, TB>(*reinterpret_cast<float (*)[64]>(&d[0]), a_desc, b_desc);
+        wgmma_m64n128<TA, TB>(*reinterpret_cast<float (*)[64]>(&d[64]), a_desc, b_desc + (16384 >> 4));
+    }
 }
 // ---------------------------------------------------------------- register reallocation (per warpgroup)
 // setmaxnreg: all four warps of a warpgroup execute it (.sync.aligned).  dec returns registers to the CTA's pool, inc blocks

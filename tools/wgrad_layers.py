@@ -34,11 +34,8 @@ def card():
         return torch.cuda.get_device_name(0) + " (nvidia-smi unavailable)"
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--json", default=None)
-    args = ap.parse_args()
+def measure(reps):
+    """(family, layer label, call index) -> (median ms over `reps` profiled eager steps, FLOPs), in call order"""
     dev = torch.device("cuda:0")
     lib = _lib.load()
     torch.manual_seed(0)
@@ -50,7 +47,7 @@ def main():
     torch.cuda.synchronize()
     times = collections.defaultdict(list)      # (family, layer label, call index) -> [ms per rep]
     work = {}
-    for _ in range(args.reps):
+    for _ in range(reps):
         rec = []
         ops.set_profile(rec)
         ts._fwd_bwd(x, m)
@@ -66,23 +63,35 @@ def main():
             seen[(fam, label)] += 1
             times[key].append(s.elapsed_time(e))
             work[key] = 2.0 * g.n * g.ho * g.wo * g.cout * (g.cin // g.groups) * g.kh * g.kw
-    rows = [(k, statistics.median(v), work[k]) for k, v in times.items()]
+    return [(k, statistics.median(v), work[k]) for k, v in times.items()]
+
+
+def report(rows, families, json_path=None):
+    """print the per-layer table of `families` and every family's total (optionally also as JSON)"""
     print(f"card: {card()}")
-    print(f"{'layer (tc_wgrad)':40s} {'GFLOP':>8s} {'ms':>8s} {'TFLOP/s':>8s}")
-    for (fam, label, i), ms, fl in rows:
-        if fam == "tc_wgrad":
-            print(f"{label:40s} {fl / 1e9:8.2f} {ms:8.3f} {fl / 1e9 / ms:8.1f}")
+    for want in families:
+        print(f"{'layer (' + want + ')':40s} {'GFLOP':>8s} {'ms':>8s} {'TFLOP/s':>8s}")
+        for (fam, label, i), ms, fl in rows:
+            if fam == want:
+                print(f"{label:40s} {fl / 1e9:8.2f} {ms:8.3f} {fl / 1e9 / ms:8.1f}")
     fams = collections.defaultdict(lambda: [0.0, 0.0, 0])
     for (fam, _label, _i), ms, fl in rows:
         f = fams[fam]
         f[0] += fl; f[1] += ms; f[2] += 1
     for fam, (fl, ms, n) in sorted(fams.items(), key=lambda kv: -kv[1][1]):
         print(f"== {fam:12s} launches={n:3d} {fl / 1e9:8.1f} GFLOP {ms:8.3f} ms {fl / 1e9 / max(ms, 1e-9):8.1f} TFLOP/s")
-    if args.json:
-        with open(args.json, "w") as f:
+    if json_path:
+        with open(json_path, "w") as f:
             json.dump({"card": card(), "rows": [{"family": k[0], "layer": k[1], "call": k[2], "ms": ms, "gflop": fl / 1e9}
                                                 for k, ms, fl in rows]}, f, indent=1)
 
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    report(measure(args.reps), ("tc_wgrad",), args.json)
 
 if __name__ == "__main__":
     main()
