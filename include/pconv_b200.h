@@ -254,6 +254,39 @@ int pcb_scse_backward(const void *gy, const void *x, const float *cse, const flo
 int pcb_seg_mask_postprocess(const void *logits, int dtype, int n, int h, int w, int cstride, int h_valid, int w_valid, int oh,
                              int ow, uint8_t *out, pcb_stream_t stream);
 
+/* ---- inpainting training data (ImageInpaintingData.process_images, Dataloader.py:110-162) -------------------------------
+ * One decoded source per image: RGB uint8 [h][rgb_stride] (3 bytes per pixel) and the text mask uint8 [h][mask_stride]. */
+typedef struct {
+    const uint8_t *rgb;
+    const uint8_t *mask;
+    int32_t h, w, rgb_stride, mask_stride;
+} pcb_inpaint_src;
+/* What one image draws: the crop box (RandomResizedCrop.get_params: top i, left j, height h, width w), the RandomGrayscale flag
+ * and random_masks' strokes in output pixels (lines x0, y0, x1, y1, width; ellipses x0, y0, x1, y1 with inclusive corners). */
+typedef struct {
+    int32_t top, left, height, width;
+    int32_t gray;
+    int32_t nlines, nellipses;
+    int32_t lines[5][5];
+    int32_t ellipses[5][4];
+} pcb_inpaint_params;
+/* Host-side check of a staged batch (h_srcs, h_params: HOST copies; h_params may be NULL): 1..cap_n images, each within the
+ * cap_h x cap_w capacity, row strides large enough, crop boxes inside their sources, stroke counts 0..5.  The capacity may be
+ * at most 8x the output size `out`. */
+int pcb_inpaint_validate(const pcb_inpaint_src *h_srcs, const pcb_inpaint_params *h_params, int n, int cap_n, int cap_h, int cap_w,
+                         int out);
+/* Draw the parameters of n <= 1024 images on the device (Philox4x32-10, key = rng[0], counter = (slot, image, rng[1])) and
+ * advance rng[1]: RandomResizedCrop.get_params(scale=(0.5, 2), ratio=(3/4, 4/3)), RandomGrayscale(0.4) and, if `strokes`,
+ * random_masks(size=out, offset=10).  srcs, rng, params: device memory. */
+int pcb_inpaint_sample(const pcb_inpaint_src *srcs, int n, int out, int strokes, uint64_t *rng, pcb_inpaint_params *params,
+                       pcb_stream_t stream);
+/* process_images for a batch from device-resident sources and parameters, two launches: Pillow-exact bicubic crop + resize of
+ * image and text mask, the strokes (if `strokes`), mask > 0.4 * 255, cv2.dilate(10x10), the grayscale flag, ToTensor and
+ * clean * (1 - mask).  tmp: uint8 [n][cap_h][out][4] scratch.  Outputs: corrupted [n][out][out][8] NHWC in `dtype` (channels
+ * 3..7 zero), mask_plane uint8 [n][out][out] (1 = valid), clean fp32 [n][3][out][out].  Grids depend on n, cap_h and out only. */
+int pcb_inpaint_prepare(const pcb_inpaint_src *srcs, const pcb_inpaint_params *params, int n, int cap_h, int cap_w, int out,
+                        int strokes, uint8_t *tmp, void *corrupted, int dtype, uint8_t *mask_plane, float *clean, pcb_stream_t stream);
+
 /* ---- loss / optimiser used by the benchmark step (SURVEY 8d: loss = out.abs().mean()) ------ */
 int pcb_l1_mean_forward(const void *x, int dtype, long long numel, float *loss /* device scalar, overwritten */,
                         double *scratch /* device, 1 double */, pcb_stream_t stream);

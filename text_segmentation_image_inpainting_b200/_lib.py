@@ -83,6 +83,10 @@ _SIGS = {
     "pcb_scse_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_ll, c_int, c_void_p]),
     "pcb_scse_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_ll,
                                   c_int, c_void_p]),
+    "pcb_inpaint_validate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int]),
+    "pcb_inpaint_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "pcb_inpaint_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                    c_void_p]),
     "pcb_l1_mean_forward": (c_int, [c_void_p, c_int, c_ll, c_void_p, c_void_p, c_void_p]),
     "pcb_l1_mean_backward": (c_int, [c_void_p, c_int, c_ll, c_float, c_void_p, c_void_p]),
     "pcb_sgd_step": (c_int, [c_void_p, c_void_p, c_void_p, c_ll, c_float, c_float, c_float, c_int, c_int, c_void_p]),

@@ -1,0 +1,359 @@
+// inpaint_data.cu -- the inpainting data path (ImageInpaintingData.process_images, Dataloader.py:110-132) for a batch, in
+// three launches:
+//   1. inpaint_sample_kernel: one thread per image draws the crop box (RandomResizedCrop.get_params), the grayscale flag and
+//      the strokes (random_masks) from Philox4x32-10; seed and step counter live in device memory and the kernel advances the
+//      counter, so every graph replay draws fresh parameters.  Skipped when the caller supplies parameters.
+//   2. inpaint_hpass_kernel: Pillow's horizontal bicubic pass over every row of each image's crop box, RGB and text mask
+//      together, into a uint8 RGBM intermediate.
+//   3. inpaint_fused_kernel: per 32x32 output tile, the vertical pass over the tile plus the 9-pixel dilation halo, the strokes,
+//      the threshold, the 10x10 dilation (separable max in shared memory), grayscale, /255, x mask and the three stores.
+// Grids are sized from the batcher's capacity (largest source), so one captured graph serves any mix of source sizes.
+// The resampler follows Pillow's fixed-point 8-bit path bit for bit: the weights are computed in double with explicitly
+// rounded operations (no FMA contraction, which Pillow's x86-64 build does not do either).
+#include "pcb_common.cuh"
+
+#define ST static_cast<cudaStream_t>(stream)
+#define PCB_API extern "C" __attribute__((visibility("default")))
+
+namespace {
+
+constexpr int KMAX = 33;      // taps of a bicubic window at scale 8 (2 * ceil(2 * 8) + 1): box / out <= 8
+constexpr int PB = 22;        // Pillow's PRECISION_BITS for 8-bit images
+constexpr int HX = 128;       // horizontal pass: output columns per block (one per thread)
+constexpr int HROWS = 16;     // horizontal pass: box rows per block
+constexpr int T = 32;         // fused kernel: output tile edge
+constexpr int HT = T + 9;     // tile + dilation halo (5 rows / columns before, 4 after: cv2's anchor of a 10x10 kernel)
+
+__device__ __forceinline__ double bicubic(double x) {
+    const double a = -0.5;
+    if (x < 0.0) x = -x;
+    if (x < 1.0) return __dadd_rn(__dmul_rn(__dmul_rn(__dsub_rn(__dmul_rn(a + 2.0, x), a + 3.0), x), x), 1.0);
+    if (x < 2.0) return __dmul_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, 5.0), x), 8.0), x), 4.0), a);
+    return 0.0;
+}
+
+// Pillow's precompute_coeffs + normalize_coeffs_8bpc for output index xx of a box of `insize` input pixels resampled to
+// `outsize`: writes the integer weights to k[0], k[stride], ... and returns the first tap; *count = number of taps.
+__device__ int pil_coeffs(int xx, int insize, int outsize, int *k, int stride, int *count) {
+    const double scale = __ddiv_rn(static_cast<double>(insize), static_cast<double>(outsize));
+    const double fs = scale < 1.0 ? 1.0 : scale;
+    const double support = __dmul_rn(2.0, fs), ss = __ddiv_rn(1.0, fs);
+    const double center = __dmul_rn(static_cast<double>(xx) + 0.5, scale);
+    int xmin = static_cast<int>(__dadd_rn(__dsub_rn(center, support), 0.5));
+    if (xmin < 0) xmin = 0;
+    int xmax = static_cast<int>(__dadd_rn(__dadd_rn(center, support), 0.5));
+    if (xmax > insize) xmax = insize;
+    xmax -= xmin;
+    if (xmax > KMAX) xmax = KMAX;                    // unreachable for box / out <= 8 (checked on the host)
+    double w[KMAX];
+    double ww = 0.0;
+#pragma unroll
+    for (int x = 0; x < KMAX; ++x) {
+        if (x < xmax) {
+            w[x] = bicubic(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(x + xmin), center), 0.5), ss));
+            ww = __dadd_rn(ww, w[x]);
+        }
+    }
+#pragma unroll
+    for (int x = 0; x < KMAX; ++x) {
+        if (x < xmax) {
+            const double v = ww != 0.0 ? __ddiv_rn(w[x], ww) : w[x];
+            const double s = __dmul_rn(v, static_cast<double>(1 << PB));
+            k[x * stride] = v < 0 ? static_cast<int>(__dadd_rn(-0.5, s)) : static_cast<int>(__dadd_rn(0.5, s));
+        }
+    }
+    *count = xmax;
+    return xmin;
+}
+
+__device__ __forceinline__ int clip8(int acc) {
+    acc >>= PB;
+    return acc < 0 ? 0 : (acc > 255 ? 255 : acc);
+}
+
+__device__ __forceinline__ bool source_ok(const pcb_inpaint_src &s, const pcb_inpaint_params &p, int cap_h, int cap_w) {
+    return s.h >= 1 && s.w >= 1 && s.h <= cap_h && s.w <= cap_w && p.top >= 0 && p.left >= 0 && p.height >= 1 && p.width >= 1 &&
+           p.top + p.height <= s.h && p.left + p.width <= s.w;
+}
+
+// ------------------------------------------------------------------------------------------------ 1. parameter sampler
+__device__ __forceinline__ uint4 philox(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+        k0 += 0x9E3779B9u;
+        k1 += 0xBB67AE85u;
+    }
+    return c;
+}
+
+struct Draws {
+    uint32_t img, c_lo, c_hi, k0, k1;
+    // uniform of slot s in [0, 1), 24 bits: word s % 4 of philox(counter = (s / 4, image, step lo, step hi), key = seed)
+    __device__ float u(int s) const {
+        const uint4 r = philox(make_uint4(static_cast<uint32_t>(s >> 2), img, c_lo, c_hi), k0, k1);
+        const int l = s & 3;
+        const uint32_t w = l == 0 ? r.x : (l == 1 ? r.y : (l == 2 ? r.z : r.w));
+        return static_cast<float>(w >> 8) * 5.9604644775390625e-8f;
+    }
+    __device__ int randint(int s, int lo, int hi) const {   // lo..hi inclusive
+        return lo + static_cast<int>(__dmul_rn(static_cast<double>(u(s)), static_cast<double>(hi - lo + 1)));
+    }
+};
+
+__global__ void __launch_bounds__(1024) inpaint_sample_kernel(const pcb_inpaint_src *__restrict__ srcs, int n, int out, int strokes,
+                                                              unsigned long long *rng, pcb_inpaint_params *__restrict__ params) {
+    const int t = threadIdx.x;
+    const unsigned long long seed = rng[0], step = rng[1];
+    __syncthreads();
+    if (t == 0) rng[1] = step + 1;
+    if (t >= n) return;
+    const Draws d{static_cast<uint32_t>(t), static_cast<uint32_t>(step), static_cast<uint32_t>(step >> 32), static_cast<uint32_t>(seed),
+                  static_cast<uint32_t>(seed >> 32)};
+    const int H = srcs[t].h, W = srcs[t].w;
+    pcb_inpaint_params &p = params[t];
+    p = pcb_inpaint_params{};
+    // RandomResizedCrop.get_params(scale=(0.5, 2.0), ratio=(3/4, 4/3)); slots 4a..4a+3 of attempt a: scale, log-aspect, top, left
+    const float lr0 = -0.28768208622932434f, span = 0.5753642320632935f;    // float32 log(3/4), log(4/3) - log(3/4) as torch has them
+    const double area = static_cast<double>(H) * static_cast<double>(W);
+    bool found = false;
+    for (int a = 0; a < 10 && !found; ++a) {
+        const float s = __fadd_rn(0.5f, __fmul_rn(1.5f, d.u(4 * a)));
+        const float r = __fadd_rn(lr0, __fmul_rn(span, d.u(4 * a + 1)));
+        const double target = __dmul_rn(area, static_cast<double>(s));
+        const double aspect = static_cast<double>(static_cast<float>(exp(static_cast<double>(r))));
+        const int w = static_cast<int>(rint(__dsqrt_rn(__dmul_rn(target, aspect))));
+        const int h = static_cast<int>(rint(__dsqrt_rn(__ddiv_rn(target, aspect))));
+        if (0 < w && w <= W && 0 < h && h <= H) {
+            p.top = d.randint(4 * a + 2, 0, H - h);
+            p.left = d.randint(4 * a + 3, 0, W - w);
+            p.height = h;
+            p.width = w;
+            found = true;
+        }
+    }
+    if (!found) {                                    // the centre-crop fallback
+        const double in_ratio = __ddiv_rn(static_cast<double>(W), static_cast<double>(H));
+        int w = W, h = H;
+        if (in_ratio < 0.75) h = static_cast<int>(rint(__ddiv_rn(static_cast<double>(W), 0.75)));
+        else if (in_ratio > 4.0 / 3.0) w = static_cast<int>(rint(__dmul_rn(static_cast<double>(H), 4.0 / 3.0)));
+        p.top = (H - h) / 2;
+        p.left = (W - w) / 2;
+        p.height = h;
+        p.width = w;
+    }
+    p.gray = static_cast<double>(d.u(40)) < 0.4 ? 1 : 0;            // RandomGrayscale(p=0.4)
+    if (strokes) {                                                   // random_masks(size=out, offset=10)
+        const int off = 10;
+        p.nlines = d.randint(41, 1, 5);
+        for (int k = 0; k < p.nlines; ++k) {
+            const int b = 42 + 5 * k;
+            const int x0 = d.randint(b, off, out - 1), y0 = d.randint(b + 1, off, out - 1);
+            const int x1 = min(max(d.randint(b + 2, off, out - 1), x0 - 75), x0 + 75);
+            const int y1 = min(max(d.randint(b + 3, off, out - 1), y0 - 75), y0 + 75);
+            p.lines[k][0] = x0; p.lines[k][1] = y0; p.lines[k][2] = x1; p.lines[k][3] = y1;
+            p.lines[k][4] = d.randint(b + 4, 15, 20);
+        }
+        p.nellipses = d.randint(67, 1, 5);
+        for (int k = 0; k < p.nellipses; ++k) {
+            const int b = 68 + 4 * k;
+            int c0 = d.randint(b, off, out - off - 1), c1 = d.randint(b + 1, off, out - off - 1);
+            if (c1 < c0) { const int tmp = c0; c0 = c1; c1 = tmp; }                // cords.sort(): x0 <= y0
+            p.ellipses[k][0] = c0; p.ellipses[k][1] = c1;
+            p.ellipses[k][2] = min(max(c0 + d.randint(b + 2, 20, 69), off), out - off);
+            p.ellipses[k][3] = min(max(c1 + d.randint(b + 3, 20, 69), off), out - off);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ 2. horizontal pass
+__global__ void __launch_bounds__(HX) inpaint_hpass_kernel(const pcb_inpaint_src *__restrict__ srcs, const pcb_inpaint_params *__restrict__ params,
+                                                           int cap_h, int cap_w, int out, uchar4 *__restrict__ tmp) {
+    __shared__ int kk[KMAX * HX];
+    const int n = blockIdx.z, x = blockIdx.x * HX + threadIdx.x, row0 = blockIdx.y * HROWS;
+    const pcb_inpaint_src s = srcs[n];
+    const pcb_inpaint_params &p = params[n];
+    const int top = p.top, left = p.left, bh = p.height, bw = p.width;
+    if (row0 >= bh || x >= out || !source_ok(s, p, cap_h, cap_w)) return;
+    int nt;
+    const int xmin = pil_coeffs(x, bw, out, kk + threadIdx.x, HX, &nt);     // this thread's column only: no barrier
+    const int rows = min(HROWS, bh - row0);
+    for (int r = row0; r < row0 + rows; ++r) {
+        const uint8_t *pr = s.rgb + static_cast<size_t>(top + r) * s.rgb_stride + static_cast<size_t>(left + xmin) * 3;
+        const uint8_t *pm = s.mask + static_cast<size_t>(top + r) * s.mask_stride + left + xmin;
+        int a0 = 1 << (PB - 1), a1 = a0, a2 = a0, a3 = a0;
+        for (int t = 0; t < nt; ++t) {
+            const int k = kk[t * HX + threadIdx.x];
+            a0 += static_cast<int>(__ldg(pr + 3 * t)) * k;
+            a1 += static_cast<int>(__ldg(pr + 3 * t + 1)) * k;
+            a2 += static_cast<int>(__ldg(pr + 3 * t + 2)) * k;
+            a3 += static_cast<int>(__ldg(pm + t)) * k;
+        }
+        tmp[(static_cast<size_t>(n) * cap_h + r) * out + x] = make_uchar4(clip8(a0), clip8(a1), clip8(a2), clip8(a3));
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ 3. fused tail
+// Stroke rules (documented in DESIGN 4.8; numpy restatement in oracle/inpaint_data.py), exact integer arithmetic:
+//   line (x0, y0, x1, y1, w): 0 <= <p - p0, d> <= |d|^2 and 4 cross(p - p0, d)^2 <= w^2 |d|^2; zero length: the pixel (x0, y0)
+//   ellipse (x0, y0, x1, y1): (2x - x0 - x1)^2 B^2 + (2y - y0 - y1)^2 A^2 <= A^2 B^2, A = x1 - x0 + 1, B = y1 - y0 + 1
+__device__ bool in_stroke(const pcb_inpaint_params &p, int x, int y) {
+    for (int k = 0; k < p.nlines; ++k) {
+        const long long x0 = p.lines[k][0], y0 = p.lines[k][1], dx = p.lines[k][2] - x0, dy = p.lines[k][3] - y0, w = p.lines[k][4];
+        const long long px = x - x0, py = y - y0;
+        if (dx == 0 && dy == 0) {
+            if (px == 0 && py == 0) return true;
+            continue;
+        }
+        const long long l2 = dx * dx + dy * dy, dot = px * dx + py * dy, cr = px * dy - py * dx;
+        if (dot >= 0 && dot <= l2 && 4 * cr * cr <= w * w * l2) return true;
+    }
+    for (int k = 0; k < p.nellipses; ++k) {
+        const long long x0 = p.ellipses[k][0], y0 = p.ellipses[k][1], x1 = p.ellipses[k][2], y1 = p.ellipses[k][3];
+        const long long A = x1 - x0 + 1, B = y1 - y0 + 1, ex = 2ll * x - x0 - x1, ey = 2ll * y - y0 - y1;
+        if (ex * ex * B * B + ey * ey * A * A <= A * A * B * B) return true;
+    }
+    return false;
+}
+
+template <typename TO>
+__global__ void __launch_bounds__(256) inpaint_fused_kernel(const pcb_inpaint_src *__restrict__ srcs, const pcb_inpaint_params *__restrict__ params,
+                                                            int cap_h, int cap_w, int out, int strokes, const uchar4 *__restrict__ tmp,
+                                                            TO *__restrict__ corrupted, uint8_t *__restrict__ plane, float *__restrict__ clean) {
+    __shared__ int vk[HT * KMAX];
+    __shared__ int vmin[HT], vcnt[HT];
+    __shared__ uint8_t hole[HT][HT];
+    __shared__ uint8_t rmax[HT][T];
+    __shared__ uchar4 rgb[T][T];
+    const int n = blockIdx.z, y0 = blockIdx.y * T, x0 = blockIdx.x * T, tid = threadIdx.x;
+    const pcb_inpaint_params &p = params[n];
+    const bool ok = source_ok(srcs[n], p, cap_h, cap_w);
+    const int bh = p.height;
+    if (tid < HT) {
+        const int yy = y0 - 5 + tid;
+        int cnt = 0, m = 0;
+        if (ok && yy >= 0 && yy < out) m = pil_coeffs(yy, bh, out, vk + tid * KMAX, 1, &cnt);
+        vmin[tid] = m;
+        vcnt[tid] = cnt;
+    }
+    __syncthreads();
+    // vertical pass over the tile + halo; the mask channel is thresholded (and stroked), RGB kept for the tile itself
+    const uchar4 *img = tmp + static_cast<size_t>(n) * cap_h * out;
+    for (int q = tid; q < HT * HT; q += blockDim.x) {
+        const int ly = q / HT, lx = q - ly * HT, gy = y0 - 5 + ly, gx = x0 - 5 + lx;
+        uint8_t h = 0;
+        if (ok && gy >= 0 && gy < out && gx >= 0 && gx < out) {
+            const uchar4 *col = img + static_cast<size_t>(vmin[ly]) * out + gx;
+            const int *k = vk + ly * KMAX;
+            int a0 = 1 << (PB - 1), a1 = a0, a2 = a0, a3 = a0;
+            for (int t = 0; t < vcnt[ly]; ++t) {
+                const uchar4 v = col[static_cast<size_t>(t) * out];
+                a0 += v.x * k[t];
+                a1 += v.y * k[t];
+                a2 += v.z * k[t];
+                a3 += v.w * k[t];
+            }
+            h = clip8(a3) >= 103 || (strokes && in_stroke(p, gx, gy));     // mask > 0.4 * 255; strokes are drawn at 255
+            if (ly >= 5 && ly < 5 + T && lx >= 5 && lx < 5 + T) rgb[ly - 5][lx - 5] = make_uchar4(clip8(a0), clip8(a1), clip8(a2), 0);
+        }
+        hole[ly][lx] = h;
+    }
+    __syncthreads();
+    for (int q = tid; q < HT * T; q += blockDim.x) {                      // 10-wide row max: columns x-5 .. x+4
+        const int ly = q / T, lx = q - ly * T;
+        uint8_t m = 0;
+#pragma unroll
+        for (int d = 0; d < 10; ++d) m |= hole[ly][lx + d];
+        rmax[ly][lx] = m;
+    }
+    __syncthreads();
+    const size_t plane_px = static_cast<size_t>(out) * out;
+    for (int q = tid; q < T * T; q += blockDim.x) {                       // 10-high column max, then the per-pixel tail
+        const int ly = q / T, lx = q - ly * T, gy = y0 + ly, gx = x0 + lx;
+        if (gy >= out || gx >= out) continue;
+        uint8_t m = ok ? 0 : 1;
+#pragma unroll
+        for (int d = 0; d < 10; ++d) m |= rmax[ly + d][lx];
+        uchar4 c = ok ? rgb[ly][lx] : make_uchar4(0, 0, 0, 0);
+        if (p.gray) {
+            const unsigned l = (19595u * c.x + 38470u * c.y + 7471u * c.z + 0x8000u) >> 16;
+            c.x = c.y = c.z = static_cast<unsigned char>(l);
+        }
+        const float binary = __fsub_rn(1.f, __fdiv_rn(m ? 255.f : 0.f, 255.f));   // 1 - ToTensor(mask)
+        const float f[3] = {__fdiv_rn(static_cast<float>(c.x), 255.f), __fdiv_rn(static_cast<float>(c.y), 255.f),
+                            __fdiv_rn(static_cast<float>(c.z), 255.f)};
+        const size_t pix = static_cast<size_t>(gy) * out + gx;
+        float v[8] = {__fmul_rn(f[0], binary), __fmul_rn(f[1], binary), __fmul_rn(f[2], binary), 0.f, 0.f, 0.f, 0.f, 0.f};
+        Vec8<TO>::store(corrupted + (static_cast<size_t>(n) * plane_px + pix) * 8, v);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) clean[(static_cast<size_t>(n) * 3 + ch) * plane_px + pix] = f[ch];
+        plane[static_cast<size_t>(n) * plane_px + pix] = m ? 0 : 1;
+    }
+}
+
+int validate(const pcb_inpaint_src *h_srcs, const pcb_inpaint_params *h_params, int n, int cap_n, int cap_h, int cap_w, int out) {
+    PCB_CHECK(h_srcs && n >= 1 && n <= cap_n, "pcb_inpaint_validate: %d images for a batch of %d", n, cap_n);
+    for (int i = 0; i < n; ++i) {
+        const pcb_inpaint_src &s = h_srcs[i];
+        PCB_CHECK(s.rgb && s.mask, "pcb_inpaint_validate: image %d has a null source", i);
+        PCB_CHECK(s.h >= 1 && s.w >= 1 && s.h <= cap_h && s.w <= cap_w, "pcb_inpaint_validate: image %d is %dx%d, capacity %dx%d", i, s.h,
+                  s.w, cap_h, cap_w);
+        PCB_CHECK(s.rgb_stride >= 3 * s.w && s.mask_stride >= s.w, "pcb_inpaint_validate: image %d row strides %d / %d too small", i,
+                  s.rgb_stride, s.mask_stride);
+        if (!h_params) continue;
+        const pcb_inpaint_params &p = h_params[i];
+        PCB_CHECK(p.top >= 0 && p.left >= 0 && p.height >= 1 && p.width >= 1 && p.top + p.height <= s.h && p.left + p.width <= s.w,
+                  "pcb_inpaint_validate: image %d crop box (%d, %d, %d, %d) is not inside its %dx%d source", i, p.top, p.left, p.height,
+                  p.width, s.h, s.w);
+        PCB_CHECK(p.height <= 8 * out && p.width <= 8 * out, "pcb_inpaint_validate: image %d crop box downscales more than 8x", i);
+        PCB_CHECK((p.gray == 0 || p.gray == 1) && p.nlines >= 0 && p.nlines <= 5 && p.nellipses >= 0 && p.nellipses <= 5,
+                  "pcb_inpaint_validate: image %d has a bad grayscale flag or stroke count", i);
+        for (int k = 0; k < 5; ++k) {
+            for (int c = 0; c < 5; ++c)
+                PCB_CHECK(p.lines[k][c] >= -4 * out && p.lines[k][c] <= 4 * out, "pcb_inpaint_validate: image %d line %d out of range", i, k);
+            for (int c = 0; c < 4; ++c)
+                PCB_CHECK(p.ellipses[k][c] >= -4 * out && p.ellipses[k][c] <= 4 * out, "pcb_inpaint_validate: image %d ellipse %d out of range",
+                          i, k);
+        }
+    }
+    return 0;
+}
+
+}  // namespace
+
+PCB_API int pcb_inpaint_validate(const pcb_inpaint_src *h_srcs, const pcb_inpaint_params *h_params, int n, int cap_n, int cap_h, int cap_w,
+                                 int out) {
+    PCB_CHECK(out >= 16 && out <= 4096 && cap_h <= 8 * out && cap_w <= 8 * out,
+              "pcb_inpaint_validate: output %d and capacity %dx%d (at most 8x the output)", out, cap_h, cap_w);
+    return validate(h_srcs, h_params, n, cap_n, cap_h, cap_w, out);
+}
+
+PCB_API int pcb_inpaint_sample(const pcb_inpaint_src *srcs, int n, int out, int strokes, uint64_t *rng, pcb_inpaint_params *params,
+                               pcb_stream_t stream) {
+    PCB_CHECK(srcs && rng && params && n >= 1 && n <= 1024 && out >= 32, "pcb_inpaint_sample: bad arguments (1..1024 images, out >= 32)");
+    inpaint_sample_kernel<<<1, (n + 31) / 32 * 32, 0, ST>>>(srcs, n, out, strokes, reinterpret_cast<unsigned long long *>(rng), params);
+    PCB_LAUNCH_CHECK();
+    return 0;
+}
+
+PCB_API int pcb_inpaint_prepare(const pcb_inpaint_src *srcs, const pcb_inpaint_params *params, int n, int cap_h, int cap_w, int out,
+                                int strokes, uint8_t *tmp, void *corrupted, int dtype, uint8_t *mask_plane, float *clean, pcb_stream_t stream) {
+    PCB_CHECK(srcs && params && tmp && corrupted && mask_plane && clean && (dtype == PCB_F32 || dtype == PCB_BF16),
+              "pcb_inpaint_prepare: bad arguments");
+    PCB_CHECK(n >= 1 && n <= 65535 && out >= 16 && out <= 4096 && cap_h >= 1 && cap_w >= 1 && cap_h <= 8 * out && cap_w <= 8 * out,
+              "pcb_inpaint_prepare: %d images, output %d, capacity %dx%d (at most 8x the output)", n, out, cap_h, cap_w);
+    const dim3 hgrid((out + HX - 1) / HX, (cap_h + HROWS - 1) / HROWS, n);
+    inpaint_hpass_kernel<<<hgrid, HX, 0, ST>>>(srcs, params, cap_h, cap_w, out, reinterpret_cast<uchar4 *>(tmp));
+    PCB_LAUNCH_CHECK();
+    const dim3 fgrid((out + T - 1) / T, (out + T - 1) / T, n);
+    if (dtype == PCB_BF16)
+        inpaint_fused_kernel<bf16><<<fgrid, 256, 0, ST>>>(srcs, params, cap_h, cap_w, out, strokes, reinterpret_cast<const uchar4 *>(tmp),
+                                                          static_cast<bf16 *>(corrupted), mask_plane, clean);
+    else
+        inpaint_fused_kernel<float><<<fgrid, 256, 0, ST>>>(srcs, params, cap_h, cap_w, out, strokes, reinterpret_cast<const uchar4 *>(tmp),
+                                                           static_cast<float *>(corrupted), mask_plane, clean);
+    PCB_LAUNCH_CHECK();
+    return 0;
+}

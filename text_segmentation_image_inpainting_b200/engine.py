@@ -337,6 +337,46 @@ class TrainStep:
             torch.cuda.synchronize()
 
 
+class InpaintTrainStep(TrainStep):
+    """TrainStep whose step begins with the GPU data path (data.InpaintBatcher.prepare): the captured graph samples the crop
+    boxes, grayscale draws and strokes, resizes, masks and dilates on the device and then runs the training step on the result.
+    Per step the host only decodes, calls ``batcher.stage(samples)`` and ``step()``.
+
+    ``step(params)`` with explicit parameters needs ``use_graph=False`` (the graph holds the device sampler)."""
+
+    def __init__(self, net: torch.nn.Module, batcher, **kwargs):
+        super().__init__(net, compute_dtype=batcher.dtype, **kwargs)
+        self.batcher = batcher
+        self._params = None
+
+    def _forward_loss(self, x, mask):
+        xin, hm, _ = self.batcher.prepare(self._params)
+        return ops.l1_mean(self.net((xin, hm)))
+
+    def warmup_and_capture(self, eager_warmup=2):
+        super().warmup_and_capture(torch.empty(0, device=self.batcher.device), None, eager_warmup=eager_warmup)
+
+    def step(self, params=None) -> torch.Tensor:
+        """One step on the staged batch.  Returns the (device) loss."""
+        if self.graph is None:
+            self._params = params
+            try:
+                loss = self._step(None, None, self.first)
+            finally:
+                self._params = None
+            self.first = False
+            return loss
+        if params is not None:
+            raise ValueError("explicit parameters need use_graph=False: the captured step draws its own")
+        self.batcher.activate()
+        self.graph.replay()
+        self.batcher.release()
+        if self.graph_update is not None:
+            self._allreduce()
+            self.graph_update.replay()
+        return self.static_loss
+
+
 class SegTrainStep(TrainStep):
     """The same step for the dense segmentation networks (models/text_segmentation.py: `net(x)`, no masks): BASELINE.json
     configs[1] (TextSegament, batch 8) and configs[3] (XceptionTextSegment, batch 16, bf16).  `mask` is ignored."""
