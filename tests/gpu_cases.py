@@ -113,9 +113,9 @@ CONV_CASES = {
     "tma_k5_s2_halo_dgrad_w256": (64, 64, 5, 2, 2, 1, 1, False, True, 1, 8, 256, BF, "uniform", "pc"),
     "tma_k3_s2_halo_dgrad_w256": (64, 128, 3, 2, 1, 1, 1, True, True, 1, 4, 256, BF, "uniform", "pc"),
     "tma_k7_s2_64_64": (64, 64, 7, 2, 3, 1, 1, False, True, 2, 16, 32, BF, "uniform", "pc"),
-    # few output tiles: the K blocks of a tile are split across CTAs (fp32 partial sums + finish kernel)
-    "tma_splitk_k3_256_128_8x8": (256, 128, 3, 1, 1, 1, 1, True, False, 2, 8, 8, BF, "uniform", "pc"),
-    "tma_splitk_k3_320_64_two_8x16": (320, 64, 3, 1, 1, 1, 1, False, False, 1, 8, 16, BF, "two64", "pc"),
+    # few output tiles: grids far smaller than the GPU, narrowed N tiles
+    "tma_few_tiles_k3_256_128_8x8": (256, 128, 3, 1, 1, 1, 1, True, False, 2, 8, 8, BF, "uniform", "pc"),
+    "tma_few_tiles_k3_320_64_two_8x16": (320, 64, 3, 1, 1, 1, 1, False, False, 1, 8, 16, BF, "two64", "pc"),
 }
 PADDED_X = {"tc_stem_rowpack_k7_s2", "tc_stem_s2d_k7_s2_tma", "tc_rowpack_k5_d2_cin4"}
 
@@ -153,15 +153,6 @@ def make_mask(kind, n, cin, h, w, seed):
 
 
 def conv_case(tag, dev, dump_dir=None):
-    if "splitk" in tag:
-        os.environ["PCB_SPLITK"] = "1"
-    try:
-        return _conv_case(tag, dev, dump_dir)
-    finally:
-        os.environ.pop("PCB_SPLITK", None)
-
-
-def _conv_case(tag, dev, dump_dir=None):
     """fwd + bwd of one PartialConv* module on the GPU vs the oracle.  Returns dict of errors + flags."""
     from text_segmentation_image_inpainting_b200 import _lib, ops
     from text_segmentation_image_inpainting_b200.models import partial_convolution as PC
@@ -225,21 +216,12 @@ LAZYCAT_CASES = {"lc_128up_64_to_64": (128, 64, 64, False), "lc_256up_64_to_128"
                  "lc_tail_64up_3_to_3": (64, 3, 3, True), "lc_64up_8_to_16": (64, 8, 16, True),
                  # TMA-fed path: the upsampled source is materialised in the workspace; second one uses row-halo tiles
                  "lc_tma_128up_64_to_64": (128, 64, 64, False, (2, 32, 32)), "lc_tma_halo_tail_64up_3_to_3": (64, 3, 3, True, (1, 8, 128)),
-                 "lc_tma_splitk_256up_64_to_128": (256, 64, 128, False, (2, 8, 8)),
+                 "lc_tma_few_tiles_256up_64_to_128": (256, 64, 128, False, (2, 8, 8)),
                  # kernel-to-row tails (conv_k2r.cu) with the 1x1 problem on the TMA-fed kernels; 4-channel second part, 2 outputs
                  "lc_k2r_tail_64up_3_to_3": (64, 3, 3, True, (2, 32, 64)), "lc_k2r_64up_4_to_2": (64, 4, 2, False, (2, 32, 32))}
 
 
 def lazycat_case(tag, dev, dtype=BF):
-    if "splitk" in tag:
-        os.environ["PCB_SPLITK"] = "1"
-    try:
-        return _lazycat_case(tag, dev, dtype)
-    finally:
-        os.environ.pop("PCB_SPLITK", None)
-
-
-def _lazycat_case(tag, dev, dtype=BF):
     """PartialConv over LazyCat([up2x(a), b]) with HoleMask cat([mask_a.upsampled(), mask_b]) vs the oracle on the
     materialised cat (image_inpainting.py:183-186)."""
     import torch.nn.functional as F

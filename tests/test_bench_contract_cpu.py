@@ -32,7 +32,7 @@ def test_ncu_family_classifier_knows_the_shipped_kernels():
     u = "void <unnamed>::"
     assert family(u + "pconv_tc_tma_kernel<64, 0, 1, 0>(<unnamed>::TcParams, CUtensorMap_st)") == "tc_fwd"
     assert family(u + "pconv_tc_tma_kernel<(int)256, (int)1, (bool)0, (bool)0>(TcParams)") == "tc_dgrad"
-    assert family(u + "pconv_tc_sp_kernel<128, 1>(TcParams)") == "tc_dgrad"
+    assert family(u + "pconv_tc_sp_kernel<(int)64>(<unnamed>::TcParams, <unnamed>::SpTable, CUtensorMap_st, CUtensorMap_st)") == "tc_dgrad"
     assert family(u + "pconv_tc_wgrad_tma_kernel<64, 4, 1>(WgParams)") == "tc_wgrad"
     assert family(u + "k2r_combine_kernel<3>(K2rParams)") == "tc_fwd"
     assert family(u + "k2r_dbuild_kernel<0, 3>(K2rParams)") == "tc_dgrad"

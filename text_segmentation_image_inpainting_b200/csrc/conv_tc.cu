@@ -83,18 +83,12 @@ struct TcParams {
     // dgrad gather source
     const bf16 *dc; int dc_cstride, dc_c8, dc_kext;
     int *abort_flag;
-    int l2pf;                 // TMA-fed fwd/dgrad: request the next tile's A boxes into L2 one tile ahead (PCB_TMA_L2_PREFETCH)
     // TMA-fed kernel: the 128 pixels of an M tile form the box {box_w, box_h, box_n} of the (x, y, image) pixel grid
     int box_w, box_h, box_n, stages, use_fix;
     int wk_base, wk_row, wk_col;   // weight-matrix K index of tap (a, b) of this launch: wk_base + a*wk_row + b*wk_col (+ part / block offset)
     // dgrad output addressing: the tile grid (h, w above) is every `sub`-th pixel of the full-resolution [fh, fw] gradient,
     // starting at (py, px) -- sub = 2 for the parity classes of a stride-2 layer, 1 otherwise
     int sub, py, px, fh, fw;
-    // split-K (layers with too few output tiles to fill the GPU): the 64-channel K blocks of every tap are dealt round-robin to
-    // `ksplit` CTAs per tile, which add their raw fp32 accumulators into `partial` [m_total][ncols]; a finish kernel applies
-    // the epilogue.  ksplit = 1: `partial` is null and the epilogue runs in the kernel.
-    int ksplit;
-    float *partial;
     // fused BatchNorm statistics (forward, MODE 0): per-channel sum / sum of squares of the bf16-ROUNDED outputs are accumulated
     // into bn_sums[0][co] / bn_sums[1][co] (doubles, pre-zeroed by the caller, row pitch bn_c = cout) -- the separate statistics
     // pass over y (nn.BatchNorm2d in training mode, partial_convolution.py:193-197) disappears.  null: off.
@@ -119,7 +113,7 @@ constexpr int EPI_STAT_SLICE = 512;
 constexpr int EPI_STAT_SQ = EPI_STAT_SLICE / 2;
 constexpr int EPI_STAT_SMEM_BYTES = EPI_WARPS * EPI_STAT_SLICE * 4;
 // TMA-fed kernels: the consumers finish the element math and stage bf16 [128 rows][BLOCK_N + 8] (a row is an odd number of
-// 16-byte units, so the epilogue warps' one-row-per-lane 16-byte loads are conflict-free); split-K stages raw fp32 partials
+// 16-byte units, so the epilogue warps' one-row-per-lane 16-byte loads are conflict-free)
 constexpr int bf16_pitch(int block_n) { return block_n + 8; }
 constexpr int bf16_stage_bytes(int block_n) { return BLOCK_M * bf16_pitch(block_n) * 2; }
 
@@ -201,10 +195,6 @@ __device__ __forceinline__ EpiRow tc_epi_row(const TcParams &P, int m, bool reno
         eh = eh * P.sub + P.py; ew = ew * P.sub + P.px;
         er.mo = (static_cast<long long>(en) * P.fh + eh) * P.fw + ew;
     }
-    if (MODE == 0 && er.rvalid && P.sub != 1) {  // sub-pixel class launch: the tile grid is every `sub`-th output pixel
-        en = m / (P.ho * P.wo); const int rem = m - en * P.ho * P.wo; eh = rem / P.wo; ew = rem - eh * P.wo;
-        er.mo = (static_cast<long long>(en) * P.fh + eh * P.sub + P.py) * P.fw + ew * P.sub + P.px;
-    }
     if (MODE == 0 && er.rvalid && renorm) {
         const float s = P.msum ? P.msum[er.mo] : 1.f;               // null: plain convolution (renormaliser 1)
         er.hole = (s == 0.f) && !P.no_guard;
@@ -225,22 +215,8 @@ __device__ __forceinline__ EpiRow tc_epi_row(const TcParams &P, int m, bool reno
 template <int BLOCK_N, int MODE>
 __device__ __forceinline__ void tc_epilogue(const TcParams &P, const EpiRow &er, const float *acc_row, int lane, int n0, float *s_stat,
                                             int cb, int ce, int sq_off) {
-                const int m = er.m;
                 const bool rvalid = er.rvalid, hole = er.hole;
                 const long long mo = er.mo;
-                if (P.partial != nullptr) {                // split-K: raw accumulators, reduced across CTAs with fp32 adds
-    #pragma unroll 1
-                    for (int c0 = cb; c0 < ce; c0 += 32) {
-                        uint32_t r[32];
-                        load_acc32(acc_row + c0, r);
-                        if (rvalid) {
-                            float *dst = P.partial + static_cast<long long>(m) * P.ncols + n0 + c0;
-    #pragma unroll
-                            for (int j = 0; j < 32; ++j) atomicAdd(dst + j, __uint_as_float(r[j]));
-                        }
-                    }
-                    return;
-                }
     #pragma unroll 1
                 for (int c0 = cb; c0 < ce; c0 += 32) {
                     uint32_t r[32];
@@ -746,7 +722,7 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
         }
         // this warpgroup's 64 rows: 8 groups of 8 rows further into the A stage
         const uint32_t a_rows = HALO ? 8u * HG * 16u : 64u * 128u;
-        float *s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
+        float *s_stat = (MODE == 0 && P.bn_sums != nullptr)
                             ? reinterpret_cast<float *>(smem_raw + (s_stat_addr - ptx::smem_u32(smem_raw))) : nullptr;
         const EpiRole<BLOCK_N> R(e);
         float *my_stat = s_stat ? s_stat + R.slice() * STAT_SLICE : nullptr;
@@ -891,11 +867,13 @@ __device__ __forceinline__ void tc_epilogue_bf16(const TcParams &P, const EpiRow
         }
         if (stats) {
             // per-channel sum and sum of squares of what was just stored (rows past the tensor contribute 0), 16 columns at a
-            // time: lane l ends up with column c0 + l
+            // time: lane l ends up with column c0 + l.  The values are read again from the staging row (the forward stores them
+            // unchanged) and the halves are not unrolled: holding o[] and both halves in registers makes the 64-register
+            // epilogue warps spill.
             const float live = er.rvalid ? 1.f : 0.f;
-            const __nv_bfloat162 *ob = reinterpret_cast<const __nv_bfloat162 *>(o);
+            const __nv_bfloat162 *ob = reinterpret_cast<const __nv_bfloat162 *>(srow + c0);
             float cs = 0.f, cq = 0.f;
-#pragma unroll
+#pragma unroll 1
             for (int h = 0; h < 2; ++h) {
                 float v[16];
 #pragma unroll
@@ -921,14 +899,12 @@ __device__ __forceinline__ void tc_epilogue_bf16(const TcParams &P, const EpiRow
 
 // epilogue warp w of the TMA-fed kernels: drains rows [32 w, 32 w + 32) x all columns of every tile the consumers stage (same
 // tile walk), one row per thread.  `tile_origin(tile, m0, n0)` gives a tile's origin, n0 < 0 for a tile the consumers skip.
-// stat_n0: N tile the statistics slice s_stat currently belongs to (-1: none / aborted).  `stage`: bf16 staging tile, or the
-// fp32 one of a split-K launch (P.partial).
+// stat_n0: N tile the statistics slice s_stat currently belongs to (-1: none / aborted).
 template <int BLOCK_N, int MODE, typename TileFn>
 __device__ __forceinline__ void tma_epilogue_warps(const TcParams &P, int tile0, int tstep, int num_tiles, TileFn tile_origin,
-                                                   const uint8_t *stage, uint32_t acc_full, uint32_t acc_empty, float *s_stat,
+                                                   const bf16 *stage, uint32_t acc_full, uint32_t acc_empty, float *s_stat,
                                                    int &stat_n0, int w, int lane, int code) {
     const int row = w * 32 + lane;
-    const bool f32 = P.partial != nullptr;
     if (s_stat) {
         for (int i = lane; i < EPI_STAT_SLICE; i += 32) s_stat[i] = 0.f;
         __syncwarp();
@@ -942,13 +918,10 @@ __device__ __forceinline__ void tma_epilogue_warps(const TcParams &P, int tile0,
             if (stat_n0 >= 0) tc_stats_flush<BLOCK_N>(P, s_stat, lane, stat_n0, 0, BLOCK_N, EPI_STAT_SQ);
             stat_n0 = n0;
         }
-        const EpiRow er = tc_epi_row<MODE>(P, m0 + row, false);     // split-K stores raw partials, bf16 was renormalised
+        const EpiRow er = tc_epi_row<MODE>(P, m0 + row, false);     // the consumers staged renormalised values
         if (!__all_sync(0xffffffffu, ptx::mbar_wait(acc_full, ph, P.abort_flag, code))) { stat_n0 = -1; return; }
         ph ^= 1;
-        if constexpr (BLOCK_N <= 128) {
-            if (f32) tc_epilogue<BLOCK_N, MODE>(P, er, reinterpret_cast<const float *>(stage) + row * acc_pitch(BLOCK_N), lane, n0, s_stat, 0, BLOCK_N, EPI_STAT_SQ);
-        }
-        if (!f32) tc_epilogue_bf16<BLOCK_N, MODE>(P, er, reinterpret_cast<const bf16 *>(stage) + row * bf16_pitch(BLOCK_N), lane, n0, s_stat);
+        tc_epilogue_bf16<BLOCK_N, MODE>(P, er, stage + row * bf16_pitch(BLOCK_N), lane, n0, s_stat);
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(acc_empty);
     }
@@ -966,7 +939,7 @@ __device__ __forceinline__ ConsRows cons_rows(const TcParams &P, int m0, int e, 
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         cr.inv[h] = 0.f; cr.hole[h] = false;
-        if (MODE == 0 && P.partial == nullptr) {
+        if (MODE == 0) {
             const EpiRow er = tc_epi_row<0>(P, m0 + 64 * (e >> 2) + 16 * (e & 3) + (lane >> 2) + 8 * h);
             cr.inv[h] = er.inv; cr.hole[h] = er.hole;
         }
@@ -1017,16 +990,13 @@ __device__ __forceinline__ void stage_acc_bf16(const TcParams &P, const float (&
 }
 
 // consumer warp e after a tile's K loop: wait until the epilogue warps have read the staging tile, write this warp's rows into
-// it (bf16 with the element math, or raw fp32 for split-K), hand it over.  false: aborted.
+// it (bf16, with the element math), hand it over.  false: aborted.
 template <int BLOCK_N, int MODE>
-__device__ __forceinline__ bool tma_stage_tile(const TcParams &P, const float (&acc)[BLOCK_N / 2], uint8_t *stage, uint32_t acc_full,
+__device__ __forceinline__ bool tma_stage_tile(const TcParams &P, const float (&acc)[BLOCK_N / 2], bf16 *stage, uint32_t acc_full,
                                                uint32_t acc_empty, uint32_t &ph, int e, int lane, int n0, const ConsRows &cr, int code) {
     if (!__all_sync(0xffffffffu, ptx::mbar_wait(acc_empty, ph, P.abort_flag, code))) return false;
     ph ^= 1;
-    if constexpr (BLOCK_N <= 128) {
-        if (P.partial != nullptr) stage_acc<BLOCK_N>(acc, reinterpret_cast<float *>(stage), e, lane);
-    }
-    if (P.partial == nullptr) stage_acc_bf16<BLOCK_N, MODE>(P, acc, reinterpret_cast<bf16 *>(stage), e, lane, n0, cr);
+    stage_acc_bf16<BLOCK_N, MODE>(P, acc, stage, e, lane, n0, cr);
     __syncwarp();
     if (lane == 0) ptx::mbar_arrive(acc_full);
     return true;
@@ -1061,9 +1031,8 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform by construction
     const int np = (MODE == 0) ? P.nparts : 1;
     const int n_tiles = P.ncols / BLOCK_N;
-    const int KS = P.ksplit;                                            // tile index = (m tile * n_tiles + n tile) * KS + split
     const int m_tiles = (P.m_total + BLOCK_M - 1) / BLOCK_M;
-    const int num_tiles = m_tiles * n_tiles * KS;
+    const int num_tiles = m_tiles * n_tiles;                           // tile index = m tile * n_tiles + n tile
     const int tile0 = static_cast<int>(blockIdx.x), tstep = static_cast<int>(gridDim.x);
     auto m0_of = [&](int mt) -> int { return mt * BLOCK_M; };
     const bool fix = (MODE == 0) && P.use_fix;
@@ -1090,7 +1059,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
     // broadcast so the compiler knows the role branch is uniform) and only the TMA instructions sit inside an elect.sync region.
     float *s_stat = nullptr;                                          // epilogue warps: private BatchNorm-statistics accumulators
     int stat_n0 = -1;                                                  // N tile they currently belong to (-1: none / aborted)
-    uint8_t *acc_stage = smem_gen + (s_acc - smem_base);
+    bf16 *acc_stage = reinterpret_cast<bf16 *>(smem_gen + (s_acc - smem_base));
     if (warp < MMA_WARPS) {
         ptx::setmaxnreg_inc<TMA_CONSUMER_REGS>();
         // ================================ consumer warpgroups ================================
@@ -1115,10 +1084,9 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
         uint32_t ph = 0, aph = 1;                                      // aph: first pass, the staging tile is free
         bool dead = false;
         for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-            const int sp = tile % KS, mn = tile / KS;
-            const int n0 = (mn % n_tiles) * BLOCK_N;
+            const int n0 = (tile % n_tiles) * BLOCK_N;
             if (!tile_active(n0)) continue;
-            const ConsRows cr = cons_rows<MODE>(P, m0_of(mn / n_tiles), e, lane);
+            const ConsRows cr = cons_rows<MODE>(P, m0_of(tile / n_tiles), e, lane);
             float acc[BLOCK_N / 2];
             zero_acc(acc);
             int held = -1;                                             // stage whose MMAs may still be reading it
@@ -1126,9 +1094,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
 #pragma unroll
                 for (int p = 0; p < TC_MAX_PARTS; ++p) {
                     const int nbp = (p == 0) ? nb0 : nb1, klast = (p == 0) ? kl0 : kl1;
-                    const int gb0 = (p == 0) ? 0 : nb0;
                     for (int cb = 0; cb < nbp; ++cb) {
-                        if (KS > 1 && (gb0 + cb) % KS != sp) continue;
                         if (!__all_sync(0xffffffffu, ptx::mbar_wait(ready + 8 * s, ph, P.abort_flag, 124))) { dead = true; break; }
                         uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16 + shift0), db = desc_b0 + static_cast<uint64_t>(s * stage16);
                         const int ksteps = (cb + 1 < nbp) ? 4 : klast;
@@ -1162,11 +1128,10 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
         if (warp >= EPI_WARP0) {
             // ================================ epilogue warps ================================
             const int w = warp - EPI_WARP0;
-            s_stat = (MODE == 0 && P.bn_sums != nullptr && P.partial == nullptr)
+            s_stat = (MODE == 0 && P.bn_sums != nullptr)
                          ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + w * EPI_STAT_SLICE : nullptr;
             auto origin = [&](int tile, int &m0, int &n0) {
-                const int mn = tile / KS;
-                m0 = m0_of(mn / n_tiles); n0 = (mn % n_tiles) * BLOCK_N;
+                m0 = m0_of(tile / n_tiles); n0 = (tile % n_tiles) * BLOCK_N;
                 if (!tile_active(n0)) n0 = -1;
             };
             tma_epilogue_warps<BLOCK_N, MODE>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, s_stat, stat_n0, w, lane, 126);
@@ -1185,27 +1150,13 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
             const int row_k = P.wk_row, col_k = P.wk_col;
             bool dead = false;
             for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-                const int sp = tile % KS, mn = tile / KS;
-                const int m0 = m0_of(mn / n_tiles), n0 = (mn % n_tiles) * BLOCK_N;
+                const int m0 = m0_of(tile / n_tiles), n0 = (tile % n_tiles) * BLOCK_N;
                 if (!tile_active(n0)) continue;
                 const int img = m0 / plane, rem = m0 - img * plane;
                 const int oy = rem / pwid, ox = rem - oy * pwid;
                 // leftmost / topmost source coordinate of tap column 0 (fwd) -- dgrad walks its taps right to left
                 const int x_org = (MODE == 0) ? ox * P.stride - P.pad_w : (HALO ? ox + P.pad_w - hx : ox + P.pad_w);
                 const int y_org = (MODE == 0) ? oy * P.stride - P.pad_h : oy + P.pad_h;
-                // optional L2 prefetch (P.l2pf): while tile t is loaded, the A boxes of this CTA's NEXT tile are requested into L2, one
-                // tile's worth of stages ahead, so that their loads find L2 instead of DRAM (the ring is round-trip-latency bound)
-                int nx_org = 0, ny_org = 0, nimg = -1;
-                if (P.l2pf && tile + tstep < num_tiles) {
-                    const int nmn = (tile + tstep) / KS;
-                    const int nm0 = m0_of(nmn / n_tiles);
-                    if (nm0 != m0) {
-                        nimg = nm0 / plane;
-                        const int nrem = nm0 - nimg * plane, noy = nrem / pwid, nox = nrem - noy * pwid;
-                        nx_org = (MODE == 0) ? nox * P.stride - P.pad_w : (HALO ? nox + P.pad_w - hx : nox + P.pad_w);
-                        ny_org = (MODE == 0) ? noy * P.stride - P.pad_h : noy + P.pad_h;
-                    }
-                }
                 int krow = P.wk_base;                                      // weight K index of (tr, tap column 0, part 0, block 0)
                 for (int tr = 0, y = y_org; tr < P.kh && !dead; ++tr, y += dstep, krow += row_k)
                     for (int ti = 0, x = x_org, kidx = krow; ti < kwi && !dead; ++ti, x += dstep, kidx = krow + ti * col_k) {
@@ -1213,9 +1164,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                         for (int p = 0; p < TC_MAX_PARTS; ++p) {
                             const int kext = (p == 0) ? kext0 : kext1;
                             const CUtensorMap *ma = (p == 0) ? &tmap_a0 : &tmap_a1;
-                            const int gb0 = (p == 0) ? 0 : kext0 / BLOCK_K;          // global K-block index of the part's first block
                             for (int c0 = 0; c0 < kext; c0 += BLOCK_K, kidx += BLOCK_K) {
-                                if (KS > 1 && (gb0 + c0 / BLOCK_K) % KS != sp) continue;
                                 if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 121))) { dead = true; break; }
                                 if (ptx::elect_one()) {
                                     const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
@@ -1224,7 +1173,6 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                                     uint32_t bdst = dst + A_ROOM;
                                     for (int tc = 0, kb = kidx; tc < nB; ++tc, kb += col_k, bdst += B_BYTES)
                                         ptx::tma_load_2d(bdst, &tmap_w, kb, n0, full);
-                                    if (nimg >= 0) ptx::tma_prefetch_4d(ma, c0, nx_org + ti * dstep, ny_org + tr * dstep, nimg);
                                 }
                                 __syncwarp();
                                 if (++s == S) { s = 0; ph ^= 1; }
@@ -1257,21 +1205,20 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
 #pragma unroll
                             for (int p = 0; p < TC_MAX_PARTS; ++p) {
                                 wnext[r][p] = 0ull;
-                                const int m = m0_of(tl / KS / n_tiles) + t + TMA_FIX_THREADS * r;
+                                const int m = m0_of(tl / n_tiles) + t + TMA_FIX_THREADS * r;
                                 if (p < P.nparts && tl < num_tiles && t + TMA_FIX_THREADS * r < BLOCK_M && m < P.m_total)
                                     wnext[r][p] = __ldg(P.parts[p].tapmask + m);
                             }
                     };
                     load_words(tile0);
                     for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-                        const int sp = tile % KS;
                         uint64_t wcur[FR][TC_MAX_PARTS];
 #pragma unroll
                         for (int r = 0; r < FR; ++r)
 #pragma unroll
                             for (int p = 0; p < TC_MAX_PARTS; ++p) wcur[r][p] = wnext[r][p];
                         load_words(tile + tstep);                      // next tile's words travel while this tile streams
-                        if (MODE == 1 && !tile_active(((tile / KS) % n_tiles) * BLOCK_N)) continue;
+                        if (MODE == 1 && !tile_active((tile % n_tiles) * BLOCK_N)) continue;
                         const int taps = P.kh * P.kw;
                         for (int tap = 0; tap < taps && !dead; ++tap) {
 #pragma unroll
@@ -1285,9 +1232,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                                 }
                                 const bool any_hole = __any_sync(0xffffffffu, mine);
                                 const int nb = ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
-                                const int gb0 = (p == 0) ? 0 : P.parts[0].kext / BLOCK_K;
                                 for (int cb = 0; cb < nb; ++cb) {
-                                    if (KS > 1 && (gb0 + cb) % KS != sp) continue;
                                     if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 122)) { dead = true; break; }
                                     if (any_hole) {
 #pragma unroll
@@ -1310,7 +1255,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
 #pragma unroll
                         for (int r = 0; r < FR; ++r) b[r] = 0;
                         if (tl >= num_tiles) return;
-                        const int m0 = m0_of(tl / KS / n_tiles);
+                        const int m0 = m0_of(tl / n_tiles);
                         const int img = m0 / plane, rem = m0 - img * plane;
                         const int oy = rem / P.wo, ox = rem - oy * P.wo;
 #pragma unroll
@@ -1333,12 +1278,11 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                     uint32_t nb_bits[FR];
                     load_bits(tile0, nb_bits);
                     for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-                        const int sp = tile % KS;
                         uint32_t cb_bits[FR];
 #pragma unroll
                         for (int r = 0; r < FR; ++r) cb_bits[r] = nb_bits[r];
                         load_bits(tile + tstep, nb_bits);
-                        if (MODE == 1 && !tile_active(((tile / KS) % n_tiles) * BLOCK_N)) continue;
+                        if (MODE == 1 && !tile_active((tile % n_tiles) * BLOCK_N)) continue;
                         for (int tr = 0; tr < P.kh && !dead; ++tr) {
 #pragma unroll
                             for (int p = 0; p < TC_MAX_PARTS; ++p) {
@@ -1348,9 +1292,7 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
                                 for (int r = 0; r < FR; ++r) { hole[r] = (cb_bits[r] >> (p * 8 + tr)) & 1u; mine = mine || hole[r]; }
                                 const bool any_hole = __any_sync(0xffffffffu, mine);
                                 const int nb = ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
-                                const int gb0 = (p == 0) ? 0 : P.parts[0].kext / BLOCK_K;
                                 for (int cb = 0; cb < nb; ++cb) {
-                                    if (KS > 1 && (gb0 + cb) % KS != sp) continue;
                                     if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 122)) { dead = true; break; }
                                     if (any_hole) {
 #pragma unroll
@@ -1375,108 +1317,83 @@ pconv_tc_tma_kernel(const __grid_constant__ TcParams P, const __grid_constant__ 
 
 
 // -------------------------------------------------------------------------------------------------
-// SUB-PIXEL (table-driven) variant of the TMA-fed kernel: convolutions whose input is cat([nearest-2x-upsample(x0), x1])
-// (models/image_inpainting.py:183-185) WITHOUT materialising the upsampled tensor and WITHOUT multiplying by replicated pixels.
+// SUB-PIXEL data gradient: for convolutions whose input is cat([nearest-2x-upsample(x0), x1]) (models/image_inpainting.py:183-185)
+// the gradient w.r.t. x0 is computed directly at SOURCE resolution -- neither the full-resolution gradient of the upsampled
+// part nor the 2x2 reduction pass over it exists.
 //
 // Output pixel (2k+py, 2j+px) of a k x k convolution over up2x(x0) reads source pixel (k + floor((py + tr*d - p)/2), ...): within
 // one parity class (py, px) the convolution over the upsampled part IS a convolution over the SOURCE with a smaller kernel whose
-// taps are sums of the original taps (3x3, pad 1: 2x2 effective taps -- 4/9 of the multiplications); the skip part x1 keeps its
-// k x k taps and is read with a traversal stride of 2.  The hole mask of the upsampled part was upsampled with it
-// (HoleMask.upsampled), so masking commutes.  One launch computes one class: its M tiles are boxes of the class grid
-// [n][h/2][w/2]; what each K step loads is listed in a small table built on the host:
-//     item = { part (tensor map), (dx, dy) added to the tile origin scaled by the part's step, nb weight tiles (taps served by
-//              one A tile through row-shifted descriptors), weight K index of the first, step between them }
-// The same kernel computes the data gradient w.r.t. x0 directly at SOURCE resolution (MODE 1): its A operand is dc read with a
-// traversal stride of 2 per (class, effective tap) item -- 16/36 of the multiplications of "full-resolution gradient + 2x2 sum",
-// and neither the full-resolution gradient nor the reduction pass exists.
-// Roles / pipeline / epilogue exactly as in pconv_tc_tma_kernel (no split-K).
+// taps are sums of the original taps (3x3, pad 1: 2x2 effective taps).  So dx0 = sum over the classes and their effective taps
+// of dc read with a traversal stride of 2 times the transposed effective weights -- 16/36 of the multiplications of
+// "full-resolution gradient + 2x2 sum".  The M tiles are boxes of the source grid [n][h/2][w/2]; what each K step loads is
+// listed in a small table built on the host:
+//     item = { (dx, dy) added to twice the tile origin (dc coordinates), weight K index }
+// Roles / pipeline / epilogue as in pconv_tc_tma_kernel; dc has no holes, so the fixer warps stay idle.
 // -------------------------------------------------------------------------------------------------
 constexpr int SP_MAX_ITEMS = 40;
-struct SpItem { int part, dx, dy, wk, nb, wk_step, shift0, dshift; };
+struct SpItem { int dx, dy, wk; };
 struct SpTable {
     int n_items;
-    int step[TC_MAX_PARTS];         // tile origin (class grid) -> part coordinates: origin * step + (dx, dy)
-    int es[TC_MAX_PARTS];           // traversal stride of the part's tensor map (pixels between consecutive tile rows)
-    int ph[TC_MAX_PARTS], pw[TC_MAX_PARTS];     // the part's own pixel grid (its mask plane has exactly this resolution)
-    int arows[TC_MAX_PARTS];        // pixel rows one TMA tile of the part delivers (128 + the halo of the part's tensor-map box)
-    int rows_max;                   // pixel rows of the largest A tile
     SpItem it[SP_MAX_ITEMS];
 };
 
-template <int BLOCK_N, int MODE>
+template <int BLOCK_N>
 __global__ void __maxnreg__(TMA_REGS)
 pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ SpTable TB, const __grid_constant__ CUtensorMap tmap_w,
-                   const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1) {
+                   const __grid_constant__ CUtensorMap tmap_a) {
     constexpr uint32_t B_BYTES = BLOCK_N * 128;
+    constexpr uint32_t STAGE = A_STAGE_BYTES + B_BYTES;               // multiple of 1024
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = align1024(ptx::smem_u32(smem_raw));
     const int S = P.stages;
-    int nb_max = 1;
-    for (int i = 0; i < TB.n_items; ++i) nb_max = max(nb_max, TB.it[i].nb);
-    const uint32_t A_ROOM = (static_cast<uint32_t>(TB.rows_max) * 128u + 1023u) & ~1023u;
-    const uint32_t STAGE = A_ROOM + nb_max * B_BYTES;
+    // shared-memory layout of pconv_tc_tma_kernel (tma_fixed_smem), the fixed-barrier and statistics slots unused
     const uint32_t sBar = smem_base + S * STAGE;
-    const uint32_t bar_full = sBar, bar_fixed = sBar + 8 * MAX_RING, bar_empty = sBar + 16 * MAX_RING;
+    const uint32_t bar_full = sBar, bar_empty = sBar + 16 * MAX_RING;
     const uint32_t acc_full = sBar + 24 * MAX_RING, acc_empty = acc_full + 8;
-    const uint32_t s_stat_addr = sBar + TMA_BAR_BYTES;
-    const uint32_t s_acc = s_stat_addr + EPI_STAT_SMEM_BYTES;
-    uint8_t *smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
+    const uint32_t s_acc = sBar + TMA_BAR_BYTES + EPI_STAT_SMEM_BYTES;
+    bf16 *acc_stage = reinterpret_cast<bf16 *>(smem_raw + (s_acc - ptx::smem_u32(smem_raw)));
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     const int n_tiles = P.ncols / BLOCK_N;
     const int m_tiles = (P.m_total + BLOCK_M - 1) / BLOCK_M;
     const int num_tiles = m_tiles * n_tiles;
     const int tile0 = static_cast<int>(blockIdx.x), tstep = static_cast<int>(gridDim.x);
-    const bool fix = P.use_fix != 0;
-    // the tile grid: [n][gh][gw] = the class grid (MODE 0: P.ho x P.wo) or the source grid (MODE 1: P.h x P.w)
-    const int gw = (MODE == 0) ? P.wo : P.w, gh = (MODE == 0) ? P.ho : P.h;
-    const int plane = gw * gh;
-    // per part: 64-channel K blocks and the K steps of the last block that hold real channels
-    int nbk[TC_MAX_PARTS], klast[TC_MAX_PARTS];
-#pragma unroll
-    for (int p = 0; p < TC_MAX_PARTS; ++p) {
-        const int kext = (MODE == 0) ? P.parts[p].kext : P.dc_kext, c8 = (MODE == 0) ? P.parts[p].c8 : P.dc_c8;
-        nbk[p] = (p < ((MODE == 0) ? P.nparts : 1)) ? kext / BLOCK_K : 0;
-        klast[p] = nbk[p] ? min(4, (c8 - (nbk[p] - 1) * BLOCK_K + 15) >> 4) : 4;
-    }
+    // the tile grid is the source grid [n][P.h][P.w]
+    const int plane = P.w * P.h;
+    // 64-channel K blocks of dc and the K steps of the last block that hold real channels
+    const int nbk = P.dc_kext / BLOCK_K;
+    const int klast = min(4, (P.dc_c8 - (nbk - 1) * BLOCK_K + 15) >> 4);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_fixed + 8 * s, TMA_FIX_THREADS / 32); ptx::mbar_init(bar_empty + 8 * s, 2); }
+        for (int s = 0; s < MAX_RING; ++s) { ptx::mbar_init(bar_full + 8 * s, 1); ptx::mbar_init(bar_empty + 8 * s, 2); }
         ptx::mbar_init(acc_full, MMA_WARPS); ptx::mbar_init(acc_empty, EPI_WARPS);     // one arrival per warp
         ptx::fence_mbar_init();
     }
-    if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_a0); ptx::prefetch_tmap(&tmap_a1); }
+    if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_a); }
     __syncthreads();
 
-    float *s_stat = nullptr;
-    int stat_n0 = -1;
-    uint8_t *acc_stage = smem_gen + (s_acc - smem_base);
     if (warp < MMA_WARPS) {
         ptx::setmaxnreg_inc<TMA_CONSUMER_REGS>();
         // ================================ consumer warpgroups ================================
         const int e = warp, g = warp >> 2;
         const bool leader = (threadIdx.x & 127) == 0;
-        const uint32_t ready = fix ? bar_fixed : bar_full;
         const uint64_t desc_a0 = ptx::make_smem_desc(smem_base + g * 64 * 128, 16, 1024);     // this warpgroup's 64 rows
-        const uint64_t desc_b0 = ptx::make_smem_desc(smem_base + A_ROOM, 16, 1024);
+        const uint64_t desc_b0 = ptx::make_smem_desc(smem_base + A_STAGE_BYTES, 16, 1024);
         const uint32_t stage16 = STAGE >> 4;
         int s = 0;
         uint32_t ph = 0, aph = 1;                                      // aph: first pass, the staging tile is free
         bool dead = false;
         for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-            const ConsRows cr = cons_rows<MODE>(P, (tile / n_tiles) * BLOCK_M, e, lane);
             float acc[BLOCK_N / 2];
             zero_acc(acc);
             int held = -1;
             for (int i = 0; i < TB.n_items && !dead; ++i) {
-                const SpItem it = TB.it[i];
-                for (int cb = 0; cb < nbk[it.part]; ++cb) {
-                    if (!__all_sync(0xffffffffu, ptx::mbar_wait(ready + 8 * s, ph, P.abort_flag, 324))) { dead = true; break; }
-                    uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16 + it.shift0), db = desc_b0 + static_cast<uint64_t>(s * stage16);
-                    const int ksteps = (cb + 1 < nbk[it.part]) ? 4 : klast[it.part];
+                for (int cb = 0; cb < nbk; ++cb) {
+                    if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 324))) { dead = true; break; }
+                    const uint64_t da = desc_a0 + static_cast<uint64_t>(s * stage16), db = desc_b0 + static_cast<uint64_t>(s * stage16);
+                    const int ksteps = (cb + 1 < nbk) ? 4 : klast;
                     ptx::wgmma_fence();
-                    for (int tc = 0; tc < it.nb; ++tc, da += it.dshift, db += B_BYTES >> 4)
-                        for (int k = 0; k < ksteps; ++k) ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + 2 * k, db + 2 * k);
+                    for (int k = 0; k < ksteps; ++k) ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + 2 * k, db + 2 * k);
                     ptx::wgmma_commit();
                     ptx::wgmma_wait<1>();
                     if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
@@ -1488,20 +1405,16 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
             ptx::wgmma_fence_regs(acc);
             if (held >= 0 && leader) ptx::mbar_arrive(bar_empty + 8 * held);
             if (dead) break;
-            if (!tma_stage_tile<BLOCK_N, MODE>(P, acc, acc_stage, acc_full, acc_empty, aph, e, lane, (tile % n_tiles) * BLOCK_N, cr, 325)) break;
+            if (!tma_stage_tile<BLOCK_N, 1>(P, acc, acc_stage, acc_full, acc_empty, aph, e, lane, (tile % n_tiles) * BLOCK_N, ConsRows{}, 325)) break;
         }
     } else {
-        ptx::setmaxnreg_dec<TMA_SUPPORT_REGS>();       // warpgroups 2 and 3, fixers included when there are no holes
+        ptx::setmaxnreg_dec<TMA_SUPPORT_REGS>();       // warpgroups 2 and 3, the idle fixer warps included
         if (warp >= EPI_WARP0) {
             // ================================ epilogue warps ================================
-            const int w = warp - EPI_WARP0;
-            s_stat = (MODE == 0 && P.bn_sums != nullptr) ? reinterpret_cast<float *>(smem_gen + (s_stat_addr - smem_base)) + w * EPI_STAT_SLICE : nullptr;
+            int stat_n0 = -1;
             auto origin = [&](int tile, int &m0, int &n0) { m0 = (tile / n_tiles) * BLOCK_M; n0 = (tile % n_tiles) * BLOCK_N; };
-            tma_epilogue_warps<BLOCK_N, MODE>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, s_stat, stat_n0, w, lane, 326);
-            // last N tile's statistics: all four slices are complete once the epilogue warpgroup passed this barrier (no CTA-wide
-            // barrier: the warpgroups run under different register limits, setmaxnreg regions must not meet again)
-            ptx::named_sync(1, EPI_WARPS * 32);
-            if (s_stat != nullptr && stat_n0 >= 0) tc_stats_final<BLOCK_N>(P, s_stat - w * EPI_STAT_SLICE, w, lane, stat_n0);
+            tma_epilogue_warps<BLOCK_N, 1>(P, tile0, tstep, num_tiles, origin, acc_stage, acc_full, acc_empty, nullptr, stat_n0,
+                                           warp - EPI_WARP0, lane, 326);
         } else if (warp == 8) {
             // ================================ TMA producer ================================
             int s = 0;
@@ -1510,100 +1423,25 @@ pconv_tc_sp_kernel(const __grid_constant__ TcParams P, const __grid_constant__ S
             for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
                 const int m0 = (tile / n_tiles) * BLOCK_M, n0 = (tile % n_tiles) * BLOCK_N;
                 const int img = m0 / plane, rem = m0 - img * plane;
-                const int oy = rem / gw, ox = rem - oy * gw;
+                const int oy = rem / P.w, ox = rem - oy * P.w;
                 for (int i = 0; i < TB.n_items && !dead; ++i) {
                     const SpItem it = TB.it[i];
-                    const CUtensorMap *ma = (it.part == 0) ? &tmap_a0 : &tmap_a1;
-                    const int x = ox * TB.step[it.part] + it.dx, y = oy * TB.step[it.part] + it.dy;
-                    const uint32_t a_bytes = static_cast<uint32_t>(TB.arows[it.part]) * 128u;      // what the part's box delivers
-                    for (int cb = 0; cb < nbk[it.part]; ++cb) {
+                    const int x = 2 * ox + it.dx, y = 2 * oy + it.dy;
+                    for (int cb = 0; cb < nbk; ++cb) {
                         if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_empty + 8 * s, ph, P.abort_flag, 321))) { dead = true; break; }
                         if (ptx::elect_one()) {
                             const uint32_t full = bar_full + 8 * s, dst = smem_base + s * STAGE;
-                            ptx::mbar_arrive_expect_tx(full, a_bytes + it.nb * B_BYTES);
-                            ptx::tma_load_4d(dst, ma, cb * BLOCK_K, x, y, img, full);
-                            uint32_t bdst = dst + A_ROOM;
-                            for (int tc = 0, kb = it.wk + cb * BLOCK_K; tc < it.nb; ++tc, kb += it.wk_step, bdst += B_BYTES)
-                                ptx::tma_load_2d(bdst, &tmap_w, kb, n0, full);
+                            ptx::mbar_arrive_expect_tx(full, STAGE);
+                            ptx::tma_load_4d(dst, &tmap_a, cb * BLOCK_K, x, y, img, full);
+                            ptx::tma_load_2d(dst + A_STAGE_BYTES, &tmap_w, it.wk + cb * BLOCK_K, n0, full);
                         }
                         __syncwarp();
                         if (++s == S) { s = 0; ph ^= 1; }
                     }
                 }
             }
-        } else {
-            // ================================ fixers: zero the hole rows of every landed A tile ================================
-            // thread t owns A-tile rows t, t + 96 and t + 192 (a part's box delivers at most 256 rows)
-            if (fix) {
-                constexpr int FR = 3;
-                const int t = (warp - 9) * 32 + lane;
-                int s = 0;
-                uint32_t ph = 0;
-                bool dead = false;
-                // bit i of b[r]: row t + 96 r of item i's A tile is a hole (rows outside the image were zero-filled by TMA)
-                auto load_bits = [&](int tl, uint64_t (&b)[FR]) {
-#pragma unroll
-                    for (int r = 0; r < FR; ++r) b[r] = 0ull;
-                    if (tl >= num_tiles) return;
-                    const int m0 = (tl / n_tiles) * BLOCK_M;
-                    const int img = m0 / plane, rem = m0 - img * plane;
-                    const int oy = rem / gw, ox = rem - oy * gw;
-                    for (int i = 0; i < TB.n_items; ++i) {
-                        const SpItem it = TB.it[i];
-                        const uint8_t *mk = P.parts[it.part].mask;
-                        if (mk == nullptr) continue;
-                        const int pwid = TB.pw[it.part], phei = TB.ph[it.part], es = TB.es[it.part];
-                        const int hrows = TB.arows[it.part] - BLOCK_M;
-                        const int x0 = ox * TB.step[it.part] + it.dx, y0 = oy * TB.step[it.part] + it.dy;
-#pragma unroll
-                        for (int r = 0; r < FR; ++r) {
-                            const int row = t + TMA_FIX_THREADS * r;
-                            if (row >= BLOCK_M + hrows) continue;
-                            int tx, ty, tn;           // rows past 128 only exist in one-row halo boxes
-                            if (hrows > 0 || (P.box_h == 1 && P.box_n == 1)) { tx = row; ty = 0; tn = 0; }
-                            else { tx = row % P.box_w; ty = (row / P.box_w) % P.box_h; tn = row / (P.box_w * P.box_h); }
-                            const int X = x0 + tx * es, Y = y0 + ty * es, IM = img + tn;
-                            if (X >= 0 && X < pwid && Y >= 0 && Y < phei && IM < P.n &&
-                                __ldg(mk + (static_cast<long long>(IM) * phei + Y) * pwid + X) == 0) b[r] |= 1ull << i;
-                        }
-                    }
-                };
-                uint64_t nb_bits[FR];
-                load_bits(tile0, nb_bits);
-                for (int tile = tile0; tile < num_tiles && !dead; tile += tstep) {
-                    uint64_t cb_bits[FR];
-#pragma unroll
-                    for (int r = 0; r < FR; ++r) cb_bits[r] = nb_bits[r];
-                    load_bits(tile + tstep, nb_bits);
-                    for (int i = 0; i < TB.n_items && !dead; ++i) {
-                        bool hole[FR], mine = false;
-#pragma unroll
-                        for (int r = 0; r < FR; ++r) { hole[r] = (cb_bits[r] >> i) & 1ull; mine = mine || hole[r]; }
-                        const bool any_hole = __any_sync(0xffffffffu, mine);
-                        const int nb_i = nbk[TB.it[i].part];
-                        for (int cb = 0; cb < nb_i; ++cb) {
-                            if (!ptx::mbar_wait(bar_full + 8 * s, ph, P.abort_flag, 322)) { dead = true; break; }
-                            if (any_hole) {
-                                const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-#pragma unroll
-                                for (int r = 0; r < FR; ++r)
-                                    if (hole[r]) {
-                                        uint4 *rw = reinterpret_cast<uint4 *>(smem_gen + s * STAGE + (t + TMA_FIX_THREADS * r) * 128);
-#pragma unroll
-                                        for (int k = 0; k < 8; ++k) rw[k] = z;
-                                    }
-                                ptx::fence_proxy_async_smem();
-                            }
-                            __syncwarp();
-                            if (lane == 0) ptx::mbar_arrive(bar_fixed + 8 * s);
-                            if (++s == S) { s = 0; ph ^= 1; }
-                        }
-                    }
-                }
-            }
         }
     }
-
 }
 
 // nearest 2x upsample of one convolution source into a dense [n, 2hs, 2ws, c8] buffer (TMA cannot replicate pixels)
@@ -2388,7 +2226,6 @@ void base_params(TcParams &P, const pcb_conv *c, const Layout &L) {
     P.pad_h = c->pad_h; P.pad_w = c->pad_w; P.dil = c->dil; P.ho = c->ho; P.wo = c->wo;
     P.nparts = c->nparts; P.no_guard = c->no_guard; P.rowpack = L.rowpack; P.ktap = L.ktap;
     P.sub = 1; P.py = 0; P.px = 0; P.fh = c->h; P.fw = c->w;
-    P.l2pf = getenv("PCB_TMA_L2_PREFETCH") != nullptr;
 }
 
 // row-halo eligibility: stride 1, output rows made of whole groups of 8 pixels, halo small enough
@@ -2424,87 +2261,6 @@ int launch_persistent(TcParams &P, const CUtensorMap &tm, cudaStream_t st) {
     return 0;
 }
 
-
-// ---- split-K: scratch buffer and finish kernels --------------------------------------------------
-// (opt-in debug path, PCB_SPLITK=1: one scratch buffer per device, single host thread / stream per device assumed)
-float *splitk_scratch(size_t bytes) {
-    static float *buf[PCB_MAX_DEVICES] = {};
-    static size_t cap[PCB_MAX_DEVICES] = {};
-    const int dev = pcb_cur_device();
-    if (bytes > cap[dev]) {
-        // the previous (smaller) buffer is deliberately not freed: a captured CUDA graph may still point into it
-        const size_t want = std::max<size_t>(bytes, 16u << 20);
-        float *fresh = nullptr;
-        if (cudaMalloc(&fresh, want) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-        buf[dev] = fresh; cap[dev] = want;
-    }
-    return buf[dev];
-}
-
-// y = hole ? 0 : acc / s + b over [m_total][y_cstride] (8 channels per thread)
-__global__ void splitk_finish_fwd_kernel(const float *__restrict__ part, int ncols, const float *__restrict__ msum, const float *__restrict__ bias, int cout,
-                                         int no_guard, long long m_total, bf16 *__restrict__ y, int y_cstride) {
-    const int cv = y_cstride >> 3;
-    const long long total = m_total * cv;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const long long m = i / cv;
-        const int col = static_cast<int>(i - m * cv) * 8;
-        const float s = msum ? msum[m] : 1.f;
-        const bool hole = (s == 0.f) && !no_guard;
-        const float inv = hole ? 0.f : 1.0f / s;
-        uint4 o;
-        __nv_bfloat162 *ob = reinterpret_cast<__nv_bfloat162 *>(&o);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int co = col + 2 * j;
-            float a = (co < ncols) ? part[m * ncols + co] : 0.f, b = (co + 1 < ncols) ? part[m * ncols + co + 1] : 0.f;
-            a = (hole || co >= cout) ? 0.f : a * inv + (bias ? bias[co] : 0.f);
-            b = (hole || co + 1 >= cout) ? 0.f : b * inv + (bias ? bias[co + 1] : 0.f);
-            ob[j] = __floats2bfloat162_rn(a, b);
-        }
-        *reinterpret_cast<uint4 *>(y + m * y_cstride + col) = o;
-    }
-}
-
-// dx_part = acc * input mask of the part (8 channels per thread); the tile grid may be a parity class of the gradient
-__global__ void splitk_finish_dgrad_kernel(const float *__restrict__ part, const TcParams P) {
-    const int cv = P.ncols >> 3;
-    const long long total = static_cast<long long>(P.m_total) * cv;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const int m = static_cast<int>(i / cv);
-        const int col = static_cast<int>(i - static_cast<long long>(m) * cv) * 8;
-        const int en = m / (P.h * P.w), rem = m - en * P.h * P.w;
-        const int eh = (rem / P.w) * P.sub + P.py, ew = (rem % P.w) * P.sub + P.px;
-        const long long mo = (static_cast<long long>(en) * P.fh + eh) * P.fw + ew;
-        for (int p = 0; p < P.nparts; ++p) {
-            const TcPart &pt = P.parts[p];
-            const int local = col - pt.koff;
-            if (local < 0 || local >= pt.c8 || pt.dx == nullptr) continue;
-            float scale = 1.f;
-            if (pt.mask != nullptr)
-                scale = pt.mask[(static_cast<long long>(en) * (P.fh >> pt.mup) + (eh >> pt.mup)) * (P.fw >> pt.mup) + (ew >> pt.mup)] ? 1.f : 0.f;
-            const float *src = part + static_cast<long long>(m) * P.ncols + col;
-            uint4 o;
-            __nv_bfloat162 *ob = reinterpret_cast<__nv_bfloat162 *>(&o);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) ob[j] = __floats2bfloat162_rn(src[2 * j] * scale, src[2 * j + 1] * scale);
-            *reinterpret_cast<uint4 *>(pt.dx + mo * pt.dx_cstride + local) = o;
-        }
-    }
-}
-
-// how many CTAs should share the K loop of one output tile
-int pick_ksplit(long long m_total, int ncols, int bn, int blocks_per_tap) {
-    // the shorter K loop of the low-resolution layers is paid back by the memset + finish kernels, so the split is opt-in
-    // (PCB_SPLITK=1; the parity tests set it)
-    if (!getenv("PCB_SPLITK")) return 1;
-    const long long tiles = ((m_total + BLOCK_M - 1) / BLOCK_M) * (ncols / bn);
-    const int sms = pcb_num_sms();
-    if (tiles * 2 > sms) return 1;
-    int ks = static_cast<int>(std::min<long long>(16, sms / tiles));
-    ks = std::min(ks, blocks_per_tap);                   // every split keeps at least one K block per tap
-    return ks < 2 ? 1 : ks;
-}
 
 // ---- TMA-fed path: eligibility, tile box, launch -------------------------------------------------
 // 128 consecutive pixels of a [n][ht][wt] grid as a box {bw, bh, bn}: possible when the extents nest in powers of two
@@ -2552,9 +2308,9 @@ size_t tapmask_bytes(const pcb_conv *c) {
 }
 
 // shared memory of a TMA-fed fwd / dgrad / sub-pixel launch outside its ring: alignment slack, barriers, statistics slices and
-// the staging tile (bf16, or fp32 for the raw partials of a split-K launch); the ring gets the rest of the opt-in maximum
-size_t tma_fixed_smem(int block_n, bool splitk) {
-    return 1024 + TMA_BAR_BYTES + EPI_STAT_SMEM_BYTES + (splitk ? acc_stage_bytes(block_n) : bf16_stage_bytes(block_n));
+// the bf16 staging tile; the ring gets the rest of the opt-in maximum
+size_t tma_fixed_smem(int block_n) {
+    return 1024 + TMA_BAR_BYTES + EPI_STAT_SMEM_BYTES + bf16_stage_bytes(block_n);
 }
 
 template <int BLOCK_N, int MODE, bool HALO>
@@ -2562,16 +2318,14 @@ int launch_tma_n(TcParams &P, const CUtensorMap &tw, const CUtensorMap &ta0, con
     const int nb = HALO ? P.kw : 1;
     const size_t a_room = (static_cast<size_t>(BLOCK_M + (HALO ? (P.kw - 1) * P.dil : 0)) * 128 + 1023) / 1024 * 1024;
     const size_t stage = a_room + static_cast<size_t>(nb) * BLOCK_N * 128;
-    PCB_CHECK(BLOCK_N <= 128 || P.partial == nullptr, "TMA-fed conv: split-K stages fp32 partials, at most 128 columns wide");
-    const size_t fixed = tma_fixed_smem(BLOCK_N, P.partial != nullptr);
+    const size_t fixed = tma_fixed_smem(BLOCK_N);
     P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (MAX_SMEM - fixed) / stage));
     PCB_CHECK(P.stages >= 2, "TMA-fed conv: stage of %zu bytes does not fit twice", stage);
     const size_t smem = fixed + P.stages * stage;
     auto kern = pconv_tc_tma_kernel<BLOCK_N, MODE, HALO>;
     PCB_SMEM_OPT_IN(kern, MAX_SMEM);
-    if (P.ksplit < 1) P.ksplit = 1;
     const int m_tiles = (P.m_total + BLOCK_M - 1) / BLOCK_M;
-    const int num_tiles = m_tiles * (P.ncols / BLOCK_N) * P.ksplit;
+    const int num_tiles = m_tiles * (P.ncols / BLOCK_N);
     const int grid = std::min(num_tiles, pcb_num_sms());
     kern<<<grid, TMA_THREADS, smem, st>>>(P, tw, ta0, ta1);
     PCB_LAUNCH_CHECK();
@@ -2626,8 +2380,7 @@ int pick_bn(int cols, long long m_total, bool fwd) {
     auto waves = [&](int b) { return (m_tiles * (cols / b) + sms - 1) / sms; };
     if (cols % 256 == 0 && 2 * waves(256) <= waves(128) && (!fwd || waves(256) == 1)) return 256;
     int bn = (cols % 128 == 0) ? 128 : 64;
-    if (!getenv("PCB_NO_NARROW_N"))
-        while (bn > 32 && cols % (bn / 2) == 0 && m_tiles * (cols / bn) < pcb_num_sms() / 2) bn /= 2;
+    while (bn > 32 && cols % (bn / 2) == 0 && m_tiles * (cols / bn) < pcb_num_sms() / 2) bn /= 2;
     return bn;
 }
 
@@ -2637,12 +2390,30 @@ int launch_tc(TcParams &P, const CUtensorMap &tm, int bn, cudaStream_t st) {
     return (bn == 128) ? launch_persistent<128, MODE, false>(P, tm, st) : launch_persistent<64, MODE, false>(P, tm, st);
 }
 
+// internal streams for the four parity-class launches of low-resolution layers: one set per device AND per host thread (two
+// host threads driving data gradients on two streams must not share the fork / join events)
+struct ClassStreams { cudaStream_t aux[3]; cudaEvent_t ev_fork, ev_join[3]; bool ready; };
+int class_streams(ClassStreams **out) {
+    static thread_local ClassStreams cs_all[PCB_MAX_DEVICES] = {};
+    ClassStreams &CS = cs_all[pcb_cur_device()];
+    if (!CS.ready) {
+        for (int i = 0; i < 3; ++i) {
+            PCB_CUDA(cudaStreamCreateWithFlags(&CS.aux[i], cudaStreamNonBlocking));
+            PCB_CUDA(cudaEventCreateWithFlags(&CS.ev_join[i], cudaEventDisableTiming));
+        }
+        PCB_CUDA(cudaEventCreateWithFlags(&CS.ev_fork, cudaEventDisableTiming));
+        CS.ready = true;
+    }
+    *out = &CS;
+    return 0;
+}
+
 }  // namespace
 
 static bool smallco_ok(const pcb_conv *c);
 namespace {
 
-// ---- sub-pixel path: plan, weights, launches -------------------------------------------------------
+// ---- sub-pixel data gradient: plan, weights, launch ---------------------------------------------------
 // one spatial axis: for output parity q, tap t of a (k, dilation d, padding p) kernel over the 2x-upsampled source reads source
 // offset floor((q + t*d - p) / 2); the distinct offsets e0 .. e0+ne-1 are the effective taps, tapbits[q][e] the original taps
 // that collapse onto effective tap e
@@ -2667,14 +2438,13 @@ SpAxis sp_axis(int k, int d, int p) {
 }
 
 struct SpPlan {
-    bool ok;                         // geometry admits the decomposition
-    bool fwd, dgrad;                 // which passes use it (see sp_plan)
+    bool ok;                         // the data gradient of the upsampled part takes the sub-pixel kernel (see sp_plan)
     int pu, ps;                      // the upsampled part and the other one (-1: none)
     SpAxis ay, ax;
     int net[4], eoff[4], net_total;  // effective taps of the upsampled part per class (class = py * 2 + px)
-    int kext_u, kext_s, c8_u, c8_s;
-    long long kc[4], clsoff[4], sp_fwd_elems, sp_dg_elems, kd_sp;
-    int bw, bh, bn;                  // M tile box of the class grid [n][h/2][w/2]
+    int kext_u, c8_u;
+    long long sp_dg_elems, kd_sp;
+    int bw, bh, bn;                  // M tile box of the source grid [n][h/2][w/2]
 };
 
 SpPlan sp_plan(const pcb_conv *c) {
@@ -2698,76 +2468,32 @@ SpPlan sp_plan(const pcb_conv *c) {
     if (!tile_box(c->w / 2, c->h / 2, &S.bw, &S.bh, &S.bn)) return S;
     const Layout L = layout_of(c);
     S.kext_u = L.kext[S.pu]; S.c8_u = rup(c->parts[S.pu].c, 8);
-    S.kext_s = S.ps >= 0 ? L.kext[S.ps] : 0; S.c8_s = S.ps >= 0 ? rup(c->parts[S.ps].c, 8) : 0;
-    const int taps = c->kh * c->kw;
-    long long off = 0;
     int eo = 0;
     for (int cls = 0; cls < 4; ++cls) {
         S.net[cls] = S.ay.ne[cls >> 1] * S.ax.ne[cls & 1];
         S.eoff[cls] = eo; eo += S.net[cls];
-        S.kc[cls] = static_cast<long long>(S.net[cls]) * S.kext_u + static_cast<long long>(S.ps >= 0 ? taps : 0) * S.kext_s;
-        S.clsoff[cls] = off; off += static_cast<long long>(L.rows_f) * S.kc[cls];
-        // worst-case item count of one class launch (no halo re-use)
-        if (S.net[cls] + (S.ps >= 0 ? taps : 0) > SP_MAX_ITEMS) return S;
     }
     S.net_total = eo;
     if (S.net_total > SP_MAX_ITEMS) return S;
     S.kd_sp = static_cast<long long>(S.net_total) * L.cout64;
-    S.ok = true;
-    //  * DATA GRADIENT: one launch over the source grid replaces the full-resolution gradient of the upsampled part AND its 2x2
-    //    reduction pass; it is used wherever the source grid has at least a third of a wave of tiles -- low-resolution layers keep
-    //    the regular kernel (their launches are latency-bound either way).
-    //  * FORWARD: 37 % fewer MMAs but MORE tile rows per output pixel (the skip part is read with a traversal stride of 2, which
-    //    costs the TMA unit two rows per delivered row, and row-halo re-use is lost where the class grid is narrower than 128).
-    //    Off by default (PCB_SUBPIXEL_FWD=1 enables it; parity-tested either way).
+    // one launch over the source grid replaces the full-resolution gradient of the upsampled part AND its 2x2 reduction pass; it
+    // is used wherever the source grid has at least a third of a wave of tiles -- low-resolution layers keep the regular kernel
+    // (their launches are latency-bound either way)
     const long long src_tiles = (static_cast<long long>(c->n) * (c->h / 2) * (c->w / 2) + BLOCK_M - 1) / BLOCK_M;
-    S.dgrad = src_tiles >= pcb_num_sms() / 3 || getenv("PCB_SUBPIXEL_ALL") != nullptr;
-    S.fwd = getenv("PCB_SUBPIXEL_FWD") != nullptr || getenv("PCB_SUBPIXEL_ALL") != nullptr;
-    S.sp_fwd_elems = S.fwd ? off : 0;
-    S.sp_dg_elems = S.dgrad ? static_cast<long long>(rup(S.kext_u, 128)) * S.kd_sp : 0;
-    if (!S.fwd && !S.dgrad) S.ok = false;
+    S.ok = src_tiles >= pcb_num_sms() / 3;
+    S.sp_dg_elems = static_cast<long long>(rup(S.kext_u, 128)) * S.kd_sp;
     return S;
 }
 
 struct SpWParams {
-    int cout, taps, cin, kw, cout64, rows_f;
-    int choff_u, c_u, kext_u, choff_s, c_s, kext_s, has_skip;
-    int net[4], eoff[4], nex[4], slot0[4];       // per class: eff taps, their prefix, eff columns, first slot index
+    int cout, taps, cin, kw, cout64, choff_u;
+    int eoff[4], nex[4];                         // per class: the prefix of its effective taps, its effective columns
     int ybits[2][4], xbits[2][4];
-    long long kc[4], clsoff[4], kd_sp;
-    int want_fwd, want_dg;
+    long long kd_sp;
 };
 
-// slot = (class, effective tap of the upsampled part | original tap of the skip part); one block per (cout, slot)
-__global__ void sp_weight_prepare_kernel(const float *__restrict__ wm, const SpWParams W, bf16 *__restrict__ w_f, bf16 *__restrict__ w_d) {
-    const int co = blockIdx.x;
-    int slot = blockIdx.y, cls = 0;
-    while (cls < 3 && slot >= W.slot0[cls + 1]) ++cls;
-    slot -= W.slot0[cls];
-    const float *wrow = wm + static_cast<long long>(co) * W.taps * W.cin;
-    if (slot < W.net[cls]) {
-        const int ey = slot / W.nex[cls], ex = slot - ey * W.nex[cls];
-        const int yb = W.ybits[cls >> 1][ey], xb = W.xbits[cls & 1][ex];
-        for (int ci = threadIdx.x; ci < W.c_u; ci += blockDim.x) {
-            float v = 0.f;
-            for (int tr = 0; tr < 4; ++tr)
-                if ((yb >> tr) & 1)
-                    for (int tc = 0; tc < 4; ++tc)
-                        if ((xb >> tc) & 1) v += wrow[static_cast<long long>(tr * W.kw + tc) * W.cin + W.choff_u + ci];
-            const bf16 b = __float2bfloat16_rn(v);
-            if (W.want_fwd) w_f[W.clsoff[cls] + static_cast<long long>(co) * W.kc[cls] + static_cast<long long>(slot) * W.kext_u + ci] = b;
-            if (W.want_dg) w_d[static_cast<long long>(ci) * W.kd_sp + static_cast<long long>(W.eoff[cls] + slot) * W.cout64 + co] = b;
-        }
-    } else if (W.has_skip && W.want_fwd) {
-        const int tap = slot - W.net[cls];
-        for (int ci = threadIdx.x; ci < W.c_s; ci += blockDim.x)
-            w_f[W.clsoff[cls] + static_cast<long long>(co) * W.kc[cls] + static_cast<long long>(W.net[cls]) * W.kext_u + static_cast<long long>(tap) * W.kext_s + ci] =
-                __float2bfloat16_rn(wrow[static_cast<long long>(tap) * W.cin + W.choff_s + ci]);
-    }
-}
-
-// dgrad-only variant: one block per (input channel of the upsampled part, slot), threads over cout -> coalesced writes of the
-// transposed matrix (the master reads are strided but L2-resident)
+// transposed effective-tap weights: one block per (input channel of the upsampled part, effective tap of a class), threads over
+// cout -> coalesced writes of the transposed matrix (the master reads are strided but L2-resident)
 __global__ void sp_weight_dg_kernel(const float *__restrict__ wm, const SpWParams W, bf16 *__restrict__ w_d) {
     const int ci = blockIdx.x;
     int slot = blockIdx.y, cls = 0;
@@ -2786,160 +2512,35 @@ __global__ void sp_weight_dg_kernel(const float *__restrict__ wm, const SpWParam
     }
 }
 
-int sp_weight_prepare(const pcb_conv *c, const SpPlan &S, const Layout &L, const float *w_master, bf16 *w_f, bf16 *w_d, cudaStream_t st) {
+int sp_weight_prepare(const pcb_conv *c, const SpPlan &S, const Layout &L, const float *w_master, bf16 *w_d, cudaStream_t st) {
     SpWParams W;
     memset(&W, 0, sizeof(W));
-    W.cout = c->cout; W.taps = c->kh * c->kw; W.cin = c->cin; W.kw = c->kw; W.cout64 = L.cout64; W.rows_f = L.rows_f;
-    int off = 0;
-    for (int p = 0; p < c->nparts; ++p) {
-        if (p == S.pu) { W.choff_u = off; W.c_u = c->parts[p].c; }
-        if (p == S.ps) { W.choff_s = off; W.c_s = c->parts[p].c; }
-        off += c->parts[p].c;
-    }
-    W.kext_u = S.kext_u; W.kext_s = S.kext_s; W.has_skip = S.ps >= 0; W.kd_sp = S.kd_sp;
-    W.want_fwd = S.fwd; W.want_dg = S.dgrad;
-    int slot = 0;
-    for (int cls = 0; cls < 4; ++cls) {
-        W.net[cls] = S.net[cls]; W.eoff[cls] = S.eoff[cls]; W.nex[cls] = S.ax.ne[cls & 1]; W.slot0[cls] = slot;
-        slot += S.net[cls] + (S.ps >= 0 ? W.taps : 0);
-        W.kc[cls] = S.kc[cls]; W.clsoff[cls] = S.clsoff[cls];
-    }
+    W.cout = c->cout; W.taps = c->kh * c->kw; W.cin = c->cin; W.kw = c->kw; W.cout64 = L.cout64; W.kd_sp = S.kd_sp;
+    for (int p = 0; p < S.pu; ++p) W.choff_u += c->parts[p].c;
+    for (int cls = 0; cls < 4; ++cls) { W.eoff[cls] = S.eoff[cls]; W.nex[cls] = S.ax.ne[cls & 1]; }
     for (int q = 0; q < 2; ++q)
         for (int e = 0; e < 4; ++e) { W.ybits[q][e] = S.ay.tapbits[q][e]; W.xbits[q][e] = S.ax.tapbits[q][e]; }
-    if (S.fwd) {
-        sp_weight_prepare_kernel<<<dim3(c->cout, slot), 128, 0, st>>>(w_master, W, w_f, w_d);
-        PCB_LAUNCH_CHECK();
-    } else if (S.dgrad) {
-        sp_weight_dg_kernel<<<dim3(W.c_u, S.net_total), 128, 0, st>>>(w_master, W, w_d);
-        PCB_LAUNCH_CHECK();
-    }
-    return 0;
-}
-
-// sub-pixel tiles are at most 64 columns wide: two stages of (A tile + up to four weight tiles) must fit next to the staging tile
-int sp_bn(int cols, long long m_total) { return std::min(pick_bn(cols, m_total, true), 64); }
-
-template <int BLOCK_N, int MODE>
-int launch_sp_n(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, cudaStream_t st) {
-    int nb_max = 1;
-    for (int i = 0; i < TB.n_items; ++i) nb_max = std::max(nb_max, TB.it[i].nb);
-    const size_t a_room = (static_cast<size_t>(TB.rows_max) * 128 + 1023) / 1024 * 1024;
-    const size_t stage = a_room + static_cast<size_t>(nb_max) * BLOCK_N * 128;
-    const size_t fixed = tma_fixed_smem(BLOCK_N, false);
-    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (MAX_SMEM - fixed) / stage));
-    PCB_CHECK(P.stages >= 2, "sub-pixel conv: stage of %zu bytes does not fit twice", stage);
-    const size_t smem = fixed + P.stages * stage;
-    auto kern = pconv_tc_sp_kernel<BLOCK_N, MODE>;
-    PCB_SMEM_OPT_IN(kern, MAX_SMEM);
-    const int num_tiles = ((P.m_total + BLOCK_M - 1) / BLOCK_M) * (P.ncols / BLOCK_N);
-    const int grid = std::min(num_tiles, pcb_num_sms());
-    kern<<<grid, TMA_THREADS, smem, st>>>(P, TB, tw, ta0, ta1);
+    sp_weight_dg_kernel<<<dim3(c->parts[S.pu].c, S.net_total), 128, 0, st>>>(w_master, W, w_d);
     PCB_LAUNCH_CHECK();
     return 0;
 }
 
-template <int MODE>
-int launch_sp(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUtensorMap &ta0, const CUtensorMap &ta1, int bn, cudaStream_t st) {
-    if (bn == 64) return launch_sp_n<64, MODE>(P, TB, tw, ta0, ta1, st);
-    return launch_sp_n<32, MODE>(P, TB, tw, ta0, ta1, st);
-}
+// sub-pixel tiles are at most 64 columns wide
+int sp_bn(int cols, long long m_total) { return std::min(pick_bn(cols, m_total, true), 64); }
 
-// internal streams for the four class launches of low-resolution layers (one set per device and host thread)
-struct ClassStreams4 { cudaStream_t aux[3]; cudaEvent_t ev_fork, ev_join[3]; bool ready; };
-int class_streams(ClassStreams4 **out) {
-    static thread_local ClassStreams4 cs_all[PCB_MAX_DEVICES] = {};
-    ClassStreams4 &CS = cs_all[pcb_cur_device()];
-    if (!CS.ready) {
-        for (int i = 0; i < 3; ++i) {
-            PCB_CUDA(cudaStreamCreateWithFlags(&CS.aux[i], cudaStreamNonBlocking));
-            PCB_CUDA(cudaEventCreateWithFlags(&CS.ev_join[i], cudaEventDisableTiming));
-        }
-        PCB_CUDA(cudaEventCreateWithFlags(&CS.ev_fork, cudaEventDisableTiming));
-        CS.ready = true;
-    }
-    *out = &CS;
-    return 0;
-}
-
-// forward over cat([up2x(x_u), x_s]): four class launches (see pconv_tc_sp_kernel)
-int sp_forward(const pcb_conv *c, const SpPlan &S, const Layout &L, const bf16 *w_sp, const float *bias, void *y, int y_cstride, const float *msum,
-               double *bn_sums, const pcb_ep *ep, int *flag, cudaStream_t st) {
-    const int hc = c->h / 2, wc = c->w / 2;
-    const long long m_class = static_cast<long long>(c->n) * hc * wc;
-    TcParams P;
-    base_params(P, c, L);
-    fill_parts(c, L, P.parts, nullptr, 0);
-    P.ho = hc; P.wo = wc; P.m_total = static_cast<int>(m_class);
-    P.sub = 2; P.fh = c->ho; P.fw = c->wo;
-    P.bias = bias; P.msum = msum; P.y = static_cast<bf16 *>(y); P.y_cstride = y_cstride; P.abort_flag = flag;
-    P.bn_sums = bn_sums; P.bn_c = c->cout;
-    set_ep(P, ep);
-    P.box_w = S.bw; P.box_h = S.bh; P.box_n = S.bn;
-    const int cols = (c->cout <= 32) ? 32 : L.rows_f;
-    const int bn = sp_bn(cols, m_class);
-    P.ncols = cols;
-    for (int p = 0; p < c->nparts; ++p)
-        if (c->parts[p].mask) P.use_fix = 1;
-    const bool row_tiles = S.bw == 128 && S.bh == 1 && S.bn == 1;       // halo re-use possible for the traversal-stride-1 part
-    const int taps = c->kh * c->kw;
-    const long long class_tiles = ((m_class + BLOCK_M - 1) / BLOCK_M) * (cols / bn);
-    const bool fork = class_tiles < pcb_num_sms() && !getenv("PCB_DISABLE_CLASS_STREAMS");
-    ClassStreams4 *CS = nullptr;
-    if (fork) {
-        if (int rc = class_streams(&CS)) return rc;
-        PCB_CUDA(cudaEventRecord(CS->ev_fork, st));
-    }
-    for (int cls = 0; cls < 4; ++cls) {
-        const int py = cls >> 1, px = cls & 1;
-        const int ney = S.ay.ne[py], nex = S.ax.ne[px], ey0 = S.ay.e0[py], ex0 = S.ax.e0[px];
-        SpTable TB;
-        memset(&TB, 0, sizeof(TB));
-        const int pu = S.pu, ps = S.ps;
-        TB.step[pu] = 1; TB.es[pu] = 1; TB.ph[pu] = hc; TB.pw[pu] = wc;
-        const bool halo_u = row_tiles && nex > 1 && !getenv("PCB_DISABLE_TMA_HALO");
-        TB.arows[pu] = BLOCK_M + (halo_u ? nex - 1 : 0);
-        int ni = 0;
-        for (int e = 0; e < ney; ++e) {
-            if (halo_u) {
-                SpItem &it = TB.it[ni++];
-                it.part = pu; it.dx = ex0; it.dy = ey0 + e; it.nb = nex; it.wk = (e * nex) * S.kext_u; it.wk_step = S.kext_u; it.shift0 = 0; it.dshift = 8;
-            } else {
-                for (int f = 0; f < nex; ++f) {
-                    SpItem &it = TB.it[ni++];
-                    it.part = pu; it.dx = ex0 + f; it.dy = ey0 + e; it.nb = 1; it.wk = (e * nex + f) * S.kext_u; it.wk_step = 0; it.shift0 = 0; it.dshift = 0;
-                }
-            }
-        }
-        if (ps >= 0) {
-            TB.step[ps] = 2; TB.es[ps] = 2; TB.ph[ps] = c->h; TB.pw[ps] = c->w;
-            TB.arows[ps] = BLOCK_M;                                      // (a 129-pixel box at traversal stride 2 would exceed the 256-element TMA box limit)
-            for (int tr = 0; tr < c->kh; ++tr)
-                for (int tc = 0; tc < c->kw; ++tc) {
-                    SpItem &it = TB.it[ni++];
-                    it.part = ps; it.dx = px + tc * c->dil - c->pad_w; it.dy = py + tr * c->dil - c->pad_h; it.nb = 1;
-                    it.wk = S.net[cls] * S.kext_u + (tr * c->kw + tc) * S.kext_s; it.wk_step = 0; it.shift0 = 0; it.dshift = 0;
-                }
-        }
-        TB.n_items = ni;
-        TB.rows_max = std::max(TB.arows[pu], ps >= 0 ? TB.arows[ps] : 0);
-        PCB_CHECK(ni <= SP_MAX_ITEMS, "sub-pixel conv: too many items");
-        CUtensorMap ta[TC_MAX_PARTS], tw;
-        memset(ta, 0, sizeof(ta));
-        if (int rc = make_tmap_nhwc(&ta[pu], c->parts[pu].x, S.c8_u, wc, hc, c->n, c->parts[pu].x_cstride, S.bw + (halo_u ? nex - 1 : 0), S.bh, S.bn, 1)) return rc;
-        if (ps >= 0) {
-            if (int rc = make_tmap_nhwc(&ta[ps], c->parts[ps].x, S.c8_s, c->w, c->h, c->n, c->parts[ps].x_cstride, S.bw, S.bh, S.bn, 2)) return rc;
-        } else ta[1 - pu] = ta[pu];
-        if (int rc = make_tmap_2d(&tw, w_sp + S.clsoff[cls], L.rows_f, S.kc[cls], S.kc[cls], bn)) return rc;
-        TcParams Q = P;
-        Q.py = py; Q.px = px;
-        cudaStream_t cs = (fork && cls > 0) ? CS->aux[cls - 1] : st;
-        if (fork && cls > 0) PCB_CUDA(cudaStreamWaitEvent(cs, CS->ev_fork, 0));
-        if (int rc = launch_sp<0>(Q, TB, tw, ta[0], ta[1], bn, cs)) return rc;
-        if (fork && cls > 0) {
-            PCB_CUDA(cudaEventRecord(CS->ev_join[cls - 1], cs));
-            PCB_CUDA(cudaStreamWaitEvent(st, CS->ev_join[cls - 1], 0));
-        }
-    }
+template <int BLOCK_N>
+int launch_sp_n(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUtensorMap &ta, cudaStream_t st) {
+    const size_t stage = A_STAGE_BYTES + static_cast<size_t>(BLOCK_N) * 128;
+    const size_t fixed = tma_fixed_smem(BLOCK_N);
+    P.stages = static_cast<int>(std::min<size_t>(MAX_RING, (MAX_SMEM - fixed) / stage));
+    PCB_CHECK(P.stages >= 2, "sub-pixel conv: stage of %zu bytes does not fit twice", stage);
+    const size_t smem = fixed + P.stages * stage;
+    auto kern = pconv_tc_sp_kernel<BLOCK_N>;
+    PCB_SMEM_OPT_IN(kern, MAX_SMEM);
+    const int num_tiles = ((P.m_total + BLOCK_M - 1) / BLOCK_M) * (P.ncols / BLOCK_N);
+    const int grid = std::min(num_tiles, pcb_num_sms());
+    kern<<<grid, TMA_THREADS, smem, st>>>(P, TB, tw, ta);
+    PCB_LAUNCH_CHECK();
     return 0;
 }
 
@@ -2966,7 +2567,6 @@ int sp_dgrad_up(const pcb_conv *c, const SpPlan &S, const Layout &L, const void 
     const int bn = sp_bn(S.kext_u, m_src);
     SpTable TB;
     memset(&TB, 0, sizeof(TB));
-    TB.step[0] = 2; TB.es[0] = 2; TB.ph[0] = c->ho; TB.pw[0] = c->wo; TB.arows[0] = BLOCK_M; TB.rows_max = BLOCK_M;
     int ni = 0;
     for (int cls = 0; cls < 4; ++cls) {
         const int py = cls >> 1, px = cls & 1;
@@ -2974,15 +2574,15 @@ int sp_dgrad_up(const pcb_conv *c, const SpPlan &S, const Layout &L, const void 
         for (int e = 0; e < ney; ++e)
             for (int f = 0; f < nex; ++f) {
                 SpItem &it = TB.it[ni++];
-                it.part = 0; it.dx = px - 2 * (S.ax.e0[px] + f); it.dy = py - 2 * (S.ay.e0[py] + e); it.nb = 1;
-                it.wk = (S.eoff[cls] + e * nex + f) * L.cout64; it.wk_step = 0; it.shift0 = 0; it.dshift = 0;
+                it.dx = px - 2 * (S.ax.e0[px] + f); it.dy = py - 2 * (S.ay.e0[py] + e);
+                it.wk = (S.eoff[cls] + e * nex + f) * L.cout64;
             }
     }
     TB.n_items = ni;
     CUtensorMap ta, tw;
     if (int rc = make_tmap_nhwc(&ta, dc, P.dc_c8, c->wo, c->ho, c->n, dc_cstride, S.bw, S.bh, S.bn, 2)) return rc;
     if (int rc = make_tmap_2d(&tw, w_sp_dg, rup(S.kext_u, 128), S.kd_sp, S.kd_sp, bn)) return rc;
-    return launch_sp<1>(P, TB, tw, ta, ta, bn, st);
+    return (bn == 64) ? launch_sp_n<64>(P, TB, tw, ta, st) : launch_sp_n<32>(P, TB, tw, ta, st);
 }
 
 }  // namespace
@@ -3023,9 +2623,9 @@ void pcb_tc_weight_layout(const pcb_conv *c, size_t *fwd_elems, size_t *dgrad_el
     const Layout L = layout_of(c);
     *fwd_elems = static_cast<size_t>(L.rows_f) * L.kf;
     *dgrad_elems = L.rowpack ? 0 : static_cast<size_t>(rup(L.ktap, 128)) * L.kd;
-    // sub-pixel path (conv over a 2x-upsampled source): the per-class effective-tap matrices follow the regular operands
+    // sub-pixel data gradient (conv over a 2x-upsampled source): the per-class effective-tap matrices follow the regular operand
     const SpPlan S = sp_plan(c);
-    if (S.ok) { *fwd_elems += static_cast<size_t>(S.sp_fwd_elems); *dgrad_elems += static_cast<size_t>(S.sp_dg_elems); }
+    if (S.ok) *dgrad_elems += static_cast<size_t>(S.sp_dg_elems);
     if (smallco_ok(c) && pcb_k2r_ok(c)) {
         size_t fb, db, fx, dx;
         k2r_bases(L, &fb, &db);
@@ -3038,8 +2638,7 @@ void pcb_tc_weight_layout(const pcb_conv *c, size_t *fwd_elems, size_t *dgrad_el
 // true when the data gradient of the 2x-upsampled part is delivered at that part's own (source) resolution
 bool pcb_tc_subpixel(const pcb_conv *c) {
     if (smallco_ok(c)) return pcb_k2r_ok(c);
-    const SpPlan S = sp_plan(c);
-    return S.ok && S.dgrad;
+    return sp_plan(c).ok;
 }
 
 int pcb_tc_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd, void *w_dgrad, bool zero_padding, cudaStream_t st) {
@@ -3063,8 +2662,7 @@ int pcb_tc_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd,
         const SpPlan S = sp_plan(c);
         if (S.ok) {
             PCB_CHECK(w_dgrad != nullptr, "sub-pixel weights need the dgrad operand buffer");
-            return sp_weight_prepare(c, S, L, w_master, static_cast<bf16 *>(w_fwd) + static_cast<size_t>(L.rows_f) * L.kf,
-                                     static_cast<bf16 *>(w_dgrad) + static_cast<size_t>(rup(L.ktap, 128)) * L.kd, st);
+            return sp_weight_prepare(c, S, L, w_master, static_cast<bf16 *>(w_dgrad) + static_cast<size_t>(rup(L.ktap, 128)) * L.kd, st);
         }
         return 0;
     }
@@ -3083,8 +2681,7 @@ int pcb_tc_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd,
     const SpPlan S = sp_plan(c);
     if (S.ok) {
         PCB_CHECK(w_dgrad != nullptr, "sub-pixel weights need the dgrad operand buffer");
-        return sp_weight_prepare(c, S, L, w_master, static_cast<bf16 *>(w_fwd) + static_cast<size_t>(L.rows_f) * L.kf,
-                                 static_cast<bf16 *>(w_dgrad) + static_cast<size_t>(rup(L.ktap, 128)) * L.kd, st);
+        return sp_weight_prepare(c, S, L, w_master, static_cast<bf16 *>(w_dgrad) + static_cast<size_t>(rup(L.ktap, 128)) * L.kd, st);
     }
     return 0;
 }
@@ -3095,7 +2692,6 @@ int pcb_tc_forward_mask_pass(const pcb_conv *c, uint64_t *tapmask, cudaStream_t 
     PCB_CHECK(m_total < (1ll << 31), "problem too large");
     const Layout L = layout_of(c);
     if (smallco_ok(c) || stem_ok(c)) return 0;            // (the stem applies its mask in the space-to-depth pass)
-    { const SpPlan S = sp_plan(c); if (S.ok && S.fwd) return 0; }   // sub-pixel forward: its fixers read the mask planes themselves
     bool any_mask = false;
     for (int p = 0; p < c->nparts; ++p) any_mask = any_mask || (c->parts[p].mask != nullptr);
     if (tma_fwd_ok(c) && !any_mask) return 0;            // no holes: TMA's out-of-range zero fill is all the validity there is
@@ -3107,15 +2703,15 @@ int pcb_tc_forward_mask_pass(const pcb_conv *c, uint64_t *tapmask, cudaStream_t 
     return launch_tapmask(c, tapmask, st);
 }
 
-// true when pcb_tc_forward_ws accumulates the BatchNorm statistics of its output itself (tensor-core kernels, no split-K)
+// true when pcb_tc_forward_ws accumulates the BatchNorm statistics of its output itself (tensor-core kernels)
 bool pcb_tc_fuses_bn_stats(const pcb_conv *c) {
     return pcb_tc_fuses_affine_act(c) && !getenv("PCB_DISABLE_FUSED_BN_STATS");
 }
 
 // true when pcb_tc_forward_ws can apply an eval-mode BatchNorm + activation in its epilogue (the same kernels as above: the
-// small-Cout / RGB-tail kernels have no such epilogue, split-K applies its epilogue in a separate finish kernel)
+// small-Cout / RGB-tail kernels have no such epilogue)
 bool pcb_tc_fuses_affine_act(const pcb_conv *c) {
-    return pcb_tc_eligible(c) && !smallco_ok(c) && !getenv("PCB_SPLITK");
+    return pcb_tc_eligible(c) && !smallco_ok(c);
 }
 
 int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, const float *msum,
@@ -3141,13 +2737,6 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
             return pcb_k2r_forward(c, smallco_layout(L), w_fwd, static_cast<const bf16 *>(w_fwd) + fb, bias, y, y_cstride, msum, tapmask, st);
         }
         return pcb_smallco_forward(c, smallco_layout(L), w_fwd, bias, y, y_cstride, msum, st);
-    }
-    {
-        const SpPlan S = sp_plan(c);
-        if (S.ok && S.fwd) {
-            PCB_CHECK(bn_sums == nullptr || pcb_tc_fuses_bn_stats(c), "fused BatchNorm statistics requested from a kernel that does not produce them");
-            return sp_forward(c, S, L, static_cast<const bf16 *>(w_fwd) + static_cast<size_t>(L.rows_f) * L.kf, bias, y, y_cstride, msum, bn_sums, ep, flag, st);
-        }
     }
     TcParams P;
     base_params(P, c, L);
@@ -3189,20 +2778,6 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
         P.ncols = (c->cout <= 32) ? 32 : L.rows_f;
         P.wk_base = 0; P.wk_col = L.ktap; P.wk_row = c->kw * L.ktap;
         if (int rc = make_tmap_2d(&tm, w_fwd, L.rows_f, L.kf, L.kf, bn)) return rc;
-        P.ksplit = pick_ksplit(m_total, P.ncols, bn, L.ktap / BLOCK_K);
-        if (P.ksplit > 1) {
-            PCB_CHECK(!P.ep_on, "split-K forward: the finish kernel does not apply a fused BatchNorm + activation");
-            const size_t bytes = static_cast<size_t>(m_total) * P.ncols * sizeof(float);
-            P.partial = splitk_scratch(bytes);
-            PCB_CHECK(P.partial != nullptr, "split-K scratch allocation failed");
-            PCB_CUDA(cudaMemsetAsync(P.partial, 0, bytes, st));
-            if (int rc = launch_tma<0>(P, tm, ta[0], ta[1], bn, halo, st)) return rc;
-            const long long work = m_total * (y_cstride / 8);
-            splitk_finish_fwd_kernel<<<static_cast<int>(std::min<long long>((work + 255) / 256, 8ll * pcb_num_sms())), 256, 0, st>>>(
-                P.partial, P.ncols, msum, bias, c->cout, c->no_guard, m_total, static_cast<bf16 *>(y), y_cstride);
-            PCB_LAUNCH_CHECK();
-            return 0;
-        }
         return launch_tma<0>(P, tm, ta[0], ta[1], bn, halo, st);
     }
     if (int rc = make_tmap_2d(&tm, w_fwd, L.rows_f, L.kf, L.kf, L.bn_f)) return rc;
@@ -3233,7 +2808,7 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
     const SpPlan SPL = sp_plan(c);
     void *dx_local[TC_MAX_PARTS] = {nullptr, nullptr};
     for (int p = 0; p < c->nparts && p < TC_MAX_PARTS; ++p) dx_local[p] = dx[p];
-    if (SPL.ok && SPL.dgrad) {
+    if (SPL.ok) {
         if (dx[SPL.pu] != nullptr)
             if (int rc = sp_dgrad_up(c, SPL, L, dc, dc_cstride, static_cast<const bf16 *>(w_dgrad) + static_cast<size_t>(rup(L.ktap, 128)) * L.kd,
                                      dx[SPL.pu], dx_cstride[SPL.pu], flag, st)) return rc;
@@ -3264,18 +2839,6 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
         CUtensorMap ta;
         if (int rc = make_tmap_nhwc(&ta, dc, P.dc_c8, c->wo, c->ho, c->n, dc_cstride, P.box_w + (halo ? (c->kw - 1) * c->dil : 0), P.box_h, P.box_n, 1)) return rc;
         if (int rc = make_tmap_2d(&tm, w_dgrad, rup(L.ktap, 128), L.kd, L.kd, bn)) return rc;
-        P.ksplit = pick_ksplit(m_total, P.ncols, bn, L.cout64 / BLOCK_K);
-        if (P.ksplit > 1) {
-            const size_t bytes = static_cast<size_t>(m_total) * P.ncols * sizeof(float);
-            P.partial = splitk_scratch(bytes);
-            PCB_CHECK(P.partial != nullptr, "split-K scratch allocation failed");
-            PCB_CUDA(cudaMemsetAsync(P.partial, 0, bytes, st));
-            if (int rc = launch_tma<1>(P, tm, ta, ta, bn, halo, st)) return rc;
-            const long long work = m_total * (P.ncols / 8);
-            splitk_finish_dgrad_kernel<<<static_cast<int>(std::min<long long>((work + 255) / 256, 8ll * pcb_num_sms())), 256, 0, st>>>(P.partial, P);
-            PCB_LAUNCH_CHECK();
-            return 0;
-        }
         return launch_tma<1>(P, tm, ta, ta, bn, halo, st);
     }
     if (tma_dgrad_s2_ok(c)) {
@@ -3291,24 +2854,12 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
         // run concurrently: fork onto three internal streams after an event on `st`, join before returning (also valid
         // inside a stream capture: the internal streams join the capture and leave it again).
         const long long class_tiles = ((m_class + BLOCK_M - 1) / BLOCK_M) * (L.ktap / bn);
-        const bool fork = class_tiles < pcb_num_sms() && !getenv("PCB_DISABLE_CLASS_STREAMS");
-        // internal streams / events: one set per device AND per host thread (two host threads driving dgrads on two streams
-        // must not share the fork / join events)
-        struct ClassStreams { cudaStream_t aux[3]; cudaEvent_t ev_fork, ev_join[3]; bool ready; };
-        static thread_local ClassStreams cs_all[PCB_MAX_DEVICES] = {};
-        ClassStreams &CS = cs_all[pcb_cur_device()];
-        cudaStream_t *aux = CS.aux;
-        cudaEvent_t *ev_join = CS.ev_join;
-        if (fork && !CS.ready) {
-            for (int i = 0; i < 3; ++i) {
-                PCB_CUDA(cudaStreamCreateWithFlags(&aux[i], cudaStreamNonBlocking));
-                PCB_CUDA(cudaEventCreateWithFlags(&ev_join[i], cudaEventDisableTiming));
-            }
-            PCB_CUDA(cudaEventCreateWithFlags(&CS.ev_fork, cudaEventDisableTiming));
-            CS.ready = true;
+        const bool fork = class_tiles < pcb_num_sms();
+        ClassStreams *CS = nullptr;
+        if (fork) {
+            if (int rc = class_streams(&CS)) return rc;
+            PCB_CUDA(cudaEventRecord(CS->ev_fork, st));
         }
-        cudaEvent_t ev_fork = CS.ev_fork;
-        if (fork) PCB_CUDA(cudaEventRecord(ev_fork, st));
         for (int cls = 0; cls < 4; ++cls) {
             TcParams Q = P;
             const int py = cls >> 1, px = cls & 1;
@@ -3323,12 +2874,12 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
                               halo_stages_fit(Q.kw, 1, bn);
             CUtensorMap ta;
             if (int rc = make_tmap_nhwc(&ta, dc, P.dc_c8, c->wo, c->ho, c->n, dc_cstride, Q.box_w + (halo ? Q.kw - 1 : 0), Q.box_h, Q.box_n, 1)) return rc;
-            cudaStream_t cs = (fork && cls > 0) ? aux[cls - 1] : st;
-            if (fork && cls > 0) PCB_CUDA(cudaStreamWaitEvent(cs, ev_fork, 0));
+            cudaStream_t cs = (fork && cls > 0) ? CS->aux[cls - 1] : st;
+            if (fork && cls > 0) PCB_CUDA(cudaStreamWaitEvent(cs, CS->ev_fork, 0));
             if (int rc = launch_tma<1>(Q, tm, ta, ta, bn, halo, cs)) return rc;
             if (fork && cls > 0) {
-                PCB_CUDA(cudaEventRecord(ev_join[cls - 1], cs));
-                PCB_CUDA(cudaStreamWaitEvent(st, ev_join[cls - 1], 0));
+                PCB_CUDA(cudaEventRecord(CS->ev_join[cls - 1], cs));
+                PCB_CUDA(cudaStreamWaitEvent(st, CS->ev_join[cls - 1], 0));
             }
         }
         return 0;

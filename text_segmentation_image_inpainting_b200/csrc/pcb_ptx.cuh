@@ -81,12 +81,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *m, 
         : "memory");
 }
 // 4-D tile (channels, x, y, image): out-of-range coordinates (negative included) are zero-filled -- the conv padding
-// L2 prefetch of a tile (no shared-memory destination, no barrier): turns the later load of the same box into an L2 hit
-__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap *m, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-                 : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap *m, int c0, int c1, int c2, int c3, uint32_t bar) {
     asm volatile(
         "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"

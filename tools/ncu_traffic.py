@@ -17,9 +17,11 @@ def family(name):
         return "tc_wgrad"
     if "dw4_s1_wgrad" in n or "dw3_wgrad" in n or "dw_wgrad" in n:
         return "dw_wgrad"
-    m = re.search(r"pconv_tc_(tma|sp|persistent)_kernel<\s*(?:\(int\))?\s*(\d+),\s*(?:\(int\))?\s*(\d+)", n)
+    m = re.search(r"pconv_tc_(tma|persistent)_kernel<\s*(?:\(int\))?\s*(\d+),\s*(?:\(int\))?\s*(\d+)", n)
     if m:
         return "tc_dgrad" if m.group(3) == "1" else "tc_fwd"
+    if "pconv_tc_sp_kernel" in n:
+        return "tc_dgrad"
     if "smallco_fwd" in n or "k2r_combine" in n:
         return "tc_fwd"
     if "smallco_dgrad" in n:
