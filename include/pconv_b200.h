@@ -142,6 +142,14 @@ int pcb_pconv_backward_data(const pcb_conv *c, const void *dc, int dc_cstride, c
  * every part is a full-resolution [n, h, w, dx_cstride] buffer and the caller reduces 2x2 blocks itself. */
 int pcb_conv_dgrad_at_source_resolution(const pcb_conv *c);
 
+/* The data gradient of a layer whose input came out of an in-place ReLU (the VGG16 blocks of loss.py:244-260), with that
+ * ReLU's backward applied in the kernel's epilogue: dx = 0 where relu_x <= 0 (torch's threshold_backward), otherwise what
+ * pcb_pconv_backward_data stores.  relu_x: the layer's input (bf16 NHWC, channel stride relu_cstride, 16-byte aligned); one part,
+ * dx[n,h,w,dx_cstride].  Only for problems with pcb_conv_dgrad_fuses_relu(c) == 1 (bf16, stride 1, the TMA-fed kernel). */
+int pcb_conv_dgrad_fuses_relu(const pcb_conv *c);
+int pcb_pconv_backward_data_relu(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_dgrad, void *dx, int dx_cstride,
+                                 const void *relu_x, int relu_cstride, pcb_stream_t stream);
+
 /* dw[co][r][s][ci] = sum_pixels dc[p][co] * (x*m)[p@tap][ci]   (fp32 KRSC, logical/unpadded, overwritten).
  * workspace: pcb_pconv_workspace(c) bytes (may be NULL when that is 0).                         */
 int pcb_pconv_backward_weight(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, pcb_stream_t stream);
@@ -286,6 +294,54 @@ int pcb_inpaint_sample(const pcb_inpaint_src *srcs, int n, int out, int strokes,
  * 3..7 zero), mask_plane uint8 [n][out][out] (1 = valid), clean fp32 [n][3][out][out].  Grids depend on n, cap_h and out only. */
 int pcb_inpaint_prepare(const pcb_inpaint_src *srcs, const pcb_inpaint_params *params, int n, int cap_h, int cap_w, int out,
                         int strokes, uint8_t *tmp, void *corrupted, int dtype, uint8_t *mask_plane, float *clean, pcb_stream_t stream);
+
+/* ---- inpainting loss (InpaintingLoss, loss.py:185-307) ---------------------------------------------------------------
+ * The VGG16 convolutions and the Gram products run on the convolution entry points above; these are the rest.  Reductions
+ * ADD into caller-zeroed fp64 sums; nothing synchronises.  Image strides are in elements (n, c, h, w order), so fp32 NCHW and
+ * NHWC (padded) views are both accepted.
+ *
+ * Pixel terms + VGG input batch, one thread per pixel: comp = m ? raw : output for the {0,1} plane m (= mask*raw +
+ * (1-mask)*output, loss.py:196); sums[0] += |output-origin| where valid, sums[1] += |output-origin| in holes, sums[2] / sums[3]
+ * += |horizontal| / |vertical| differences of comp (loss.py:303-307); vgg_in = [3n][h][w][8] in `dtype`: comp | output | origin,
+ * channels 3..7 zero.  raw, origin: fp32 NCHW [n,3,h,w]; output: `out_dtype`, 3 channels through out_strides (host [4]). */
+int pcb_inpaint_loss_pixel_forward(const float *raw, const float *origin, const void *output, int out_dtype, const long long *out_strides,
+                                   const uint8_t *plane, int n, int h, int w, void *vgg_in, int dtype, double *sums, pcb_stream_t stream);
+/* d loss / d output = gs * (coef[0] * m + coef[1] * (1-m)) * sign(output - origin) + (1-m) * (gs * d tv / d comp + dvgg_in[comp])
+ * + dvgg_in[output], gs = *gscale (device).  coef (host [4]): valid, hole, horizontal-TV and vertical-TV weights over their element
+ * counts.  dvgg_in: [2n][h][w][8] in `dtype` (comp | output) or NULL.  grad: `out_dtype`, through grad_strides (host [4]). */
+int pcb_inpaint_loss_pixel_backward(const float *raw, const float *origin, const void *output, int out_dtype, const long long *out_strides,
+                                    const uint8_t *plane, int n, int h, int w, const void *dvgg_in, int dtype, const float *coef,
+                                    const float *gscale, void *grad, const long long *grad_strides, pcb_stream_t stream);
+/* nn.MaxPool2d(2, 2) on NHWC [n,h,w,c] (h, w even, c % 8 == 0), torch's rule: a tap replaces the running maximum when it is
+ * greater or NaN (row-major order), so ties go to the first maximum and NaN propagates.  The backward recomputes the window
+ * maximum from x and writes every element of gx: gy at the maximum, 0 elsewhere; relu_mask != 0 also applies the backward of the
+ * in-place ReLU that produced x (0 where x <= 0). */
+int pcb_maxpool2x2_forward(const void *x, void *y, int dtype, int n, int h, int w, int c, pcb_stream_t stream);
+int pcb_maxpool2x2_backward(const void *gy, const void *x, void *gx, int dtype, int n, int h, int w, int c, int relu_mask, pcb_stream_t stream);
+/* f: NHWC features of 3n images (comp | output | origin), hw pixels x c channels each (c % 8 == 0):
+ * sums[0] += sum |f_comp - f_origin|, sums[1] += sum |f_output - f_origin|   (the perceptual L1 sums, loss.py:211-212). */
+int pcb_feature_l1_forward(const void *f, int dtype, int n, long long hw, int c, double *sums, pcb_stream_t stream);
+/* df (2n images comp | output) = gs * (l1_coef * sign(f - f_origin) + gram_coef * g_gram) + g_next; g_gram, g_next: [2n][hw][c]
+ * or NULL. */
+int pcb_feature_loss_backward(const void *f, int dtype, int n, long long hw, int c, const void *g_next, const void *g_gram, float l1_coef,
+                              float gram_coef, const float *gscale, void *df, pcb_stream_t stream);
+/* gram: fp32 [3n][c][c] unnormalised products F F^T (comp | output | origin); G = gram / norm (loss.py:294-300):
+ * sums[0] += sum |G_comp - G_origin|, sums[1] += sum |G_output - G_origin|. */
+int pcb_gram_l1_forward(const float *gram, int n, int c, float norm, double *sums, pcb_stream_t stream);
+/* t: fp32 [2n][c][c] = S + S^T, S = sign(G_i - G_origin) for the images comp | output: the weight of the Gram backward
+ * dF = F (S + S^T) k (a 1x1 convolution; integer-valued, so exact in bf16). */
+int pcb_gram_sign_sym(const float *gram, int n, int c, float norm, float *t, pcb_stream_t stream);
+/* Data gradient of a 3x3 / pad 1 / stride 1 convolution with 3 input channels (VGG16 conv1_1) in kernel-to-row form:
+ * pcb_k2r_image_weight writes the fp32 [32][cout] weight of the 1x1 problem Z[p][tap*3 + ci] = sum_co dc[p][co] W[co][ci][tap]
+ * (W: fp32 OIHW [cout][3][3][3]; rows 27..31 zero), which the caller lays out with pcb_conv_weight_prepare and runs with
+ * pcb_pconv_forward (1x1, cout -> 32, plain) into z [n][h][w][32];  pcb_k2r_image_dgrad then sums the taps:
+ * dx[q][ci] = sum_tap z[q - tap + 1][tap*3 + ci], dx: [n][h][w][8] in `dtype` (channels 3..7 zero). */
+int pcb_k2r_image_weight(const float *w_oihw, int cout, float *wz, pcb_stream_t stream);
+int pcb_k2r_image_dgrad(const void *z, int dtype, int n, int h, int w, void *dx, pcb_stream_t stream);
+/* sums: the 16 fp64 sums [valid, hole, tv_h, tv_v, perceptual comp|output per stage (3x2), style comp|output per stage (3x2)];
+ * h_inv (host [16]): their normalisers.  terms (fp32 [5], unweighted): valid, hole, tv, perceptual, style;
+ * loss = 1 valid + 6 hole + 0.1 tv + 0.05 perceptual + 120 style (loss.py:223-224). */
+int pcb_inpaint_loss_finalize(const double *sums, const double *h_inv, float *loss, float *terms, pcb_stream_t stream);
 
 /* ---- loss / optimiser used by the benchmark step (SURVEY 8d: loss = out.abs().mean()) ------ */
 int pcb_l1_mean_forward(const void *x, int dtype, long long numel, float *loss /* device scalar, overwritten */,

@@ -87,6 +87,22 @@ _SIGS = {
     "pcb_inpaint_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_inpaint_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                     c_void_p]),
+    "pcb_inpaint_loss_pixel_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
+                                               c_int, c_void_p, c_void_p]),
+    "pcb_inpaint_loss_pixel_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
+                                                c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcb_maxpool2x2_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "pcb_maxpool2x2_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "pcb_feature_l1_forward": (c_int, [c_void_p, c_int, c_int, c_ll, c_int, c_void_p, c_void_p]),
+    "pcb_feature_loss_backward": (c_int, [c_void_p, c_int, c_int, c_ll, c_int, c_void_p, c_void_p, c_float, c_float, c_void_p, c_void_p,
+                                          c_void_p]),
+    "pcb_gram_l1_forward": (c_int, [c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "pcb_gram_sign_sym": (c_int, [c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "pcb_inpaint_loss_finalize": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcb_k2r_image_weight": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "pcb_k2r_image_dgrad": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pcb_conv_dgrad_fuses_relu": (c_int, [ctypes.POINTER(Conv)]),
+    "pcb_pconv_backward_data_relu": (c_int, [ctypes.POINTER(Conv), c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "pcb_l1_mean_forward": (c_int, [c_void_p, c_int, c_ll, c_void_p, c_void_p, c_void_p]),
     "pcb_l1_mean_backward": (c_int, [c_void_p, c_int, c_ll, c_float, c_void_p, c_void_p]),
     "pcb_sgd_step": (c_int, [c_void_p, c_void_p, c_void_p, c_ll, c_float, c_float, c_float, c_int, c_int, c_void_p]),

@@ -184,6 +184,22 @@ PCB_API int pcb_pconv_backward_data(const pcb_conv *c, const void *dc, int dc_cs
     return pcb_generic_dgrad(c, dc, dc_cstride, w_fwd, dx, dx_cstride, st);
 }
 
+PCB_API int pcb_conv_dgrad_fuses_relu(const pcb_conv *c) {
+    if (!c || c->force_generic || validate(c, false) || use_dw(c) || !use_tc(c) || !pcb_tc_dgrad_supported(c)) return 0;
+    return pcb_tc_dgrad_fuses_relu(c) ? 1 : 0;
+}
+
+PCB_API int pcb_pconv_backward_data_relu(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_dgrad, void *dx, int dx_cstride,
+                                         const void *relu_x, int relu_cstride, pcb_stream_t stream) {
+    PCB_CHECK(dc && w_dgrad && dx && relu_x && dc_cstride >= c->cout, "pcb_pconv_backward_data_relu: bad arguments");
+    PCB_CHECK(pcb_conv_dgrad_fuses_relu(c), "pcb_pconv_backward_data_relu: this problem's kernel does not fuse the ReLU backward "
+                                            "(ask pcb_conv_dgrad_fuses_relu first)");
+    PCB_CHECK((reinterpret_cast<uintptr_t>(dc) & 15) == 0, "pcb_pconv_backward_data_relu: dc misaligned");
+    void *dxs[1] = {dx};
+    const int cs[1] = {dx_cstride};
+    return pcb_tc_dgrad(c, dc, dc_cstride, w_dgrad, dxs, cs, static_cast<cudaStream_t>(stream), relu_x, relu_cstride);
+}
+
 static int backward_weight_impl(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, pcb_stream_t stream) {
     if (int rc = validate(c, true)) return rc;
     PCB_CHECK(dc && dw && dc_cstride >= c->cout, "pcb_pconv_backward_weight: bad arguments");

@@ -82,6 +82,9 @@ struct TcParams {
     const float *bias; const float *msum; bf16 *y; int y_cstride;
     // dgrad gather source
     const bf16 *dc; int dc_cstride, dc_c8, dc_kext;
+    // dgrad (TMA-fed kernel, one part): backward of the in-place ReLU that produced the layer's input -- the stored gradient is 0
+    // where relu_x <= 0 (torch's threshold_backward).  null: off.
+    const bf16 *relu_x; int relu_cstride;
     int *abort_flag;
     // TMA-fed kernel: the 128 pixels of an M tile form the box {box_w, box_h, box_n} of the (x, y, image) pixel grid
     int box_w, box_h, box_n, stages, use_fix;
@@ -831,6 +834,7 @@ __device__ __forceinline__ void tc_epilogue_bf16(const TcParams &P, const EpiRow
         const int col = n0 + c0;
         bf16 *orow = nullptr;
         int nstore = 0;                                  // channels to store from this 32-column chunk (multiple of 8)
+        int xlocal = 0;                                  // dgrad: channel of the part's input that column col is
         float scale = 1.f;
         if (MODE == 0) {
             if (er.rvalid && col < P.y_cstride) { orow = P.y + er.mo * P.y_cstride + col; nstore = min(32, P.y_cstride - col); }
@@ -844,6 +848,7 @@ __device__ __forceinline__ void tc_epilogue_bf16(const TcParams &P, const EpiRow
                     orow = pt.dx + er.mo * pt.dx_cstride + local;
                     nstore = min(32, pt.c8 - local);
                     scale = er.dscale[p];
+                    xlocal = local;
                 }
             }
         }
@@ -857,6 +862,23 @@ __device__ __forceinline__ void tc_epilogue_bf16(const TcParams &P, const EpiRow
             for (int j = 0; j < 16; ++j) {
                 const float2 f = __bfloat1622float2(ob[j]);
                 ob[j] = __floats2bfloat162_rn(f.x * scale, f.y * scale);
+            }
+        }
+        if (MODE == 1 && P.relu_x != nullptr && nstore > 0) {
+            // in-place ReLU backward: one 16-byte load of the layer's input per 8 channels, a select per element
+            const uint4 *xr = reinterpret_cast<const uint4 *>(P.relu_x + er.mo * P.relu_cstride + xlocal);
+#pragma unroll 1
+            for (int j = 0; j < 4; ++j) {
+                if (j * 8 >= nstore) break;
+                const uint4 xv = xr[j];
+                const __nv_bfloat162 *xb = reinterpret_cast<const __nv_bfloat162 *>(&xv);
+                __nv_bfloat162 *ob = reinterpret_cast<__nv_bfloat162 *>(&o[j]);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const float2 xf = __bfloat1622float2(xb[k]);
+                    const __nv_bfloat162 z = __float2bfloat162_rn(0.f);
+                    ob[k] = __halves2bfloat162(xf.x <= 0.f ? z.x : ob[k].x, xf.y <= 0.f ? z.y : ob[k].y);
+                }
             }
         }
         if (nstore > 0) {
@@ -2787,8 +2809,17 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
 
 bool pcb_tc_dgrad_supported(const pcb_conv *c) { return pcb_tc_eligible(c) && !is_rowpack(c); }
 
+// the data-gradient problems whose kernel can apply the ReLU backward of the layer's input in its epilogue: the TMA-fed
+// stride-1 kernel on a single-part layer (not the small-Cout, sub-pixel or gather kernels)
+bool pcb_tc_dgrad_fuses_relu(const pcb_conv *c) {
+    return c->nparts == 1 && !smallco_ok(c) && !sp_plan(c).ok && tma_dgrad_ok(c);
+}
+
 int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_dgrad, void *const *dx, const int *dx_cstride,
-                 cudaStream_t st) {
+                 cudaStream_t st, const void *relu_x, int relu_cstride) {
+    PCB_CHECK(relu_x == nullptr || (pcb_tc_dgrad_fuses_relu(c) && relu_cstride % 8 == 0 && relu_cstride >= rup(c->cin, 8) &&
+                                    (reinterpret_cast<uintptr_t>(relu_x) & 15) == 0),
+              "tensor-core dgrad: the ReLU backward is fused only on the TMA-fed stride-1 kernel (16-byte aligned input, channel stride %% 8 == 0)");
     int *flag = abort_flag_ptr();
     PCB_CHECK(flag != nullptr, "cudaMalloc(abort flag) failed");
     const long long m_total = static_cast<long long>(c->n) * c->h * c->w;
@@ -2827,6 +2858,7 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
                   "tensor-core dgrad: dx[%d] must be 16-byte aligned with a channel stride that is a multiple of 8", p);
     }
     P.dc = static_cast<const bf16 *>(dc); P.dc_cstride = dc_cstride; P.dc_c8 = rup(c->cout, 8); P.dc_kext = L.cout64;
+    P.relu_x = static_cast<const bf16 *>(relu_x); P.relu_cstride = relu_cstride;
     P.abort_flag = flag;
     int bn = (L.ktap % 128 == 0) ? 128 : 64;
     P.ncols = L.ktap;

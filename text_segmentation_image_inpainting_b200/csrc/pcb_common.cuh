@@ -157,8 +157,11 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
 bool pcb_tc_fuses_bn_stats(const pcb_conv *c);
 bool pcb_tc_fuses_affine_act(const pcb_conv *c);
 bool pcb_tc_subpixel(const pcb_conv *c);
+// relu_x (optional, TMA-fed single-part stride-1 problems only: pcb_tc_dgrad_fuses_relu): the epilogue also applies the backward
+// of the in-place ReLU that produced the layer's input, dx = 0 where relu_x <= 0 (relu_x: bf16 NHWC, channel stride relu_cstride)
 int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_dgrad, void *const *dx, const int *dx_cstride,
-                 cudaStream_t st);
+                 cudaStream_t st, const void *relu_x = nullptr, int relu_cstride = 0);
+bool pcb_tc_dgrad_fuses_relu(const pcb_conv *c);
 int pcb_tc_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st);
 int pcb_tc_read_abort_flag(int *value);
 // layers with <= 8 output channels (conv_smallco.cu); weights are read from the tensor-core operand layouts

@@ -377,6 +377,34 @@ class InpaintTrainStep(TrainStep):
         return self.static_loss
 
 
+class InpaintLossTrainStep(InpaintTrainStep):
+    """InpaintTrainStep trained on the reference's InpaintingLoss (loss.py:185-225) instead of the benchmark's L1 stand-in:
+    the batcher's clean image is both `raw_input` (where the mask is valid they agree) and `origin`.  The loss runs inside the
+    same captured graph.  The extractor's frozen parameters stay out of the gradient arena; its operand buffers are laid out
+    once (keyed on the weights, not the step's weight epoch, so they are not refreshed every step) and kept alive with the
+    graph's captured operands.  `last_terms` holds the five unweighted terms of the last step (device fp32 [5]:
+    valid, hole, tv, perceptual, style)."""
+
+    def __init__(self, net: torch.nn.Module, batcher, extractor, feature_range=3, **kwargs):
+        from .loss import InpaintingLoss
+        super().__init__(net, batcher, **kwargs)
+        self.criterion = InpaintingLoss(extractor, feature_range)
+        self._frozen_caches = [m.__dict__ for m in extractor.modules() if isinstance(getattr(m, "_wcache", None), dict)]
+
+    def warmup_and_capture(self, eager_warmup=2):
+        super().warmup_and_capture(eager_warmup=eager_warmup)
+        if self._captured_operands is not None:
+            self._captured_operands += [(d["_wcache"].get("val"), d.get("_pcb_k2r_cache", {}).get("val")) for d in self._frozen_caches]
+
+    @property
+    def last_terms(self):
+        return self.criterion.last_terms
+
+    def _forward_loss(self, x, mask):
+        xin, hm, clean = self.batcher.prepare(self._params)
+        return self.criterion(clean, hm, self.net((xin, hm)), clean)
+
+
 class SegTrainStep(TrainStep):
     """The same step for the dense segmentation networks (models/text_segmentation.py: `net(x)`, no masks): BASELINE.json
     configs[1] (TextSegament, batch 8) and configs[3] (XceptionTextSegment, batch 16, bf16).  `mask` is ignored."""
