@@ -295,6 +295,37 @@ int pcb_inpaint_sample(const pcb_inpaint_src *srcs, int n, int out, int strokes,
 int pcb_inpaint_prepare(const pcb_inpaint_src *srcs, const pcb_inpaint_params *params, int n, int cap_h, int cap_w, int out,
                         int strokes, uint8_t *tmp, void *corrupted, int dtype, uint8_t *mask_plane, float *clean, pcb_stream_t stream);
 
+/* ---- segmentation training data (TextSegmentationData.process_images, Dataloader.py:66-74) -------------------------------
+ * One decoded source per image: the gray (`L`) page uint8 [h][page_stride] and its text mask uint8 [h][mask_stride]. */
+typedef struct {
+    const uint8_t *page;
+    const uint8_t *mask;
+    int32_t h, w, page_stride, mask_stride;
+} pcb_seg_src;
+/* What one image draws: the crop box (RandomResizedCrop.get_params(scale=(0.1, 2)): top i, left j, height h, width w), whether
+ * ColorJitter applies brightness before contrast, and the two factors (float32, as Pillow's blend uses them). */
+typedef struct {
+    int32_t top, left, height, width;
+    int32_t brightness_first;
+    float brightness, contrast;
+    int32_t reserved;
+} pcb_seg_params;
+/* Host-side check of a staged batch (h_srcs, h_params: HOST copies; h_params may be NULL): 1..cap_n images, each within the
+ * cap_h x cap_w capacity, row strides large enough, crop boxes inside their sources and at most 8x the output size `out`,
+ * order flag 0 / 1, finite non-negative factors. */
+int pcb_seg_validate(const pcb_seg_src *h_srcs, const pcb_seg_params *h_params, int n, int cap_n, int cap_h, int cap_w, int out);
+/* Draw the parameters of n <= 1024 images on the device (Philox4x32-10, key = rng[0], counter = (slot, image, rng[1])) and
+ * advance rng[1]: RandomResizedCrop.get_params(scale=(0.1, 2), ratio=(3/4, 4/3)), the brightness / contrast order of
+ * ColorJitter's randperm(4) and both factors on [0.8, 1.2].  srcs, rng, params: device memory. */
+int pcb_seg_sample(const pcb_seg_src *srcs, int n, uint64_t *rng, pcb_seg_params *params, pcb_stream_t stream);
+/* process_images for a batch, three launches: Pillow-exact bicubic crop + resize of page and mask, the page histogram,
+ * ColorJitter's brightness and contrast blends in the drawn order (contrast about int(mean + 0.5) of the image it is applied
+ * to), ToTensor and, if h_norm (host [6]: mean[3], std[3]) is given, Normalize.  tmp: uint8 [n][cap_h][out][2], planes: uint8
+ * [2][n][out][out], hist: int32 [n][256] (scratch).  Outputs: x [n][out][out][8] NHWC in `dtype`, the page in channels 0..2,
+ * channels 3..7 zero; target fp32 [n][out][out] (the mask's ToTensor).  Grids depend on n, cap_h and out only. */
+int pcb_seg_prepare(const pcb_seg_src *srcs, const pcb_seg_params *params, int n, int cap_h, int cap_w, int out, uint8_t *tmp,
+                    uint8_t *planes, int *hist, const float *h_norm, void *x, int dtype, float *target, pcb_stream_t stream);
+
 /* ---- inpainting loss (InpaintingLoss, loss.py:185-307) ---------------------------------------------------------------
  * The VGG16 convolutions and the Gram products run on the convolution entry points above; these are the rest.  Reductions
  * ADD into caller-zeroed fp64 sums; nothing synchronises.  Image strides are in elements (n, c, h, w order), so fp32 NCHW and
@@ -342,6 +373,23 @@ int pcb_k2r_image_dgrad(const void *z, int dtype, int n, int h, int w, void *dx,
  * h_inv (host [16]): their normalisers.  terms (fp32 [5], unweighted): valid, hole, tv, perceptual, style;
  * loss = 1 valid + 6 hole + 0.1 tv + 0.05 perceptual + 120 style (loss.py:223-224). */
 int pcb_inpaint_loss_finalize(const double *sums, const double *h_inv, float *loss, float *terms, pcb_stream_t stream);
+
+/* ---- segmentation losses (BinaryFocalLoss, SoftBootstrapCrossEntropy, loss.py:58-121) ------------------------------------
+ * x: [n, 1, h, w] logits in `dtype` through x_strides (host [4], elements, n c h w order): NCHW or a channel-padded NHWC view.
+ * target: fp32 [n][h][w].  loss PCB_SEG_FOCAL (p0 = gamma, reduction PCB_SEG_MEAN only) or PCB_SEG_BOOTSTRAP (p0 = beta,
+ * one_minus_beta = 1 - beta).  Forward: out = the fp32 loss (a scalar, or [n*h*w] for PCB_SEG_NONE), reduced deterministically
+ * through `partials` (device, pcb_seg_loss_partials(n*h*w) doubles) and `counter` (device, one zero-initialised uint32 per
+ * concurrent call; the kernel leaves it zero).  Backward: dx = gout * d loss / d x in `dtype` through dx_strides; gout (device):
+ * the upstream gradient, a scalar or [n*h*w] for PCB_SEG_NONE. */
+enum { PCB_SEG_FOCAL = 0, PCB_SEG_BOOTSTRAP = 1 };
+enum { PCB_SEG_NONE = 0, PCB_SEG_MEAN = 1, PCB_SEG_SUM = 2 };
+int pcb_seg_loss_partials(long long count);
+int pcb_seg_loss_forward(const void *x, int dtype, const long long *x_strides, const float *target, int n, int h, int w, int loss,
+                         int reduction, float p0, float one_minus_beta, float background_weight, float words_weight, double *partials,
+                         unsigned int *counter, float *out, pcb_stream_t stream);
+int pcb_seg_loss_backward(const void *x, int dtype, const long long *x_strides, const float *target, int n, int h, int w, int loss,
+                          int reduction, float p0, float one_minus_beta, float background_weight, float words_weight, const float *gout,
+                          void *dx, const long long *dx_strides, pcb_stream_t stream);
 
 /* ---- loss / optimiser used by the benchmark step (SURVEY 8d: loss = out.abs().mean()) ------ */
 int pcb_l1_mean_forward(const void *x, int dtype, long long numel, float *loss /* device scalar, overwritten */,

@@ -11,6 +11,8 @@ from . import build as _build
 PCB_F32, PCB_BF16 = 0, 1
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_RELU6 = 0, 1, 2, 3
 MAX_PARTS = 8
+SEG_FOCAL, SEG_BOOTSTRAP = 0, 1
+SEG_NONE, SEG_MEAN, SEG_SUM = 0, 1, 2
 
 c_int, c_ll, c_float, c_void_p, c_size_t = ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
@@ -87,6 +89,15 @@ _SIGS = {
     "pcb_inpaint_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_inpaint_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                     c_void_p]),
+    "pcb_seg_validate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int]),
+    "pcb_seg_sample": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "pcb_seg_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                c_void_p, c_void_p]),
+    "pcb_seg_loss_partials": (c_int, [c_ll]),
+    "pcb_seg_loss_forward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
+                                     c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcb_seg_loss_backward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
+                                      c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcb_inpaint_loss_pixel_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                                c_int, c_void_p, c_void_p]),
     "pcb_inpaint_loss_pixel_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,

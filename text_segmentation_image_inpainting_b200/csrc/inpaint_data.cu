@@ -8,68 +8,23 @@
 //   3. inpaint_fused_kernel: per 32x32 output tile, the vertical pass over the tile plus the 9-pixel dilation halo, the strokes,
 //      the threshold, the 10x10 dilation (separable max in shared memory), grayscale, /255, x mask and the three stores.
 // Grids are sized from the batcher's capacity (largest source), so one captured graph serves any mix of source sizes.
-// The resampler follows Pillow's fixed-point 8-bit path bit for bit: the weights are computed in double with explicitly
-// rounded operations (no FMA contraction, which Pillow's x86-64 build does not do either).
-#include "pcb_common.cuh"
+// The resampler follows Pillow's fixed-point 8-bit path bit for bit (pil_data.cuh, shared with seg_data.cu).
+#include "pil_data.cuh"
 
 #define ST static_cast<cudaStream_t>(stream)
 #define PCB_API extern "C" __attribute__((visibility("default")))
 
 namespace {
 
-constexpr int KMAX = 33;      // taps of a bicubic window at scale 8 (2 * ceil(2 * 8) + 1): box / out <= 8
-constexpr int PB = 22;        // Pillow's PRECISION_BITS for 8-bit images
+using pil::KMAX;
+using pil::PB;
+using pil::clip8;
+using pil::pil_coeffs;
+
 constexpr int HX = 128;       // horizontal pass: output columns per block (one per thread)
 constexpr int HROWS = 16;     // horizontal pass: box rows per block
 constexpr int T = 32;         // fused kernel: output tile edge
 constexpr int HT = T + 9;     // tile + dilation halo (5 rows / columns before, 4 after: cv2's anchor of a 10x10 kernel)
-
-__device__ __forceinline__ double bicubic(double x) {
-    const double a = -0.5;
-    if (x < 0.0) x = -x;
-    if (x < 1.0) return __dadd_rn(__dmul_rn(__dmul_rn(__dsub_rn(__dmul_rn(a + 2.0, x), a + 3.0), x), x), 1.0);
-    if (x < 2.0) return __dmul_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, 5.0), x), 8.0), x), 4.0), a);
-    return 0.0;
-}
-
-// Pillow's precompute_coeffs + normalize_coeffs_8bpc for output index xx of a box of `insize` input pixels resampled to
-// `outsize`: writes the integer weights to k[0], k[stride], ... and returns the first tap; *count = number of taps.
-__device__ int pil_coeffs(int xx, int insize, int outsize, int *k, int stride, int *count) {
-    const double scale = __ddiv_rn(static_cast<double>(insize), static_cast<double>(outsize));
-    const double fs = scale < 1.0 ? 1.0 : scale;
-    const double support = __dmul_rn(2.0, fs), ss = __ddiv_rn(1.0, fs);
-    const double center = __dmul_rn(static_cast<double>(xx) + 0.5, scale);
-    int xmin = static_cast<int>(__dadd_rn(__dsub_rn(center, support), 0.5));
-    if (xmin < 0) xmin = 0;
-    int xmax = static_cast<int>(__dadd_rn(__dadd_rn(center, support), 0.5));
-    if (xmax > insize) xmax = insize;
-    xmax -= xmin;
-    if (xmax > KMAX) xmax = KMAX;                    // unreachable for box / out <= 8 (checked on the host)
-    double w[KMAX];
-    double ww = 0.0;
-#pragma unroll
-    for (int x = 0; x < KMAX; ++x) {
-        if (x < xmax) {
-            w[x] = bicubic(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(x + xmin), center), 0.5), ss));
-            ww = __dadd_rn(ww, w[x]);
-        }
-    }
-#pragma unroll
-    for (int x = 0; x < KMAX; ++x) {
-        if (x < xmax) {
-            const double v = ww != 0.0 ? __ddiv_rn(w[x], ww) : w[x];
-            const double s = __dmul_rn(v, static_cast<double>(1 << PB));
-            k[x * stride] = v < 0 ? static_cast<int>(__dadd_rn(-0.5, s)) : static_cast<int>(__dadd_rn(0.5, s));
-        }
-    }
-    *count = xmax;
-    return xmin;
-}
-
-__device__ __forceinline__ int clip8(int acc) {
-    acc >>= PB;
-    return acc < 0 ? 0 : (acc > 255 ? 255 : acc);
-}
 
 __device__ __forceinline__ bool source_ok(const pcb_inpaint_src &s, const pcb_inpaint_params &p, int cap_h, int cap_w) {
     return s.h >= 1 && s.w >= 1 && s.h <= cap_h && s.w <= cap_w && p.top >= 0 && p.left >= 0 && p.height >= 1 && p.width >= 1 &&
@@ -77,32 +32,6 @@ __device__ __forceinline__ bool source_ok(const pcb_inpaint_src &s, const pcb_in
 }
 
 // ------------------------------------------------------------------------------------------------ 1. parameter sampler
-__device__ __forceinline__ uint4 philox(uint4 c, uint32_t k0, uint32_t k1) {
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
-        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
-        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-        k0 += 0x9E3779B9u;
-        k1 += 0xBB67AE85u;
-    }
-    return c;
-}
-
-struct Draws {
-    uint32_t img, c_lo, c_hi, k0, k1;
-    // uniform of slot s in [0, 1), 24 bits: word s % 4 of philox(counter = (s / 4, image, step lo, step hi), key = seed)
-    __device__ float u(int s) const {
-        const uint4 r = philox(make_uint4(static_cast<uint32_t>(s >> 2), img, c_lo, c_hi), k0, k1);
-        const int l = s & 3;
-        const uint32_t w = l == 0 ? r.x : (l == 1 ? r.y : (l == 2 ? r.z : r.w));
-        return static_cast<float>(w >> 8) * 5.9604644775390625e-8f;
-    }
-    __device__ int randint(int s, int lo, int hi) const {   // lo..hi inclusive
-        return lo + static_cast<int>(__dmul_rn(static_cast<double>(u(s)), static_cast<double>(hi - lo + 1)));
-    }
-};
-
 __global__ void __launch_bounds__(1024) inpaint_sample_kernel(const pcb_inpaint_src *__restrict__ srcs, int n, int out, int strokes,
                                                               unsigned long long *rng, pcb_inpaint_params *__restrict__ params) {
     const int t = threadIdx.x;
@@ -110,40 +39,15 @@ __global__ void __launch_bounds__(1024) inpaint_sample_kernel(const pcb_inpaint_
     __syncthreads();
     if (t == 0) rng[1] = step + 1;
     if (t >= n) return;
-    const Draws d{static_cast<uint32_t>(t), static_cast<uint32_t>(step), static_cast<uint32_t>(step >> 32), static_cast<uint32_t>(seed),
-                  static_cast<uint32_t>(seed >> 32)};
+    const pil::Draws d(static_cast<uint32_t>(t), step, seed);
     const int H = srcs[t].h, W = srcs[t].w;
     pcb_inpaint_params &p = params[t];
     p = pcb_inpaint_params{};
-    // RandomResizedCrop.get_params(scale=(0.5, 2.0), ratio=(3/4, 4/3)); slots 4a..4a+3 of attempt a: scale, log-aspect, top, left
-    const float lr0 = -0.28768208622932434f, span = 0.5753642320632935f;    // float32 log(3/4), log(4/3) - log(3/4) as torch has them
-    const double area = static_cast<double>(H) * static_cast<double>(W);
-    bool found = false;
-    for (int a = 0; a < 10 && !found; ++a) {
-        const float s = __fadd_rn(0.5f, __fmul_rn(1.5f, d.u(4 * a)));
-        const float r = __fadd_rn(lr0, __fmul_rn(span, d.u(4 * a + 1)));
-        const double target = __dmul_rn(area, static_cast<double>(s));
-        const double aspect = static_cast<double>(static_cast<float>(exp(static_cast<double>(r))));
-        const int w = static_cast<int>(rint(__dsqrt_rn(__dmul_rn(target, aspect))));
-        const int h = static_cast<int>(rint(__dsqrt_rn(__ddiv_rn(target, aspect))));
-        if (0 < w && w <= W && 0 < h && h <= H) {
-            p.top = d.randint(4 * a + 2, 0, H - h);
-            p.left = d.randint(4 * a + 3, 0, W - w);
-            p.height = h;
-            p.width = w;
-            found = true;
-        }
-    }
-    if (!found) {                                    // the centre-crop fallback
-        const double in_ratio = __ddiv_rn(static_cast<double>(W), static_cast<double>(H));
-        int w = W, h = H;
-        if (in_ratio < 0.75) h = static_cast<int>(rint(__ddiv_rn(static_cast<double>(W), 0.75)));
-        else if (in_ratio > 4.0 / 3.0) w = static_cast<int>(rint(__dmul_rn(static_cast<double>(H), 4.0 / 3.0)));
-        p.top = (H - h) / 2;
-        p.left = (W - w) / 2;
-        p.height = h;
-        p.width = w;
-    }
+    const pil::Box box = pil::crop_box(d, H, W, 0.5f, 1.5f);        // RandomResizedCrop.get_params(scale=(0.5, 2.0))
+    p.top = box.top;
+    p.left = box.left;
+    p.height = box.height;
+    p.width = box.width;
     p.gray = static_cast<double>(d.u(40)) < 0.4 ? 1 : 0;            // RandomGrayscale(p=0.4)
     if (strokes) {                                                   // random_masks(size=out, offset=10)
         const int off = 10;

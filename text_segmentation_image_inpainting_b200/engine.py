@@ -337,21 +337,12 @@ class TrainStep:
             torch.cuda.synchronize()
 
 
-class InpaintTrainStep(TrainStep):
-    """TrainStep whose step begins with the GPU data path (data.InpaintBatcher.prepare): the captured graph samples the crop
-    boxes, grayscale draws and strokes, resizes, masks and dilates on the device and then runs the training step on the result.
-    Per step the host only decodes, calls ``batcher.stage(samples)`` and ``step()``.
+class _BatcherStep:
+    """`warmup_and_capture()` and `step(params=None)` of a training step whose step begins with a GPU batcher's `prepare()`
+    (data.InpaintBatcher, data.SegBatcher): the captured graph draws the parameters and prepares the batch on the device.  Per
+    step the host only decodes, calls ``batcher.stage(samples)`` and ``step()``.
 
     ``step(params)`` with explicit parameters needs ``use_graph=False`` (the graph holds the device sampler)."""
-
-    def __init__(self, net: torch.nn.Module, batcher, **kwargs):
-        super().__init__(net, compute_dtype=batcher.dtype, **kwargs)
-        self.batcher = batcher
-        self._params = None
-
-    def _forward_loss(self, x, mask):
-        xin, hm, _ = self.batcher.prepare(self._params)
-        return ops.l1_mean(self.net((xin, hm)))
 
     def warmup_and_capture(self, eager_warmup=2):
         super().warmup_and_capture(torch.empty(0, device=self.batcher.device), None, eager_warmup=eager_warmup)
@@ -375,6 +366,23 @@ class InpaintTrainStep(TrainStep):
             self._allreduce()
             self.graph_update.replay()
         return self.static_loss
+
+
+class InpaintTrainStep(_BatcherStep, TrainStep):
+    """TrainStep whose step begins with the GPU data path (data.InpaintBatcher.prepare): the captured graph samples the crop
+    boxes, grayscale draws and strokes, resizes, masks and dilates on the device and then runs the training step on the result.
+    Per step the host only decodes, calls ``batcher.stage(samples)`` and ``step()``.
+
+    ``step(params)`` with explicit parameters needs ``use_graph=False`` (the graph holds the device sampler)."""
+
+    def __init__(self, net: torch.nn.Module, batcher, **kwargs):
+        super().__init__(net, compute_dtype=batcher.dtype, **kwargs)
+        self.batcher = batcher
+        self._params = None
+
+    def _forward_loss(self, x, mask):
+        xin, hm, _ = self.batcher.prepare(self._params)
+        return ops.l1_mean(self.net((xin, hm)))
 
 
 class InpaintLossTrainStep(InpaintTrainStep):
@@ -415,6 +423,23 @@ class SegTrainStep(TrainStep):
         xin = buf[:, :c]
         xin.copy_(x)
         return ops.l1_mean(self.net(xin))
+
+
+class SegLossTrainStep(_BatcherStep, SegTrainStep):
+    """SegTrainStep trained on the reference's data and losses: the step begins with the GPU segmentation data path
+    (data.SegBatcher.prepare: crop, resize, ColorJitter, ToTensor on the device) and ends in ``criterion(net(x), target)``
+    (loss.BinaryFocalLoss or loss.SoftBootstrapCrossEntropy with a reduced output), all in the one captured graph.  The
+    logits reach the loss as the network returns them, the [n, 1, h, w] view of a channel-padded NHWC buffer."""
+
+    def __init__(self, net: torch.nn.Module, batcher, criterion, **kwargs):
+        super().__init__(net, compute_dtype=batcher.dtype, **kwargs)
+        self.batcher = batcher
+        self.criterion = criterion
+        self._params = None
+
+    def _forward_loss(self, x, mask=None):
+        xin, target = self.batcher.prepare(self._params)
+        return self.criterion(self.net(xin), target)
 
 
 class InferStep:

@@ -1,5 +1,7 @@
-"""The reference's inpainting loss on the GPU (loss.py:185-307): `InpaintingLoss`, `FeatureExtractor`, `VggExtractor`,
-`gram_matrix` and `total_variation_loss` under the reference's names and signatures.
+"""The reference's losses on the GPU under the reference's names and signatures: the inpainting loss (loss.py:185-307:
+`InpaintingLoss`, `FeatureExtractor`, `VggExtractor`, `gram_matrix`, `total_variation_loss`) and the segmentation losses
+(loss.py:58-121: `BinaryFocalLoss`, `SoftBootstrapCrossEntropy`, csrc/seg_loss.cu).  `MultiClassFocalLoss` (multi-class logits;
+both segmentation networks have one output channel) and `BCERegionLoss` (the LSTM classifier head) have no GPU path.
 
     loss = 1 valid + 6 hole + 0.1 tv + 0.05 perceptual + 120 style          (loss.py:223-224)
 
@@ -453,3 +455,113 @@ def total_variation_loss(image):
     _lib.check(lib.pcb_inpaint_loss_pixel_forward(img.data_ptr(), img.data_ptr(), img.data_ptr(), ops._dtype_code(img), _strides(img),
                                                   plane.data_ptr(), n, h, w, X.data_ptr(), ops._dtype_code(img), sums.data_ptr(), _stream()))
     return (sums[2] / (n * 3 * h * (w - 1)) + sums[3] / (n * 3 * (h - 1) * w)).float()
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# segmentation losses (loss.py:58-121)
+# ------------------------------------------------------------------------------------------------------------------------------
+class _SegLossFn(torch.autograd.Function):
+    """One forward and one backward launch of csrc/seg_loss.cu over [n, 1, h, w] logits read in place through their strides."""
+
+    @staticmethod
+    def forward(ctx, crit, x, target):
+        lib = _lib.load()
+        n, _, h, w = x.shape
+        count = n * h * w
+        ws = crit._workspace(x.device, count)
+        out = torch.empty((count, 1) if crit._reduction == _lib.SEG_NONE else (), dtype=torch.float32, device=x.device)
+        _lib.check(lib.pcb_seg_loss_forward(x.data_ptr(), ops._dtype_code(x), _strides(x), target.data_ptr(), n, h, w, crit._kind,
+                                            crit._reduction, *crit._coefs(), ws[0].data_ptr(), ws[1].data_ptr(), out.data_ptr(), _stream()))
+        ctx.crit = crit
+        ctx.save_for_backward(x, target)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        lib = _lib.load()
+        x, target = ctx.saved_tensors
+        crit = ctx.crit
+        n, _, h, w = x.shape
+        g = gout.detach().float().contiguous()
+        # the gradient in the input's own layout family: NHWC (channel-padded) for NHWC views, dense otherwise
+        if ops.nhwc_layout(x) is not None and not x.is_contiguous():
+            dx = ops.padded_empty(*x.shape, x.dtype, x.device)
+        else:
+            dx = torch.empty_like(x)
+        _lib.check(lib.pcb_seg_loss_backward(x.data_ptr(), ops._dtype_code(x), _strides(x), target.data_ptr(), n, h, w, crit._kind,
+                                             crit._reduction, *crit._coefs(), g.data_ptr(), dx.data_ptr(), _strides(dx), _stream()))
+        return None, dx, None
+
+
+class _SegLoss(nn.Module):
+    """Shared plumbing: input checks and the device workspace of the deterministic reduction."""
+
+    _kind = _lib.SEG_FOCAL
+    _reduction = _lib.SEG_MEAN
+
+    def _coefs(self):
+        raise NotImplementedError
+
+    def _workspace(self, dev, count):
+        """(fp64 partials, uint32 counter): the counter is zeroed once here and left zero by every forward launch."""
+        key = (str(dev), _lib.load().pcb_seg_loss_partials(count))
+        ws = self.__dict__.get("_pcb_ws")
+        if ws is None or ws[0] != key:
+            if torch.cuda.is_current_stream_capturing():
+                raise _lib.PcbError(f"{type(self).__name__}: run the loss once before capturing it for this input size")
+            ws = (key, (torch.empty((key[1],), dtype=torch.float64, device=dev), torch.zeros((1,), dtype=torch.int32, device=dev)))
+            self.__dict__["_pcb_ws"] = ws
+        return ws[1]
+
+    def forward(self, input, target):
+        assert input.dim() == 4 and input.size(1) == 1          # the reference's flatten_images assertion
+        assert target.dim() == 4 and target.size(1) == 1
+        if not input.is_cuda or input.dtype not in (torch.float32, torch.bfloat16):
+            raise _lib.PcbError(f"{type(self).__name__}: input must be a CUDA float32 or bfloat16 tensor")
+        if tuple(target.shape) != tuple(input.shape):
+            raise _lib.PcbError(f"{type(self).__name__}: target {tuple(target.shape)} does not match input {tuple(input.shape)}")
+        t = target.detach()
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            t = t.float().contiguous()
+        return _SegLossFn.apply(self, input, t)
+
+
+class BinaryFocalLoss(_SegLoss):
+    """loss.py:58-83 on the GPU: mean(exp(gamma * logsigmoid(-x (2t - 1))) * w * bce(x, t)), w = words_weights where t > 0,
+    background_weights elsewhere.  `input`: [n, 1, h, w] logits, fp32 or bf16, dense or the channel-padded NHWC view the
+    segmentation networks return (read in place); `target`: [n, 1, h, w] in [0, 1].  Returns the fp32 scalar loss (device);
+    the gradient goes to `input` only, through pt as well when gamma != 0."""
+
+    def __init__(self, gamma=0, background_weights=1, words_weights=2):
+        super().__init__()
+        self.gamma = gamma
+        self.background_weights = background_weights
+        self.words_weights = words_weights
+
+    def _coefs(self):
+        return float(self.gamma), 0.0, float(self.background_weights), float(self.words_weights)
+
+
+class SoftBootstrapCrossEntropy(_SegLoss):
+    """loss.py:86-121 on the GPU: w * bce(x, beta t + (1 - beta) [sigmoid(x) > 0.5]) reduced by mean (default), sum
+    (`size_average=False`) or not at all (`reduce=False`: fp32 [n*h*w, 1]).  The indicator carries no gradient; it equals
+    torch's CPU float32 `sigmoid(x) > 0.5` for every input value.  Inputs as for BinaryFocalLoss."""
+
+    _kind = _lib.SEG_BOOTSTRAP
+
+    def __init__(self, beta=0.95, background_weight=1, words_weight=2, size_average=True, reduce=True):
+        super().__init__()
+        self.beta = beta
+        self.background_weight = background_weight
+        self.words_weight = words_weight
+        self.size_average = size_average
+        self.reduce = reduce
+
+    @property
+    def _reduction(self):
+        if self.reduce is not None and not self.reduce:
+            return _lib.SEG_NONE
+        return _lib.SEG_SUM if self.size_average is not None and not self.size_average else _lib.SEG_MEAN
+
+    def _coefs(self):
+        return float(self.beta), float(1 - self.beta), float(self.background_weight), float(self.words_weight)

@@ -747,10 +747,24 @@ def side_streams():
     return list(_SIDE_STREAMS.values())
 
 
+def _in_capture(st) -> bool:
+    """True when `st` takes part in the capture of the current stream (it waited on captured work and holds captured work)."""
+    with torch.cuda.stream(st):
+        return torch.cuda.is_current_stream_capturing()
+
+
 def join_side_streams():
-    """Make the current stream wait for every weight gradient still running on a side stream (gradient sinks only)."""
+    """Make the current stream wait for every weight gradient still running on a side stream (gradient sinks only).
+
+    Inside a graph capture only the streams this capture forked are joined: a stream the captured step never used (the mask
+    stream of an earlier partial-convolution network, during the capture of a segmentation step) holds no captured work, and
+    waiting on it would end the capture with cudaErrorStreamCaptureIsolation."""
+    cur = torch.cuda.current_stream()
+    capturing = torch.cuda.is_current_stream_capturing()
     for st in list(_SIDE_STREAMS.values()) + list(_MASK_STREAMS.values()) + list(_PREFETCH_STREAMS.values()):
-        torch.cuda.current_stream().wait_stream(st)
+        if capturing and not _in_capture(st):
+            continue
+        cur.wait_stream(st)
     _DEFERRED.clear()
 
 
