@@ -116,8 +116,7 @@ int pcb_pconv_forward_bn(const pcb_conv *c, const void *w_fwd, const float *bias
  * Channels [cout, y_cstride) are zeros.  scale / shift: fp32 [cout] from pcb_bn_finalize(training = 0), or both NULL for an
  * activation alone ([PartialConv, PartialActivation] blocks).  act: PCB_ACT_*, slope: LeakyReLU's negative slope.
  * Only for problems with pcb_conv_fuses_affine_act(c) == 1 (the tensor-core kernels other than the small-Cout ones, and the
- * depthwise 3x3 kernels -- the problems pcb_conv_fuses_bn_stats accepts, whether or not PCB_DISABLE_FUSED_BN_STATS is set);
- * others are rejected.  mask_pass_done: see pcb_pconv_forward_premasked.                                                                */
+ * depthwise 3x3 kernels -- the problems pcb_conv_fuses_bn_stats accepts); others are rejected.  mask_pass_done: see pcb_pconv_forward_premasked.                                                                */
 int pcb_conv_fuses_affine_act(const pcb_conv *c);
 int pcb_pconv_forward_affine_act(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
                                  uint8_t *newmask, void *workspace, int mask_pass_done, const float *scale, const float *shift,

@@ -1,0 +1,131 @@
+"""Generate tests/golden/conv_dispatch.json for tests/test_conv_dispatch_cpu.py, in two steps:
+
+  1. on a GPU, record the `pcb_conv` descriptor (geometry and parts, no pointers) of every distinct convolution of the following
+     runs -- every descriptor `ops.ConvGeom.struct` hands to the library, so also the calls loss.py's VGG16 makes directly --
+       * one eager forward + backward of ImageFillOrigin 512^2 b8, TextSegament 512^2 b8 and XceptionTextSegment 512^2 b16 (bf16),
+       * the eager eval forward of XceptionTextSegment at 600^2 b1 (non-power-of-two grids: the gather kernels),
+       * one forward + backward of InpaintingLoss at 512^2 b8: the VGG16 forward over 3n = 24 images, its data gradient over
+         the 16 images the loss differentiates, and the 1x1 problem of conv1_1's data gradient,
+       * the cases of tests/gpu_cases.py, test_gpu_fwd_tiles.py and test_gpu_wgrad_tiles.py:
+         python tests/golden/make_golden_conv_dispatch.py --record descriptors.json
+  2. on any machine, evaluate every host query of the library on them and write the fixture:
+         python tests/golden/make_golden_conv_dispatch.py descriptors.json
+
+The queries depend on the SM count; without a visible device the library assumes 132 (H100 SXM), which is what the fixture
+holds.  Step 2 was run with the library of the commit before the dispatch was gathered into one plan per problem, so the
+test pins that the refactor kept every choice."""
+import json
+import os
+import sys
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(os.path.dirname(HERE))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+
+from test_conv_dispatch_cpu import FIELDS, FIXTURE, PART_FIELDS, conv_of, host_queries  # noqa: E402
+
+
+def describe(c):
+    d = {k: getattr(c, k) for k in FIELDS}
+    d["parts"] = [dict({k: getattr(c.parts[i], k) for k in PART_FIELDS}, mask=int(bool(c.parts[i].mask))) for i in range(c.nparts)]
+    return d
+
+
+def _tile_case_descs(cases, with_mode):
+    from text_segmentation_image_inpainting_b200 import _lib
+    out = []
+    for name, case in cases.items():
+        n, h, w, parts, cout, k, s, d = case[:8]
+        pad = d * (k - 1) // 2
+        c = _lib.Conv()
+        c.n, c.h, c.w, c.cin, c.cout, c.kh, c.kw = n, h, w, sum(p[0] for p in parts), cout, k, k
+        c.stride, c.pad_h, c.pad_w, c.dil, c.groups = s, pad, pad, d, 1
+        c.ho, c.wo = (h + 2 * pad - d * (k - 1) - 1) // s + 1, (w + 2 * pad - d * (k - 1) - 1) // s + 1
+        c.dtype, c.nparts, c.no_guard = _lib.PCB_BF16, len(parts), int(with_mode and case[8] == "no_guard")
+        for i, (ch, up, masked) in enumerate(parts):
+            c.parts[i].c, c.parts[i].x_cstride, c.parts[i].x_up, c.parts[i].mask_up = ch, ch, up, up
+            c.parts[i].mask = 1 if masked else None
+        out.append(describe(c))
+    return out
+
+
+def record(path):
+    import torch
+
+    import gpu_cases as G
+    import test_gpu_fwd_tiles
+    import test_gpu_wgrad_tiles
+    from oracle.detfill import det_fill_state_dict, det_tensor
+    from oracle.inpaint_loss import vgg_state_dict
+    from text_segmentation_image_inpainting_b200 import ops
+    from text_segmentation_image_inpainting_b200.engine import SegInferStep, SegTrainStep, TrainStep
+    from text_segmentation_image_inpainting_b200.loss import InpaintingLoss, VggExtractor
+    from text_segmentation_image_inpainting_b200.models import image_inpainting, text_segmentation
+    from text_segmentation_image_inpainting_b200.synthetic import random_hole_masks
+
+    dev = torch.device("cuda")
+    rec = []
+    struct = ops.ConvGeom.struct
+
+    def recording_struct(self, xs, force_generic=False):
+        c = struct(self, xs, force_generic)
+        rec.append(describe(c))
+        return c
+    ops.ConvGeom.struct = recording_struct
+    torch.manual_seed(0)
+    for mod, cls, batch, masks in ((image_inpainting, "ImageFillOrigin", 8, True), (text_segmentation, "TextSegament", 8, False),
+                                   (text_segmentation, "XceptionTextSegment", 16, False)):
+        net = getattr(mod, cls)().to(dev)
+        ts = (TrainStep if masks else SegTrainStep)(net, compute_dtype=torch.bfloat16, use_graph=False)
+        x = torch.randn(batch, 3, 512, 512, device=dev)
+        m = torch.from_numpy(random_hole_masks(batch, 512, 512, seed=0)).to(dev) if masks else None
+        ts._fwd_bwd(x, m)
+        torch.cuda.synchronize()
+        del net, ts
+    net = text_segmentation.XceptionTextSegment()
+    net.load_state_dict(det_fill_state_dict(net.state_dict()))
+    net = net.to(dev).eval()
+    with torch.no_grad():
+        SegInferStep(net)._forward(det_tensor("conv_dispatch.x", (1, 3, 600, 600)).to(dev))
+    torch.cuda.synchronize()
+    del net
+    vgg = VggExtractor(pretrained=False)
+    vgg.load_state_dict(vgg_state_dict(0))
+    crit = InpaintingLoss(vgg.to(dev))
+    clean = torch.rand(8, 3, 512, 512, device=dev)
+    mask = torch.from_numpy(random_hole_masks(8, 512, 512, seed=1)).to(dev)
+    out = ops.padded_empty(8, 3, 512, 512, torch.bfloat16, dev)
+    with torch.no_grad():
+        out.copy_(clean.to(torch.bfloat16))
+    out.requires_grad_(True)
+    crit(clean * mask, mask, out, clean).backward()
+    torch.cuda.synchronize()
+    for tag in G.CONV_CASES:
+        G.conv_case(tag, dev)
+    for tag in G.LAZYCAT_CASES:
+        G.lazycat_case(tag, dev)
+    torch.cuda.synchronize()
+    ops.ConvGeom.struct = struct
+    descs = rec + _tile_case_descs(test_gpu_fwd_tiles.CASES, True) + _tile_case_descs(test_gpu_wgrad_tiles.CASES, False)
+    uniq = {json.dumps(d, sort_keys=True): d for d in descs}
+    with open(path, "w") as f:
+        json.dump(sorted(uniq.values(), key=lambda d: json.dumps(d, sort_keys=True)), f)
+    print(f"{len(rec)} descriptors, {len(uniq)} distinct -> {path}")
+
+
+def expect(path):
+    from text_segmentation_image_inpainting_b200 import _lib
+    lib = _lib.load()
+    with open(path) as f:
+        descs = json.load(f)
+    cases = [{"conv": d, "expect": host_queries(lib, conv_of(d))} for d in descs]
+    with open(FIXTURE, "w") as f:
+        f.write('{"cases": [\n' + ",\n".join(json.dumps(c, sort_keys=True) for c in cases) + "\n]}\n")
+    print(f"{len(cases)} cases -> {FIXTURE}")
+
+
+if __name__ == "__main__":
+    if sys.argv[1] == "--record":
+        record(sys.argv[2])
+    else:
+        expect(sys.argv[1])

@@ -47,22 +47,30 @@ static int validate(const pcb_conv *c, bool need_x) {
     return 0;
 }
 
-static bool use_dw(const pcb_conv *c) { return pcb_dw_eligible(c); }
-static bool use_tc(const pcb_conv *c) { return !c->force_generic && !use_dw(c) && pcb_tc_eligible(c); }
+// the kernel family a problem dispatches to: the depthwise kernels, the tensor-core kernels or the shape-general ones
+// (force_generic: always the latter)
+enum Family { FAMILY_GENERIC, FAMILY_DW, FAMILY_TC };
+
+static Family family_of(const pcb_conv *c) {
+    if (c->force_generic) return FAMILY_GENERIC;
+    if (pcb_dw_eligible(c)) return FAMILY_DW;
+    return pcb_tc_eligible(c) ? FAMILY_TC : FAMILY_GENERIC;
+}
 
 #define PCB_API extern "C" __attribute__((visibility("default")))
 
-PCB_API int pcb_conv_uses_tensor_cores(const pcb_conv *c) { return (c && use_tc(c)) ? 1 : 0; }
+PCB_API int pcb_conv_uses_tensor_cores(const pcb_conv *c) { return (c && family_of(c) == FAMILY_TC) ? 1 : 0; }
 
 // 1 when pcb_pconv_backward_data writes the gradient of a 2x-UPSAMPLED source directly at that source's own (half) resolution:
 // dx[p] of such a part is then a [n, h/2, w/2, dx_cstride] buffer and no 2x2 reduction pass follows (the tensor-core sub-pixel path)
-PCB_API int pcb_conv_dgrad_at_source_resolution(const pcb_conv *c) { return (c && use_tc(c) && pcb_tc_subpixel(c)) ? 1 : 0; }
+PCB_API int pcb_conv_dgrad_at_source_resolution(const pcb_conv *c) { return (c && family_of(c) == FAMILY_TC && pcb_tc_subpixel(c)) ? 1 : 0; }
 
-PCB_API size_t pcb_pconv_workspace(const pcb_conv *c) { return (c && use_tc(c)) ? pcb_tc_workspace(c) : 0; }
+PCB_API size_t pcb_pconv_workspace(const pcb_conv *c) { return (c && family_of(c) == FAMILY_TC) ? pcb_tc_workspace(c) : 0; }
 
 PCB_API void pcb_conv_weight_layout(const pcb_conv *c, size_t *fwd_elems, size_t *dgrad_elems) {
-    if (use_dw(c)) { *fwd_elems = static_cast<size_t>(c->cin) * c->kh * c->kw; *dgrad_elems = 0; return; }   // [taps][c]
-    if (use_tc(c)) { pcb_tc_weight_layout(c, fwd_elems, dgrad_elems); return; }
+    const Family f = family_of(c);
+    if (f == FAMILY_DW) { *fwd_elems = static_cast<size_t>(c->cin) * c->kh * c->kw; *dgrad_elems = 0; return; }   // [taps][c]
+    if (f == FAMILY_TC) { pcb_tc_weight_layout(c, fwd_elems, dgrad_elems); return; }
     *fwd_elems = static_cast<size_t>(c->cout) * c->kh * c->kw * (c->cin / c->groups);
     *dgrad_elems = 0;
 }
@@ -72,8 +80,9 @@ int pcb_cast_weights(const float *src, void *dst, long long n, int dtype, cudaSt
 static int weight_prepare(const pcb_conv *c, const float *w_master_krsc, void *w_fwd, void *w_dgrad, bool zero_padding, pcb_stream_t stream) {
     PCB_CHECK(c && w_master_krsc && w_fwd, "pcb_conv_weight_prepare: null pointer");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (use_dw(c)) return pcb_dw_weight_prepare(c, w_master_krsc, w_fwd, st);
-    if (use_tc(c)) return pcb_tc_weight_prepare(c, w_master_krsc, w_fwd, w_dgrad, zero_padding, st);
+    const Family f = family_of(c);
+    if (f == FAMILY_DW) return pcb_dw_weight_prepare(c, w_master_krsc, w_fwd, st);
+    if (f == FAMILY_TC) return pcb_tc_weight_prepare(c, w_master_krsc, w_fwd, w_dgrad, zero_padding, st);
     return pcb_cast_weights(w_master_krsc, w_fwd, static_cast<long long>(c->cout) * c->kh * c->kw * (c->cin / c->groups), c->dtype, st);
 }
 
@@ -85,20 +94,18 @@ PCB_API int pcb_conv_weight_refresh(const pcb_conv *c, const float *w_master_krs
     return weight_prepare(c, w_master_krsc, w_fwd, w_dgrad, false, stream);
 }
 
-// 1 when the forward kernel this problem dispatches to can accumulate the per-channel BatchNorm statistics of its output itself
-PCB_API int pcb_conv_fuses_bn_stats(const pcb_conv *c) {
-    if (!c || c->force_generic) return 0;
-    if (use_dw(c)) return pcb_dw_fuses_bn_stats(c) ? 1 : 0;
-    return (use_tc(c) && pcb_tc_fuses_bn_stats(c)) ? 1 : 0;
+static bool fuses_epilogue(const pcb_conv *c) {
+    if (!c) return false;
+    const Family f = family_of(c);
+    return (f == FAMILY_DW && pcb_dw_fuses_epilogue(c)) || (f == FAMILY_TC && pcb_tc_fuses_epilogue(c));
 }
 
+// 1 when the forward kernel this problem dispatches to can accumulate the per-channel BatchNorm statistics of its output itself
+PCB_API int pcb_conv_fuses_bn_stats(const pcb_conv *c) { return fuses_epilogue(c) ? 1 : 0; }
+
 // 1 when the forward kernel this problem dispatches to can apply an eval-mode BatchNorm + activation in its epilogue: the same
-// problems as pcb_conv_fuses_bn_stats, independent of PCB_DISABLE_FUSED_BN_STATS (which only concerns the training statistics)
-PCB_API int pcb_conv_fuses_affine_act(const pcb_conv *c) {
-    if (!c || c->force_generic) return 0;
-    if (use_dw(c)) return pcb_dw_fuses_affine_act(c) ? 1 : 0;
-    return (use_tc(c) && pcb_tc_fuses_affine_act(c)) ? 1 : 0;
-}
+// problems as pcb_conv_fuses_bn_stats
+PCB_API int pcb_conv_fuses_affine_act(const pcb_conv *c) { return fuses_epilogue(c) ? 1 : 0; }
 
 static int pconv_forward_impl(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, float *msum,
                               uint8_t *newmask, void *workspace, bool mask_pass_done, double *bn_sums, const pcb_ep *ep,
@@ -111,11 +118,12 @@ static int pconv_forward_impl(const pcb_conv *c, const void *w_fwd, const float 
         if (int rc = pcb_mask_sums(c, msum, newmask, st)) return rc;
     PCB_CHECK(bn_sums == nullptr || pcb_conv_fuses_bn_stats(c), "pcb_pconv_forward_bn: this problem's kernel does not fuse the BatchNorm statistics (ask pcb_conv_fuses_bn_stats first)");
     PCB_CHECK(ep == nullptr || pcb_conv_fuses_affine_act(c), "pcb_pconv_forward_affine_act: this problem's kernel does not apply a fused BatchNorm + activation (ask pcb_conv_fuses_affine_act first)");
-    if (use_dw(c)) {
+    const Family f = family_of(c);
+    if (f == FAMILY_DW) {
         PCB_CHECK(y_cstride % 8 == 0, "depthwise forward: y channel stride must be a multiple of 8");
         return pcb_dw_forward(c, w_fwd, bias, y, y_cstride, msum, bn_sums, ep, st);
     }
-    if (use_tc(c)) {
+    if (f == FAMILY_TC) {
         PCB_CHECK(workspace != nullptr, "pcb_pconv_forward: workspace required for the tensor-core path");
         PCB_CHECK((reinterpret_cast<uintptr_t>(w_fwd) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0, "w / y must be 16-byte aligned");
         return pcb_tc_forward_ws(c, w_fwd, bias, y, y_cstride, msum, static_cast<uint64_t *>(workspace), mask_pass_done, bn_sums, ep, st);
@@ -154,7 +162,7 @@ PCB_API int pcb_pconv_mask_pass(const pcb_conv *c, float *msum, uint8_t *newmask
     PCB_CHECK(msum && newmask, "pcb_pconv_mask_pass: bad arguments");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (int rc = pcb_mask_sums(c, msum, newmask, st)) return rc;
-    if (use_tc(c) && !use_dw(c)) {
+    if (family_of(c) == FAMILY_TC) {
         PCB_CHECK(workspace != nullptr, "pcb_pconv_mask_pass: workspace required for the tensor-core path");
         return pcb_tc_forward_mask_pass(c, static_cast<uint64_t *>(workspace), st);
     }
@@ -171,21 +179,18 @@ PCB_API int pcb_pconv_backward_data(const pcb_conv *c, const void *dc, int dc_cs
     if (int rc = validate(c, false)) return rc;
     PCB_CHECK(dc && w_fwd && dx && dx_cstride && dc_cstride >= c->cout, "pcb_pconv_backward_data: bad arguments");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (use_dw(c)) {
+    const Family f = family_of(c);
+    if (f == FAMILY_DW) {
         if (!dx[0]) return 0;
         PCB_CHECK(dc_cstride % 8 == 0 && dx_cstride[0] % 8 == 0, "depthwise dgrad: channel strides must be multiples of 8");
         return pcb_dw_dgrad(c, dc, dc_cstride, w_fwd, dx[0], dx_cstride[0], st);
     }
-    if (use_tc(c)) {
-        PCB_CHECK(pcb_tc_dgrad_supported(c), "data gradient of a row-packed (cin <= 8) tensor-core layer: set force_generic and pass KRSC weights");
-        PCB_CHECK(w_dgrad != nullptr && (reinterpret_cast<uintptr_t>(dc) & 15) == 0, "pcb_pconv_backward_data: w_dgrad required / dc misaligned");
-        return pcb_tc_dgrad(c, dc, dc_cstride, w_dgrad, dx, dx_cstride, st);
-    }
+    if (f == FAMILY_TC) return pcb_tc_dgrad(c, dc, dc_cstride, w_dgrad, dx, dx_cstride, st);
     return pcb_generic_dgrad(c, dc, dc_cstride, w_fwd, dx, dx_cstride, st);
 }
 
 PCB_API int pcb_conv_dgrad_fuses_relu(const pcb_conv *c) {
-    if (!c || c->force_generic || validate(c, false) || use_dw(c) || !use_tc(c) || !pcb_tc_dgrad_supported(c)) return 0;
+    if (!c || validate(c, false) || family_of(c) != FAMILY_TC) return 0;
     return pcb_tc_dgrad_fuses_relu(c) ? 1 : 0;
 }
 
@@ -204,11 +209,12 @@ static int backward_weight_impl(const pcb_conv *c, const void *dc, int dc_cstrid
     if (int rc = validate(c, true)) return rc;
     PCB_CHECK(dc && dw && dc_cstride >= c->cout, "pcb_pconv_backward_weight: bad arguments");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (use_dw(c)) {
+    const Family f = family_of(c);
+    if (f == FAMILY_DW) {
         PCB_CHECK(dc_cstride % 8 == 0, "depthwise wgrad: dc channel stride must be a multiple of 8");
         return pcb_dw_wgrad(c, dc, dc_cstride, dw, zero_dw, st);
     }
-    if (use_tc(c)) {
+    if (f == FAMILY_TC) {
         PCB_CHECK(workspace != nullptr && (reinterpret_cast<uintptr_t>(dc) & 15) == 0, "pcb_pconv_backward_weight: workspace required / dc misaligned");
         return pcb_tc_wgrad(c, dc, dc_cstride, dw, workspace, zero_dw, st);
     }

@@ -12,7 +12,7 @@
 //     du[s][c] = m_u[s] * sum_k D[s][k] W'[k][c]         1x1 data gradient, delivered at SOURCE resolution (no 2x2 reduction pass)
 //     dW'[k][c] = sum_s D[s][k] u[s][c] m_u[s]           1x1 weight gradient, scattered back into the [co][tap][c] master layout
 // and the 81 weight gradients of the image part are reduced on CUDA cores inside the D pass.
-// The mma.sync kernels of conv_smallco.cu stay as the general path (other kernel sizes, wider second parts, PCB_DISABLE_K2R=1).
+// The mma.sync kernels of conv_smallco.cu stay as the general path (other kernel sizes, wider second parts).
 #include <string.h>
 
 #include <algorithm>
@@ -25,19 +25,15 @@ constexpr int K2R_N = 32;          // columns of the 1x1 problem: (tap, co) = ta
 constexpr int K2R_CO = 3;
 constexpr int K2R_TAPS = 9;
 
-struct K2rPlan {
-    bool ok;
-    int pu, ps;                    // upsampled (wide) part, full-resolution (narrow) part
-    int cu, cs, choff_u, choff_s;
-    pcb_conv sub;                  // the 1x1 problem at source resolution
-    size_t sub_fe, sub_de;         // its operand sizes (bf16 elements)
-    size_t fwd_extra, dg_extra;    // elements appended to the layer's operand buffers (sub operands + fp32 staging of W')
-};
+size_t rup256(size_t v) { return (v + 255) / 256 * 256; }
+size_t zbytes(const pcb_conv *c) { return rup256(static_cast<size_t>(c->n) * (c->h >> 1) * (c->w >> 1) * K2R_N * sizeof(bf16)); }
 
-K2rPlan plan_of(const pcb_conv *c) {
+}  // namespace
+
+K2rPlan pcb_k2r_plan(const pcb_conv *c) {
     K2rPlan K;
     memset(&K, 0, sizeof(K));
-    if (getenv("PCB_DISABLE_K2R") || !pcb_smallco_eligible(c)) return K;
+    if (!pcb_smallco_eligible(c)) return K;
     if (c->kh != 3 || c->kw != 3 || c->pad_h != 1 || c->pad_w != 1 || c->cout > K2R_CO || c->nparts != 2) return K;
     if (c->ho != c->h || c->wo != c->w || ((c->h | c->w) & 1)) return K;
     K.pu = c->parts[0].x_up ? 0 : 1;
@@ -58,12 +54,12 @@ K2rPlan plan_of(const pcb_conv *c) {
     K.sub_de = (K.sub_de + 63) / 64 * 64;
     K.fwd_extra = K.sub_fe + 2 * static_cast<size_t>(K2R_N) * K.cu;      // + fp32 W' [32][cu]
     K.dg_extra = K.sub_de;
+    K.workspace = zbytes(c) + rup256(sizeof(float) * K2R_N * K.cu) + pcb_tc_workspace(&S);
     K.ok = true;
     return K;
 }
 
-size_t rup256(size_t v) { return (v + 255) / 256 * 256; }
-size_t zbytes(const pcb_conv *c) { return rup256(static_cast<size_t>(c->n) * (c->h >> 1) * (c->w >> 1) * K2R_N * sizeof(bf16)); }
+namespace {
 
 // W'[k = tap*3 + co][c] (fp32, the KRSC master of the 1x1 problem) from the layer's master weights [co][tap][cin]
 __global__ void k2r_weight_kernel(const float *__restrict__ w, float *__restrict__ wsub, int cout, int cin, int choff_u, int cu) {
@@ -338,22 +334,8 @@ bf16 *dgrad_scratch(size_t bytes) {
 
 }  // namespace
 
-bool pcb_k2r_ok(const pcb_conv *c) { return plan_of(c).ok; }
-
-void pcb_k2r_weight_layout(const pcb_conv *c, size_t *fwd_extra, size_t *dg_extra) {
-    const K2rPlan K = plan_of(c);
-    *fwd_extra = K.ok ? K.fwd_extra : 0;
-    *dg_extra = K.ok ? K.dg_extra : 0;
-}
-
-size_t pcb_k2r_workspace(const pcb_conv *c) {
-    const K2rPlan K = plan_of(c);
-    if (!K.ok) return 0;
-    return zbytes(c) + rup256(sizeof(float) * K2R_N * K.cu) + pcb_tc_workspace(&K.sub);
-}
-
-int pcb_k2r_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd_extra, void *w_dg_extra, bool zero_padding, cudaStream_t st) {
-    const K2rPlan K = plan_of(c);
+int pcb_k2r_weight_prepare(const pcb_conv *c, const K2rPlan &K, const float *w_master, void *w_fwd_extra, void *w_dg_extra, bool zero_padding,
+                           cudaStream_t st) {
     PCB_CHECK(K.ok && w_fwd_extra && w_dg_extra, "k2r weight prepare: not a kernel-to-row layer / missing operand buffers");
     float *wsub = reinterpret_cast<float *>(static_cast<bf16 *>(w_fwd_extra) + K.sub_fe);
     k2r_weight_kernel<<<(K2R_N * K.cu + 255) / 256, 256, 0, st>>>(w_master, wsub, c->cout, c->cin, K.choff_u, K.cu);
@@ -361,9 +343,8 @@ int pcb_k2r_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd
     return pcb_tc_weight_prepare(&K.sub, wsub, w_fwd_extra, w_dg_extra, zero_padding, st);
 }
 
-int pcb_k2r_forward(const pcb_conv *c, const pcb_smallco_layout &L, const void *w_fwd, const void *w_fwd_extra, const float *bias, void *y, int y_cstride,
-                    const float *msum, void *workspace, cudaStream_t st) {
-    const K2rPlan K = plan_of(c);
+int pcb_k2r_forward(const pcb_conv *c, const K2rPlan &K, const pcb_smallco_layout &L, const void *w_fwd, const void *w_fwd_extra, const float *bias,
+                    void *y, int y_cstride, const float *msum, void *workspace, cudaStream_t st) {
     PCB_CHECK(K.ok && workspace, "k2r forward: not a kernel-to-row layer / no workspace");
     PCB_CHECK(y_cstride % 8 == 0 && y_cstride >= 8 && (reinterpret_cast<uintptr_t>(y) & 15) == 0, "small-cout forward: y must be 16-byte aligned with a channel stride that is a multiple of 8");
     uint8_t *ws = static_cast<uint8_t *>(workspace);
@@ -382,9 +363,8 @@ int pcb_k2r_forward(const pcb_conv *c, const pcb_smallco_layout &L, const void *
 }
 
 // dx[pu] is a SOURCE-resolution buffer (pcb_conv_dgrad_at_source_resolution); dx[ps], when wanted, comes from the mma.sync kernel
-int pcb_k2r_dgrad(const pcb_conv *c, const pcb_smallco_layout &L, const void *dc, int dc_cstride, const void *w_dgrad, const void *w_dg_extra,
-                  void *const *dx, const int *dx_cstride, cudaStream_t st) {
-    const K2rPlan K = plan_of(c);
+int pcb_k2r_dgrad(const pcb_conv *c, const K2rPlan &K, const pcb_smallco_layout &L, const void *dc, int dc_cstride, const void *w_dgrad,
+                  const void *w_dg_extra, void *const *dx, const int *dx_cstride, cudaStream_t st) {
     PCB_CHECK(K.ok, "k2r dgrad: not a kernel-to-row layer");
     PCB_CHECK(dc_cstride % 8 == 0 && dc_cstride >= 8, "small-cout dgrad: dc channel stride must be a multiple of 8");
     if (dx[K.pu]) {
@@ -407,8 +387,7 @@ int pcb_k2r_dgrad(const pcb_conv *c, const pcb_smallco_layout &L, const void *dc
     return 0;
 }
 
-int pcb_k2r_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st) {
-    const K2rPlan K = plan_of(c);
+int pcb_k2r_wgrad(const pcb_conv *c, const K2rPlan &K, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st) {
     PCB_CHECK(K.ok && workspace, "k2r wgrad: not a kernel-to-row layer / no workspace");
     PCB_CHECK(dc_cstride % 8 == 0 && dc_cstride >= 8, "small-cout wgrad: dc channel stride must be a multiple of 8");
     if (zero_dw) PCB_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * c->cout * K2R_TAPS * c->cin, st));

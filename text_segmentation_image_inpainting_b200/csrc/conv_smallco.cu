@@ -417,7 +417,6 @@ int launch(void (*kern)(const ScParams), bool (&attr_done)[PCB_MAX_DEVICES], con
 }  // namespace
 
 bool pcb_smallco_eligible(const pcb_conv *c) {
-    if (getenv("PCB_DISABLE_SMALLCO")) return false;
     if (c->dtype != PCB_BF16 || c->groups != 1 || c->stride != 1 || c->dil != 1 || c->kh > 3 || c->kw > 3 || c->cout > 8) return false;
     if (c->nparts < 1 || c->nparts > 2 || c->cin < 16) return false;
     int cp = 0;

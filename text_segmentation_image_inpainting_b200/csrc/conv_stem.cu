@@ -21,17 +21,15 @@ namespace {
 constexpr int S2D_C = 32;          // (a, b, ch8)
 constexpr int SK = 4;              // sub-kernel size
 
-struct StemPlan {
-    bool ok;
-    pcb_conv sub;
-    size_t sub_fe;                 // bf16 elements of the sub-problem's forward operand (rounded to 64)
-    size_t fwd_extra;              // + fp32 staging of the re-indexed master weights
-};
+size_t rup256(size_t v) { return (v + 255) / 256 * 256; }
+size_t s2d_bytes(const pcb_conv *c) { return rup256(static_cast<size_t>(c->n) * (c->h / 2) * (c->w / 2) * S2D_C * sizeof(bf16)); }
+size_t dwsub_bytes(const pcb_conv *c) { return rup256(sizeof(float) * c->cout * SK * SK * S2D_C); }
 
-StemPlan plan_of(const pcb_conv *c) {
+}  // namespace
+
+StemPlan pcb_stem_plan(const pcb_conv *c) {
     StemPlan K;
     memset(&K, 0, sizeof(K));
-    if (getenv("PCB_DISABLE_S2D_STEM")) return K;
     if (c->dtype != PCB_BF16 || c->groups != 1 || c->nparts != 1 || c->kh != 7 || c->kw != 7 || c->stride != 2 || c->pad_h != 3 || c->pad_w != 3 ||
         c->dil != 1) return K;
     const pcb_part &p = c->parts[0];
@@ -47,13 +45,12 @@ StemPlan plan_of(const pcb_conv *c) {
     pcb_tc_weight_layout(&S, &K.sub_fe, &de);
     K.sub_fe = (K.sub_fe + 63) / 64 * 64;
     K.fwd_extra = K.sub_fe + 2 * static_cast<size_t>(c->cout) * SK * SK * S2D_C;
+    K.workspace = s2d_bytes(c) + dwsub_bytes(c) + pcb_tc_workspace(&S);
     K.ok = true;
     return K;
 }
 
-size_t rup256(size_t v) { return (v + 255) / 256 * 256; }
-size_t s2d_bytes(const pcb_conv *c) { return rup256(static_cast<size_t>(c->n) * (c->h / 2) * (c->w / 2) * S2D_C * sizeof(bf16)); }
-size_t dwsub_bytes(const pcb_conv *c) { return rup256(sizeof(float) * c->cout * SK * SK * S2D_C); }
+namespace {
 
 // one thread per (cell, a): two horizontally adjacent pixels (32 contiguous bytes) -> 16 channels of the cell, times the hole mask
 __global__ void s2d_kernel(const bf16 *__restrict__ x, const uint8_t *__restrict__ mask, bf16 *__restrict__ xs, int n, int h, int w) {
@@ -107,21 +104,7 @@ int run_s2d(const pcb_conv *c, bf16 *xs, cudaStream_t st) {
 
 }  // namespace
 
-bool pcb_stem_ok(const pcb_conv *c) { return plan_of(c).ok; }
-
-size_t pcb_stem_weight_extra(const pcb_conv *c) {
-    const StemPlan K = plan_of(c);
-    return K.ok ? K.fwd_extra : 0;
-}
-
-size_t pcb_stem_workspace(const pcb_conv *c) {
-    StemPlan K = plan_of(c);
-    if (!K.ok) return 0;
-    return s2d_bytes(c) + dwsub_bytes(c) + pcb_tc_workspace(&K.sub);
-}
-
-int pcb_stem_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd_extra, bool zero_padding, cudaStream_t st) {
-    const StemPlan K = plan_of(c);
+int pcb_stem_weight_prepare(const pcb_conv *c, const StemPlan &K, const float *w_master, void *w_fwd_extra, bool zero_padding, cudaStream_t st) {
     PCB_CHECK(K.ok && w_fwd_extra, "space-to-depth stem: weight prepare on a layer that does not take this path");
     float *wsub = reinterpret_cast<float *>(static_cast<bf16 *>(w_fwd_extra) + K.sub_fe);
     const int total = c->cout * SK * SK * S2D_C;
@@ -130,25 +113,25 @@ int pcb_stem_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fw
     return pcb_tc_weight_prepare(&K.sub, wsub, w_fwd_extra, nullptr, zero_padding, st);
 }
 
-int pcb_stem_forward(const pcb_conv *c, const void *w_fwd_extra, const float *bias, void *y, int y_cstride, const float *msum, void *workspace,
-                     double *bn_sums, const pcb_ep *ep, cudaStream_t st) {
-    StemPlan K = plan_of(c);
+int pcb_stem_forward(const pcb_conv *c, const StemPlan &K, const void *w_fwd_extra, const float *bias, void *y, int y_cstride,
+                     const float *msum, void *workspace, double *bn_sums, const pcb_ep *ep, cudaStream_t st) {
     PCB_CHECK(K.ok && workspace, "space-to-depth stem forward: wrong layer / no workspace");
     uint8_t *ws = static_cast<uint8_t *>(workspace);
     bf16 *xs = reinterpret_cast<bf16 *>(ws);
     if (int rc = run_s2d(c, xs, st)) return rc;
-    K.sub.parts[0].x = xs;
+    pcb_conv sub = K.sub;
+    sub.parts[0].x = xs;
     uint64_t *sub_ws = reinterpret_cast<uint64_t *>(ws + s2d_bytes(c) + dwsub_bytes(c));
     // tap-validity words of the 4x4 problem (in-bounds bits only: no holes) where its kernel wants them (the gather kernels of
     // non-power-of-two grids; the TMA-fed kernels zero-fill out-of-range coordinates themselves)
-    if (int rc = pcb_tc_forward_mask_pass(&K.sub, sub_ws, st)) return rc;
+    if (int rc = pcb_tc_forward_mask_pass(&sub, sub_ws, st)) return rc;
     // the layer's own mask sums drive the epilogue (renormalise, zero at holes, bias, BatchNorm statistics or the eval-mode
     // BatchNorm + activation); no hole rows in the GEMM
-    return pcb_tc_forward_ws(&K.sub, w_fwd_extra, bias, y, y_cstride, msum, sub_ws, true, bn_sums, ep, st);
+    return pcb_tc_forward_ws(&sub, w_fwd_extra, bias, y, y_cstride, msum, sub_ws, true, bn_sums, ep, st);
 }
 
-int pcb_stem_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st) {
-    StemPlan K = plan_of(c);
+int pcb_stem_wgrad(const pcb_conv *c, const StemPlan &K, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw,
+                   cudaStream_t st) {
     PCB_CHECK(K.ok && workspace, "space-to-depth stem wgrad: wrong layer / no workspace");
     if (zero_dw) PCB_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * c->cout * 49 * c->cin, st));
     uint8_t *ws = static_cast<uint8_t *>(workspace);
@@ -156,8 +139,9 @@ int pcb_stem_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw,
     float *dwsub = reinterpret_cast<float *>(ws + s2d_bytes(c));
     void *sub_ws = ws + s2d_bytes(c) + dwsub_bytes(c);
     if (int rc = run_s2d(c, xs, st)) return rc;
-    K.sub.parts[0].x = xs;
-    if (int rc = pcb_tc_wgrad(&K.sub, dc, dc_cstride, dwsub, sub_ws, true, st)) return rc;
+    pcb_conv sub = K.sub;
+    sub.parts[0].x = xs;
+    if (int rc = pcb_tc_wgrad(&sub, dc, dc_cstride, dwsub, sub_ws, true, st)) return rc;
     const int total = c->cout * 49 * c->cin;
     stem_dw_gather_kernel<<<(total + 255) / 256, 256, 0, st>>>(dwsub, dw, c->cout, c->cin);
     PCB_LAUNCH_CHECK();

@@ -2252,7 +2252,7 @@ void base_params(TcParams &P, const pcb_conv *c, const Layout &L) {
 
 // row-halo eligibility: stride 1, output rows made of whole groups of 8 pixels, halo small enough
 int halo_hg(const pcb_conv *c, bool rowpack) {
-    if (rowpack || c->stride != 1 || getenv("PCB_DISABLE_HALO")) return 0;
+    if (rowpack || c->stride != 1) return 0;
     const int hg = 8 + (c->kw - 1) * c->dil;
     if (c->kw < 2 || hg > HALO_MAX_HG || c->kh > 8) return 0;
     if (c->wo % 8 != 0 || c->w % 8 != 0 || c->wo != c->w) return 0;
@@ -2298,28 +2298,43 @@ bool tile_box(int wt, int ht, int *bw, int *bh, int *bn) {
     return true;
 }
 
-bool tma_fwd_ok(const pcb_conv *c) {
-    if (getenv("PCB_DISABLE_TMA") || is_rowpack(c)) return false;
-    int bw, bh, bn;
-    if (!tile_box(c->wo, c->ho, &bw, &bh, &bn)) return false;
-    if (c->stride > 2 || bw * c->stride > 256 || bh * c->stride > 256) return false;
+// 64 consecutive pixels of a [n][ht][wt] grid as a box {bw, bh, bn} (the K blocks of the weight gradient)
+bool kblock_box(int wt, int ht, int *bw, int *bh, int *bn) {
+    if (wt < 4) return false;
+    if (wt % 64 == 0) { *bw = 64; *bh = 1; *bn = 1; return true; }
+    if (64 % wt) return false;
+    const int rows = 64 / wt;
+    *bw = wt;
+    if (ht % rows == 0) { *bh = rows; *bn = 1; return true; }
+    if (rows % ht) return false;
+    *bh = ht; *bn = rows / ht;
+    return true;
+}
+
+bool even_upsampled_parts(const pcb_conv *c) {
     for (int p = 0; p < c->nparts; ++p)
         if (c->parts[p].x_up && ((c->h | c->w) & 1)) return false;
     return true;
 }
 
-bool tma_dgrad_ok(const pcb_conv *c) {
-    if (getenv("PCB_DISABLE_TMA") || is_rowpack(c) || c->stride != 1) return false;
-    int bw, bh, bn;
-    return tile_box(c->w, c->h, &bw, &bh, &bn);
+// the TMA-fed kernels of each direction take the problem when its M tile box exists (the row-packed layout has no TMA path)
+bool tma_fwd_ok(const pcb_conv *c, int *bw, int *bh, int *bn) {
+    if (is_rowpack(c) || !tile_box(c->wo, c->ho, bw, bh, bn)) return false;
+    if (c->stride > 2 || *bw * c->stride > 256 || *bh * c->stride > 256) return false;
+    return even_upsampled_parts(c);
 }
 
-// stride-2 data gradient as four stride-1 parity-class problems (see pcb_tc_dgrad)
-bool tma_dgrad_s2_ok(const pcb_conv *c) {
-    if (getenv("PCB_DISABLE_TMA") || getenv("PCB_DISABLE_TMA_S2") || is_rowpack(c)) return false;
+// stride-2 data gradient of a layer that is not row-packed as four stride-1 parity-class problems (see pcb_tc_dgrad)
+bool tma_dgrad_s2_ok(const pcb_conv *c, int *bw, int *bh, int *bn) {
     if (c->stride != 2 || c->dil != 1 || c->kh < 2 || c->kw < 2 || ((c->h | c->w) & 1) || c->ho != c->h / 2 || c->wo != c->w / 2) return false;
-    int bw, bh, bn;
-    return tile_box(c->w / 2, c->h / 2, &bw, &bh, &bn);
+    return tile_box(c->w / 2, c->h / 2, bw, bh, bn);
+}
+
+// kernel columns of the parity class with input column parity px: the taps with (px + pad - tc) even
+int class_kw(const pcb_conv *c, int px) { return (c->kw - ((px + c->pad_w) & 1) + 1) / 2; }
+
+bool tma_wgrad_ok(const pcb_conv *c, int *bw, int *bh, int *bn) {
+    return !is_rowpack(c) && c->stride <= 2 && kblock_box(c->wo, c->ho, bw, bh, bn) && even_upsampled_parts(c);
 }
 
 size_t up_bytes(const pcb_conv *c, int p) {
@@ -2377,11 +2392,10 @@ bool halo_stages_fit(int kw, int dil, int block_n) {
     return 3 * stage + acc_stage_bytes(block_n) <= RING_BUDGET;
 }
 
-// halo tiles: stride 1, the M tile is one image-row segment, a kernel row's halo fits the 256-pixel TMA box, and the stages fit
-bool tma_halo_ok(const pcb_conv *c, int bw, int bh, int bn, int block_n) {
-    if (getenv("PCB_DISABLE_TMA_HALO")) return false;
-    if (!(c->stride == 1 && bw == 128 && bh == 1 && bn == 1 && c->kw >= 2 && 128 + (c->kw - 1) * c->dil <= 256 && c->kh <= 8)) return false;
-    return halo_stages_fit(c->kw, c->dil, block_n);
+// row-halo tiles of the TMA-fed forward / data gradient for a (stride-1) kernel row of kw taps: the M tile is one image-row
+// segment, a kernel row's halo fits the 256-pixel TMA box, and the stages fit
+bool halo_ok(int kw, int dil, int bw, int bh, int bn, int block_n) {
+    return bw == 128 && bh == 1 && bn == 1 && kw >= 2 && 128 + (kw - 1) * dil <= 256 && halo_stages_fit(kw, dil, block_n);
 }
 
 // widest N tile that divides `cols` and still leaves at least one tile per SM; low-resolution layers (a handful of M tiles
@@ -2395,14 +2409,13 @@ bool tma_halo_ok(const pcb_conv *c, int bw, int bh, int bn, int block_n) {
 // 0.133 ms; dec5 768 columns, 768 tiles: 0.262 -> 0.252 ms), the forward only where 256 columns take ONE wave instead of two
 // (dec1, 128 tiles: 0.199 -> 0.191 ms).  With more waves the forward lost (enc2 and dec5, 256 tiles: 0.164 -> 0.172 and
 // 0.271 -> 0.295 ms; enc3: 0.082 -> 0.089 ms): its consumers also do the epilogue's element math, twice as much per tile.
-int pick_bn(int cols, long long m_total, bool fwd) {
+int pick_bn(int cols, long long m_total, bool fwd, int sms) {
     const long long m_tiles = (m_total + BLOCK_M - 1) / BLOCK_M;
     if (cols <= 32) return 32;
-    const long long sms = pcb_num_sms();
     auto waves = [&](int b) { return (m_tiles * (cols / b) + sms - 1) / sms; };
     if (cols % 256 == 0 && 2 * waves(256) <= waves(128) && (!fwd || waves(256) == 1)) return 256;
     int bn = (cols % 128 == 0) ? 128 : 64;
-    while (bn > 32 && cols % (bn / 2) == 0 && m_tiles * (cols / bn) < pcb_num_sms() / 2) bn /= 2;
+    while (bn > 32 && cols % (bn / 2) == 0 && m_tiles * (cols / bn) < sms / 2) bn /= 2;
     return bn;
 }
 
@@ -2429,11 +2442,6 @@ int class_streams(ClassStreams **out) {
     *out = &CS;
     return 0;
 }
-
-}  // namespace
-
-static bool smallco_ok(const pcb_conv *c);
-namespace {
 
 // ---- sub-pixel data gradient: plan, weights, launch ---------------------------------------------------
 // one spatial axis: for output parity q, tap t of a (k, dilation d, padding p) kernel over the 2x-upsampled source reads source
@@ -2467,13 +2475,14 @@ struct SpPlan {
     int kext_u, c8_u;
     long long sp_dg_elems, kd_sp;
     int bw, bh, bn;                  // M tile box of the source grid [n][h/2][w/2]
+    int block_n;                     // N tile width (at most 64)
 };
 
-SpPlan sp_plan(const pcb_conv *c) {
+// for a tensor-core problem that is neither row-packed nor small-Cout
+SpPlan sp_plan(const pcb_conv *c, const Layout &L, int sms) {
     SpPlan S;
     memset(&S, 0, sizeof(S));
     S.pu = S.ps = -1;
-    if (getenv("PCB_DISABLE_SUBPIXEL") || getenv("PCB_DISABLE_TMA") || !common_ok(c) || is_rowpack(c)) return S;
     if (c->stride != 1 || c->ho != c->h || c->wo != c->w || ((c->h | c->w) & 1) || c->nparts > 2) return S;
     for (int p = 0; p < c->nparts; ++p) {
         if (c->parts[p].x_up) { if (S.pu >= 0) return S; S.pu = p; }
@@ -2483,12 +2492,10 @@ SpPlan sp_plan(const pcb_conv *c) {
     // the hole mask of each part must live at the part's own resolution (HoleMask.upsampled keeps them together)
     if (c->parts[S.pu].mask && c->parts[S.pu].mask_up != 1) return S;
     if (S.ps >= 0 && c->parts[S.ps].mask && c->parts[S.ps].mask_up != 0) return S;
-    if (smallco_ok(c)) return S;
     S.ay = sp_axis(c->kh, c->dil, c->pad_h);
     S.ax = sp_axis(c->kw, c->dil, c->pad_w);
     if (!S.ay.ok || !S.ax.ok) return S;
     if (!tile_box(c->w / 2, c->h / 2, &S.bw, &S.bh, &S.bn)) return S;
-    const Layout L = layout_of(c);
     S.kext_u = L.kext[S.pu]; S.c8_u = rup(c->parts[S.pu].c, 8);
     int eo = 0;
     for (int cls = 0; cls < 4; ++cls) {
@@ -2501,9 +2508,10 @@ SpPlan sp_plan(const pcb_conv *c) {
     // one launch over the source grid replaces the full-resolution gradient of the upsampled part AND its 2x2 reduction pass; it
     // is used wherever the source grid has at least a third of a wave of tiles -- low-resolution layers keep the regular kernel
     // (their launches are latency-bound either way)
-    const long long src_tiles = (static_cast<long long>(c->n) * (c->h / 2) * (c->w / 2) + BLOCK_M - 1) / BLOCK_M;
-    S.ok = src_tiles >= pcb_num_sms() / 3;
+    const long long m_src = static_cast<long long>(c->n) * (c->h / 2) * (c->w / 2);
+    S.ok = (m_src + BLOCK_M - 1) / BLOCK_M >= sms / 3;
     S.sp_dg_elems = static_cast<long long>(rup(S.kext_u, 128)) * S.kd_sp;
+    S.block_n = std::min(pick_bn(S.kext_u, m_src, true, sms), 64);
     return S;
 }
 
@@ -2547,9 +2555,6 @@ int sp_weight_prepare(const pcb_conv *c, const SpPlan &S, const Layout &L, const
     return 0;
 }
 
-// sub-pixel tiles are at most 64 columns wide
-int sp_bn(int cols, long long m_total) { return std::min(pick_bn(cols, m_total, true), 64); }
-
 template <int BLOCK_N>
 int launch_sp_n(TcParams &P, const SpTable &TB, const CUtensorMap &tw, const CUtensorMap &ta, cudaStream_t st) {
     const size_t stage = A_STAGE_BYTES + static_cast<size_t>(BLOCK_N) * 128;
@@ -2586,7 +2591,7 @@ int sp_dgrad_up(const pcb_conv *c, const SpPlan &S, const Layout &L, const void 
     P.abort_flag = flag;
     P.ncols = S.kext_u;
     P.box_w = S.bw; P.box_h = S.bh; P.box_n = S.bn;
-    const int bn = sp_bn(S.kext_u, m_src);
+    const int bn = S.block_n;
     SpTable TB;
     memset(&TB, 0, sizeof(TB));
     int ni = 0;
@@ -2607,66 +2612,202 @@ int sp_dgrad_up(const pcb_conv *c, const SpPlan &S, const Layout &L, const void 
     return (bn == 64) ? launch_sp_n<64>(P, TB, tw, ta, st) : launch_sp_n<32>(P, TB, tw, ta, st);
 }
 
-}  // namespace
+// ---- the plan ---------------------------------------------------------------------------------------------------------------
+// Every choice the tensor-core path makes for one problem, taken once from the descriptor and the SM count: the kernel of each
+// direction and its tiles, where the extra operands sit in the weight buffers, and the layout of the workspace.  Every pcb_tc_*
+// entry point works from this plan, so the mask pass, the workspace and the weight layout agree with the kernels that use them.
+enum TcRoute { ROUTE_NONE, ROUTE_STEM, ROUTE_K2R, ROUTE_SMALLCO, ROUTE_TMA, ROUTE_TMA_S2, ROUTE_GATHER };
 
-static bool smallco_ok(const pcb_conv *c) { return common_ok(c) && !is_rowpack(c) && pcb_smallco_eligible(c); }
-static pcb_smallco_layout smallco_layout(const Layout &L) {
+struct DirPlan {
+    TcRoute route;
+    int box_w, box_h, box_n;           // M tile box of the TMA-fed kernels
+    int bn;                            // N tile width
+    bool halo;                         // TMA-fed row-halo tiles
+    int hg;                            // row-halo group of the cp.async gather kernels (0: none)
+};
+
+struct TcPlan {
+    bool ok;                           // the tensor-core path takes the problem
+    Layout L;
+    long long m_out, m_in;             // output / input pixels
+    size_t fwd_elems, dg_elems;        // operand buffer sizes (bf16 elements)
+    size_t extra_fwd_off, extra_dg_off;  // the operands of the stem's / the tail's sub-problem follow the layer's own
+    size_t sp_off;                     // the sub-pixel matrices follow the regular data-gradient operand
+    size_t workspace;                  // tap-validity words first, then the dense copies of the 2x-upsampled parts
+    size_t up_off[TC_MAX_PARTS];       // workspace offset of each 2x-upsampled part's copy
+    DirPlan fwd, dg, wg;
+    bool fwd_tapmask, wg_tapmask;      // the forward / weight-gradient kernel reads tap-validity words from the workspace
+    StemPlan stem;                     // ROUTE_STEM: the 4x4 problem over the space-to-depth image (conv_stem.cu)
+    K2rPlan k2r;                       // ROUTE_K2R: the 1x1 problem at source resolution (conv_k2r.cu)
+    SpPlan sp;                         // the data gradient of the 2x-upsampled part at source resolution (sp.ok)
+    bool cls_halo[4];                  // ROUTE_TMA_S2: row-halo tiles per parity class (py * 2 + px)
+    bool cls_fork;                     // ROUTE_TMA_S2: one class does not fill the GPU, the four run concurrently
+    bool fuses_epilogue;               // the forward accumulates the BatchNorm statistics / applies the eval-mode epilogue
+    bool dg_fuses_relu;                // the data gradient applies the ReLU backward of the layer's input
+    bool dg_at_source;                 // see pcb_conv_dgrad_at_source_resolution
+};
+
+TcPlan tc_plan(const pcb_conv *c) {
+    TcPlan T;
+    memset(&T, 0, sizeof(T));
+    T.sp.pu = T.sp.ps = -1;
+    if (!common_ok(c)) return T;
+    T.ok = true;
+    const int sms = pcb_num_sms();
+    T.L = layout_of(c);
+    const Layout &L = T.L;
+    T.m_out = static_cast<long long>(c->n) * c->ho * c->wo;
+    T.m_in = static_cast<long long>(c->n) * c->h * c->w;
+    bool any_mask = false;
+    for (int p = 0; p < c->nparts; ++p) any_mask = any_mask || (c->parts[p].mask != nullptr);
+    const bool smallco = !L.rowpack && pcb_smallco_eligible(c);
+    if (L.rowpack) T.stem = pcb_stem_plan(c);
+    if (smallco) T.k2r = pcb_k2r_plan(c);
+    const bool stem = T.stem.ok, k2r = T.k2r.ok;
+    if (!L.rowpack && !smallco) T.sp = sp_plan(c, L, sms);
+
+    T.fwd_elems = static_cast<size_t>(L.rows_f) * L.kf;
+    T.sp_off = static_cast<size_t>(rup(L.ktap, 128)) * L.kd;
+    T.dg_elems = L.rowpack ? 0 : T.sp_off;
+    if (T.sp.ok) T.dg_elems += static_cast<size_t>(T.sp.sp_dg_elems);
+    T.extra_fwd_off = (T.fwd_elems + 63) / 64 * 64;
+    T.extra_dg_off = (T.sp_off + 63) / 64 * 64;
+    if (k2r) {
+        T.fwd_elems = T.extra_fwd_off + T.k2r.fwd_extra;
+        T.dg_elems = T.extra_dg_off + T.k2r.dg_extra;
+    }
+    if (stem) T.fwd_elems = T.extra_fwd_off + T.stem.fwd_extra;
+
+    int bw, bh, bn;
+    const bool fwd_tma = tma_fwd_ok(c, &bw, &bh, &bn);
+    DirPlan &F = T.fwd;
+    if (stem) F.route = ROUTE_STEM;                      // (the stem applies its mask in the space-to-depth pass)
+    else if (k2r) F.route = ROUTE_K2R;
+    else if (smallco) F.route = ROUTE_SMALLCO;
+    else if (fwd_tma) {
+        F.route = ROUTE_TMA;
+        F.box_w = bw; F.box_h = bh; F.box_n = bn;
+        F.bn = pick_bn(c->cout <= 32 ? 32 : L.rows_f, T.m_out, true, sms);
+        F.halo = c->stride == 1 && c->kh <= 8 && halo_ok(c->kw, c->dil, bw, bh, bn, F.bn);
+        // without holes TMA's out-of-range zero fill is all the validity there is; row-halo tiles read the mask planes themselves
+        T.fwd_tapmask = any_mask && !F.halo;
+    } else {
+        F.route = ROUTE_GATHER;
+        F.bn = L.bn_f;
+        F.hg = halo_hg(c, L.rowpack);
+        T.fwd_tapmask = true;
+    }
+
+    DirPlan &D = T.dg;
+    if (k2r) D.route = ROUTE_K2R;
+    else if (smallco) D.route = ROUTE_SMALLCO;
+    else if (L.rowpack) D.route = ROUTE_NONE;            // row-packed layers take their data gradient on the generic kernels
+    else if (c->stride == 1 && tile_box(c->w, c->h, &bw, &bh, &bn)) {
+        D.route = ROUTE_TMA;
+        D.box_w = bw; D.box_h = bh; D.box_n = bn;
+        D.bn = pick_bn(L.ktap, T.m_in, false, sms);
+        D.halo = c->kh <= 8 && halo_ok(c->kw, c->dil, bw, bh, bn, D.bn);
+    } else if (tma_dgrad_s2_ok(c, &bw, &bh, &bn)) {
+        D.route = ROUTE_TMA_S2;
+        D.box_w = bw; D.box_h = bh; D.box_n = bn;
+        const long long m_class = static_cast<long long>(c->n) * (c->h / 2) * (c->w / 2);
+        D.bn = pick_bn(L.ktap, m_class, false, sms);
+        for (int cls = 0; cls < 4; ++cls) T.cls_halo[cls] = halo_ok(class_kw(c, cls & 1), 1, bw, bh, bn, D.bn);
+        T.cls_fork = ((m_class + BLOCK_M - 1) / BLOCK_M) * (L.ktap / D.bn) < sms;
+    } else {
+        D.route = ROUTE_GATHER;
+        D.bn = (L.ktap % 128 == 0) ? 128 : 64;
+        D.hg = halo_hg(c, false);
+    }
+
+    const bool wg_tma = tma_wgrad_ok(c, &bw, &bh, &bn);
+    DirPlan &W = T.wg;
+    if (stem) W.route = ROUTE_STEM;
+    else if (k2r) W.route = ROUTE_K2R;
+    else if (smallco) W.route = ROUTE_SMALLCO;
+    else if (wg_tma) {
+        W.route = ROUTE_TMA;
+        W.box_w = bw; W.box_h = bh; W.box_n = bn;
+        // row-halo tiles for kw == 3: the three taps of a kernel row are three 64 x 64 register accumulators per consumer thread
+        W.halo = c->stride == 1 && c->kw == 3 && bw == 64 && bh == 1 && bn == 1 && 64 + (c->kw - 1) * c->dil <= 256;
+        // 128 output channels per tile, except for layers with at most 64 and for short reductions (< 128 K blocks of 64
+        // pixels): there each CTA has few K blocks and its red.global.add epilogue, twice as long at 128 columns, dominates
+        W.bn = (c->cout > 64 && T.m_out >= 128 * 64) ? 128 : 64;
+        T.wg_tapmask = any_mask;                         // without holes the TMA-fed kernel needs no validity words
+    } else {
+        W.route = ROUTE_GATHER;
+        T.wg_tapmask = true;
+    }
+
+    if (k2r) T.workspace = T.k2r.workspace;
+    else if (stem) T.workspace = std::max(T.stem.workspace, tapmask_bytes(c));
+    else {
+        T.workspace = tapmask_bytes(c);
+        // dense copies of the 2x-upsampled sources for the TMA-fed kernels (TMA cannot replicate pixels), reserved wherever the
+        // geometry allows them (small-Cout layers included)
+        if (fwd_tma || wg_tma)
+            for (int p = 0; p < c->nparts; ++p)
+                if (c->parts[p].x_up) { T.up_off[p] = T.workspace; T.workspace += up_bytes(c, p); }
+    }
+
+    T.fuses_epilogue = !smallco;                         // the small-Cout / RGB-tail kernels have no such epilogue
+    T.dg_fuses_relu = c->nparts == 1 && !T.sp.ok && D.route == ROUTE_TMA;
+    T.dg_at_source = smallco ? k2r : T.sp.ok;
+    return T;
+}
+
+// A-operand tensor maps of the TMA-fed forward and weight gradient, one per part (the second repeats a single part): a
+// 2x-upsampled part is first copied densely into the workspace at the plan's offset.  *use_fix is set when a part has holes.
+int a_operand_maps(const pcb_conv *c, const TcPlan &T, void *workspace, int bx, int by, int bn, CUtensorMap (&ta)[TC_MAX_PARTS],
+                   int *use_fix, cudaStream_t st) {
+    memset(ta, 0, sizeof(ta));
+    for (int p = 0; p < c->nparts; ++p) {
+        const pcb_part &pt = c->parts[p];
+        const void *src = pt.x;
+        long long cs = pt.x_cstride;
+        const int c8 = rup(pt.c, 8);
+        if (pt.x_up) {
+            bf16 *up = reinterpret_cast<bf16 *>(static_cast<uint8_t *>(workspace) + T.up_off[p]);
+            const long long pix = static_cast<long long>(c->n) * (c->h >> 1) * (c->w >> 1);
+            const long long work = pix * (c8 >> 3);
+            const int grid = static_cast<int>(std::min<long long>((work + 255) / 256, 16ll * pcb_num_sms()));
+            upsample_part_kernel<<<grid, 256, 0, st>>>(static_cast<const bf16 *>(pt.x), pt.x_cstride, c8, pix, c->h >> 1, c->w >> 1, up);
+            PCB_LAUNCH_CHECK();
+            src = up; cs = c8;
+        }
+        if (pt.mask) *use_fix = 1;
+        if (int rc = make_tmap_nhwc(&ta[p], src, c8, c->w, c->h, c->n, cs, bx, by, bn, c->stride)) return rc;
+    }
+    if (c->nparts < 2) ta[1] = ta[0];
+    return 0;
+}
+
+pcb_smallco_layout smallco_layout(const Layout &L) {
     pcb_smallco_layout S;
     S.ktap = L.ktap; S.koff[0] = L.koff[0]; S.koff[1] = L.koff[1]; S.cout64 = L.cout64; S.kf = L.kf; S.kd = L.kd;
     return S;
 }
 
-// ---- eligibility / layouts -----------------------------------------------------------------------
-bool pcb_tc_eligible(const pcb_conv *c) { return common_ok(c) && !getenv("PCB_DISABLE_TC"); }
+}  // namespace
 
-static bool tma_wgrad_ok(const pcb_conv *c);
+// ---- entry points --------------------------------------------------------------------------------------------------------
+bool pcb_tc_eligible(const pcb_conv *c) { return common_ok(c); }
 
-// kernel-to-row tails (conv_k2r.cu): their 1x1 operands follow the layer's regular ones, at 64-element boundaries
-static void k2r_bases(const Layout &L, size_t *fe, size_t *de) {
-    *fe = (static_cast<size_t>(L.rows_f) * L.kf + 63) / 64 * 64;
-    *de = (static_cast<size_t>(rup(L.ktap, 128)) * L.kd + 63) / 64 * 64;
-}
-
-// space-to-depth stems (conv_stem.cu): the 4x4 problem's operand (+ staging) follows the row-packed operand
-static bool stem_ok(const pcb_conv *c) { return common_ok(c) && is_rowpack(c) && pcb_stem_ok(c); }
-static size_t stem_base(const Layout &L) { return (static_cast<size_t>(L.rows_f) * L.kf + 63) / 64 * 64; }
-
-size_t pcb_tc_workspace(const pcb_conv *c) {
-    if (smallco_ok(c) && pcb_k2r_ok(c)) return pcb_k2r_workspace(c);
-    if (stem_ok(c)) return std::max(pcb_stem_workspace(c), tapmask_bytes(c));
-    size_t bytes = tapmask_bytes(c);
-    if (tma_fwd_ok(c) || tma_wgrad_ok(c))                // dense copies of the 2x-upsampled sources (TMA cannot replicate pixels)
-        for (int p = 0; p < c->nparts; ++p)
-            if (c->parts[p].x_up) bytes += up_bytes(c, p);
-    return bytes;
-}
+size_t pcb_tc_workspace(const pcb_conv *c) { return tc_plan(c).workspace; }
 
 void pcb_tc_weight_layout(const pcb_conv *c, size_t *fwd_elems, size_t *dgrad_elems) {
-    const Layout L = layout_of(c);
-    *fwd_elems = static_cast<size_t>(L.rows_f) * L.kf;
-    *dgrad_elems = L.rowpack ? 0 : static_cast<size_t>(rup(L.ktap, 128)) * L.kd;
-    // sub-pixel data gradient (conv over a 2x-upsampled source): the per-class effective-tap matrices follow the regular operand
-    const SpPlan S = sp_plan(c);
-    if (S.ok) *dgrad_elems += static_cast<size_t>(S.sp_dg_elems);
-    if (smallco_ok(c) && pcb_k2r_ok(c)) {
-        size_t fb, db, fx, dx;
-        k2r_bases(L, &fb, &db);
-        pcb_k2r_weight_layout(c, &fx, &dx);
-        *fwd_elems = fb + fx; *dgrad_elems = db + dx;
-    }
-    if (stem_ok(c)) *fwd_elems = stem_base(L) + pcb_stem_weight_extra(c);
+    const TcPlan T = tc_plan(c);
+    *fwd_elems = T.fwd_elems;
+    *dgrad_elems = T.dg_elems;
 }
 
 // true when the data gradient of the 2x-upsampled part is delivered at that part's own (source) resolution
-bool pcb_tc_subpixel(const pcb_conv *c) {
-    if (smallco_ok(c)) return pcb_k2r_ok(c);
-    return sp_plan(c).ok;
-}
+bool pcb_tc_subpixel(const pcb_conv *c) { return tc_plan(c).dg_at_source; }
 
 int pcb_tc_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd, void *w_dgrad, bool zero_padding, cudaStream_t st) {
-    const Layout L = layout_of(c);
-    size_t fe, de;
-    pcb_tc_weight_layout(c, &fe, &de);
+    const TcPlan T = tc_plan(c);
+    const Layout &L = T.L;
+    const size_t fe = T.fwd_elems, de = T.dg_elems;
     if (zero_padding) {                                  // a refresh of buffers filled before leaves the (never written) padding alone
         PCB_CUDA(cudaMemsetAsync(w_fwd, 0, fe * 2, st));
         if (w_dgrad && de) PCB_CUDA(cudaMemsetAsync(w_dgrad, 0, de * 2, st));
@@ -2677,179 +2818,114 @@ int pcb_tc_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd,
     W.ktap = L.ktap; W.cout64 = L.cout64; W.kf = L.kf; W.kd = L.kd;
     int off = 0;
     for (int p = 0; p < c->nparts; ++p) { W.choff[p] = off; W.c[p] = c->parts[p].c; W.koff[p] = L.koff[p]; off += c->parts[p].c; }
+    bf16 *wf = static_cast<bf16 *>(w_fwd), *wd = static_cast<bf16 *>(w_dgrad);
     if (!L.rowpack && W.taps <= 65535 && c->cout >= 32 && c->cin >= 32) {
         dim3 tg((c->cin + 31) / 32, (c->cout + 31) / 32, W.taps);
-        tc_weight_prepare_tiled_kernel<<<tg, 256, 0, st>>>(w_master, W, static_cast<bf16 *>(w_fwd), (w_dgrad && de) ? static_cast<bf16 *>(w_dgrad) : nullptr);
-        PCB_LAUNCH_CHECK();
-        const SpPlan S = sp_plan(c);
-        if (S.ok) {
-            PCB_CHECK(w_dgrad != nullptr, "sub-pixel weights need the dgrad operand buffer");
-            return sp_weight_prepare(c, S, L, w_master, static_cast<bf16 *>(w_dgrad) + static_cast<size_t>(rup(L.ktap, 128)) * L.kd, st);
-        }
-        return 0;
+        tc_weight_prepare_tiled_kernel<<<tg, 256, 0, st>>>(w_master, W, wf, (w_dgrad && de) ? wd : nullptr);
+    } else {
+        const long long total = static_cast<long long>(c->cout) * W.taps * c->cin;
+        const int grid = static_cast<int>(std::min<long long>((total + 1023) / 1024, 8ll * pcb_num_sms()));
+        tc_weight_prepare_kernel<<<grid < 1 ? 1 : grid, 256, 0, st>>>(w_master, W, wf, (w_dgrad && de) ? wd : nullptr);
     }
-    const long long total = static_cast<long long>(c->cout) * W.taps * c->cin;
-    const int grid = static_cast<int>(std::min<long long>((total + 1023) / 1024, 8ll * pcb_num_sms()));
-    tc_weight_prepare_kernel<<<grid < 1 ? 1 : grid, 256, 0, st>>>(w_master, W, static_cast<bf16 *>(w_fwd),
-                                                                   (w_dgrad && de) ? static_cast<bf16 *>(w_dgrad) : nullptr);
     PCB_LAUNCH_CHECK();
-    if (stem_ok(c)) return pcb_stem_weight_prepare(c, w_master, static_cast<bf16 *>(w_fwd) + stem_base(L), zero_padding, st);
-    if (smallco_ok(c) && pcb_k2r_ok(c)) {
+    if (T.fwd.route == ROUTE_STEM) return pcb_stem_weight_prepare(c, T.stem, w_master, wf + T.extra_fwd_off, zero_padding, st);
+    if (T.fwd.route == ROUTE_K2R) {
         PCB_CHECK(w_dgrad != nullptr, "kernel-to-row weights need the dgrad operand buffer");
-        size_t fb, db;
-        k2r_bases(L, &fb, &db);
-        return pcb_k2r_weight_prepare(c, w_master, static_cast<bf16 *>(w_fwd) + fb, static_cast<bf16 *>(w_dgrad) + db, zero_padding, st);
+        return pcb_k2r_weight_prepare(c, T.k2r, w_master, wf + T.extra_fwd_off, wd + T.extra_dg_off, zero_padding, st);
     }
-    const SpPlan S = sp_plan(c);
-    if (S.ok) {
+    if (T.sp.ok) {
         PCB_CHECK(w_dgrad != nullptr, "sub-pixel weights need the dgrad operand buffer");
-        return sp_weight_prepare(c, S, L, w_master, static_cast<bf16 *>(w_dgrad) + static_cast<size_t>(rup(L.ktap, 128)) * L.kd, st);
+        return sp_weight_prepare(c, T.sp, L, w_master, wd + T.sp_off, st);
     }
     return 0;
 }
 
 // the part of the forward that only depends on the masks: tap-validity words for the kernels that want them
 int pcb_tc_forward_mask_pass(const pcb_conv *c, uint64_t *tapmask, cudaStream_t st) {
-    const long long m_total = static_cast<long long>(c->n) * c->ho * c->wo;
-    PCB_CHECK(m_total < (1ll << 31), "problem too large");
-    const Layout L = layout_of(c);
-    if (smallco_ok(c) || stem_ok(c)) return 0;            // (the stem applies its mask in the space-to-depth pass)
-    bool any_mask = false;
-    for (int p = 0; p < c->nparts; ++p) any_mask = any_mask || (c->parts[p].mask != nullptr);
-    if (tma_fwd_ok(c) && !any_mask) return 0;            // no holes: TMA's out-of-range zero fill is all the validity there is
-    if (tma_fwd_ok(c)) {                                  // row-halo tiles: the fixers read the mask planes themselves
-        int bw, bh, bn;
-        tile_box(c->wo, c->ho, &bw, &bh, &bn);
-        if (tma_halo_ok(c, bw, bh, bn, pick_bn(c->cout <= 32 ? 32 : L.rows_f, m_total, true))) return 0;
-    }
-    return launch_tapmask(c, tapmask, st);
+    const TcPlan T = tc_plan(c);
+    PCB_CHECK(T.m_out < (1ll << 31), "problem too large");
+    return T.fwd_tapmask ? launch_tapmask(c, tapmask, st) : 0;
 }
 
-// true when pcb_tc_forward_ws accumulates the BatchNorm statistics of its output itself (tensor-core kernels)
-bool pcb_tc_fuses_bn_stats(const pcb_conv *c) {
-    return pcb_tc_fuses_affine_act(c) && !getenv("PCB_DISABLE_FUSED_BN_STATS");
-}
-
-// true when pcb_tc_forward_ws can apply an eval-mode BatchNorm + activation in its epilogue (the same kernels as above: the
-// small-Cout / RGB-tail kernels have no such epilogue)
-bool pcb_tc_fuses_affine_act(const pcb_conv *c) {
-    return pcb_tc_eligible(c) && !smallco_ok(c);
-}
+// true when pcb_tc_forward_ws can accumulate the BatchNorm statistics of its output / apply an eval-mode BatchNorm + activation
+// in its epilogue
+bool pcb_tc_fuses_epilogue(const pcb_conv *c) { return tc_plan(c).fuses_epilogue; }
 
 int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, const float *msum,
                       uint64_t *tapmask, bool mask_pass_done, double *bn_sums, const pcb_ep *ep, cudaStream_t st) {
     int *flag = abort_flag_ptr();
     PCB_CHECK(flag != nullptr, "cudaMalloc(abort flag) failed");
-    const long long m_total = static_cast<long long>(c->n) * c->ho * c->wo;
-    PCB_CHECK(m_total < (1ll << 31), "problem too large");
+    const TcPlan T = tc_plan(c);
+    const Layout &L = T.L;
+    const DirPlan &F = T.fwd;
+    PCB_CHECK(T.m_out < (1ll << 31), "problem too large");
     PCB_CHECK(y_cstride % 8 == 0 && y_cstride >= c->cout, "tensor-core forward: y channel stride must be a multiple of 8 and >= cout");
-    const Layout L = layout_of(c);
-    if (!mask_pass_done)
-        if (int rc = pcb_tc_forward_mask_pass(c, tapmask, st)) return rc;
-    if (stem_ok(c)) {
-        PCB_CHECK(bn_sums == nullptr || pcb_tc_fuses_bn_stats(c), "fused BatchNorm statistics requested from a kernel that does not produce them");
-        PCB_CHECK(ep == nullptr || pcb_tc_fuses_affine_act(c), "fused BatchNorm + activation requested from a kernel that does not apply it");
-        return pcb_stem_forward(c, static_cast<const bf16 *>(w_fwd) + stem_base(L), bias, y, y_cstride, msum, tapmask, bn_sums, ep, st);
-    }
-    if (smallco_ok(c)) {
-        PCB_CHECK(ep == nullptr, "fused BatchNorm + activation requested from a small-Cout kernel that does not apply it");
-        if (pcb_k2r_ok(c)) {
-            size_t fb, db;
-            k2r_bases(L, &fb, &db);
-            return pcb_k2r_forward(c, smallco_layout(L), w_fwd, static_cast<const bf16 *>(w_fwd) + fb, bias, y, y_cstride, msum, tapmask, st);
-        }
-        return pcb_smallco_forward(c, smallco_layout(L), w_fwd, bias, y, y_cstride, msum, st);
-    }
+    PCB_CHECK(bn_sums == nullptr || T.fuses_epilogue, "fused BatchNorm statistics requested from a kernel that does not produce them");
+    PCB_CHECK(ep == nullptr || T.fuses_epilogue, "fused BatchNorm + activation requested from a kernel that does not apply it");
+    if (!mask_pass_done && T.fwd_tapmask)
+        if (int rc = launch_tapmask(c, tapmask, st)) return rc;
+    const bf16 *wf = static_cast<const bf16 *>(w_fwd);
+    if (F.route == ROUTE_STEM) return pcb_stem_forward(c, T.stem, wf + T.extra_fwd_off, bias, y, y_cstride, msum, tapmask, bn_sums, ep, st);
+    if (F.route == ROUTE_K2R) return pcb_k2r_forward(c, T.k2r, smallco_layout(L), w_fwd, wf + T.extra_fwd_off, bias, y, y_cstride, msum, tapmask, st);
+    if (F.route == ROUTE_SMALLCO) return pcb_smallco_forward(c, smallco_layout(L), w_fwd, bias, y, y_cstride, msum, st);
     TcParams P;
     base_params(P, c, L);
-    P.m_total = static_cast<int>(m_total);
-    fill_parts(c, L, P.parts, tapmask, m_total);
+    P.m_total = static_cast<int>(T.m_out);
+    fill_parts(c, L, P.parts, tapmask, T.m_out);
     P.bias = bias; P.msum = msum; P.y = static_cast<bf16 *>(y); P.y_cstride = y_cstride; P.abort_flag = flag;
-    PCB_CHECK(bn_sums == nullptr || pcb_tc_fuses_bn_stats(c), "fused BatchNorm statistics requested from a kernel that does not produce them");
     P.bn_sums = bn_sums; P.bn_c = c->cout;
-    PCB_CHECK(ep == nullptr || pcb_tc_fuses_affine_act(c), "fused BatchNorm + activation requested from a kernel that does not apply it");
     set_ep(P, ep);
     P.ncols = L.rows_f;
     CUtensorMap tm;
-    if (tma_fwd_ok(c)) {
-        tile_box(c->wo, c->ho, &P.box_w, &P.box_h, &P.box_n);
-        const int bn = pick_bn(c->cout <= 32 ? 32 : L.rows_f, m_total, true);
-        const bool halo = tma_halo_ok(c, P.box_w, P.box_h, P.box_n, bn);
-        const int hx = halo ? (c->kw - 1) * c->dil : 0;
+    if (int rc = make_tmap_2d(&tm, w_fwd, L.rows_f, L.kf, L.kf, F.bn)) return rc;
+    if (F.route == ROUTE_TMA) {
+        P.box_w = F.box_w; P.box_h = F.box_h; P.box_n = F.box_n;
         CUtensorMap ta[TC_MAX_PARTS];
-        memset(ta, 0, sizeof(ta));
-        uint8_t *extra = reinterpret_cast<uint8_t *>(tapmask) + tapmask_bytes(c);
-        for (int p = 0; p < c->nparts; ++p) {
-            const pcb_part &pt = c->parts[p];
-            const void *src = pt.x;
-            long long cs = pt.x_cstride;
-            const int c8 = rup(pt.c, 8);
-            if (pt.x_up) {
-                const long long pix = static_cast<long long>(c->n) * (c->h >> 1) * (c->w >> 1);
-                const long long work = pix * (c8 >> 3);
-                const int grid = static_cast<int>(std::min<long long>((work + 255) / 256, 16ll * pcb_num_sms()));
-                upsample_part_kernel<<<grid, 256, 0, st>>>(static_cast<const bf16 *>(pt.x), pt.x_cstride, c8, pix, c->h >> 1, c->w >> 1, reinterpret_cast<bf16 *>(extra));
-                PCB_LAUNCH_CHECK();
-                src = extra; cs = c8;
-                extra += up_bytes(c, p);
-            }
-            if (pt.mask) P.use_fix = 1;
-            if (int rc = make_tmap_nhwc(&ta[p], src, c8, c->w, c->h, c->n, cs, P.box_w + hx, P.box_h, P.box_n, c->stride)) return rc;
-        }
-        if (c->nparts < 2) ta[1] = ta[0];
+        if (int rc = a_operand_maps(c, T, tapmask, F.box_w + (F.halo ? (c->kw - 1) * c->dil : 0), F.box_h, F.box_n, ta, &P.use_fix, st)) return rc;
         P.ncols = (c->cout <= 32) ? 32 : L.rows_f;
         P.wk_base = 0; P.wk_col = L.ktap; P.wk_row = c->kw * L.ktap;
-        if (int rc = make_tmap_2d(&tm, w_fwd, L.rows_f, L.kf, L.kf, bn)) return rc;
-        return launch_tma<0>(P, tm, ta[0], ta[1], bn, halo, st);
+        return launch_tma<0>(P, tm, ta[0], ta[1], F.bn, F.halo, st);
     }
-    if (int rc = make_tmap_2d(&tm, w_fwd, L.rows_f, L.kf, L.kf, L.bn_f)) return rc;
-    P.hg = halo_hg(c, L.rowpack);
-    return launch_tc<0>(P, tm, L.bn_f, st);
+    P.hg = F.hg;
+    return launch_tc<0>(P, tm, F.bn, st);
 }
-
-bool pcb_tc_dgrad_supported(const pcb_conv *c) { return pcb_tc_eligible(c) && !is_rowpack(c); }
 
 // the data-gradient problems whose kernel can apply the ReLU backward of the layer's input in its epilogue: the TMA-fed
 // stride-1 kernel on a single-part layer (not the small-Cout, sub-pixel or gather kernels)
-bool pcb_tc_dgrad_fuses_relu(const pcb_conv *c) {
-    return c->nparts == 1 && !smallco_ok(c) && !sp_plan(c).ok && tma_dgrad_ok(c);
-}
+bool pcb_tc_dgrad_fuses_relu(const pcb_conv *c) { return tc_plan(c).dg_fuses_relu; }
 
 int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_dgrad, void *const *dx, const int *dx_cstride,
                  cudaStream_t st, const void *relu_x, int relu_cstride) {
-    PCB_CHECK(relu_x == nullptr || (pcb_tc_dgrad_fuses_relu(c) && relu_cstride % 8 == 0 && relu_cstride >= rup(c->cin, 8) &&
+    const TcPlan T = tc_plan(c);
+    const Layout &L = T.L;
+    const DirPlan &D = T.dg;
+    PCB_CHECK(D.route != ROUTE_NONE, "data gradient of a row-packed (cin <= 8) tensor-core layer: set force_generic and pass KRSC weights");
+    PCB_CHECK(w_dgrad != nullptr && (reinterpret_cast<uintptr_t>(dc) & 15) == 0, "pcb_pconv_backward_data: w_dgrad required / dc misaligned");
+    PCB_CHECK(relu_x == nullptr || (T.dg_fuses_relu && relu_cstride % 8 == 0 && relu_cstride >= rup(c->cin, 8) &&
                                     (reinterpret_cast<uintptr_t>(relu_x) & 15) == 0),
               "tensor-core dgrad: the ReLU backward is fused only on the TMA-fed stride-1 kernel (16-byte aligned input, channel stride %% 8 == 0)");
     int *flag = abort_flag_ptr();
     PCB_CHECK(flag != nullptr, "cudaMalloc(abort flag) failed");
-    const long long m_total = static_cast<long long>(c->n) * c->h * c->w;
-    PCB_CHECK(m_total < (1ll << 31), "problem too large");
+    PCB_CHECK(T.m_in < (1ll << 31), "problem too large");
     PCB_CHECK(dc_cstride % 8 == 0 && dc_cstride >= rup(c->cout, 8), "tensor-core dgrad: dc channel stride must be a multiple of 8");
-    const Layout L = layout_of(c);
-    if (smallco_ok(c)) {
-        if (pcb_k2r_ok(c)) {
-            size_t fb, db;
-            k2r_bases(L, &fb, &db);
-            return pcb_k2r_dgrad(c, smallco_layout(L), dc, dc_cstride, w_dgrad, static_cast<const bf16 *>(w_dgrad) + db, dx, dx_cstride, st);
-        }
-        return pcb_smallco_dgrad(c, smallco_layout(L), dc, dc_cstride, w_dgrad, dx, dx_cstride, st);
-    }
+    const bf16 *wd = static_cast<const bf16 *>(w_dgrad);
+    if (D.route == ROUTE_K2R) return pcb_k2r_dgrad(c, T.k2r, smallco_layout(L), dc, dc_cstride, w_dgrad, wd + T.extra_dg_off, dx, dx_cstride, st);
+    if (D.route == ROUTE_SMALLCO) return pcb_smallco_dgrad(c, smallco_layout(L), dc, dc_cstride, w_dgrad, dx, dx_cstride, st);
     // sub-pixel path: the gradient of the upsampled part is computed directly at source resolution (dx[pu] is a SOURCE-resolution
     // buffer, see pcb_conv_dgrad_at_source_resolution); the other part goes through the regular kernel below
-    const SpPlan SPL = sp_plan(c);
+    const SpPlan &SPL = T.sp;
     void *dx_local[TC_MAX_PARTS] = {nullptr, nullptr};
     for (int p = 0; p < c->nparts && p < TC_MAX_PARTS; ++p) dx_local[p] = dx[p];
     if (SPL.ok) {
         if (dx[SPL.pu] != nullptr)
-            if (int rc = sp_dgrad_up(c, SPL, L, dc, dc_cstride, static_cast<const bf16 *>(w_dgrad) + static_cast<size_t>(rup(L.ktap, 128)) * L.kd,
-                                     dx[SPL.pu], dx_cstride[SPL.pu], flag, st)) return rc;
+            if (int rc = sp_dgrad_up(c, SPL, L, dc, dc_cstride, wd + T.sp_off, dx[SPL.pu], dx_cstride[SPL.pu], flag, st)) return rc;
         dx_local[SPL.pu] = nullptr;
         if (SPL.ps < 0 || dx[SPL.ps] == nullptr) return 0;
     }
     dx = dx_local;
     TcParams P;
     base_params(P, c, L);
-    P.m_total = static_cast<int>(m_total);
+    P.m_total = static_cast<int>(T.m_in);
     fill_parts(c, L, P.parts, nullptr, 0);
     for (int p = 0; p < c->nparts; ++p) {
         P.parts[p].dx = static_cast<bf16 *>(dx[p]);
@@ -2860,33 +2936,26 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
     P.dc = static_cast<const bf16 *>(dc); P.dc_cstride = dc_cstride; P.dc_c8 = rup(c->cout, 8); P.dc_kext = L.cout64;
     P.relu_x = static_cast<const bf16 *>(relu_x); P.relu_cstride = relu_cstride;
     P.abort_flag = flag;
-    int bn = (L.ktap % 128 == 0) ? 128 : 64;
     P.ncols = L.ktap;
     CUtensorMap tm;
-    if (tma_dgrad_ok(c)) {
-        tile_box(c->w, c->h, &P.box_w, &P.box_h, &P.box_n);
-        bn = pick_bn(L.ktap, m_total, false);
-        const bool halo = tma_halo_ok(c, P.box_w, P.box_h, P.box_n, bn);
+    if (int rc = make_tmap_2d(&tm, w_dgrad, rup(L.ktap, 128), L.kd, L.kd, D.bn)) return rc;
+    if (D.route == ROUTE_TMA) {
+        P.box_w = D.box_w; P.box_h = D.box_h; P.box_n = D.box_n;
         P.wk_base = 0; P.wk_col = L.cout64; P.wk_row = c->kw * L.cout64;
         CUtensorMap ta;
-        if (int rc = make_tmap_nhwc(&ta, dc, P.dc_c8, c->wo, c->ho, c->n, dc_cstride, P.box_w + (halo ? (c->kw - 1) * c->dil : 0), P.box_h, P.box_n, 1)) return rc;
-        if (int rc = make_tmap_2d(&tm, w_dgrad, rup(L.ktap, 128), L.kd, L.kd, bn)) return rc;
-        return launch_tma<1>(P, tm, ta, ta, bn, halo, st);
+        if (int rc = make_tmap_nhwc(&ta, dc, P.dc_c8, c->wo, c->ho, c->n, dc_cstride, D.box_w + (D.halo ? (c->kw - 1) * c->dil : 0), D.box_h, D.box_n, 1)) return rc;
+        return launch_tma<1>(P, tm, ta, ta, D.bn, D.halo, st);
     }
-    if (tma_dgrad_s2_ok(c)) {
+    if (D.route == ROUTE_TMA_S2) {
         // Stride 2: an input pixel (y, x) only sees the taps with (y + pad - tr) even, so the four parity classes
         // (y & 1, x & 1) are four independent STRIDE-1 problems on the half-resolution grid -- which is dc's own grid --
         // each with its subset of taps (3x3 / 3x2 / 2x3 / 2x2 for a 5x5 kernel) and no multiplications by inserted zeros.
         const int hh = c->h / 2, hw = c->w / 2;
-        const long long m_class = static_cast<long long>(c->n) * hh * hw;
-        tile_box(hw, hh, &P.box_w, &P.box_h, &P.box_n);
-        bn = pick_bn(L.ktap, m_class, false);
-        if (int rc = make_tmap_2d(&tm, w_dgrad, rup(L.ktap, 128), L.kd, L.kd, bn)) return rc;
+        P.box_w = D.box_w; P.box_h = D.box_h; P.box_n = D.box_n;
         // The classes write disjoint pixels.  When one class does not fill the GPU (low-resolution layers) the four launches
         // run concurrently: fork onto three internal streams after an event on `st`, join before returning (also valid
         // inside a stream capture: the internal streams join the capture and leave it again).
-        const long long class_tiles = ((m_class + BLOCK_M - 1) / BLOCK_M) * (L.ktap / bn);
-        const bool fork = class_tiles < pcb_num_sms();
+        const bool fork = T.cls_fork;
         ClassStreams *CS = nullptr;
         if (fork) {
             if (int rc = class_streams(&CS)) return rc;
@@ -2896,19 +2965,18 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
             TcParams Q = P;
             const int py = cls >> 1, px = cls & 1;
             const int tr0 = (py + c->pad_h) & 1, tc0 = (px + c->pad_w) & 1;
-            Q.kh = (c->kh - tr0 + 1) / 2; Q.kw = (c->kw - tc0 + 1) / 2;
+            Q.kh = (c->kh - tr0 + 1) / 2; Q.kw = class_kw(c, px);
             Q.pad_h = (py + c->pad_h - tr0) / 2; Q.pad_w = (px + c->pad_w - tc0) / 2;
             Q.h = hh; Q.w = hw; Q.stride = 1; Q.dil = 1;
-            Q.m_total = static_cast<int>(m_class);
+            Q.m_total = static_cast<int>(static_cast<long long>(c->n) * hh * hw);
             Q.sub = 2; Q.py = py; Q.px = px; Q.fh = c->h; Q.fw = c->w;
             Q.wk_base = (tr0 * c->kw + tc0) * L.cout64; Q.wk_row = 2 * c->kw * L.cout64; Q.wk_col = 2 * L.cout64;
-            const bool halo = !getenv("PCB_DISABLE_TMA_HALO") && Q.box_w == 128 && Q.box_h == 1 && Q.box_n == 1 && Q.kw >= 2 &&
-                              halo_stages_fit(Q.kw, 1, bn);
+            const bool halo = T.cls_halo[cls];
             CUtensorMap ta;
             if (int rc = make_tmap_nhwc(&ta, dc, P.dc_c8, c->wo, c->ho, c->n, dc_cstride, Q.box_w + (halo ? Q.kw - 1 : 0), Q.box_h, Q.box_n, 1)) return rc;
             cudaStream_t cs = (fork && cls > 0) ? CS->aux[cls - 1] : st;
             if (fork && cls > 0) PCB_CUDA(cudaStreamWaitEvent(cs, CS->ev_fork, 0));
-            if (int rc = launch_tma<1>(Q, tm, ta, ta, bn, halo, cs)) return rc;
+            if (int rc = launch_tma<1>(Q, tm, ta, ta, D.bn, halo, cs)) return rc;
             if (fork && cls > 0) {
                 PCB_CUDA(cudaEventRecord(CS->ev_join[cls - 1], cs));
                 PCB_CUDA(cudaStreamWaitEvent(st, CS->ev_join[cls - 1], 0));
@@ -2916,35 +2984,12 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
         }
         return 0;
     }
-    if (int rc = make_tmap_2d(&tm, w_dgrad, rup(L.ktap, 128), L.kd, L.kd, bn)) return rc;
-    P.hg = halo_hg(c, L.rowpack);
-    return launch_tc<1>(P, tm, bn, st);
+    P.hg = D.hg;
+    return launch_tc<1>(P, tm, D.bn, st);
 }
 
 
 // ---- TMA-fed weight gradient ---------------------------------------------------------------------
-// 64 consecutive pixels of a [n][ht][wt] grid as a box {bw, bh, bn}
-static bool kblock_box(int wt, int ht, int *bw, int *bh, int *bn) {
-    if (wt < 4) return false;
-    if (wt % 64 == 0) { *bw = 64; *bh = 1; *bn = 1; return true; }
-    if (64 % wt) return false;
-    const int rows = 64 / wt;
-    *bw = wt;
-    if (ht % rows == 0) { *bh = rows; *bn = 1; return true; }
-    if (rows % ht) return false;
-    *bh = ht; *bn = rows / ht;
-    return true;
-}
-
-static bool tma_wgrad_ok(const pcb_conv *c) {
-    if (getenv("PCB_DISABLE_TMA") || getenv("PCB_DISABLE_TMA_WGRAD") || is_rowpack(c) || c->stride > 2) return false;
-    int bw, bh, bn;
-    if (!kblock_box(c->wo, c->ho, &bw, &bh, &bn)) return false;
-    for (int p = 0; p < c->nparts; ++p)
-        if (c->parts[p].x_up && ((c->h | c->w) & 1)) return false;
-    return true;
-}
-
 template <int BLOCK_N, int T, bool HALO>
 int launch_wgrad_tma(WgParams &P, const CUtensorMap &tdc, const CUtensorMap &ta0, const CUtensorMap &ta1, cudaStream_t st) {
     const int rows_a = 64 + (HALO ? (P.kw - 1) * P.dil : 0);
@@ -2998,66 +3043,34 @@ int pcb_tc_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, v
     int *flag = abort_flag_ptr();
     PCB_CHECK(flag != nullptr, "cudaMalloc(abort flag) failed");
     PCB_CHECK(workspace != nullptr, "pcb_tc_wgrad: workspace required");
-    const long long m_total = static_cast<long long>(c->n) * c->ho * c->wo;
-    PCB_CHECK(m_total < (1ll << 31), "problem too large");
+    const TcPlan T = tc_plan(c);
+    const Layout &L = T.L;
+    const DirPlan &W = T.wg;
+    PCB_CHECK(T.m_out < (1ll << 31), "problem too large");
     PCB_CHECK(dc_cstride % 8 == 0 && dc_cstride >= c->cout, "tensor-core wgrad: dc channel stride must be a multiple of 8");
-    if (stem_ok(c)) return pcb_stem_wgrad(c, dc, dc_cstride, dw, workspace, zero_dw, st);
-    if (smallco_ok(c)) {
-        if (pcb_k2r_ok(c)) return pcb_k2r_wgrad(c, dc, dc_cstride, dw, workspace, zero_dw, st);
-        return pcb_smallco_wgrad(c, smallco_layout(layout_of(c)), dc, dc_cstride, dw, zero_dw, st);
-    }
+    if (W.route == ROUTE_STEM) return pcb_stem_wgrad(c, T.stem, dc, dc_cstride, dw, workspace, zero_dw, st);
+    if (W.route == ROUTE_K2R) return pcb_k2r_wgrad(c, T.k2r, dc, dc_cstride, dw, workspace, zero_dw, st);
+    if (W.route == ROUTE_SMALLCO) return pcb_smallco_wgrad(c, smallco_layout(L), dc, dc_cstride, dw, zero_dw, st);
     uint64_t *tapmask = static_cast<uint64_t *>(workspace);
-    bool any_mask = false;
-    for (int p = 0; p < c->nparts; ++p) any_mask = any_mask || (c->parts[p].mask != nullptr);
-    if (any_mask || !tma_wgrad_ok(c))                     // the TMA-fed kernel without holes needs no validity words
+    if (T.wg_tapmask)
         if (int rc = launch_tapmask(c, tapmask, st)) return rc;
     const size_t dw_bytes = sizeof(float) * c->cout * c->kh * c->kw * c->cin;
     if (zero_dw) PCB_CUDA(cudaMemsetAsync(dw, 0, dw_bytes, st));
-    const Layout L = layout_of(c);
     WgParams P;
     memset(&P, 0, sizeof(P));
     P.n = c->n; P.h = c->h; P.w = c->w; P.cin = c->cin; P.cout = c->cout; P.kh = c->kh; P.kw = c->kw; P.stride = c->stride;
-    P.pad_h = c->pad_h; P.pad_w = c->pad_w; P.dil = c->dil; P.ho = c->ho; P.wo = c->wo; P.m_total = static_cast<int>(m_total);
+    P.pad_h = c->pad_h; P.pad_w = c->pad_w; P.dil = c->dil; P.ho = c->ho; P.wo = c->wo; P.m_total = static_cast<int>(T.m_out);
     P.nparts = c->nparts; P.rowpack = L.rowpack; P.ktap = L.ktap; P.ntaps = L.rowpack ? c->kh : c->kh * c->kw;
-    fill_parts(c, L, P.parts, tapmask, m_total);
+    fill_parts(c, L, P.parts, tapmask, T.m_out);
     P.dw = dw; P.abort_flag = flag;
     CUtensorMap tm;
-    if (int rc = make_tmap_2d(&tm, dc, m_total, c->cout, dc_cstride, 64)) return rc;
-    if (tma_wgrad_ok(c)) {
-        kblock_box(c->wo, c->ho, &P.box_w, &P.box_h, &P.box_n);
-        // row-halo tiles for kw == 3: the three taps of a kernel row are three 64 x 64 register accumulators per consumer thread
-        const bool halo = !getenv("PCB_DISABLE_TMA_HALO") && c->stride == 1 && c->kw == 3 && P.box_w == 64 &&
-                          P.box_h == 1 && P.box_n == 1 && 64 + (c->kw - 1) * c->dil <= 256;
-        const int hx = halo ? (c->kw - 1) * c->dil : 0;
+    if (int rc = make_tmap_2d(&tm, dc, T.m_out, c->cout, dc_cstride, 64)) return rc;
+    if (W.route == ROUTE_TMA) {
+        P.box_w = W.box_w; P.box_h = W.box_h; P.box_n = W.box_n;
         CUtensorMap ta[TC_MAX_PARTS];
-        memset(ta, 0, sizeof(ta));
-        uint8_t *extra = reinterpret_cast<uint8_t *>(workspace) + tapmask_bytes(c);
-        for (int p = 0; p < c->nparts; ++p) {
-            const pcb_part &pt = c->parts[p];
-            const void *src = pt.x;
-            long long cs = pt.x_cstride;
-            const int c8 = rup(pt.c, 8);
-            if (pt.x_up) {
-                const long long pix = static_cast<long long>(c->n) * (c->h >> 1) * (c->w >> 1);
-                const long long work = pix * (c8 >> 3);
-                const int grid = static_cast<int>(std::min<long long>((work + 255) / 256, 16ll * pcb_num_sms()));
-                upsample_part_kernel<<<grid, 256, 0, st>>>(static_cast<const bf16 *>(pt.x), pt.x_cstride, c8, pix, c->h >> 1, c->w >> 1, reinterpret_cast<bf16 *>(extra));
-                PCB_LAUNCH_CHECK();
-                src = extra; cs = c8;
-                extra += up_bytes(c, p);
-            }
-            if (pt.mask) P.use_fix = 1;
-            if (int rc = make_tmap_nhwc(&ta[p], src, c8, c->w, c->h, c->n, cs, P.box_w + hx, P.box_h, P.box_n, c->stride)) return rc;
-        }
-        if (c->nparts < 2) ta[1] = ta[0];
-        // 128 output channels per tile, except for layers with at most 64 and for short reductions (< 128 K blocks of 64
-        // pixels): there each CTA has few K blocks and its red.global.add epilogue, twice as long at 128 columns, dominates
-        if (c->cout > 64 && m_total >= 128 * 64) {
-            if (halo) return launch_wgrad_tma<128, 3, true>(P, tm, ta[0], ta[1], st);
-            return launch_wgrad_tma<128, 3, false>(P, tm, ta[0], ta[1], st);
-        }
-        if (halo) return launch_wgrad_tma<64, 3, true>(P, tm, ta[0], ta[1], st);
-        return launch_wgrad_tma<64, 3, false>(P, tm, ta[0], ta[1], st);
+        if (int rc = a_operand_maps(c, T, workspace, W.box_w + (W.halo ? (c->kw - 1) * c->dil : 0), W.box_h, W.box_n, ta, &P.use_fix, st)) return rc;
+        if (W.bn == 128) return W.halo ? launch_wgrad_tma<128, 3, true>(P, tm, ta[0], ta[1], st) : launch_wgrad_tma<128, 3, false>(P, tm, ta[0], ta[1], st);
+        return W.halo ? launch_wgrad_tma<64, 3, true>(P, tm, ta[0], ta[1], st) : launch_wgrad_tma<64, 3, false>(P, tm, ta[0], ta[1], st);
     }
     return launch_wgrad<64, 3, 3>(P, tm, c->cout, st);
 }

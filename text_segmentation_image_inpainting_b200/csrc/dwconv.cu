@@ -728,9 +728,15 @@ __global__ void __launch_bounds__(256, 2) dw4_s1_wgrad_kernel(const T *__restric
     }
 }
 
-bool dw4_ok(const pcb_conv *c) {
-    return c->kh == 3 && c->kw == 3 && c->stride == 1 && c->pad_h == c->dil && c->pad_w == c->dil && c->plain && c->parts[0].mask == nullptr &&
-           c->cin % 4 == 0 && !getenv("PCB_DW_GEN2") && !getenv("PCB_DW_GEN1");
+// the kernel generation a direction takes: dw4 (plain 3x3 stride 1, pad == dil; the data gradient is the same convolution with
+// flipped taps), dw3 (any other 3x3; its data gradient walks the input grid with shifts, so power-of-two strides only), or
+// the first generation (every other shape)
+enum DwRoute { DW_GEN1, DW3, DW4 };
+
+DwRoute dw_route(const pcb_conv *c, bool dgrad) {
+    if (c->kh != 3 || c->kw != 3) return DW_GEN1;
+    if (c->stride == 1 && c->pad_h == c->dil && c->pad_w == c->dil && c->plain && c->parts[0].mask == nullptr && c->cin % 4 == 0) return DW4;
+    return (dgrad && (c->stride & (c->stride - 1))) ? DW_GEN1 : DW3;
 }
 
 template <typename T>
@@ -759,7 +765,6 @@ inline int dw_grid(long long items) {
 }  // namespace
 
 bool pcb_dw_eligible(const pcb_conv *c) {
-    if (c->force_generic || getenv("PCB_DISABLE_DW")) return false;
     if (!(c->groups == c->cin && c->cin == c->cout && c->groups > 1 && c->nparts == 1)) return false;
     const pcb_part &pt = c->parts[0];
     if (c->cin % 8 != 0 || c->cin > 2048 || pt.x_cstride % 8 != 0 || pt.x_up != 0) return false;
@@ -777,25 +782,21 @@ int pcb_dw_weight_prepare(const pcb_conv *c, const float *w_master, void *w_t, c
     return 0;
 }
 
-bool pcb_dw_fuses_bn_stats(const pcb_conv *c) {
-    return pcb_dw_fuses_affine_act(c) && !getenv("PCB_DISABLE_FUSED_BN_STATS");
-}
-
-// the 3x3 kernels (dw3_fwd_kernel, dw4_s1_kernel) can apply an eval-mode BatchNorm + activation before they store
-bool pcb_dw_fuses_affine_act(const pcb_conv *c) {
-    return pcb_dw_eligible(c) && c->kh == 3 && c->kw == 3 && !getenv("PCB_DW_GEN1");
-}
+// the 3x3 kernels (dw3_fwd_kernel, dw4_s1_kernel) can accumulate the BatchNorm statistics of their output / apply an eval-mode
+// BatchNorm + activation before they store
+bool pcb_dw_fuses_epilogue(const pcb_conv *c) { return dw_route(c, false) != DW_GEN1; }
 
 int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *y, int y_cstride, const float *msum, double *bn_sums,
                    const pcb_ep *ep, cudaStream_t st) {
-    PCB_CHECK(bn_sums == nullptr || pcb_dw_fuses_bn_stats(c), "depthwise forward: fused BatchNorm statistics need the 3x3 kernels");
-    PCB_CHECK(ep == nullptr || pcb_dw_fuses_affine_act(c), "depthwise forward: fused BatchNorm + activation needs the 3x3 kernels");
+    const DwRoute route = dw_route(c, false);
+    PCB_CHECK(bn_sums == nullptr || route != DW_GEN1, "depthwise forward: fused BatchNorm statistics need the 3x3 kernels");
+    PCB_CHECK(ep == nullptr || route != DW_GEN1, "depthwise forward: fused BatchNorm + activation needs the 3x3 kernels");
     DwParams P;
     fill(P, c);
     P.ep = dw_ep(ep);
     P.y_cstride = y_cstride;
     P.msum = msum;       // plain mode: mask_sums wrote 1.0 everywhere, so the same epilogue applies
-    if (dw4_ok(c)) {
+    if (route == DW4) {
         const Dw4Geom g = dw4_geom(c->cin, c->w, c->h, c->dil);
         const dim3 grid(g.chunks, g.xtiles, c->n * g.pgroups * g.nseg);
 #define PCB_DW4_FWD(TT, EP_) dw4_s1_kernel<TT, false, EP_><<<grid, 256, 0, st>>>(static_cast<const TT *>(c->parts[0].x), c->parts[0].x_cstride, static_cast<const TT *>(w_t), bias, static_cast<TT *>(y), y_cstride, bn_sums, P.ep, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb)
@@ -805,7 +806,7 @@ int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *
         PCB_LAUNCH_CHECK();
         return 0;
     }
-    if (c->kh == 3 && c->kw == 3 && !getenv("PCB_DW_GEN1")) {
+    if (route == DW3) {
         const Dw3Geom g = dw3_geom(c->cin);
         const dim3 grid(g.chunks, (c->n * c->ho + DW3_ROWS - 1) / DW3_ROWS);
         const bool plain = c->plain && c->parts[0].mask == nullptr;
@@ -831,7 +832,8 @@ int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *
 int pcb_dw_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_t, void *dx, int dx_cstride, cudaStream_t st) {
     DwParams P;
     fill(P, c);
-    if (dw4_ok(c)) {                                      // stride 1, pad == dil: the data gradient is the same convolution with flipped taps
+    const DwRoute route = dw_route(c, true);
+    if (route == DW4) {
         const Dw4Geom g = dw4_geom(c->cin, c->w, c->h, c->dil);
         const dim3 grid(g.chunks, g.xtiles, c->n * g.pgroups * g.nseg);
         if (c->dtype == PCB_BF16) dw4_s1_kernel<bf16, true, false><<<grid, 256, 0, st>>>(static_cast<const bf16 *>(dc), dc_cstride, static_cast<const bf16 *>(w_t), nullptr, static_cast<bf16 *>(dx), dx_cstride, nullptr, P.ep, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
@@ -839,7 +841,7 @@ int pcb_dw_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
         PCB_LAUNCH_CHECK();
         return 0;
     }
-    if (c->kh == 3 && c->kw == 3 && (c->stride & (c->stride - 1)) == 0 && !getenv("PCB_DW_GEN1")) {
+    if (route == DW3) {
         const Dw3Geom g = dw3_geom(c->cin);
         const dim3 grid(g.chunks, (c->n * c->h + DW3_ROWS - 1) / DW3_ROWS);
         const bool plain = c->plain && c->parts[0].mask == nullptr;
@@ -864,7 +866,8 @@ int pcb_dw_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, b
     fill(P, c);
     const int taps = c->kh * c->kw;
     if (zero_dw) PCB_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * c->cin * taps, st));
-    if (dw4_ok(c)) {
+    const DwRoute route = dw_route(c, false);
+    if (route == DW4) {
         const Dw4Geom g = dw4_geom(c->cin, c->w, c->h, c->dil);
         const dim3 grid(g.chunks, g.xtiles, c->n * g.pgroups * g.nseg);
         if (c->dtype == PCB_BF16) dw4_s1_wgrad_kernel<bf16><<<grid, 256, 0, st>>>(static_cast<const bf16 *>(c->parts[0].x), c->parts[0].x_cstride, static_cast<const bf16 *>(dc), dc_cstride, dw, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
@@ -872,7 +875,7 @@ int pcb_dw_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, b
         PCB_LAUNCH_CHECK();
         return 0;
     }
-    if (c->kh == 3 && c->kw == 3 && !getenv("PCB_DW_GEN1")) {
+    if (route == DW3) {
         const Dw3Geom g = dw3_geom(c->cin);
         // about two resident waves of blocks; every block ends with cvb * 72 atomics
         const int rows_total = c->n * c->ho;

@@ -147,15 +147,13 @@ int pcb_generic_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *
 // mask box sums (all paths): msum fp32 [mg][n,ho,wo] (0 at holes), newmask u8 [mg][n,ho,wo]
 int pcb_mask_sums(const pcb_conv *c, float *msum, uint8_t *newmask, cudaStream_t st);
 bool pcb_tc_eligible(const pcb_conv *c);
-bool pcb_tc_dgrad_supported(const pcb_conv *c);
 size_t pcb_tc_workspace(const pcb_conv *c);
 void pcb_tc_weight_layout(const pcb_conv *c, size_t *fwd_elems, size_t *dgrad_elems);
 int pcb_tc_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd, void *w_dgrad, bool zero_padding, cudaStream_t st);
 int pcb_tc_forward_mask_pass(const pcb_conv *c, uint64_t *tapmask, cudaStream_t st);
 int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, void *y, int y_cstride, const float *msum,
                       uint64_t *tapmask, bool mask_pass_done, double *bn_sums, const pcb_ep *ep, cudaStream_t st);
-bool pcb_tc_fuses_bn_stats(const pcb_conv *c);
-bool pcb_tc_fuses_affine_act(const pcb_conv *c);
+bool pcb_tc_fuses_epilogue(const pcb_conv *c);
 bool pcb_tc_subpixel(const pcb_conv *c);
 // relu_x (optional, TMA-fed single-part stride-1 problems only: pcb_tc_dgrad_fuses_relu): the epilogue also applies the backward
 // of the in-place ReLU that produced the layer's input, dx = 0 where relu_x <= 0 (relu_x: bf16 NHWC, channel stride relu_cstride)
@@ -173,29 +171,42 @@ int pcb_smallco_dgrad(const pcb_conv *c, const pcb_smallco_layout &L, const void
                       cudaStream_t st);
 int pcb_smallco_wgrad(const pcb_conv *c, const pcb_smallco_layout &L, const void *dc, int dc_cstride, float *dw, bool zero_dw, cudaStream_t st);
 // RGB tails as a 1x1 GEMM at source resolution (conv_k2r.cu); the *_extra operands follow the layer's regular ones
-bool pcb_k2r_ok(const pcb_conv *c);
-void pcb_k2r_weight_layout(const pcb_conv *c, size_t *fwd_extra, size_t *dg_extra);
-size_t pcb_k2r_workspace(const pcb_conv *c);
-int pcb_k2r_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd_extra, void *w_dg_extra, bool zero_padding, cudaStream_t st);
-int pcb_k2r_forward(const pcb_conv *c, const pcb_smallco_layout &L, const void *w_fwd, const void *w_fwd_extra, const float *bias, void *y, int y_cstride,
-                    const float *msum, void *workspace, cudaStream_t st);
-int pcb_k2r_dgrad(const pcb_conv *c, const pcb_smallco_layout &L, const void *dc, int dc_cstride, const void *w_dgrad, const void *w_dg_extra,
-                  void *const *dx, const int *dx_cstride, cudaStream_t st);
-int pcb_k2r_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st);
+struct K2rPlan {
+    bool ok;
+    int pu, ps;                    // upsampled (wide) part, full-resolution (narrow) part
+    int cu, cs, choff_u, choff_s;
+    pcb_conv sub;                  // the 1x1 problem at source resolution
+    size_t sub_fe, sub_de;         // its operand sizes (bf16 elements)
+    size_t fwd_extra, dg_extra;    // elements appended to the layer's operand buffers (sub operands + fp32 staging of W')
+    size_t workspace;
+};
+K2rPlan pcb_k2r_plan(const pcb_conv *c);
+int pcb_k2r_weight_prepare(const pcb_conv *c, const K2rPlan &K, const float *w_master, void *w_fwd_extra, void *w_dg_extra, bool zero_padding,
+                           cudaStream_t st);
+int pcb_k2r_forward(const pcb_conv *c, const K2rPlan &K, const pcb_smallco_layout &L, const void *w_fwd, const void *w_fwd_extra, const float *bias,
+                    void *y, int y_cstride, const float *msum, void *workspace, cudaStream_t st);
+int pcb_k2r_dgrad(const pcb_conv *c, const K2rPlan &K, const pcb_smallco_layout &L, const void *dc, int dc_cstride, const void *w_dgrad,
+                  const void *w_dg_extra, void *const *dx, const int *dx_cstride, cudaStream_t st);
+int pcb_k2r_wgrad(const pcb_conv *c, const K2rPlan &K, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st);
 // 7x7 stride-2 image stems as a 4x4 convolution over the space-to-depth image (conv_stem.cu)
-bool pcb_stem_ok(const pcb_conv *c);
-size_t pcb_stem_weight_extra(const pcb_conv *c);
-size_t pcb_stem_workspace(const pcb_conv *c);
-int pcb_stem_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd_extra, bool zero_padding, cudaStream_t st);
-int pcb_stem_forward(const pcb_conv *c, const void *w_fwd_extra, const float *bias, void *y, int y_cstride, const float *msum, void *workspace,
-                     double *bn_sums, const pcb_ep *ep, cudaStream_t st);
-int pcb_stem_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st);
+struct StemPlan {
+    bool ok;
+    pcb_conv sub;                  // the 4x4 problem over the space-to-depth image
+    size_t sub_fe;                 // bf16 elements of the sub-problem's forward operand (rounded to 64)
+    size_t fwd_extra;              // + fp32 staging of the re-indexed master weights
+    size_t workspace;
+};
+StemPlan pcb_stem_plan(const pcb_conv *c);
+int pcb_stem_weight_prepare(const pcb_conv *c, const StemPlan &K, const float *w_master, void *w_fwd_extra, bool zero_padding, cudaStream_t st);
+int pcb_stem_forward(const pcb_conv *c, const StemPlan &K, const void *w_fwd_extra, const float *bias, void *y, int y_cstride,
+                     const float *msum, void *workspace, double *bn_sums, const pcb_ep *ep, cudaStream_t st);
+int pcb_stem_wgrad(const pcb_conv *c, const StemPlan &K, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw,
+                   cudaStream_t st);
 // depthwise fast path (dwconv.cu)
 bool pcb_dw_eligible(const pcb_conv *c);
 int pcb_dw_weight_prepare(const pcb_conv *c, const float *w_master, void *w_t, cudaStream_t st);
 int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *y, int y_cstride, const float *msum, double *bn_sums,
                    const pcb_ep *ep, cudaStream_t st);
-bool pcb_dw_fuses_bn_stats(const pcb_conv *c);
-bool pcb_dw_fuses_affine_act(const pcb_conv *c);
+bool pcb_dw_fuses_epilogue(const pcb_conv *c);
 int pcb_dw_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_t, void *dx, int dx_cstride, cudaStream_t st);
 int pcb_dw_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, bool zero_dw, cudaStream_t st);
