@@ -87,7 +87,8 @@ int pcb_conv_weight_refresh(const pcb_conv *c, const float *w_master_krsc, void 
  *   new_mask = (s != 0).
  * w_fwd  : from pcb_conv_weight_prepare
  * bias   : fp32 [cout] or NULL
- * y      : NHWC [n,ho,wo,y_cstride], y_cstride >= cout (channels [cout, y_cstride) are written as zeros)
+ * y      : NHWC [n,ho,wo,y_cstride], y_cstride >= cout (channels [cout, rup(cout, 8)) are written as zeros; channels past
+ *          that are not outputs and may be left untouched)
  * msum   : fp32 [mg][n,ho,wo]  mask sums s (0 at holes); mg = 1, or groups when groups>1 && !same_holes
  * newmask: u8   [mg][n,ho,wo]
  * workspace : pcb_pconv_workspace(c) bytes (may be NULL when that is 0)                        */
@@ -113,7 +114,7 @@ int pcb_pconv_forward_bn(const pcb_conv *c, const void *w_fwd, const float *bias
  * pcb_pconv_forward would store (0 at holes),
  *   y = act(v * scale[co] + shift[co])      rounded to the storage type once,
  * so hole pixels hold act(shift[co]) -- the reference's BatchNorm runs over the zeros the partial convolution wrote.
- * Channels [cout, y_cstride) are zeros.  scale / shift: fp32 [cout] from pcb_bn_finalize(training = 0), or both NULL for an
+ * Channels [cout, rup(cout, 8)) are zeros.  scale / shift: fp32 [cout] from pcb_bn_finalize(training = 0), or both NULL for an
  * activation alone ([PartialConv, PartialActivation] blocks).  act: PCB_ACT_*, slope: LeakyReLU's negative slope.
  * Only for problems with pcb_conv_fuses_affine_act(c) == 1 (the tensor-core kernels other than the small-Cout ones, and the
  * depthwise 3x3 kernels -- the problems pcb_conv_fuses_bn_stats accepts); others are rejected.  mask_pass_done: see pcb_pconv_forward_premasked.                                                                */
@@ -159,6 +160,14 @@ int pcb_pconv_backward_weight_acc(const pcb_conv *c, const void *dc, int dc_cstr
 /* Debug aid: after a device synchronise, returns the (sticky) pipeline-timeout code set by a tensor-core
  * kernel whose mbarrier wait expired (0 = none) and clears it. */
 int pcb_debug_pipeline_status(int *code);
+/* Debug aid (host only, nothing is launched): the kernel family each direction of this problem runs on, as PCB_ROUTE_* codes in
+ * routes[0..2] = forward, data gradient, weight gradient.  GENERIC: conv_generic.cu; DEPTHWISE: dwconv.cu; the tensor-core routes:
+ * STEM (space-to-depth 4x4 problem, conv_stem.cu), K2R (kernel-to-row RGB tail, conv_k2r.cu), SMALLCO (mma.sync, cout <= 8,
+ * conv_smallco.cu), TMA (TMA-fed wgmma), TMA_S2 (the stride-2 data gradient as four stride-1 parity classes), GATHER (cp.async-fed
+ * wgmma); NONE: the direction is refused (the data gradient of a row-packed layer, which its callers run with force_generic). */
+enum { PCB_ROUTE_NONE = 0, PCB_ROUTE_GENERIC = 1, PCB_ROUTE_DEPTHWISE = 2, PCB_ROUTE_STEM = 3, PCB_ROUTE_K2R = 4,
+       PCB_ROUTE_SMALLCO = 5, PCB_ROUTE_TMA = 6, PCB_ROUTE_TMA_S2 = 7, PCB_ROUTE_GATHER = 8 };
+int pcb_debug_conv_routes(const pcb_conv *c, int32_t routes[3]);
 
 /* ---- masks ----------------------------------------------------------------------------- */
 /* dense fp32 NCHW mask (the reference API, partial_convolution.py:50) -> c u8 planes [c][n,h,w]. */

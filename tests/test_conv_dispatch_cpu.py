@@ -36,7 +36,10 @@ def host_queries(lib, c):
     ref = ctypes.byref(c)
     fe, de = ctypes.c_size_t(), ctypes.c_size_t()
     lib.pcb_conv_weight_layout(ref, ctypes.byref(fe), ctypes.byref(de))
+    routes = (ctypes.c_int32 * 3)()
+    _lib.check(lib.pcb_debug_conv_routes(ref, routes))
     return {"uses_tensor_cores": lib.pcb_conv_uses_tensor_cores(ref), "workspace": lib.pcb_pconv_workspace(ref),
+            "routes": [_lib.ROUTES[r] for r in routes],
             "weight_fwd_elems": fe.value, "weight_dgrad_elems": de.value, "fuses_bn_stats": lib.pcb_conv_fuses_bn_stats(ref),
             "fuses_affine_act": lib.pcb_conv_fuses_affine_act(ref),
             "dgrad_at_source_resolution": lib.pcb_conv_dgrad_at_source_resolution(ref),

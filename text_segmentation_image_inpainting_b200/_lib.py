@@ -13,6 +13,8 @@ ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_RELU6 = 0, 1, 2, 3
 MAX_PARTS = 8
 SEG_FOCAL, SEG_BOOTSTRAP = 0, 1
 SEG_NONE, SEG_MEAN, SEG_SUM = 0, 1, 2
+# PCB_ROUTE_* of pcb_debug_conv_routes, by code
+ROUTES = ("none", "generic", "depthwise", "stem", "k2r", "smallco", "tma", "tma_s2", "gather")
 
 c_int, c_ll, c_float, c_void_p, c_size_t = ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
@@ -53,6 +55,7 @@ _SIGS = {
     "pcb_pconv_backward_weight": (c_int, [ctypes.POINTER(Conv), c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_pconv_backward_weight_acc": (c_int, [ctypes.POINTER(Conv), c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_debug_pipeline_status": (c_int, [ctypes.POINTER(c_int)]),
+    "pcb_debug_conv_routes": (c_int, [ctypes.POINTER(Conv), ctypes.POINTER(ctypes.c_int32)]),
     "pcb_mask_planes_from_dense": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pcb_mask_plane_to_dense": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pcb_bn_stats": (c_int, [c_void_p, c_int, c_ll, c_int, c_void_p, c_void_p, c_void_p]),

@@ -235,3 +235,15 @@ PCB_API int pcb_debug_pipeline_status(int *code) {
     PCB_CHECK(code != nullptr, "null code");
     return pcb_tc_read_abort_flag(code);
 }
+
+PCB_API int pcb_debug_conv_routes(const pcb_conv *c, int32_t routes[3]) {
+    PCB_CHECK(routes != nullptr, "null routes");
+    if (int rc = validate(c, false)) return rc;
+    const Family f = family_of(c);
+    if (f == FAMILY_TC) {
+        pcb_tc_routes(c, routes);
+        return 0;
+    }
+    routes[0] = routes[1] = routes[2] = (f == FAMILY_DW) ? PCB_ROUTE_DEPTHWISE : PCB_ROUTE_GENERIC;
+    return 0;
+}

@@ -2804,6 +2804,13 @@ void pcb_tc_weight_layout(const pcb_conv *c, size_t *fwd_elems, size_t *dgrad_el
 // true when the data gradient of the 2x-upsampled part is delivered at that part's own (source) resolution
 bool pcb_tc_subpixel(const pcb_conv *c) { return tc_plan(c).dg_at_source; }
 
+void pcb_tc_routes(const pcb_conv *c, int32_t routes[3]) {
+    static const int32_t code[] = {PCB_ROUTE_NONE, PCB_ROUTE_STEM, PCB_ROUTE_K2R, PCB_ROUTE_SMALLCO, PCB_ROUTE_TMA, PCB_ROUTE_TMA_S2,
+                                   PCB_ROUTE_GATHER};
+    const TcPlan T = tc_plan(c);
+    routes[0] = code[T.fwd.route]; routes[1] = code[T.dg.route]; routes[2] = code[T.wg.route];
+}
+
 int pcb_tc_weight_prepare(const pcb_conv *c, const float *w_master, void *w_fwd, void *w_dgrad, bool zero_padding, cudaStream_t st) {
     const TcPlan T = tc_plan(c);
     const Layout &L = T.L;

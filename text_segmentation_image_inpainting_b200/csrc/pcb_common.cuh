@@ -162,6 +162,8 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
 bool pcb_tc_dgrad_fuses_relu(const pcb_conv *c);
 int pcb_tc_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st);
 int pcb_tc_read_abort_flag(int *value);
+// the plan's route of the forward, data gradient and weight gradient as PCB_ROUTE_* codes (pcb_debug_conv_routes)
+void pcb_tc_routes(const pcb_conv *c, int32_t routes[3]);
 // layers with <= 8 output channels (conv_smallco.cu); weights are read from the tensor-core operand layouts
 struct pcb_smallco_layout { int ktap, koff[2], cout64; long long kf, kd; };
 bool pcb_smallco_eligible(const pcb_conv *c);
