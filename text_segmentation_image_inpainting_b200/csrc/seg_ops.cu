@@ -439,11 +439,12 @@ PCB_API int pcb_scse_forward(const void *x, const float *cse, const float *ws, v
 
 PCB_API int pcb_scse_backward(const void *gy, const void *x, const float *cse, const float *ws, const float *sse, void *dx, float *dcse,
                               float *dws, int dtype, int n, long long hw, int c, pcb_stream_t stream) {
-    PCB_CHECK(gy && x && cse && ws && sse && dx && dcse && dws && c % 8 == 0 && c <= 4096, "pcb_scse_backward: bad arguments");
+    // checked before the memsets: a refused call leaves dcse and dws untouched
+    PCB_CHECK(gy && x && cse && ws && sse && dx && dcse && dws && c % 8 == 0 && c <= 8 * 32 * SCSE_VM_MAX,
+              "pcb_scse_backward: bad arguments (channels a multiple of 8, at most %d)", 8 * 32 * SCSE_VM_MAX);
     const long long npix = static_cast<long long>(n) * hw;
     PCB_CUDA(cudaMemsetAsync(dcse, 0, sizeof(float) * n * c, ST));
     PCB_CUDA(cudaMemsetAsync(dws, 0, sizeof(float) * c, ST));
-    PCB_CHECK(c <= 8 * 32 * SCSE_VM_MAX, "scSE backward: at most %d channels", 8 * 32 * SCSE_VM_MAX);
     const int gw = scse_group_width(c);
     // blocks per sample: ~2048 lane-slots of work per block, at most ~4 blocks per SM in total
     const long long want = std::max<long long>(1, (hw * gw + 2047) / 2048), cap = std::max<long long>(1, 4ll * pcb_num_sms() / n);
