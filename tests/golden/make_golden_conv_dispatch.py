@@ -6,14 +6,16 @@
        * the eager eval forward of XceptionTextSegment at 600^2 b1 (non-power-of-two grids: the gather kernels),
        * one forward + backward of InpaintingLoss at 512^2 b8: the VGG16 forward over 3n = 24 images, its data gradient over
          the 16 images the loss differentiates, and the 1x1 problem of conv1_1's data gradient,
-       * the cases of tests/gpu_cases.py, test_gpu_fwd_tiles.py and test_gpu_wgrad_tiles.py:
+       * the cases of tests/gpu_cases.py and the tile cases of test_gpu_conv_routes.py (TILE_CASES):
          python tests/golden/make_golden_conv_dispatch.py --record descriptors.json
   2. on any machine, evaluate every host query of the library on them and write the fixture:
          python tests/golden/make_golden_conv_dispatch.py descriptors.json
 
 The queries depend on the SM count; without a visible device the library assumes 132 (H100 SXM), which is what the fixture
 holds.  Step 2 was run with the library of the commit before the dispatch was gathered into one plan per problem, so the
-test pins that the refactor kept every choice."""
+test pins that the refactor kept every choice.  One descriptor came later: the tile case two_parts_one_upsampled moved from
+batch 1 to batch 6 (where it reaches the sub-pixel data gradient), and its batch-1 descriptor, which no other run records,
+was replaced by the batch-6 one with its host queries evaluated by the library of that change."""
 import json
 import os
 import sys
@@ -31,17 +33,17 @@ def describe(c):
     return d
 
 
-def _tile_case_descs(cases, with_mode):
+def _tile_case_descs(cases):
     from text_segmentation_image_inpainting_b200 import _lib
     out = []
-    for name, case in cases.items():
+    for case in cases.values():
         n, h, w, parts, cout, k, s, d = case[:8]
         pad = d * (k - 1) // 2
         c = _lib.Conv()
         c.n, c.h, c.w, c.cin, c.cout, c.kh, c.kw = n, h, w, sum(p[0] for p in parts), cout, k, k
         c.stride, c.pad_h, c.pad_w, c.dil, c.groups = s, pad, pad, d, 1
         c.ho, c.wo = (h + 2 * pad - d * (k - 1) - 1) // s + 1, (w + 2 * pad - d * (k - 1) - 1) // s + 1
-        c.dtype, c.nparts, c.no_guard = _lib.PCB_BF16, len(parts), int(with_mode and case[8] == "no_guard")
+        c.dtype, c.nparts, c.no_guard = _lib.PCB_BF16, len(parts), int(case[8:] == ("no_guard",))
         for i, (ch, up, masked) in enumerate(parts):
             c.parts[i].c, c.parts[i].x_cstride, c.parts[i].x_up, c.parts[i].mask_up = ch, ch, up, up
             c.parts[i].mask = 1 if masked else None
@@ -53,8 +55,7 @@ def record(path):
     import torch
 
     import gpu_cases as G
-    import test_gpu_fwd_tiles
-    import test_gpu_wgrad_tiles
+    from test_gpu_conv_routes import TILE_CASES
     from oracle.detfill import det_fill_state_dict, det_tensor
     from oracle.inpaint_loss import vgg_state_dict
     from text_segmentation_image_inpainting_b200 import ops
@@ -106,7 +107,7 @@ def record(path):
         G.lazycat_case(tag, dev)
     torch.cuda.synchronize()
     ops.ConvGeom.struct = struct
-    descs = rec + _tile_case_descs(test_gpu_fwd_tiles.CASES, True) + _tile_case_descs(test_gpu_wgrad_tiles.CASES, False)
+    descs = rec + _tile_case_descs(TILE_CASES)
     uniq = {json.dumps(d, sort_keys=True): d for d in descs}
     with open(path, "w") as f:
         json.dump(sorted(uniq.values(), key=lambda d: json.dumps(d, sort_keys=True)), f)

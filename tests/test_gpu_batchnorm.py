@@ -9,7 +9,7 @@ computed on the device.  Cases:
     rpb * 16, a c = 8 tensor of 2^24 rows (about 166 grid-stride sweeps per thread), the one-launch small backward at 1, 1023,
     1025, 16384 and 2^20 rows, every activation with and without a residual, and ill-conditioned channels.
 
-Routes (kernel names asserted from one complete torch.profiler trace per case, see _traced):
+Routes (kernel names asserted from one complete torch.profiler trace per case, see kernel_harness.traced):
     vector  (c % 8 == 0, c <= 2048)  bn_stats_kernel, bn_fwd_fused_kernel, bn_finalize_kernel, bn_act_fwd_kernel,
                                      bn_bwd_reduce_kernel, bn_bwd_apply_kernel               every case with such c
     small   (vector, rows <= 2^20)   bn_bwd_small_kernel                                    every vector case of <= 2^20 rows
@@ -54,21 +54,14 @@ Gaussian regime (fp32 storage, the forward's own coefficients).  Higham (Accurac
 Ill-conditioned channels (mean >= 64 x spread, the "spread below one bf16 ulp of its mean" case) run through the same bounds:
 E[x^2] - m^2 from fp32 partials loses about (L + 2) u m^2 / var of relative variance, which dv carries.
 """
-import ctypes
-import json
 import math
-import os
-import re
-import time
-import warnings
 
 import pytest
 import torch
-from torch.profiler import ProfilerActivity, profile
 
+from kernel_harness import act_ref, assert_bitwise, assert_within, elementwise_sites, nan, traced
 from text_segmentation_image_inpainting_b200 import _lib
 
-FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "elementwise_sites.json")
 MAX_ELEMS = 1 << 27
 SMALL_MAX = 1 << 20               # the row limit of pcb_bn_act_backward_small
 U = 2.0 ** -24
@@ -77,10 +70,6 @@ EPS_F, MOM_F = (float(torch.tensor(v, dtype=torch.float32)) for v in (EPS, MOM))
 SLOPE_INT, SLOPE = 0.25, 0.2      # LeakyReLU slope: dyadic in the integer regime, the networks' 0.2 in the Gaussian one
 ACTS = (_lib.ACT_NONE, _lib.ACT_RELU, _lib.ACT_LEAKY, _lib.ACT_RELU6)
 DTYPES = {_lib.PCB_BF16: ("bf16", torch.bfloat16), _lib.PCB_F32: ("f32", torch.float32)}
-KERNEL_NAME = re.compile(r"(?<![A-Za-z_])(bn_\w*?_kernel)")
-PROFILER_PAD_S = 0.05             # idle margins: the profiler drops device activity at the edges of its window
-PROFILER_TRIES = 20               # traces taken at most per case (see _traced)
-MARKER, MARKER_CYCLES = "spin_kernel", 1000   # torch.cuda._sleep's kernel brackets every trace
 VEC_KERNELS = {"bn_stats_kernel", "bn_fwd_fused_kernel", "bn_finalize_kernel", "bn_act_fwd_kernel", "bn_bwd_reduce_kernel",
                "bn_bwd_apply_kernel"}
 SCALAR_KERNELS = {"bn_stats_scalar_kernel", "bn_finalize_kernel", "bn_act_fwd_scalar_kernel", "bn_bwd_reduce_scalar_kernel",
@@ -100,13 +89,8 @@ def _site_case(site):
     return name, _spec(dt, max(2, min(count, MAX_ELEMS // c)), c, act, res)
 
 
-def _load_sites():
-    with open(FIXTURE) as f:
-        return json.load(f)
-
-
 def _fixture_cases():
-    return dict(_site_case(s) for s in _load_sites() if s["fn"].startswith("pcb_bn_"))
+    return dict(_site_case(s) for s in elementwise_sites() if s["fn"].startswith("pcb_bn_"))
 
 
 BF, F32 = _lib.PCB_BF16, _lib.PCB_F32
@@ -131,7 +115,7 @@ def _cases():
 
 def test_fixture_sites_map_to_cases():
     """every BatchNorm site of the fixture names exactly one case, and every case name is distinct from the hand cases"""
-    sites = [s for s in _load_sites() if s["fn"].startswith("pcb_bn_")]
+    sites = [s for s in elementwise_sites() if s["fn"].startswith("pcb_bn_")]
     assert sites, "the fixture holds no BatchNorm site"
     names = [_site_case(s)[0] for s in sites]
     assert all(n.startswith("fx_") for n in names) and not set(names) & set(HAND_CASES)
@@ -163,16 +147,6 @@ def _rows_per_block(count, c, per_thread_rows):
     return rpb * math.ceil(count / (grid * rpb))
 
 
-def _act(z, act, slope):
-    if act == _lib.ACT_RELU:
-        return torch.where(z > 0, z, torch.zeros_like(z))
-    if act == _lib.ACT_LEAKY:
-        return torch.where(z > 0, z, z * torch.tensor(slope, dtype=torch.float32, device=z.device).to(z.dtype))
-    if act == _lib.ACT_RELU6:
-        return z.clamp(0, 6)
-    return z
-
-
 def _act_grad(z, act, slope):
     one = torch.ones_like(z)
     if act == _lib.ACT_RELU:
@@ -184,71 +158,8 @@ def _act_grad(z, act, slope):
     return one
 
 
-def _assert_bitwise(name, got, want):
-    ok = got == want
-    if not bool(ok.all()):
-        bad = (~ok).nonzero()[0].tolist()
-        raise AssertionError(f"{name}: {int((~ok).sum())} of {ok.numel()} elements differ from the exact result; first at {bad}: "
-                             f"got {float(got[tuple(bad)])}, want {float(want[tuple(bad)])}")
-
-
-def _assert_either(name, got, a, b):
-    ok = (got == a) | (got == b)
-    if not bool(ok.all()):
-        bad = (~ok).nonzero()[0].tolist()
-        raise AssertionError(f"{name}: {int((~ok).sum())} of {ok.numel()} elements match neither rounding; first at {bad}: "
-                             f"got {float(got[tuple(bad)])}, want {float(a[tuple(bad)])} or {float(b[tuple(bad)])}")
-
-
-def _assert_within(name, got, ref, bound):
-    got = got.double()
-    assert bool(torch.isfinite(got).all()), f"{name}: output left unwritten or not finite"
-    excess = (got - ref).abs() - bound
-    worst = int(excess.argmax())
-    assert float(excess.max()) <= 0.0, (f"{name}: |err| exceeds the bound at flat index {worst}: err "
-                                        f"{float((got - ref).abs().flatten()[worst]):.3e}, bound {float(bound.flatten()[worst]):.3e}")
-
-
-def _traced(name, fn, want, state):
-    """Run fn inside a torch.profiler trace and assert that the kernels it launched are exactly `want`.  The profiler loses
-    device activity records now and then (whole traces come back empty, even of several kernels and after an idle margin),
-    so every trace is bracketed by two marker kernels, the second after a synchronisation, and a trace in which either
-    marker is missing is not evidence either way.  Such a trace, or one whose kernels differ from `want`, is taken again, up
-    to PROFILER_TRIES times, from the same state: `state` lists (tensor, initial value) pairs reset before each attempt
-    (outputs back to NaN, accumulators and running statistics back to their operands), so the last attempt is the one the
-    checks read.  The route is a host-side decision on the arguments alone: a wrong route repeats on every complete trace
-    and still fails.  Losses come in stretches of seconds, so a case may see no complete trace at all: it then warns that
-    its route went unchecked (other cases of the same route still check it) and keeps every value check."""
-    last = None
-    for _ in range(PROFILER_TRIES):
-        for t, v in state:
-            t.copy_(v) if isinstance(v, torch.Tensor) else t.fill_(v)
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            time.sleep(PROFILER_PAD_S)
-            torch.cuda._sleep(MARKER_CYCLES)
-            fn()
-            torch.cuda.synchronize()
-            torch.cuda._sleep(MARKER_CYCLES)
-            torch.cuda.synchronize()
-            time.sleep(PROFILER_PAD_S)
-        ev = prof.events()
-        if sum(MARKER in e.name for e in ev) == 2:
-            last = {m.group(1) for e in ev for m in [KERNEL_NAME.search(e.name)] if m}
-            if last == want:
-                return
-    if last is None:       # no complete trace: the route cannot be judged, the value checks that follow still run
-        warnings.warn(f"{name}: the profiler recorded no complete trace in {PROFILER_TRIES} attempts; route not checked")
-        return
-    assert last == want, f"{name}: ran {sorted(last)}, the case covers {sorted(want)}"
-
-
 def _p(t):
     return None if t is None else t.data_ptr()
-
-
-def _nan(*shape, dtype=torch.float32):
-    return torch.full(shape, float("nan"), dtype=dtype, device="cuda")
 
 
 def _fl(x):
@@ -261,7 +172,7 @@ def _fwd_candidates(x64, sc, sh, act, slope, res):
     x32 = x64.float()
     outs = []
     for z in ((x32 * sc.float()) + sh.float(), (x64 * sc.double() + sh.double()).float()):
-        z = _act(z, act, slope)
+        z = act_ref(z, act, slope, f32_slope=True)
         if res is not None:
             z = z + res.float()
         outs.append(z)
@@ -288,7 +199,7 @@ def _coef_ref(S, Q, dS, dQ, count, g, b):
 def _check_coef(name, R, mean, invstd, scale, shift):
     for tag, got, ref, bd in (("mean", mean, R["m"], R["dm"]), ("invstd", invstd, R["inv"], R["d_inv"]),
                               ("scale", scale, R["sc"], R["d_sc"]), ("shift", shift, R["sh"], R["d_sh"])):
-        _assert_within(f"{name}: {tag}", got, ref, bd)
+        assert_within(f"{name}: {tag}", got, ref, bd)
 
 
 def _check_running(name, R, rm0, rv0, rm, rv, count):
@@ -297,8 +208,8 @@ def _check_running(name, R, rm0, rv0, rm, rv, count):
     d_unb = (R["dv"] + 2 * U * R["var"]) * (count / (count - 1) if count > 1 else 1) + 3 * U * unb
     rm_ref = (1 - MOM) * rm0.double() + MOM * R["m"]
     rv_ref = (1 - MOM) * rv0.double() + MOM * unb
-    _assert_within(f"{name}: running mean", rm, rm_ref, MOM * R["dm"] + 3 * U * ((1 - MOM) * rm0.double().abs() + MOM * R["m"].abs()) + 1e-7 * MOM * R["m"].abs())
-    _assert_within(f"{name}: running var", rv, rv_ref, MOM * d_unb + 3 * U * ((1 - MOM) * rv0.double().abs() + MOM * unb) + 1e-7 * MOM * unb)
+    assert_within(f"{name}: running mean", rm, rm_ref, MOM * R["dm"] + 3 * U * ((1 - MOM) * rm0.double().abs() + MOM * R["m"].abs()) + 1e-7 * MOM * R["m"].abs())
+    assert_within(f"{name}: running var", rv, rv_ref, MOM * d_unb + 3 * U * ((1 - MOM) * rv0.double().abs() + MOM * unb) + 1e-7 * MOM * unb)
 
 
 # ------------------------------------------------------------------------------------------------ the test
@@ -347,23 +258,23 @@ def test_batchnorm_vs_fp64(name):
     msum = torch.randint(0, 10, (count,), generator=gen, device=dev).float()           # 0 = hole; 3, 5, 6, 7, 9: not 2^k
     coef_b = torch.stack([bsc, bsh, bmu, binv]).contiguous()
 
-    sum_a, sq_a = _nan(c, dtype=torch.float64), _nan(c, dtype=torch.float64)
-    sums_al = _nan(2, c, dtype=torch.float64)
+    sum_a, sq_a = nan(c, dtype=torch.float64), nan(c, dtype=torch.float64)
+    sums_al = nan(2, c, dtype=torch.float64)
     acc0 = ints(2, c, lo=-1000, hi=1000)
     sums_acc = acc0.clone()
-    y_fused, coef = _nan(count, c, dtype=dt), _nan(4, c)
+    y_fused, coef = nan(count, c, dtype=dt), nan(4, c)
     rm_f, rv_f, nbt_f = rm0.clone(), rv0.clone(), torch.tensor([5], dtype=torch.int64, device=dev)
-    scale_t, shift_t, mean_t, inv_t = _nan(c), _nan(c), _nan(c), _nan(c)
+    scale_t, shift_t, mean_t, inv_t = nan(c), nan(c), nan(c), nan(c)
     rm_t, rv_t, nbt_t = rm0.clone(), rv0.clone(), torch.tensor([7], dtype=torch.int64, device=dev)
-    y_t = _nan(count, c, dtype=dt)
-    scale_e, shift_e = _nan(c), _nan(c)
-    y_e, y_a = _nan(count, c, dtype=dt), _nan(count, c, dtype=dt)
-    sg_a, sgx_a, red_al = _nan(c, dtype=torch.float64), _nan(c, dtype=torch.float64), _nan(2, c, dtype=torch.float64)
+    y_t = nan(count, c, dtype=dt)
+    scale_e, shift_e = nan(c), nan(c)
+    y_e, y_a = nan(count, c, dtype=dt), nan(count, c, dtype=dt)
+    sg_a, sgx_a, red_al = nan(c, dtype=torch.float64), nan(c, dtype=torch.float64), nan(2, c, dtype=torch.float64)
     red_acc = acc0.clone()
     exact = torch.stack([SG, SGX])
-    dx_t, dx_r, dx_e, dx_a = (_nan(count, c, dtype=dt) for _ in range(4))
-    dg_t, db_t, dg_r, db_r = _nan(c), _nan(c), _nan(c), _nan(c)
-    dx_s, dx_sm, dg_s, db_s, dg_sm, db_sm = _nan(count, c, dtype=dt), _nan(count, c, dtype=dt), _nan(c), _nan(c), _nan(c), _nan(c)
+    dx_t, dx_r, dx_e, dx_a = (nan(count, c, dtype=dt) for _ in range(4))
+    dg_t, db_t, dg_r, db_r = nan(c), nan(c), nan(c), nan(c)
+    dx_s, dx_sm, dg_s, db_s, dg_sm, db_sm = nan(count, c, dtype=dt), nan(count, c, dtype=dt), nan(c), nan(c), nan(c), nan(c)
     exact_sums = torch.stack([S, Q]).contiguous()
     bargs = (bsc.data_ptr(), bsh.data_ptr(), bmu.data_ptr(), binv.data_ptr(), act, SLOPE_INT)
     ex = exact.contiguous()
@@ -413,13 +324,17 @@ def test_batchnorm_vs_fp64(name):
                                                      msum.data_ptr(), dx_sm.data_ptr(), dg_sm.data_ptr(), db_sm.data_ptr(), st))
 
     want = (VEC_KERNELS | ({"bn_bwd_small_kernel"} if small else set())) if vec else SCALAR_KERNELS
-    _traced(name, run, want, state)
+
+    def check(records):
+        ran = {k for k, _ in records if k.startswith("bn_")}
+        assert ran == want, f"{name}: ran {sorted(ran)}, the case covers {sorted(want)}"
+    traced(name, run, check, state)
 
     # statistics: exact
     for tag, a, b in (("separate", sum_a, sq_a), ("aliased", sums_al[0], sums_al[1])):
-        _assert_bitwise(f"{name}: sum ({tag})", a, S)
-        _assert_bitwise(f"{name}: sum of squares ({tag})", b, Q)
-    _assert_bitwise(f"{name}: accumulated sums", sums_acc, acc0 + torch.stack([S, Q]))
+        assert_bitwise(f"{name}: sum ({tag})", a, S)
+        assert_bitwise(f"{name}: sum of squares ({tag})", b, Q)
+    assert_bitwise(f"{name}: accumulated sums", sums_acc, acc0 + torch.stack([S, Q]))
 
     # forward: coefficients within the bounds, y exact given them
     R = _coef_ref(S, Q, 0 * S, 0 * Q, count, gamma.double(), beta.double())
@@ -427,25 +342,25 @@ def test_batchnorm_vs_fp64(name):
         _check_coef(f"{name}: fused forward", R, coef[2], coef[3], coef[0], coef[1])
         _check_running(f"{name}: fused forward", R, rm0, rv0, rm_f, rv_f, count)
         assert int(nbt_f) == 6, f"{name}: num_batches_tracked must grow by exactly 1 per call, got {int(nbt_f) - 5}"
-        _assert_either(f"{name}: fused forward y", y_fused, *(v.to(dt) for v in _fwd_candidates(x64, coef[0], coef[1], act, SLOPE_INT, res)))
+        assert_bitwise(f"{name}: fused forward y", y_fused, *(v.to(dt) for v in _fwd_candidates(x64, coef[0], coef[1], act, SLOPE_INT, res)))
     _check_coef(f"{name}: finalize", R, mean_t, inv_t, scale_t, shift_t)
     _check_running(f"{name}: finalize", R, rm0, rv0, rm_t, rv_t, count)
     assert int(nbt_t) == 8, f"{name}: pcb_bn_finalize must bump num_batches_tracked by 1"
-    _assert_either(f"{name}: finalize + apply y", y_t, *(v.to(dt) for v in _fwd_candidates(x64, scale_t, shift_t, act, SLOPE_INT, res)))
+    assert_bitwise(f"{name}: finalize + apply y", y_t, *(v.to(dt) for v in _fwd_candidates(x64, scale_t, shift_t, act, SLOPE_INT, res)))
     inv_e = 1 / torch.sqrt(rv0.double() + EPS)
-    _assert_within(f"{name}: eval scale", scale_e, gamma.double() * inv_e, (gamma.double() * inv_e).abs() * 4 * U)
-    _assert_within(f"{name}: eval shift", shift_e, beta.double() - rm0.double() * gamma.double() * inv_e,
+    assert_within(f"{name}: eval scale", scale_e, gamma.double() * inv_e, (gamma.double() * inv_e).abs() * 4 * U)
+    assert_within(f"{name}: eval shift", shift_e, beta.double() - rm0.double() * gamma.double() * inv_e,
                    (rm0.double() * gamma.double() * inv_e).abs() * 6 * U + U * beta.double().abs() * 2)
-    _assert_either(f"{name}: eval forward y", y_e, *(v.to(dt) for v in _fwd_candidates(x64, scale_e, shift_e, act, SLOPE_INT, res)))
-    ya = _act(x64.float(), act, SLOPE_INT) + (res.float() if res is not None else 0)
-    _assert_bitwise(f"{name}: activation-only forward y", y_a, ya.to(dt))
+    assert_bitwise(f"{name}: eval forward y", y_e, *(v.to(dt) for v in _fwd_candidates(x64, scale_e, shift_e, act, SLOPE_INT, res)))
+    ya = act_ref(x64.float(), act, SLOPE_INT, f32_slope=True) + (res.float() if res is not None else 0)
+    assert_bitwise(f"{name}: activation-only forward y", y_a, ya.to(dt))
 
     # backward: exact
     for tag, a, b in (("separate", sg_a, sgx_a), ("aliased", red_al[0], red_al[1])):
-        _assert_bitwise(f"{name}: sum gz ({tag})", a, SG)
-        _assert_bitwise(f"{name}: sum gz xhat ({tag})", b, SGX)
+        assert_bitwise(f"{name}: sum gz ({tag})", a, SG)
+        assert_bitwise(f"{name}: sum gz xhat ({tag})", b, SGX)
     if vec:
-        _assert_bitwise(f"{name}: accumulated backward sums", red_acc, acc0 + exact)
+        assert_bitwise(f"{name}: accumulated backward sums", red_acc, acc0 + exact)
     inv_n = torch.tensor(1.0, dtype=torch.float32, device=dev) / torch.tensor(float(count), dtype=torch.float32, device=dev)
     sc32, mu64 = bsc, bmu.double()
     B = ((-sc32 * binv) * SGX.float()) * inv_n
@@ -455,11 +370,11 @@ def test_batchnorm_vs_fp64(name):
     rs = torch.where(msum == 0, torch.zeros_like(msum), (1 / msum.double()).float())
     d_r = d * rs[:, None]
     if vec:
-        _assert_bitwise(f"{name}: apply dx", dx_t, d.to(dt))
-        _assert_bitwise(f"{name}: apply_renorm dx", dx_r, d_r.to(dt))
+        assert_bitwise(f"{name}: apply dx", dx_t, d.to(dt))
+        assert_bitwise(f"{name}: apply_renorm dx", dx_r, d_r.to(dt))
         for tag, dg, db in (("apply", dg_t, db_t), ("apply_renorm", dg_r, db_r)):
-            _assert_bitwise(f"{name}: {tag} dgamma", dg, SGX.float())
-            _assert_bitwise(f"{name}: {tag} dbeta", db, SG.float())
+            assert_bitwise(f"{name}: {tag} dgamma", dg, SGX.float())
+            assert_bitwise(f"{name}: {tag} dbeta", db, SG.float())
     else:
         # sc * ((gz - sg * ic) - (xhat * sgx) * ic): either subtraction may be contracted with its product
         xhat = (x64 - mu64) * binv.double()
@@ -469,24 +384,24 @@ def test_batchnorm_vs_fp64(name):
                 for t1 in (_fl(gz - _fl(p1)), _fl(gz - p1)) for t2 in (_fl(t1 - _fl(q * ic)), _fl(t1 - q * ic))]
         ok = (dx_t == outs[0]) | (dx_t == outs[1]) | (dx_t == outs[2]) | (dx_t == outs[3])
         assert bool(ok.all()), f"{name}: scalar apply dx: {int((~ok).sum())} elements match none of the four roundings"
-        _assert_bitwise(f"{name}: dgamma", dg_t, SGX.float())
-        _assert_bitwise(f"{name}: dbeta", db_t, SG.float())
+        assert_bitwise(f"{name}: dgamma", dg_t, SGX.float())
+        assert_bitwise(f"{name}: dbeta", db_t, SG.float())
         assert bool(dx_r.isnan().all()) and bool(dg_r.isnan().all()), f"{name}: apply_renorm must not run on this route"
-    _assert_bitwise(f"{name}: eval apply dx", dx_e, (sc32.double() * gz).float().to(dt))
-    _assert_bitwise(f"{name}: activation-only apply dx", dx_a, (g64 * _act_grad(x64, act, SLOPE_INT)).float().to(dt))
+    assert_bitwise(f"{name}: eval apply dx", dx_e, (sc32.double() * gz).float().to(dt))
+    assert_bitwise(f"{name}: activation-only apply dx", dx_a, (g64 * _act_grad(x64, act, SLOPE_INT)).float().to(dt))
     if small:
-        _assert_bitwise(f"{name}: small dx", dx_s, d.to(dt))
-        _assert_bitwise(f"{name}: small dx (renorm)", dx_sm, d_r.to(dt))
+        assert_bitwise(f"{name}: small dx", dx_s, d.to(dt))
+        assert_bitwise(f"{name}: small dx (renorm)", dx_sm, d_r.to(dt))
         for tag, dg, db in (("small", dg_s, db_s), ("small renorm", dg_sm, db_sm)):
-            _assert_bitwise(f"{name}: {tag} dgamma", dg, SGX.float())
-            _assert_bitwise(f"{name}: {tag} dbeta", db, SG.float())
+            assert_bitwise(f"{name}: {tag} dgamma", dg, SGX.float())
+            assert_bitwise(f"{name}: {tag} dbeta", db, SG.float())
 
     # refusals on the scalar route: nothing launched, nothing written
     if not vec:
         before = _lib.launch_count()
-        y0, cf0, nb0 = _nan(count, c, dtype=dt), _nan(4, c), torch.tensor([5], dtype=torch.int64, device=dev)
+        y0, cf0, nb0 = nan(count, c, dtype=dt), nan(4, c), torch.tensor([5], dtype=torch.int64, device=dev)
         rm1, rv1, s0 = rm0.clone(), rv0.clone(), acc0.clone()
-        dx0 = _nan(count, c, dtype=dt)
+        dx0 = nan(count, c, dtype=dt)
         assert lib.pcb_bn_forward_fused(x.data_ptr(), dcode, count, c, exact_sums.data_ptr(), gamma.data_ptr(), beta.data_ptr(),
                                         rm1.data_ptr(), rv1.data_ptr(), nb0.data_ptr(), MOM, EPS, act, SLOPE_INT, None, y0.data_ptr(),
                                         cf0.data_ptr(), st) != 0
@@ -509,11 +424,11 @@ def test_batchnorm_vs_fp64(name):
     ax = xg64.abs()
     Sg, Qg = xg64.sum(0), (xg64 * xg64).sum(0)
     dS, dQ = (L + 1) * U * ax.sum(0), (L + 2) * U * (ax * ax).sum(0)
-    sums = _nan(2, c, dtype=torch.float64)
+    sums = nan(2, c, dtype=torch.float64)
     _lib.check(lib.pcb_bn_stats(xg.data_ptr(), F32, count, c, sums[0].data_ptr(), sums[1].data_ptr(), st))
     torch.cuda.synchronize()
-    _assert_within(f"{name}: Gaussian sum", sums[0], Sg, dS)
-    _assert_within(f"{name}: Gaussian sum of squares", sums[1], Qg, dQ)
+    assert_within(f"{name}: Gaussian sum", sums[0], Sg, dS)
+    assert_within(f"{name}: Gaussian sum of squares", sums[1], Qg, dQ)
     # the two-pass reference of mean and variance
     m2 = Sg / count
     var2 = ((xg64 - m2) ** 2).sum(0) / count
@@ -521,7 +436,7 @@ def test_batchnorm_vs_fp64(name):
     Rg["var"] = var2
     if not vec:
         return
-    y, cf = _nan(count, c), _nan(4, c)
+    y, cf = nan(count, c), nan(4, c)
     rm_g, rv_g, nb_g = rm0.clone(), rv0.clone(), torch.tensor([0], dtype=torch.int64, device=dev)
     _lib.check(lib.pcb_bn_forward_fused(xg.data_ptr(), F32, count, c, sums.data_ptr(), gamma.data_ptr(), beta.data_ptr(), rm_g.data_ptr(),
                                         rv_g.data_ptr(), nb_g.data_ptr(), MOM, EPS, act, SLOPE, _p(rg), y.data_ptr(), cf.data_ptr(), st))
@@ -531,8 +446,8 @@ def test_batchnorm_vs_fp64(name):
     assert int(nb_g) == 1
     sc, sh, mu, iv = (cf[i].double() for i in range(4))
     zg = xg64 * sc + sh
-    yref = _act(zg, act, SLOPE) + (rg.double() if rg is not None else 0)
-    _assert_within(f"{name}: Gaussian y", y, yref, 2 * U * ((xg64 * sc).abs() + sh.abs()) + U * yref.abs() * 2)
+    yref = act_ref(zg, act, SLOPE, f32_slope=True) + (rg.double() if rg is not None else 0)
+    assert_within(f"{name}: Gaussian y", y, yref, 2 * U * ((xg64 * sc).abs() + sh.abs()) + U * yref.abs() * 2)
     if sp["illcond"]:                    # for comparison: torch's own (Welford) statistics kernel on the same fp32 input
         ref_inv = 1 / torch.sqrt(var2 + EPS)
         err = float(((cf[3].double() - ref_inv) / ref_inv).abs().max())
@@ -552,18 +467,18 @@ def test_batchnorm_vs_fp64(name):
     Lb = _chain(count, c, 16)
     dSG = (Lb + 1) * U * gzg.abs().sum(0) + (gg64.abs() * kink).sum(0)
     dSGX = (Lb + 4) * U * (gzg * xm * iv).abs().sum(0) + (gg64.abs() * kink * xm.abs() * iv).sum(0)
-    rsum = _nan(2, c, dtype=torch.float64)
+    rsum = nan(2, c, dtype=torch.float64)
     _lib.check(lib.pcb_bn_act_backward_reduce(gg.data_ptr(), xg.data_ptr(), F32, count, c, cf[0].data_ptr(), cf[1].data_ptr(),
                                               cf[2].data_ptr(), cf[3].data_ptr(), act, SLOPE, rsum[0].data_ptr(), rsum[1].data_ptr(), st))
-    dxg, dgg, dbg = _nan(count, c), _nan(c), _nan(c)
+    dxg, dgg, dbg = nan(count, c), nan(c), nan(c)
     _lib.check(lib.pcb_bn_act_backward_apply_renorm(gg.data_ptr(), xg.data_ptr(), F32, count, c, cf[0].data_ptr(), cf[1].data_ptr(),
                                                     cf[2].data_ptr(), cf[3].data_ptr(), act, SLOPE, rsum[0].data_ptr(), rsum[1].data_ptr(),
                                                     1, msum.data_ptr(), dxg.data_ptr(), dgg.data_ptr(), dbg.data_ptr(), st))
     torch.cuda.synchronize()
-    _assert_within(f"{name}: Gaussian sum gz", rsum[0], SGg, dSG)
-    _assert_within(f"{name}: Gaussian sum gz xhat", rsum[1], SGXg, dSGX)
-    _assert_within(f"{name}: Gaussian dbeta", dbg, SGg, dSG + U * SGg.abs())
-    _assert_within(f"{name}: Gaussian dgamma", dgg, SGXg, dSGX + U * SGXg.abs())
+    assert_within(f"{name}: Gaussian sum gz", rsum[0], SGg, dSG)
+    assert_within(f"{name}: Gaussian sum gz xhat", rsum[1], SGXg, dSGX)
+    assert_within(f"{name}: Gaussian dbeta", dbg, SGg, dSG + U * SGg.abs())
+    assert_within(f"{name}: Gaussian dgamma", dgg, SGXg, dSGX + U * SGXg.abs())
     Bg, Cg = -sc * iv * SGXg / count, -sc * SGg / count
     dB = (sc * iv / count).abs() * (dSGX + 4 * U * SGXg.abs())
     dC = (sc / count).abs() * (dSG + 3 * U * SGg.abs())
@@ -571,18 +486,18 @@ def test_batchnorm_vs_fp64(name):
     bd = xm.abs() * dB + dC + U * (xm.abs() * Bg.abs() + 2 * (Bg * xm + Cg).abs() + 2 * dref.abs()) + (sc * gg64).abs() * kink + 2 * U * (sc * gzg).abs()
     s64 = msum.double()[:, None]
     rsd = torch.where(s64 == 0, torch.zeros_like(s64), 1 / torch.where(s64 == 0, torch.ones_like(s64), s64))
-    _assert_within(f"{name}: Gaussian apply_renorm dx", dxg, dref * rsd, (bd + 2 * U * dref.abs()) * rsd)
+    assert_within(f"{name}: Gaussian apply_renorm dx", dxg, dref * rsd, (bd + 2 * U * dref.abs()) * rsd)
     if small:
-        dxs, dgg, dbg = _nan(count, c), _nan(c), _nan(c)
+        dxs, dgg, dbg = nan(count, c), nan(c), nan(c)
         _lib.check(lib.pcb_bn_act_backward_small(gg.data_ptr(), xg.data_ptr(), F32, count, c, cf.data_ptr(), act, SLOPE, None,
                                                  dxs.data_ptr(), dgg.data_ptr(), dbg.data_ptr(), st))
         torch.cuda.synchronize()
         Ls = math.ceil(count / 1024) + 5 + 32
         dSGs = (Ls + 1) * U * gzg.abs().sum(0) + (gg64.abs() * kink).sum(0)
         dSGXs = (Ls + 4) * U * (gzg * xm * iv).abs().sum(0) + (gg64.abs() * kink * xm.abs() * iv).sum(0)
-        _assert_within(f"{name}: Gaussian small dbeta", dbg, SGg, dSGs)
-        _assert_within(f"{name}: Gaussian small dgamma", dgg, SGXg, dSGXs)
+        assert_within(f"{name}: Gaussian small dbeta", dbg, SGg, dSGs)
+        assert_within(f"{name}: Gaussian small dgamma", dgg, SGXg, dSGXs)
         dBs = (sc * iv / count).abs() * (dSGXs + 4 * U * SGXg.abs())
         dCs = (sc / count).abs() * (dSGs + 3 * U * SGg.abs())
         bds = xm.abs() * dBs + dCs + U * (xm.abs() * Bg.abs() + 2 * (Bg * xm + Cg).abs() + 2 * dref.abs()) + (sc * gg64).abs() * kink + 2 * U * (sc * gzg).abs()
-        _assert_within(f"{name}: Gaussian small dx", dxs, dref, bds)
+        assert_within(f"{name}: Gaussian small dx", dxs, dref, bds)

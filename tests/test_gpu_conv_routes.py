@@ -3,7 +3,7 @@ computed on the device (F.conv2d / torch.nn.grad.conv2d_input / conv2d_weight, c
 sum), on every route the plan of a problem can take: the TMA-fed and cp.async-gather wgmma kernels (conv_tc.cu), the stride-2
 data gradient as four parity classes, the sub-pixel data gradient of a 2x-upsampled part, the space-to-depth stem
 (conv_stem.cu), the kernel-to-row RGB tail (conv_k2r.cu), the mma.sync small-Cout kernels (conv_smallco.cu) and the
-shape-general kernels (conv_generic.cu).  Two sets of cases:
+shape-general kernels (conv_generic.cu).  Three sets of cases:
 
   * one per dense descriptor of tests/golden/conv_dispatch.json (the layers the workloads run), batch capped at 2 -- or the
     smallest batch above that whose routes (pcb_debug_conv_routes) equal those of the uncapped descriptor;
@@ -11,12 +11,21 @@ shape-general kernels (conv_generic.cu).  Two sets of cases:
     a non-power-of-two grid, dilation; row-packed layers with cin 1 / 3 / 8 and kw 3 / 5 / 7; stems with holes, no_guard, cout
     32 / 40 and a grid that is not a whole number of tiles; RGB tails with 1 / 3 / 4 image channels, 32 / 64 upsampled channels
     and holes in both parts; small-Cout layers at 80 packed channels, ragged h and w, 1x1, an upsampled part; the stride-2 data
-    gradient with and without its four-stream fork; grouped, many-part, kh != kw and fp32 no_guard generic layers.
+    gradient with and without its four-stream fork; grouped, many-part, kh != kw and fp32 no_guard generic layers;
+  * tile cases (TILE_CASES, at their own batch), one per tile configuration of the TMA-fed kernels, each asserting the tiles it
+    is named for (TILE_KERNELS) from the template arguments of its kernels: 256-wide forward and data-gradient tiles and the
+    eval epilogue at 256; cout 320 and 384 on 64- and 128-wide forward tiles; the sub-pixel data gradient of a 2x-upsampled
+    part; row-halo forward and data-gradient tiles at dilation 48 (halo rows up to 224, past the fixers' third row at 192);
+    no_guard on the row-halo forward; the stride-2 data gradient as four parity classes.  Weight gradient: 128-wide
+    output-channel tiles with and without row-halo A blocks, ragged (cout 192, 320), an input-channel tile straddling two
+    parts, a 2x-upsampled part; one 64-channel input block shared by both consumer warpgroups at N = 128 (each takes 64 output
+    channels) and alone at N = 64 (the second warpgroup idles: DESIGN 4.1); 64-wide tiles for a short reduction (fewer than
+    8192 output pixels); row-halo A blocks taller than 128 rows (dilation 48).
 
-Each case asserts that the routes the query reports are the routes its kernels take: the kernel names of one torch.profiler
-trace of the forward, data gradient and both weight gradients are mapped back to a route per direction.  A row-packed layer
-has no data-gradient route (the query says none); its callers run that gradient on the generic kernels with force_generic and
-KRSC weights (ops.py), and so does this test.
+Each case asserts that the routes the query reports are the routes its kernels take: the kernel names of a torch.profiler
+trace of the forward, data gradient and both weight gradients (kernel_harness.traced) are mapped back to a route per
+direction.  A row-packed layer has no data-gradient route (the query says none); its callers run that gradient on the generic
+kernels with force_generic and KRSC weights (ops.py), and so does this test.
 
 Integer regime (every case, bit-exact).  x, w and dc are small integers (|x|, |w|, |dc| <= 4; <= 2 where noted below) and the bias a
 multiple of 1/8, all exact in bf16.  Each case asserts that every partial sum stays below 2^24 (max|x| max|w| times the number of
@@ -43,9 +52,14 @@ hold zeros in channels [cout, rup(cout, 8)) and may only zero the channels past 
 leave them bitwise equal to pcb_conv_weight_prepare(W2) -- including the extra operands the stem, the tail and the sub-pixel
 kernels keep behind the layer's own.
 
-Gaussian regime (every case, error bounds, as test_gpu_fwd_tiles.py).  Each of the n nonzero products of an element costs at most
-two fp32 roundings (bf16 products are exact), so the accumulation is off by at most n * 2^-22 * M, M = the sum of |products|
-(Higham, Accuracy and Stability of Numerical Algorithms, 4.2).  The renormalisation and the bias add two roundings (2^-22 of
+Gaussian regime (every case, error bounds).  Every product of two bf16 values is exact in fp32, so a kernel differs from the
+exact sum only in how it adds the products of an element: fp32 tensor-core accumulation, plus fp32 red.global.add of the
+split-K partials in the weight gradient, in an order the test does not know.  Adding an exact zero is exact, so only the n
+nonzero products count.  Any order of n - 1 additions with unit roundoff u is off by at most (n - 1) u / (1 - (n - 1) u) * M,
+M = the sum of |products| (Higham, Accuracy and Stability of Numerical Algorithms, 4.2).  The tensor cores' fp32 adder is
+not guaranteed to round to nearest, so u = 2^-23 (one ulp) instead of 2^-24, and 1 / (1 - (n - 1) u) < 2 here: the
+accumulation is off by at most n * 2^-22 * M (fp32 storage: each product and its add round once each, the same bound).
+The renormalisation and the bias add two roundings (2^-22 of
 |acc| / s and of the result), the eval epilogue's fma one (2^-23 of |z| + |shift|), LeakyReLU's multiply one (2^-23 of the
 result); activations are 1-Lipschitz; a bf16 store adds half an ulp (2^-8 relative is used).  Rounding an intermediate to bf16
 adds half an ulp of it, at most 2^-9 of the sum of the |products| it holds, bounded by 2^-8 M: the tail's Z (forward) and D
@@ -55,31 +69,22 @@ calls must be refused and write nothing.
 """
 import collections
 import ctypes
-import json
-import os
-import re
-import time
 
 import pytest
 import torch
 import torch.nn.functional as F
-from torch.autograd import DeviceType
 from torch.nn.grad import conv2d_input, conv2d_weight
-from torch.profiler import ProfilerActivity, profile
 
+from kernel_harness import (HOLE_VALUE, SENTINEL, act_ref, assert_bitwise, assert_within, conv_dispatch_cases, holes, nchw,
+                            sentinel_kept, strided, traced)
 from text_segmentation_image_inpainting_b200 import _lib
 
 pytestmark = pytest.mark.gpu
 
-FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "conv_dispatch.json")
-HOLE_VALUE = 1024.0          # x under the holes: a read that ignores the mask is far outside any bound (exact in bf16)
-SENTINEL = -8192.0           # channels past rup(c, 8) of a strided view: inputs must not be read there, outputs not written
 SLOPE = 0.2
 ACTS = (_lib.ACT_NONE, _lib.ACT_RELU, _lib.ACT_LEAKY, _lib.ACT_RELU6)
 DTYPES = {"bf16": (torch.bfloat16, _lib.PCB_BF16), "f32": (torch.float32, _lib.PCB_F32)}
 TC_ROUTES = {"stem", "k2r", "smallco", "tma", "tma_s2", "gather"}
-KERNEL_NAME = re.compile(r"(?<![A-Za-z0-9_])([a-z0-9_]+_kernel)(?:<([^<>]*)>)?")
-PROFILER_PAD_S = 0.05        # idle margins: the profiler drops device activity that falls outside its window
 
 
 def _rup8(v):
@@ -130,10 +135,8 @@ def _fixture_cases():
     """one case per distinct dense descriptor of the dispatch fixture, at the smallest batch >= min(n, 2) whose routes equal those
     of the uncapped descriptor"""
     lib = _lib.load()
-    with open(FIXTURE) as f:
-        fixture = json.load(f)["cases"]
     out = {}
-    for case in fixture:
+    for case in conv_dispatch_cases():
         d = case["conv"]
         if case["expect"]["routes"][0] == "depthwise":
             continue
@@ -202,42 +205,86 @@ HAND_CASES = {
     "generic_force_bf16_s2": _case(2, 26, 30, [P_(64, mask=True)], 64, 3, 2, force_generic=True, route=("generic",) * 3),
     "generic_f32_plain_d3_s2": _case(2, 25, 27, [P_(16)], 24, 3, 2, dil=3, dtype="f32", plain=True, route=("generic",) * 3),
 }
-CASES = {**_fixture_cases(), **HAND_CASES}
+
+# name: (n, h, w, parts [(channels, upsampled, masked)], cout, k, stride, dilation[, mode]), "same" padding; an upsampled part
+# is stored at (h/2, w/2) with its hole plane at that resolution; mode "no_guard": NaN at empty boxes (every case runs the
+# fused BatchNorm sums and the eval epilogue).  tests/golden/make_golden_conv_dispatch.py records these descriptors too.
+TILE_CASES = {
+    "n256_two_parts_1024_512": (8, 32, 32, [(512, 0, 1), (512, 0, 1)], 512, 3, 1, 1, "bn"),
+    "eval_affine_leaky_n256": (8, 32, 32, [(256, 0, 1)], 512, 3, 1, 1, "eval"),
+    "ragged_cout320": (2, 32, 64, [(128, 0, 1)], 320, 3, 1, 1, "bn"),
+    "ragged_cout384": (2, 32, 64, [(128, 0, 1)], 384, 3, 1, 1, "bn"),
+    # batch 6, not 1: the sub-pixel data gradient runs where the source grid has at least a third of a wave of 128-pixel tiles
+    # (44 on 132 SMs); at batches 1 to 5 (8 to 40 tiles) the plan keeps the regular kernel and pconv_tc_sp_kernel never launches
+    "two_parts_one_upsampled": (6, 64, 64, [(128, 1, 1), (64, 0, 1)], 64, 3, 1, 1, "bn"),
+    "holes_no_guard_nan": (2, 32, 128, [(128, 0, 1)], 128, 3, 1, 1, "no_guard"),
+    "s2_parity_dgrad_cin256": (2, 64, 64, [(256, 0, 1)], 512, 3, 2, 1, "bn"),
+    "halo_n64_d48_holes_over_large_x": (2, 64, 128, [(64, 0, 1)], 64, 3, 1, 48, "bn"),
+    "halo_n128_holes": (2, 32, 128, [(128, 0, 1)], 128, 3, 1, 1),
+    "decoder_upsampled_two_parts_n128": (1, 64, 128, [(128, 1, 1), (64, 0, 1)], 128, 3, 1, 1),
+    "enc1_like_k5_s2_64_128_split_n": (2, 128, 128, [(64, 0, 1)], 128, 5, 2, 1),
+    "k3_s2_256_512": (2, 128, 128, [(256, 0, 1)], 512, 3, 2, 1),
+    # the input-channel tile holding only the 64 skip channels is one 64-channel block: at N = 64 the second consumer warpgroup
+    # idles (DESIGN 4.1: splitting the K blocks between the warpgroups is not used)
+    "dec7_like_192_64_one_block_n64": (1, 16, 128, [(128, 1, 1), (64, 0, 1)], 64, 3, 1, 1),
+    "ragged_cout192_halo": (1, 64, 128, [(128, 0, 1)], 192, 3, 1, 1),
+    "ragged_cout320_split_n": (8, 32, 32, [(64, 0, 1)], 320, 3, 1, 1),
+    "ci_tile_straddles_parts": (1, 128, 64, [(64, 0, 1), (128, 0, 1)], 128, 3, 1, 1),
+    "short_reduction_n64_tiles": (2, 8, 64, [(256, 0, 1)], 256, 3, 1, 1),
+    "halo_d48_holes_over_large_x": (1, 64, 128, [(128, 0, 1)], 128, 3, 1, 48),
+}
+
+
+def _tma(bn, mode, halo):
+    return ("pconv_tc_tma_kernel", (str(bn), str(mode), str(halo).lower()))
+
+
+def _wg(bn, halo):
+    return ("pconv_tc_wgrad_tma_kernel", (str(bn), "3", str(halo).lower()))
+
+
+# the launches each tile case is named for, per trace (one forward, one data gradient, two weight gradients)
+TILE_KERNELS = {
+    "n256_two_parts_1024_512": {_tma(256, 0, False): 1, _tma(256, 1, False): 1},
+    "eval_affine_leaky_n256": {_tma(256, 0, False): 1},
+    "ragged_cout320": {_tma(64, 0, False): 1},
+    "ragged_cout384": {_tma(128, 0, False): 1},
+    # the upsampled part's gradient at source resolution, the other part's on the regular kernel
+    "two_parts_one_upsampled": {("pconv_tc_sp_kernel", ("64",)): 1, _tma(64, 1, False): 1},
+    "holes_no_guard_nan": {_tma(64, 0, True): 1},
+    "s2_parity_dgrad_cin256": {_tma(32, 1, False): 4},
+    "halo_n64_d48_holes_over_large_x": {_tma(64, 0, True): 1, _tma(64, 1, True): 1},
+    "halo_n128_holes": {_wg(128, True): 2},
+    "decoder_upsampled_two_parts_n128": {_wg(128, True): 2},
+    "enc1_like_k5_s2_64_128_split_n": {_wg(128, False): 2},
+    "k3_s2_256_512": {_wg(128, False): 2},
+    "dec7_like_192_64_one_block_n64": {_wg(64, True): 2},
+    "ragged_cout192_halo": {_wg(128, True): 2},
+    "ragged_cout320_split_n": {_wg(128, False): 2},
+    "ci_tile_straddles_parts": {_wg(128, True): 2},
+    "short_reduction_n64_tiles": {_wg(64, True): 2},
+    "halo_d48_holes_over_large_x": {_wg(128, True): 2},
+}
+
+
+def _tile_cases():
+    """every tile case covers the TMA-fed kernels: the stride-2 data gradient as parity classes"""
+    out = {}
+    for name, case in TILE_CASES.items():
+        n, h, w, parts, cout, k, s, d = case[:8]
+        sp = _case(n, h, w, [_part(c, up, masked) for c, up, masked in parts], cout, k, s, dil=d, no_guard=case[8:] == ("no_guard",),
+                   route=("tma", "tma_s2" if s == 2 else "tma", "tma"))
+        sp["tiles"] = TILE_KERNELS[name]
+        out["tile_" + name] = sp
+    return out
+
+
+CASES = {**_fixture_cases(), **HAND_CASES, **_tile_cases()}
 
 
 # ------------------------------------------------------------------------------------------------------------------------
-def _holes(n, h, w, gen):
-    """uint8 plane, 1 = valid: a rectangle per image plus scattered single pixels"""
-    m = (torch.rand(n, h, w, generator=gen) > 0.15).to(torch.uint8)
-    for i in range(n):
-        y0, x0 = int(torch.randint(0, max(1, h // 2), (1,), generator=gen)), int(torch.randint(0, max(1, w // 2), (1,), generator=gen))
-        m[i, y0:y0 + max(1, h // 3), x0:x0 + max(2, w // 3)] = 0
-    return m
-
-
 def _up2(t):
     return t.repeat_interleave(2, -2).repeat_interleave(2, -1)
-
-
-def _same(got, want):
-    """bitwise equality with NaN == NaN (a NaN prefill left unwritten still fails: want is never NaN there)"""
-    return (got == want) | (got.isnan() & want.isnan())
-
-
-def _assert_bitwise(name, got, want, alt=None):
-    ok = _same(got, want) if alt is None else (_same(got, want) | _same(got, alt))
-    if not bool(ok.all()):
-        bad = tuple((~ok).nonzero()[0].tolist())
-        raise AssertionError(f"{name}: {int((~ok).sum())} of {ok.numel()} elements differ from the exact result; first at {list(bad)}: "
-                             f"got {float(got[bad])}, want {float(want[bad])}" + ("" if alt is None else f" or {float(alt[bad])}"))
-
-
-def _assert_within(name, got, ref, bound):
-    assert torch.isfinite(got).all(), f"{name}: output left unwritten or not finite"
-    excess = (got - ref).abs() - bound
-    worst = int(excess.argmax())
-    assert float(excess.max()) <= 0.0, (f"{name}: |err| exceeds the bound at flat index {worst}: "
-                                       f"err {float((got - ref).abs().flatten()[worst]):.3e}, bound {float(bound.flatten()[worst]):.3e}")
 
 
 def _fl32_sum(t, b):
@@ -254,30 +301,15 @@ def _fl32_sum(t, b):
     return torch.where(tie, toward_e, f)
 
 
-def _act(z, act):
-    if act == _lib.ACT_RELU:
-        return z.clamp_min(0)
-    if act == _lib.ACT_LEAKY:
-        return torch.where(z > 0, z, z * SLOPE)
-    if act == _lib.ACT_RELU6:
-        return z.clamp(0, 6)
-    return z
-
-
-def _kernel_routes(prof):
-    """(forward, data gradient, weight gradient) route names from the kernels of a trace holding one forward, one data gradient
-    and two weight gradients: the route-specific kernels first (a stem or a tail also runs its sub-problem on the tensor-core
-    kernels), then the tensor-core kernels by their MODE template argument (0 forward, 1 data gradient); the stride-2 data
-    gradient launches the stride-1 TMA kernel once per parity class"""
+def _kernel_routes(records):
+    """(forward, data gradient, weight gradient) route names from the kernel records of a trace holding one forward, one data
+    gradient and two weight gradients: the route-specific kernels first (a stem or a tail also runs its sub-problem on the
+    tensor-core kernels), then the tensor-core kernels by their MODE template argument (0 forward, 1 data gradient); the
+    stride-2 data gradient launches the stride-1 TMA kernel once per parity class"""
     cnt = collections.Counter()
-    for e in prof.events():
-        if getattr(e, "device_type", DeviceType.CUDA) != DeviceType.CUDA:
-            continue
-        m = KERNEL_NAME.search(e.name)
-        if m:
-            args = [a.strip() for a in (m.group(2) or "").split(",")]
-            cnt[(m.group(1), args[1] if m.group(1) in ("pconv_tc_tma_kernel", "pconv_tc_persistent_kernel") else
-                 args[0] if m.group(1) == "k2r_dbuild_kernel" else "")] += 1
+    for (k, args), launches in records.items():
+        cnt[(k, args[1] if k in ("pconv_tc_tma_kernel", "pconv_tc_persistent_kernel") else
+             args[0] if k == "k2r_dbuild_kernel" else "")] += launches
 
     def one(options):
         found = [r for r, k in options if cnt[k]]
@@ -305,7 +337,7 @@ class _Problem:
         for p in sp["parts"]:
             if p["mask"]:
                 mu = p["mup"]
-                mk = _holes(n, h >> mu, w >> mu, gen).to(dev)
+                mk = holes(n, h >> mu, w >> mu, gen).to(dev)
                 self.masks.append(mk)
                 m = mk.double()
                 mfull.append(_up2(m) if mu else m)
@@ -347,19 +379,17 @@ class _Problem:
         for p, v, m in zip(sp["parts"], vals, self.mfull):
             mx = F.max_pool2d(m[:, None], 2)[:, 0] if p["up"] else m
             v = torch.where(mx[..., None] == 0, torch.full_like(v, HOLE_VALUE), v)
-            buf = torch.full((*v.shape[:-1], p["xcs"]), SENTINEL, dtype=self.dtype, device=self.dev)
-            buf[..., :_rup8(p["c"])] = 0
-            buf[..., :p["c"]] = v.to(self.dtype)
+            buf = self.operand(v, p["xcs"])
             self.xbufs.append(buf)
-            xv = buf[..., :p["c"]].double().permute(0, 3, 1, 2)
+            xv = nchw(buf, p["c"])
             xm.append((_up2(xv) if p["up"] else xv) * m[:, None])
         for i, b in enumerate(self.xbufs):
             self.conv.parts[i].x = b.data_ptr()
         self.XM = torch.cat(xm, 1)
 
-    def strided(self, vals, cs):
-        buf = torch.full((*vals.shape[:-1], cs), SENTINEL, dtype=self.dtype, device=self.dev)
-        buf[..., :_rup8(vals.shape[-1])] = 0
+    def operand(self, vals, cs):
+        """vals [..., c] in the storage type, zeros in channels [c, rup(c, 8)), SENTINEL past that"""
+        buf = strided((*vals.shape[:-1], _rup8(vals.shape[-1])), cs, 0, self.dtype)
         buf[..., :vals.shape[-1]] = vals.to(self.dtype)
         return buf
 
@@ -369,9 +399,7 @@ class _Problem:
         self.W = wm.to(self.dtype).double().permute(0, 3, 1, 2).contiguous()
 
     def new_y(self):
-        buf = torch.full((self.sp["n"], self.ho, self.wo, self.sp["ycs"]), SENTINEL, dtype=self.dtype, device=self.dev)
-        buf[..., :_rup8(self.sp["cout"])] = float("nan")
-        return buf
+        return strided((self.sp["n"], self.ho, self.wo, _rup8(self.sp["cout"])), self.sp["ycs"], float("nan"), self.dtype)
 
     def y_padding_ok(self, y):
         """zeros in channels [cout, rup(cout, 8)); past that, channels that are no output: the sentinel, or zeros"""
@@ -383,9 +411,7 @@ class _Problem:
         sp, out = self.sp, []
         for p, cs in zip(sp["parts"], sp["dxcs"]):
             sh = p["up"] if at_src else 0
-            buf = torch.full((sp["n"], sp["h"] >> sh, sp["w"] >> sh, cs), SENTINEL, dtype=self.dtype, device=self.dev)
-            buf[..., :p["c"]] = float("nan")
-            out.append(buf)
+            out.append(strided((sp["n"], sp["h"] >> sh, sp["w"] >> sh, p["c"]), cs, float("nan"), self.dtype))
         return out
 
     # ---- fp64 references
@@ -414,10 +440,6 @@ class _Problem:
             out.append(g)
             off += p["c"]
         return out
-
-
-def _nchw(buf, c):
-    return buf[..., :c].permute(0, 3, 1, 2)
 
 
 def _ws(lib, cref, dev):
@@ -463,30 +485,28 @@ def test_conv_route_vs_fp64(name):
         _lib.check(lib.pcb_conv_weight_prepare(cref, wm.data_ptr(), wf.data_ptr(), wd.data_ptr() if wd is not None else None, stream))
         return wf, wd
 
-    def run_dgrad(dc, wf, wd, wm):
-        dxs = P.new_dx(at_src)
+    def run_dgrad(dc, wf, wd, wk, dxs):
+        """into the prefilled dxs; wk: the KRSC weights in the storage type (row-packed layers)"""
         ptrs = (ctypes.c_void_p * len(dxs))(*[b.data_ptr() for b in dxs])
         strides = (ctypes.c_int32 * len(dxs))(*sp["dxcs"])
         if route[1] == "none":
-            wk = wm.to(dt).contiguous()
             _lib.check(lib.pcb_pconv_backward_data(dg_ref, dc.data_ptr(), dcs, wk.data_ptr(), None, ptrs, strides, stream))
         else:
             _lib.check(lib.pcb_pconv_backward_data(cref, dc.data_ptr(), dcs, wf.data_ptr(), wd.data_ptr() if wd is not None else None,
                                                    ptrs, strides, stream))
-        return dxs
 
     def ints(r, *shape):
         return torch.randint(-r, r + 1, shape, generator=dgen, device=dev).to(torch.float32)
 
     def check_dx(tag, dxs, want_parts, alt_parts=None):
         for i, (p, buf, want) in enumerate(zip(sp["parts"], dxs, want_parts)):
-            got = _nchw(buf, p["c"]).float()
+            got = nchw(buf, p["c"]).float()
             if alt_parts is None:
-                _assert_bitwise(f"{name}: {tag}, part {i}", got, want)
+                assert_bitwise(f"{name}: {tag}, part {i}", got, want, nan_equal=True)
             else:
-                _assert_within(f"{name}: {tag}, part {i}", got.double(), want, alt_parts[i])
+                assert_within(f"{name}: {tag}, part {i}", got.double(), want, alt_parts[i])
             c8 = _rup8(p["c"])
-            assert bool((buf[..., c8:] == SENTINEL).all()), f"{name}: {tag} wrote past rup(c, 8) of part {i}"
+            assert sentinel_kept(buf, c8), f"{name}: {tag} wrote past rup(c, 8) of part {i}"
             pad = buf[..., p["c"]:c8]
             assert bool(((pad == SENTINEL) | (pad == 0)).all()), f"{name}: {tag} wrote garbage into the channel padding of part {i}"
 
@@ -496,8 +516,8 @@ def test_conv_route_vs_fp64(name):
     P.master(ints(iw, cout, kh, kw, P.cig))
     bias = torch.randint(-16, 17, (cout,), generator=dgen, device=dev).to(torch.float32) / 8
     dcv = ints(4, n, ho, wo, cout)
-    dc = P.strided(dcv, dcs)
-    G = _nchw(dc, cout).double()
+    dc = P.operand(dcv, dcs)
+    G = nchw(dc, cout)
     # every partial sum below 2^24: at most (number of valid terms) x max|a| x max|b|
     big = max(float(P.nz_fwd.max()) * ix * iw, float(P.nz_dg.max()) * 4 * iw, float(P.nz_wg.max()) * 4 * ix)
     assert big < 2 ** 24, f"{name}: partial sums could round ({big:.3g}): not an exact case"
@@ -505,25 +525,31 @@ def test_conv_route_vs_fp64(name):
         cu = max(p["c"] for p in sp["parts"] if p["up"])
         assert cu * ix * iw <= 256, f"{name}: the tail's bf16 Z rows would round"
     wf, wd = prepare(P.wm)
-    y = P.new_y()
+    wk = P.wm.to(dt).contiguous()
+    y, dxs = P.new_y(), P.new_dx(at_src)
     msum = torch.full((mg, N), float("nan"), device=dev)
     newmask = torch.full((mg, N), 77, dtype=torch.uint8, device=dev)
     dw = torch.full((cout, kh, kw, P.cig), float("nan"), device=dev)
     dw0 = ints(4, cout, kh, kw, P.cig)
     dw_acc = dw0.clone()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        time.sleep(PROFILER_PAD_S)
+    state = [(y, y.clone()), (msum, float("nan")), (newmask, 77), (dw, float("nan")), (dw_acc, dw0)] + [(b, b.clone()) for b in dxs]
+
+    def run():
         _lib.check(lib.pcb_pconv_forward(cref, wf.data_ptr(), bias.data_ptr(), y.data_ptr(), ycs, msum.data_ptr(), newmask.data_ptr(),
                                          ws.data_ptr(), stream))
-        dxs = run_dgrad(dc, wf, wd, P.wm)
+        run_dgrad(dc, wf, wd, wk, dxs)
         _lib.check(lib.pcb_pconv_backward_weight(cref, dc.data_ptr(), dcs, dw.data_ptr(), ws.data_ptr(), stream))
         _lib.check(lib.pcb_pconv_backward_weight_acc(cref, dc.data_ptr(), dcs, dw_acc.data_ptr(), ws.data_ptr(), stream))
-        torch.cuda.synchronize()
-        time.sleep(PROFILER_PAD_S)
-    ran, cnt = _kernel_routes(prof)
+
     want_ran = tuple("generic" if r == "none" else r for r in route)
-    assert ran == want_ran, f"{name}: the kernels ran {ran}, the plan says {route}; kernels: {dict(cnt)}"
+
+    def check(records):
+        ran, cnt = _kernel_routes(records)
+        assert ran == want_ran, f"{name}: the kernels ran {ran}, the plan says {route}; kernels: {dict(cnt)}"
+        for (k, args), launches in sp.get("tiles", {}).items():
+            assert records[(k, args)] == launches, (f"{name}: {k}<{', '.join(args)}> launched {records[(k, args)]} times, the case is "
+                                                    f"named for {launches}; kernels: {dict(records)}")
+    traced(name, run, check, state)
 
     # mask pass: the fp64 box sums; a plain convolution leaves msum / newmask alone
     s_ref = P.box.permute(1, 0, 2, 3).reshape(mg, N)
@@ -531,8 +557,8 @@ def test_conv_route_vs_fp64(name):
     if sp["plain"]:
         assert bool(msum.isnan().all()) and bool((newmask == 77).all()), f"{name}: a plain convolution must not touch msum / newmask"
     else:
-        _assert_bitwise(f"{name}: msum", msum.double(), s_ref)
-        _assert_bitwise(f"{name}: newmask", newmask, nm_ref)
+        assert_bitwise(f"{name}: msum", msum.double(), s_ref, nan_equal=True)
+        assert_bitwise(f"{name}: newmask", newmask, nm_ref, nan_equal=True)
     # the two-call forward: mask pass, then the rest, bitwise equal to the one-call forward
     msum2 = torch.full((mg, N), float("nan"), device=dev)
     newmask2 = torch.full((mg, N), 77, dtype=torch.uint8, device=dev)
@@ -542,9 +568,9 @@ def test_conv_route_vs_fp64(name):
                                                newmask2.data_ptr(), ws2.data_ptr(), stream))
     torch.cuda.synchronize()
     if not sp["plain"]:
-        _assert_bitwise(f"{name}: mask pass msum", msum2.double(), s_ref)
-        _assert_bitwise(f"{name}: mask pass newmask", newmask2, nm_ref)
-    _assert_bitwise(f"{name}: mask pass + premasked forward vs one-call forward", y2, y)
+        assert_bitwise(f"{name}: mask pass msum", msum2.double(), s_ref, nan_equal=True)
+        assert_bitwise(f"{name}: mask pass newmask", newmask2, nm_ref, nan_equal=True)
+    assert_bitwise(f"{name}: mask pass + premasked forward vs one-call forward", y2, y, nan_equal=True)
 
     # forward
     S = P.conv_ref(P.XM, P.W).round()
@@ -562,29 +588,29 @@ def test_conv_route_vs_fp64(name):
     hole = torch.full_like(want, float("nan") if sp["no_guard"] else 0.0)
     want = torch.where(empty, hole, want).to(dt)
     alt = torch.where(empty, hole, alt).to(dt) if alt is not None else None
-    _assert_bitwise(f"{name}: forward", _nchw(y, cout), want, alt)
+    assert_bitwise(f"{name}: forward", nchw(y, cout), want, alt, nan_equal=True)
     assert P.y_padding_ok(y), f"{name}: forward must write zeros into channels [cout, rup(cout, 8)) and nothing past them"
 
     # renormalisation backward: which of the three kernels runs is decided by the layout, each has its own last operation
     dyv = ints(4, n, ho, wo, cout)
-    dy = P.strided(dyv, ycs)
+    dy = P.operand(dyv, ycs)
     dco = torch.full((n, ho, wo, dcs), float("nan"), dtype=dt, device=dev)
     dbias = torch.full((cout,), float("nan"), device=dev)
     _lib.check(lib.pcb_pconv_renorm_backward(cref, dy.data_ptr(), ycs, msum.data_ptr(), dco.data_ptr(), dcs, dbias.data_ptr(), stream))
     torch.cuda.synchronize()
-    Y = _nchw(dy, cout).float()
+    Y = nchw(dy, cout).float()
     sf = P.s.float()
     vec = mg == 1 and cout % 8 == 0 and cout <= 2048 and dcs == cout and ycs % 8 == 0
     pix8 = mg == 1 and cout <= 8 and dcs == 8
     d = Y * (1.0 / sf) if (vec or pix8) else Y / sf
     keep = ~empty if not sp["no_guard"] else torch.ones_like(empty)
     d = torch.where(keep, d, torch.zeros_like(d))
-    _assert_bitwise(f"{name}: renormalisation backward", _nchw(dco, cout).float(), d.to(dt).float())
+    assert_bitwise(f"{name}: renormalisation backward", nchw(dco, cout).float(), d.to(dt).float(), nan_equal=True)
     assert bool((dco[..., cout:] == 0).all()), f"{name}: renormalisation backward must zero channels [cout, dc_cstride)"
     dbias_want = (Y.double() * (~empty)).sum((0, 2, 3))
     if sp["no_guard"] and bool(empty.any()):
         dbias_want = torch.where(empty.any(3).any(2).any(0), torch.full_like(dbias_want, float("nan")), dbias_want)
-    _assert_bitwise(f"{name}: bias gradient", dbias.double(), dbias_want)
+    assert_bitwise(f"{name}: bias gradient", dbias.double(), dbias_want, nan_equal=True)
 
     # data gradient: m * S, zero under the holes, at source resolution where the query says so
     gfull = P.dgrad_ref(G, P.W).round() * P.M
@@ -597,15 +623,15 @@ def test_conv_route_vs_fp64(name):
         _lib.check(lib.pcb_pconv_backward_data_relu(cref, dc.data_ptr(), dcs, wd.data_ptr(), dxr.data_ptr(), sp["dxcs"][0],
                                                     rx.data_ptr(), sp["parts"][0]["xcs"], stream))
         torch.cuda.synchronize()
-        relu_keep = _nchw(rx, cin).float() > 0
+        relu_keep = nchw(rx, cin).float() > 0
         check_dx("data gradient with the ReLU backward", [dxr], [torch.where(relu_keep, wants[0], torch.zeros_like(wants[0]))])
 
     # weight gradient: S, and fl(dw0 + S) accumulating
     gw = P.wgrad_ref(P.XM, G).round().permute(0, 2, 3, 1)
-    _assert_bitwise(f"{name}: weight gradient", dw, gw.float())
-    _assert_bitwise(f"{name}: weight gradient (accumulating)", dw_acc, (dw0.double() + gw).float())
+    assert_bitwise(f"{name}: weight gradient", dw, gw.float(), nan_equal=True)
+    assert_bitwise(f"{name}: weight gradient (accumulating)", dw_acc, (dw0.double() + gw).float(), nan_equal=True)
     for i, (p, buf) in enumerate(zip(sp["parts"], P.xbufs)):
-        assert bool((buf[..., _rup8(p["c"]):] == SENTINEL).all()), f"{name}: x of part {i} was written"
+        assert sentinel_kept(buf, _rup8(p["c"])), f"{name}: x of part {i} was written"
 
     # weight refresh: refresh(W2) over prepare(W1) is bitwise prepare(W2), extra operands included
     wm2 = ints(iw, cout, kh, kw, P.cig)
@@ -634,11 +660,11 @@ def test_conv_route_vs_fp64(name):
 
     def check_y(tag, y, v, e, nan_at_empty=True):
         assert P.y_padding_ok(y), f"{name}: {tag} must write zeros into channels [cout, rup(cout, 8)) and nothing past them"
-        got = _nchw(y, cout).double()
+        got = nchw(y, cout)
         if sp["no_guard"]:                       # (an activation of NaN is whatever fmaxf / fminf make of it)
             assert not nan_at_empty or bool(got[~live].isnan().all()), f"{name}: {tag}: NaN expected where the box is empty"
             got = torch.where(live, got, v)
-        _assert_within(f"{name}: {tag}", got, v, e + store * (v.abs() + e))
+        assert_within(f"{name}: {tag}", got, v, e + store * (v.abs() + e))
 
     y = P.new_y()
     _lib.check(lib.pcb_pconv_forward(cref, wf.data_ptr(), bias.data_ptr(), y.data_ptr(), ycs, msum.data_ptr(), newmask.data_ptr(),
@@ -668,7 +694,7 @@ def test_conv_route_vs_fp64(name):
                                                         newmask.data_ptr(), ws.data_ptr(), 0, scale.data_ptr(), shift.data_ptr(), act,
                                                         SLOPE, stream))
             torch.cuda.synchronize()
-            va = _act(z, act)
+            va = act_ref(z, act, SLOPE)
             check_y(f"eval epilogue, activation {act}", y, va, ez + 2.0 ** -23 * va.abs(), act == _lib.ACT_NONE)
     else:
         y = P.new_y()
@@ -683,9 +709,10 @@ def test_conv_route_vs_fp64(name):
         torch.cuda.synchronize()
         assert bool(y[..., :_rup8(cout)].isnan().all()) and bool((sums == 0).all()), f"{name}: a refused call must not run"
 
-    dc = P.strided(torch.randn(n, ho, wo, cout, generator=dgen, device=dev), dcs)
-    G = _nchw(dc, cout).double()
-    dxs = run_dgrad(dc, wf, wd, P.wm)
+    dc = P.operand(torch.randn(n, ho, wo, cout, generator=dgen, device=dev), dcs)
+    G = nchw(dc, cout)
+    dxs = P.new_dx(at_src)
+    run_dgrad(dc, wf, wd, P.wm.to(dt).contiguous(), dxs)
     dw = torch.full((cout, kh, kw, P.cig), float("nan"), device=dev)
     _lib.check(lib.pcb_pconv_backward_weight(cref, dc.data_ptr(), dcs, dw.data_ptr(), ws.data_ptr(), stream))
     torch.cuda.synchronize()
@@ -699,4 +726,4 @@ def test_conv_route_vs_fp64(name):
     wref = P.wgrad_ref(P.XM, G)
     wmag = P.wgrad_ref(P.XM.abs(), G.abs())
     werr = P.nz_wg * 2.0 ** -22 * wmag + (2.0 ** -8 * wmag if route[2] == "k2r" else 0.0)
-    _assert_within(f"{name}: Gaussian weight gradient", dw.double(), wref.permute(0, 2, 3, 1), werr.permute(0, 2, 3, 1))
+    assert_within(f"{name}: Gaussian weight gradient", dw.double(), wref.permute(0, 2, 3, 1), werr.permute(0, 2, 3, 1))

@@ -9,7 +9,7 @@ reference is a direct sum).  Two sets of cases:
     x-tile and dilation-phase edges in both storage types, a "valid" 3x3 on dw3, and the first-generation kernels (k5, k7,
     kh != kw, the stride-3 data gradient).
 
-Each case asserts the route it covers from the kernel names of one torch.profiler trace, then checks:
+Each case asserts the route it covers from the kernel names of a torch.profiler trace (kernel_harness.traced), then checks:
 
   * mask pass: msum and newmask equal the fp64 box sums exactly (times cin with same_holes); a plain convolution leaves both
     untouched;
@@ -32,28 +32,22 @@ two fp32 roundings (product, or the fma, and add; bf16 products are exact), so t
 n * 2^-22 * S, S = sum of |products| (Higham, Accuracy and Stability of Numerical Algorithms, 4.2; n u < 1/2 here).  The
 division by s and the bias add round twice more (2^-22 relative of |acc| / s and the result), the eval epilogue's fma once
 (2^-23 of |z| + |shift|) and LeakyReLU's multiply once (2^-23 of the result); every activation is 1-Lipschitz.  A bf16 store
-adds half an ulp (2^-8 relative is used, as in test_gpu_fwd_tiles.py).  The BatchNorm sums are checked against the stored
+adds half an ulp (2^-8 relative is used, as in test_gpu_conv_routes.py).  The BatchNorm sums are checked against the stored
 values: M fp32 additions of terms bounded by |y| are off by at most M * 2^-23 * sum |y|.
 """
 import ctypes
-import json
-import os
-import re
-import time
 
 import pytest
 import torch
 import torch.nn.functional as F
 from torch.nn.grad import conv2d_input, conv2d_weight
-from torch.profiler import ProfilerActivity, profile
 
+from kernel_harness import (HOLE_VALUE, act_ref, assert_bitwise, assert_within, conv_dispatch_cases, holes, nchw, sentinel_kept,
+                            strided, traced)
 from text_segmentation_image_inpainting_b200 import _lib
 
 pytestmark = pytest.mark.gpu
 
-FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "conv_dispatch.json")
-HOLE_VALUE = 1024.0          # x under the holes: a read that ignores the mask is far outside any bound (exact in bf16)
-SENTINEL = -8192.0           # channels [c, cstride) of a strided view: inputs must not be read there, outputs not written
 INT_RANGE = 4                # |x|, |w|, |dc| <= 4 in the integer regime
 SLOPE = 0.2
 ACTS = (_lib.ACT_NONE, _lib.ACT_RELU, _lib.ACT_LEAKY, _lib.ACT_RELU6)
@@ -63,10 +57,6 @@ DTYPES = {"bf16": (torch.bfloat16, _lib.PCB_BF16), "f32": (torch.float32, _lib.P
 KERNELS = {"dw4": ("dw4_s1_kernel", "dw4_s1_kernel", "dw4_s1_wgrad_kernel"),
            "dw3": ("dw3_fwd_kernel", "dw3_dgrad_kernel", "dw3_wgrad_kernel"),
            "gen1": ("dw_fwd_kernel", "dw_dgrad_kernel", "dw_wgrad_kernel")}
-KERNEL_NAME = re.compile(r"(?<![A-Za-z_])(dw\w*?_kernel)")
-# the profiler keeps only the device activity whose timestamps, converted to host time, fall inside its window: idle margins
-# keep a workload of a few microseconds from being dropped at the window's edges
-PROFILER_PAD_S = 0.05
 
 
 def _case(n, h, w, c, k=3, s=1, pad=None, dil=1, dtype="bf16", holes=False, mask_up=0, same_holes=False, plain=None,
@@ -90,10 +80,8 @@ def _case(n, h, w, c, k=3, s=1, pad=None, dil=1, dtype="bf16", holes=False, mask
 
 def _fixture_cases():
     """one case per distinct depthwise descriptor of the dispatch fixture (the depthwise family's eligibility test, n <= 2)"""
-    with open(FIXTURE) as f:
-        descs = [case["conv"] for case in json.load(f)["cases"]]
     out = {}
-    for d in descs:
+    for d in (case["conv"] for case in conv_dispatch_cases()):
         p = d["parts"]
         if not (d["groups"] == d["cin"] == d["cout"] > 1 and len(p) == 1):
             continue
@@ -157,56 +145,6 @@ HAND_CASES = {
 CASES = {**_fixture_cases(), **HAND_CASES}
 
 
-def _holes(n, h, w, gen):
-    """uint8 plane, 1 = valid: a rectangle per image plus scattered single pixels"""
-    m = (torch.rand(n, h, w, generator=gen) > 0.15).to(torch.uint8)
-    for i in range(n):
-        y0, x0 = int(torch.randint(0, max(1, h // 2), (1,), generator=gen)), int(torch.randint(0, max(1, w // 2), (1,), generator=gen))
-        m[i, y0:y0 + max(1, h // 3), x0:x0 + max(2, w // 3)] = 0
-    return m
-
-
-def _strided(shape, cs, fill, dtype, dev):
-    """[..., cs] buffer: channels [0, c) = fill (a tensor, or a value), [c, cs) = SENTINEL"""
-    buf = torch.full((*shape[:-1], cs), SENTINEL, dtype=dtype, device=dev)
-    buf[..., :shape[-1]] = fill
-    return buf
-
-
-def _sentinel_kept(buf, c):
-    return bool((buf[..., c:] == SENTINEL).all())
-
-
-def _nchw(buf, c):
-    return buf[..., :c].double().permute(0, 3, 1, 2)
-
-
-def _act(z, act):
-    if act == _lib.ACT_RELU:
-        return z.clamp_min(0)
-    if act == _lib.ACT_LEAKY:
-        return torch.where(z > 0, z, z * SLOPE)
-    if act == _lib.ACT_RELU6:
-        return z.clamp(0, 6)
-    return z
-
-
-def _assert_within(name, got, ref, bound):
-    assert torch.isfinite(got).all(), f"{name}: output left unwritten or not finite"
-    excess = (got - ref).abs() - bound
-    worst = int(excess.argmax())
-    assert float(excess.max()) <= 0.0, (f"{name}: |err| exceeds the bound at flat index {worst}: "
-                                       f"err {float((got - ref).abs().flatten()[worst]):.3e}, bound {float(bound.flatten()[worst]):.3e}")
-
-
-def _assert_bitwise(name, got, want):
-    ok = got == want                                                  # NaN (unwritten) compares unequal
-    if not bool(ok.all()):
-        bad = (~ok).nonzero()[0].tolist()
-        raise AssertionError(f"{name}: {int((~ok).sum())} of {ok.numel()} elements differ from the exact result; first at "
-                             f"{bad}: got {float(got[tuple(bad)])}, want {float(want[tuple(bad)])}")
-
-
 class _Problem:
     """one depthwise problem: the descriptor, the hole plane and the fp64 reference helpers"""
 
@@ -220,7 +158,7 @@ class _Problem:
         self.mg = 1 if sp["same_holes"] else c
         if sp["holes"]:
             mu = sp["mask_up"]
-            self.mask = _holes(n, h >> mu, w >> mu, gen).to(dev)
+            self.mask = holes(n, h >> mu, w >> mu, gen).to(dev)
             m = self.mask.double()
             if mu:
                 m = m.repeat_interleave(2, 1).repeat_interleave(2, 2)
@@ -245,9 +183,9 @@ class _Problem:
         """x: [n, h, w, c] values; HOLE_VALUE under the holes, the sentinel past c"""
         if self.mask is not None:
             x = torch.where(self.M[:, 0, :, :, None] == 0, torch.full_like(x, HOLE_VALUE), x)
-        self.x = _strided(x.shape, self.sp["cs"][0], x.to(self.dtype), self.dtype, self.dev)
+        self.x = strided(x.shape, self.sp["cs"][0], x.to(self.dtype), self.dtype)
         self.conv.parts[0].x = self.x.data_ptr()
-        self.XM = _nchw(self.x, self.sp["c"]) * self.M
+        self.XM = nchw(self.x, self.sp["c"]) * self.M
 
     def prepare_weights(self, wm, stream, lib):
         fe, de = ctypes.c_size_t(), ctypes.c_size_t()
@@ -273,22 +211,13 @@ class _Problem:
         return r.reshape(sp["c"], self.taps)
 
     def new_y(self):
-        return _strided((self.sp["n"], self.ho, self.wo, self.sp["c"]), self.sp["cs"][1], float("nan"), self.dtype, self.dev)
+        return strided((self.sp["n"], self.ho, self.wo, self.sp["c"]), self.sp["cs"][1], float("nan"), self.dtype)
 
     def new_dc(self, vals):
-        return _strided(vals.shape, self.sp["cs"][2], vals.to(self.dtype), self.dtype, self.dev)
+        return strided(vals.shape, self.sp["cs"][2], vals.to(self.dtype), self.dtype)
 
     def new_dx(self):
-        return _strided((self.sp["n"], self.sp["h"], self.sp["w"], self.sp["c"]), self.sp["cs"][3], float("nan"), self.dtype, self.dev)
-
-
-def _kernels_in(prof):
-    names = set()
-    for e in prof.events():
-        m = KERNEL_NAME.search(e.name)
-        if m:
-            names.add(m.group(1))
-    return names
+        return strided((self.sp["n"], self.sp["h"], self.sp["w"], self.sp["c"]), self.sp["cs"][3], float("nan"), self.dtype)
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
@@ -323,27 +252,30 @@ def test_dwconv_vs_fp64(name):
     dw = torch.full((c, P.taps), float("nan"), device=dev)
     dw0 = ints(c, P.taps)
     dw_acc = dw0.clone()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        time.sleep(PROFILER_PAD_S)
+    state = [(y, y.clone()), (dx, dx.clone()), (msum, float("nan")), (newmask, 77), (dw, float("nan")), (dw_acc, dw0)]
+
+    def run():
         _lib.check(lib.pcb_pconv_forward(cref, P.w_t.data_ptr(), bias.data_ptr(), y.data_ptr(), ycs, msum.data_ptr(),
                                          newmask.data_ptr(), None, stream))
         _lib.check(lib.pcb_pconv_backward_data(cref, dc.data_ptr(), dcs, P.w_t.data_ptr(), None, (ctypes.c_void_p * 1)(dx.data_ptr()),
                                                (ctypes.c_int32 * 1)(dxcs), stream))
         _lib.check(lib.pcb_pconv_backward_weight(cref, dc.data_ptr(), dcs, dw.data_ptr(), None, stream))
         _lib.check(lib.pcb_pconv_backward_weight_acc(cref, dc.data_ptr(), dcs, dw_acc.data_ptr(), None, stream))
-        torch.cuda.synchronize()
-        time.sleep(PROFILER_PAD_S)
-    want, ran = {KERNELS[r][i] for i, r in enumerate(sp["route"])}, _kernels_in(prof)
-    assert ran == want, f"{name}: ran {sorted(ran)}, the case covers {sorted(want)} ({len(prof.events())} events in the trace)"
+
+    want = {KERNELS[r][i] for i, r in enumerate(sp["route"])}
+
+    def check(records):
+        ran = {k for k, _ in records if k.startswith("dw")}
+        assert ran == want, f"{name}: ran {sorted(ran)}, the case covers {sorted(want)}"
+    traced(name, run, check, state)
 
     # mask pass
     if sp["plain"]:
         assert bool(msum.isnan().all()) and bool((newmask == 77).all()), f"{name}: a plain convolution must not touch msum / newmask"
     else:
         s_ref = P.msum[:, 0].reshape(1, N).expand(P.mg, N)
-        _assert_bitwise(f"{name}: msum", msum.double(), s_ref)
-        _assert_bitwise(f"{name}: newmask", newmask, (s_ref != 0).to(torch.uint8))
+        assert_bitwise(f"{name}: msum", msum.double(), s_ref)
+        assert_bitwise(f"{name}: newmask", newmask, (s_ref != 0).to(torch.uint8))
 
     # forward: fl(S + b) or fl(fl(S / s) + b)
     S = P.conv_ref(P.XM, P.W).round()
@@ -354,23 +286,23 @@ def test_dwconv_vs_fp64(name):
         s = P.msum
         q = (S / torch.where(s == 0, torch.ones_like(s), s)).float().double()
         v = torch.where(s == 0, torch.zeros_like(S), q + b).float()
-    _assert_bitwise(f"{name}: forward", y[..., :c].permute(0, 3, 1, 2), v.to(dt))
-    assert _sentinel_kept(y, c), f"{name}: forward wrote past c"
+    assert_bitwise(f"{name}: forward", y[..., :c].permute(0, 3, 1, 2), v.to(dt))
+    assert sentinel_kept(y, c), f"{name}: forward wrote past c"
 
     # data gradient: m * S, zero under the holes
-    G = _nchw(dc, c)
+    G = nchw(dc, c)
     gx = (P.dgrad_ref(G, P.W).round() * P.M).float()
     got = dx[..., :c].permute(0, 3, 1, 2)
-    _assert_bitwise(f"{name}: data gradient", got, gx.to(dt))
+    assert_bitwise(f"{name}: data gradient", got, gx.to(dt))
     assert bool((got.float() * (P.M == 0) == 0).all()), f"{name}: data gradient under the holes"
-    assert _sentinel_kept(dx, c), f"{name}: data gradient wrote past c"
+    assert sentinel_kept(dx, c), f"{name}: data gradient wrote past c"
 
     # weight gradient: S, and fl(dw0 + S) accumulating
     gw = P.wgrad_ref(P.XM, G).round()
     assert float(P.wgrad_ref(P.XM.abs(), G.abs()).max()) < 2 ** 24, f"{name}: partial sums could round: not an exact case"
-    _assert_bitwise(f"{name}: weight gradient", dw, gw.float())
-    _assert_bitwise(f"{name}: weight gradient (accumulating)", dw_acc, (dw0.double() + gw).float())
-    assert _sentinel_kept(P.x, c) and _sentinel_kept(dc, c)
+    assert_bitwise(f"{name}: weight gradient", dw, gw.float())
+    assert_bitwise(f"{name}: weight gradient (accumulating)", dw_acc, (dw0.double() + gw).float())
+    assert sentinel_kept(P.x, c) and sentinel_kept(dc, c)
 
     # ================= Gaussian regime: error bounds
     P.set_x(torch.randn(n, h, w, c, generator=dgen, device=dev))
@@ -388,8 +320,8 @@ def test_dwconv_vs_fp64(name):
     store = 2.0 ** -8 if dt == torch.bfloat16 else 0.0
 
     def check_y(tag, y, v, e):
-        assert _sentinel_kept(y, c), f"{name}: {tag} wrote past c"
-        _assert_within(f"{name}: {tag}", _nchw(y, c), v, e + store * (v.abs() + e))
+        assert sentinel_kept(y, c), f"{name}: {tag} wrote past c"
+        assert_within(f"{name}: {tag}", nchw(y, c), v, e + store * (v.abs() + e))
 
     scale = torch.rand(c, generator=dgen, device=dev) + 0.5
     shift = torch.randn(c, generator=dgen, device=dev) * 0.1
@@ -413,7 +345,7 @@ def test_dwconv_vs_fp64(name):
                                                         newmask.data_ptr(), None, 0, scale.data_ptr(), shift.data_ptr(), act, SLOPE,
                                                         stream))
             torch.cuda.synchronize()
-            va = _act(z, act)
+            va = act_ref(z, act, SLOPE)
             check_y(f"eval epilogue, activation {act}", y, va, ez + 2.0 ** -23 * va.abs())
     else:
         y = P.new_y()
@@ -440,11 +372,11 @@ def test_dwconv_vs_fp64(name):
         _lib.check(lib.pcb_pconv_backward_weight(cref, dc.data_ptr(), dcs, dw.data_ptr(), None, stream))
         torch.cuda.synchronize()
         check_y("fp32 forward", y, v_ref, e_ref)
-        G = _nchw(dc, c)
+        G = nchw(dc, c)
         gref = P.dgrad_ref(G, P.W) * P.M
         gb = P.dgrad_ref((G != 0).double(), (P.W != 0).double()) * 2.0 ** -22 * P.dgrad_ref(G.abs(), P.W.abs()) * P.M
-        _assert_within(f"{name}: fp32 data gradient", _nchw(dx, c), gref, gb)
-        assert _sentinel_kept(dx, c), f"{name}: data gradient wrote past c"
+        assert_within(f"{name}: fp32 data gradient", nchw(dx, c), gref, gb)
+        assert sentinel_kept(dx, c), f"{name}: data gradient wrote past c"
         wref = P.wgrad_ref(P.XM, G)
         wb = P.wgrad_ref((P.XM != 0).double(), (G != 0).double()) * 2.0 ** -22 * P.wgrad_ref(P.XM.abs(), G.abs())
-        _assert_within(f"{name}: fp32 weight gradient", dw.double(), wref, wb)
+        assert_within(f"{name}: fp32 weight gradient", dw.double(), wref, wb)

@@ -3,7 +3,8 @@ computed on the device: average pooling, bilinear upsampling, GAP and the scSE g
 2x upsampling, mask-format conversion, the L1-mean loss and SGD (elementwise.cu).  Cases: one per distinct call site of
 tests/golden/elementwise_sites.json (the layers of the three training workloads, the eval forward and one optimiser step, at
 the recorded size), plus hand cases for the edges production does not reach.  Outputs are prefilled with NaN, and each case
-asserts its route from the kernel names (and template arguments) of one complete torch.profiler trace (see _traced):
+asserts its route from the kernel names (and template arguments) of one complete torch.profiler trace (see
+kernel_harness.traced):
 
     route                 kernel                                  cases
     avgpool fwd / bwd     avgpool_kernel<T, false / true>         avgpool_*, fx_avgpool_*
@@ -43,28 +44,18 @@ Bounds:
     |p| + |lr d| for the update), propagated through the momentum and learning-rate factors.
 """
 import ctypes
-import json
 import math
-import os
-import re
-import time
-import warnings
 
 import pytest
 import torch
 import torch.nn.functional as F
-from torch.profiler import ProfilerActivity, profile
 
+from kernel_harness import assert_bitwise, assert_within, elementwise_sites, nan, nchw, traced
 from text_segmentation_image_inpainting_b200 import _lib
 
-FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "elementwise_sites.json")
 U = 2.0 ** -24
 BF, F32 = _lib.PCB_BF16, _lib.PCB_F32
 DT = {BF: torch.bfloat16, F32: torch.float32}
-KERNEL_NAME = re.compile(r"(?<![A-Za-z_])(\w+?_kernel)(?:<([^()]*)>)?\(")
-PROFILER_PAD_S = 0.05             # idle margins: the profiler drops device activity at the edges of its window
-PROFILER_TRIES = 20               # traces taken at most per case (see _traced)
-MARKER, MARKER_CYCLES = "spin_kernel", 1000   # torch.cuda._sleep's kernel brackets every trace
 NAN = float("nan")
 FAMILIES = ("avgpool", "bilinear", "gap", "scse", "concat", "upsample2x", "mask", "l1", "sgd")
 
@@ -88,18 +79,13 @@ def _site_case(s):
     return fam, name, dict(s)
 
 
-def _load_sites():
-    with open(FIXTURE) as f:
-        return json.load(f)
-
-
 def _fixture(fam):
-    return {name: sp for f, name, sp in map(_site_case, _load_sites()) if f == fam}
+    return {name: sp for f, name, sp in map(_site_case, elementwise_sites()) if f == fam}
 
 
 def test_fixture_sites_map_to_cases():
     """every non-BatchNorm site of the fixture names exactly one case of one family"""
-    sites = [s for s in _load_sites() if not s["fn"].startswith("pcb_bn_")]
+    sites = [s for s in elementwise_sites() if not s["fn"].startswith("pcb_bn_")]
     assert sites
     for s in sites:
         fam, name, _ = _site_case(s)
@@ -107,89 +93,14 @@ def test_fixture_sites_map_to_cases():
         assert name in _fixture(fam) and name not in HAND[fam]
 
 
-def _names(prof):
-    """(library kernels with their template arguments, number of marker kernels) of a trace"""
-    out, markers = set(), 0
-    for e in prof.events():
-        if MARKER in e.name:
-            markers += 1
-            continue
-        m = KERNEL_NAME.search(e.name)
-        if m:
-            out.add((m.group(1), re.sub(r"\s+", "", m.group(2) or "")))
-    return out, markers
-
-
-def _traced(name, fn, want, state):
-    """Run fn inside a torch.profiler trace and assert its route (see _assert_route).  The profiler loses device activity
-    records now and then (whole traces come back empty, even of several kernels and after an idle margin), so every trace
-    is bracketed by two marker kernels, the second after a synchronisation, and a trace in which either marker is missing
-    is not evidence either way.  Such a trace, or one whose kernels differ from `want`, is taken again, up to PROFILER_TRIES
-    times, from the same state: `state` lists (tensor, initial value) pairs reset before each attempt (outputs back to NaN,
-    accumulators back to their operands), so the last attempt is the one the checks read.  The route of these kernels is a
-    host-side decision on the arguments alone: a wrong route repeats on every complete trace and still fails.  Losses come
-    in stretches of seconds, so a case may see no complete trace at all: it then warns that its route went unchecked (other
-    cases of the same route still check it) and keeps every value check."""
-    last = None
-    for _ in range(PROFILER_TRIES):
-        for t, v in state:
-            t.copy_(v) if isinstance(v, torch.Tensor) else t.fill_(v)
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            time.sleep(PROFILER_PAD_S)
-            torch.cuda._sleep(MARKER_CYCLES)
-            fn()
-            torch.cuda.synchronize()
-            torch.cuda._sleep(MARKER_CYCLES)
-            torch.cuda.synchronize()
-            time.sleep(PROFILER_PAD_S)
-        ran, markers = _names(prof)
-        if markers == 2:
-            last = ran
-            if _route_ok(ran, want):
-                return
-    if last is None:       # no complete trace: the route cannot be judged, the value checks that follow still run
-        warnings.warn(f"{name}: the profiler recorded no complete trace in {PROFILER_TRIES} attempts; route not checked")
-        return
-    _assert_route(name, last, want)
-
-
-def _route_ok(ran, want):
-    return {r[0] for r in ran} == {k for k, _ in want} and \
-        all(any(r[0] == k and (suffix is None or r[1].endswith(suffix)) for r in ran) for k, suffix in want)
-
-
-def _assert_route(name, ran, want):
-    """want: {(kernel, template-argument suffix or None)}"""
-    for k, suffix in want:
-        assert any(r[0] == k and (suffix is None or r[1].endswith(suffix)) for r in ran), \
-            f"{name}: {k}<...{suffix or ''}> did not run; ran {sorted(ran)}"
-    assert {r[0] for r in ran} == {k for k, _ in want}, f"{name}: ran {sorted(ran)}, the case covers {sorted(want)}"
-
-
-def _assert_bitwise(name, got, want):
-    ok = got == want
-    if not bool(ok.all()):
-        bad = (~ok).nonzero()[0].tolist()
-        raise AssertionError(f"{name}: {int((~ok).sum())} of {ok.numel()} elements differ from the exact result; first at {bad}: "
-                             f"got {float(got[tuple(bad)])}, want {float(want[tuple(bad)])}")
-
-
-def _assert_either(name, got, a, b):
-    ok = (got == a) | (got == b)
-    if not bool(ok.all()):
-        bad = (~ok).nonzero()[0].tolist()
-        raise AssertionError(f"{name}: {int((~ok).sum())} elements match neither rounding; first at {bad}: got "
-                             f"{float(got[tuple(bad)])}, want {float(a[tuple(bad)])} or {float(b[tuple(bad)])}")
-
-
-def _assert_within(name, got, ref, bound):
-    got = got.double()
-    assert bool(torch.isfinite(got).all()), f"{name}: output left unwritten or not finite"
-    excess = (got - ref).abs() - bound
-    worst = int(excess.argmax())
-    assert float(excess.max()) <= 0.0, (f"{name}: |err| exceeds the bound at flat index {worst}: err "
-                                        f"{float((got - ref).abs().flatten()[worst]):.3e}, bound {float(bound.flatten()[worst]):.3e}")
+def _route(name, want):
+    """the check of traced for want = {(kernel, last template argument or None)}: those kernels ran, and no other"""
+    def check(records):
+        for k, last in want:
+            assert any(r == k and (last is None or args[-1:] == (last,)) for r, args in records), \
+                f"{name}: {k}<...{last or ''}> did not run; ran {sorted(records)}"
+        assert {r for r, _ in records} == {k for k, _ in want}, f"{name}: ran {sorted(records)}, the case covers {sorted(want)}"
+    return check
 
 
 def _gen(name):
@@ -200,20 +111,8 @@ def _ints(gen, *shape, lo=-4, hi=4):
     return torch.randint(lo, hi + 1, shape, generator=gen, device="cuda").double()
 
 
-def _nan(*shape, dtype=torch.float32):
-    return torch.full(shape, float("nan"), dtype=dtype, device="cuda")
-
-
 def _st():
     return torch.cuda.current_stream().cuda_stream
-
-
-def _nchw(t):
-    return t.double().permute(0, 3, 1, 2)
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
 
 
 # ------------------------------------------------------------------------------------------------ hand cases
@@ -290,22 +189,22 @@ def test_avgpool_vs_fp64(name):
     ho, wo = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
     x = _ints(gen, n, h, w, c).to(dt)
     gy = _ints(gen, n, ho, wo, c).to(dt)
-    y, gx = _nan(n, ho, wo, c, dtype=dt), _nan(n, h, w, c, dtype=dt)
-    _traced(name, lambda: (_lib.check(lib.pcb_avgpool_forward(x.data_ptr(), y.data_ptr(), sp["dtype"], n, h, w, c, k, s, p, st)),
-                           _lib.check(lib.pcb_avgpool_backward(gy.data_ptr(), gx.data_ptr(), sp["dtype"], n, h, w, c, k, s, p, st))),
-            {("avgpool_kernel", "false"), ("avgpool_kernel", "true")}, [(y, NAN), (gx, NAN)])
+    y, gx = nan(n, ho, wo, c, dtype=dt), nan(n, h, w, c, dtype=dt)
+    traced(name, lambda: (_lib.check(lib.pcb_avgpool_forward(x.data_ptr(), y.data_ptr(), sp["dtype"], n, h, w, c, k, s, p, st)),
+                          _lib.check(lib.pcb_avgpool_backward(gy.data_ptr(), gx.data_ptr(), sp["dtype"], n, h, w, c, k, s, p, st))),
+            _route(name, {("avgpool_kernel", "false"), ("avgpool_kernel", "true")}), [(y, NAN), (gx, NAN)])
     inv = torch.tensor(1.0 / (k * k), dtype=torch.float32).double().item()     # fl(1/k^2): 1.0f / (float)(k*k)
-    S = F.avg_pool2d(_nchw(x), k, s, p, count_include_pad=True, divisor_override=1)
+    S = F.avg_pool2d(nchw(x), k, s, p, count_include_pad=True, divisor_override=1)
     # backward: scatter every output's gradient over its window in padded coordinates (output o, tap a -> row o s + a)
-    G = _nchw(gy)
+    G = nchw(gy)
     hp, wp = max((ho - 1) * s + k, p + h), max((wo - 1) * s + k, p + w)
     acc = torch.zeros(n, c, hp, wp, dtype=torch.float64, device="cuda")
     for a in range(k):
         for b in range(k):
             acc[:, :, a:a + (ho - 1) * s + 1:s, b:b + (wo - 1) * s + 1:s] += G
     Sb = acc[:, :, p:p + h, p:p + w]
-    _assert_bitwise(f"{name}: forward", _nchw(y), (S * inv).float().to(dt).double())
-    _assert_bitwise(f"{name}: backward", _nchw(gx), (Sb * inv).float().to(dt).double())
+    assert_bitwise(f"{name}: forward", nchw(y), (S * inv).float().to(dt).double())
+    assert_bitwise(f"{name}: backward", nchw(gx), (Sb * inv).float().to(dt).double())
 
 
 # ------------------------------------------------------------------------------------------------ bilinear
@@ -317,24 +216,24 @@ def test_bilinear_vs_fp64(name):
     dt, n, h, w, c, s = DT[sp["dtype"]], sp["n"], sp["h"], sp["w"], sp["c"], sp["scale"]
     x = _ints(gen, n, h, w, c).to(dt)
     gy = _ints(gen, n, h * s, w * s, c).to(dt)
-    y, gx = _nan(n, h * s, w * s, c, dtype=dt), _nan(n, h, w, c, dtype=dt)
-    _traced(name, lambda: (_lib.check(lib.pcb_bilinear_forward(x.data_ptr(), y.data_ptr(), sp["dtype"], n, h, w, c, s, st)),
-                           _lib.check(lib.pcb_bilinear_backward(gy.data_ptr(), gx.data_ptr(), sp["dtype"], n, h, w, c, s, st))),
-            {("bilinear_fwd_kernel", None), ("bilinear_bwd_kernel", None)}, [(y, NAN), (gx, NAN)])
-    xr = _nchw(x).requires_grad_(True)
+    y, gx = nan(n, h * s, w * s, c, dtype=dt), nan(n, h, w, c, dtype=dt)
+    traced(name, lambda: (_lib.check(lib.pcb_bilinear_forward(x.data_ptr(), y.data_ptr(), sp["dtype"], n, h, w, c, s, st)),
+                          _lib.check(lib.pcb_bilinear_backward(gy.data_ptr(), gx.data_ptr(), sp["dtype"], n, h, w, c, s, st))),
+            _route(name, {("bilinear_fwd_kernel", None), ("bilinear_bwd_kernel", None)}), [(y, NAN), (gx, NAN)])
+    xr = nchw(x).requires_grad_(True)
     Y = F.interpolate(xr, scale_factor=s, mode="bilinear", align_corners=False)
-    G, = torch.autograd.grad(Y, xr, _nchw(gy))
+    G, = torch.autograd.grad(Y, xr, nchw(gy))
     if s & (s - 1) == 0:
-        _assert_bitwise(f"{name}: forward", _nchw(y), Y.detach().float().to(dt).double())
-        _assert_bitwise(f"{name}: backward", _nchw(gx), G.float().to(dt).double())
+        assert_bitwise(f"{name}: forward", nchw(y), Y.detach().float().to(dt).double())
+        assert_bitwise(f"{name}: backward", nchw(gx), G.float().to(dt).double())
     else:
         store = 2.0 ** -8 if dt == torch.bfloat16 else 0.0
         # a weight 1 - l or l is off by 2u (|src| + 1) in absolute terms, src < max(h, w), whatever its size; with the
         # products and the additions each term is off by at most 8u (max(h, w) + 2) |x|, |x| <= 4: 4 terms per output
         # forward, at most (2 s + 2)^2 per input backward
         wb = 8 * U * (max(h, w) + 2) * 4
-        _assert_within(f"{name}: forward", _nchw(y), Y.detach(), 4 * wb + store * Y.detach().abs())
-        _assert_within(f"{name}: backward", _nchw(gx), G, (2 * s + 2) ** 2 * wb + store * G.abs())
+        assert_within(f"{name}: forward", nchw(y), Y.detach(), 4 * wb + store * Y.detach().abs())
+        assert_within(f"{name}: backward", nchw(gx), G, (2 * s + 2) ** 2 * wb + store * G.abs())
 
 
 # ------------------------------------------------------------------------------------------------ GAP
@@ -347,26 +246,26 @@ def test_gap_vs_fp64(name):
     x = _ints(gen, n, hw, c).to(dt)
     g = _ints(gen, n, c).float()
     dx0 = _ints(gen, n, hw, c).to(dt)
-    out, dx, dxa = _nan(n, c), _nan(n, hw, c, dtype=dt), dx0.clone()
-    _traced(name, lambda: (_lib.check(lib.pcb_gap_forward(x.data_ptr(), sp["dtype"], n, hw, c, out.data_ptr(), st)),
-                           _lib.check(lib.pcb_gap_backward(g.data_ptr(), dx.data_ptr(), sp["dtype"], n, hw, c, 0, st)),
-                           _lib.check(lib.pcb_gap_backward(g.data_ptr(), dxa.data_ptr(), sp["dtype"], n, hw, c, 1, st))),
-            {("gap_kernel", None), ("gap_bwd_kernel", None)}, [(out, NAN), (dx, NAN), (dxa, dx0)])
+    out, dx, dxa = nan(n, c), nan(n, hw, c, dtype=dt), dx0.clone()
+    traced(name, lambda: (_lib.check(lib.pcb_gap_forward(x.data_ptr(), sp["dtype"], n, hw, c, out.data_ptr(), st)),
+                          _lib.check(lib.pcb_gap_backward(g.data_ptr(), dx.data_ptr(), sp["dtype"], n, hw, c, 0, st)),
+                          _lib.check(lib.pcb_gap_backward(g.data_ptr(), dxa.data_ptr(), sp["dtype"], n, hw, c, 1, st))),
+            _route(name, {("gap_kernel", None), ("gap_bwd_kernel", None)}), [(out, NAN), (dx, NAN), (dxa, dx0)])
     inv32 = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(float(hw), dtype=torch.float32)
     inv = float(inv32)
     S = x.double().sum(1)
     if hw & (hw - 1) == 0:
-        _assert_bitwise(f"{name}: forward", out.double(), S * inv)
+        assert_bitwise(f"{name}: forward", out.double(), S * inv)
     else:
         rpb = 256 // (c // 8)
         nsm = torch.cuda.get_device_properties(0).multi_processor_count
         chunks = max(1, min(math.ceil(hw / (rpb * 8)), max(1, 4 * nsm // n)))
-        _assert_within(f"{name}: forward", out, S / hw, (chunks + 1) * U * x.double().abs().sum(1) / hw + 2 * U * (S / hw).abs())
+        assert_within(f"{name}: forward", out, S / hw, (chunks + 1) * U * x.double().abs().sum(1) / hw + 2 * U * (S / hw).abs())
     gi = (g.double() * inv)[:, None, :]
-    _assert_bitwise(f"{name}: backward", dx, gi.float().expand(n, hw, c).to(dt))
+    assert_bitwise(f"{name}: backward", dx, gi.float().expand(n, hw, c).to(dt))
     unf = (dx0.float() + (g * inv32.cuda())[:, None, :])
     fus = (dx0.double() + gi).float()
-    _assert_either(f"{name}: backward (accumulate)", dxa, unf.to(dt), fus.to(dt))
+    assert_bitwise(f"{name}: backward (accumulate)", dxa, unf.to(dt), fus.to(dt))
 
 
 # ------------------------------------------------------------------------------------------------ scSE
@@ -389,8 +288,8 @@ def test_scse_vs_fp64(name):
         gy = gy * (torch.rand(npix, 1, generator=gen, device="cuda") < 2 ** 22 / tot)
     gy = gy.to(dt)
     g64 = gy.double()
-    y, sse_out = _nan(npix, c, dtype=dt), _nan(npix)
-    dx, dcse, dws = _nan(npix, c, dtype=dt), _nan(n, c), _nan(c)
+    y, sse_out = nan(npix, c, dtype=dt), nan(npix)
+    dx, dcse, dws = nan(npix, c, dtype=dt), nan(n, c), nan(c)
     if c > 1024:                                                        # refused before anything is written or launched
         before = _lib.launch_count()
         assert lib.pcb_scse_backward(gy.data_ptr(), x.data_ptr(), cse.data_ptr(), ws.data_ptr(), sse.data_ptr(), dx.data_ptr(),
@@ -400,11 +299,12 @@ def test_scse_vs_fp64(name):
         assert bool(dcse.isnan().all()) and bool(dws.isnan().all()) and bool(dx.isnan().all()), f"{name}: a refused call wrote"
         return
     vm = 1 if c <= 256 else (2 if c <= 512 else 4)
-    _traced(name, lambda: (_lib.check(lib.pcb_scse_forward(x.data_ptr(), cse.data_ptr(), ws.data_ptr(), y.data_ptr(), sse_out.data_ptr(),
-                                                           sp["dtype"], n, hw, c, st)),
-                           _lib.check(lib.pcb_scse_backward(gy.data_ptr(), x.data_ptr(), cse.data_ptr(), ws.data_ptr(), sse.data_ptr(),
-                                                            dx.data_ptr(), dcse.data_ptr(), dws.data_ptr(), sp["dtype"], n, hw, c, st))),
-            {("scse_fwd_kernel", None), ("scse_bwd_kernel", f",{vm}")}, [(y, NAN), (sse_out, NAN), (dx, NAN), (dcse, NAN), (dws, NAN)])
+    traced(name, lambda: (_lib.check(lib.pcb_scse_forward(x.data_ptr(), cse.data_ptr(), ws.data_ptr(), y.data_ptr(), sse_out.data_ptr(),
+                                                          sp["dtype"], n, hw, c, st)),
+                          _lib.check(lib.pcb_scse_backward(gy.data_ptr(), x.data_ptr(), cse.data_ptr(), ws.data_ptr(), sse.data_ptr(),
+                                                           dx.data_ptr(), dcse.data_ptr(), dws.data_ptr(), sp["dtype"], n, hw, c, st))),
+            _route(name, {("scse_fwd_kernel", None), ("scse_bwd_kernel", str(vm))}),
+            [(y, NAN), (sse_out, NAN), (dx, NAN), (dcse, NAN), (dws, NAN)])
     # forward: sse within the __expf bound, y exact given the kernel's sse
     cse_p = cse.repeat_interleave(hw, 0)                                # [npix, c]
     dot = x64 @ ws.double()
@@ -415,14 +315,14 @@ def test_scse_vs_fp64(name):
     d_dot = (c / gw + math.log2(gw) + 1) * U * (x64.abs() @ ws.double().abs())
     ref = torch.sigmoid(dot)
     bound = d_dot / 4 + ref * (1 - ref) * (2 + (1.173 * dot).abs().floor()) * 2.0 ** -23 + 2 * U
-    _assert_within(f"{name}: sse", sse_out, ref, bound)
-    _assert_bitwise(f"{name}: forward y", y, (x.float() * (cse_p + sse_out[:, None])).to(dt))
+    assert_within(f"{name}: sse", sse_out, ref, bound)
+    assert_bitwise(f"{name}: forward y", y, (x.float() * (cse_p + sse_out[:, None])).to(dt))
     # backward from the given sse: exact
     s64 = sse.double()[:, None]
     dpre = (g64 * x64).sum(1, keepdim=True) * s64 * (1 - s64)
-    _assert_bitwise(f"{name}: dx", dx, (g64 * (cse_p.double() + s64) + ws.double() * dpre).float().to(dt))
-    _assert_bitwise(f"{name}: dcse", dcse, (g64 * x64).reshape(n, hw, c).sum(1).float())
-    _assert_bitwise(f"{name}: dws", dws, (x64 * dpre).sum(0).float())
+    assert_bitwise(f"{name}: dx", dx, (g64 * (cse_p.double() + s64) + ws.double() * dpre).float().to(dt))
+    assert_bitwise(f"{name}: dcse", dcse, (g64 * x64).reshape(n, hw, c).sum(1).float())
+    assert_bitwise(f"{name}: dws", dws, (x64 * dpre).sum(0).float())
 
 
 # ------------------------------------------------------------------------------------------------ concat / upsample2x
@@ -444,27 +344,27 @@ def _concat_case(sp, name, lib):
         arr[i].x, arr[i].mask, arr[i].c, arr[i].x_cstride, arr[i].x_up, arr[i].mask_up = view.data_ptr(), None, c, cs, up, 0
         off += c
     null = set(sp.get("null", []))
-    y = _nan(n, h, w, ctot, dtype=dt)
+    y = nan(n, h, w, ctot, dtype=dt)
     gy = _ints(gen, n, h, w, ctot).to(dt)
-    gxs = [None if i in null else _nan(n, h >> p[2], w >> p[2], p[0], dtype=dt) for i, p in enumerate(parts)]
+    gxs = [None if i in null else nan(n, h >> p[2], w >> p[2], p[0], dtype=dt) for i, p in enumerate(parts)]
     ptrs = (ctypes.c_void_p * np_)(*[None if g is None else g.data_ptr() for g in gxs])
     carr = (ctypes.c_int32 * np_)(*[p[0] for p in parts])
     uarr = (ctypes.c_int32 * np_)(*[p[2] for p in parts])
     vec_f = all(p[0] % 8 == 0 and max(p[1], p[0]) % 8 == 0 for p in parts) and not sp.get("misalign")
     vec_b = [(p[0] % 8 == 0 and sum(q[0] for q in parts[:i]) % 8 == 0 and ctot % 8 == 0) for i, p in enumerate(parts)]
-    want = {("concat_fwd_kernel", ",8" if vec_f else ",1")}
-    want |= {("concat_bwd_kernel", ",8" if v else ",1") for i, v in enumerate(vec_b) if i not in null}
-    _traced(name, lambda: (_lib.check(lib.pcb_concat_forward(arr, np_, code, n, h, w, y.data_ptr(), st)),
-                           _lib.check(lib.pcb_concat_backward(gy.data_ptr(), carr, uarr, np_, code, n, h, w, ptrs, st))),
-            want, [(y, NAN)] + [(g, NAN) for g in gxs if g is not None])
+    want = {("concat_fwd_kernel", "8" if vec_f else "1")}
+    want |= {("concat_bwd_kernel", "8" if v else "1") for i, v in enumerate(vec_b) if i not in null}
+    traced(name, lambda: (_lib.check(lib.pcb_concat_forward(arr, np_, code, n, h, w, y.data_ptr(), st)),
+                          _lib.check(lib.pcb_concat_backward(gy.data_ptr(), carr, uarr, np_, code, n, h, w, ptrs, st))),
+            _route(name, want), [(y, NAN)] + [(g, NAN) for g in gxs if g is not None])
     ref = torch.cat([v.repeat_interleave(1 << p[2], 1).repeat_interleave(1 << p[2], 2) for v, p in zip(views, parts)], dim=3)
-    _assert_bitwise(f"{name}: forward", y, ref)
+    assert_bitwise(f"{name}: forward", y, ref)
     off = 0
     for i, (c, _, up) in enumerate(parts):
         if gxs[i] is not None:
             f = 1 << up
             g = gy[..., off:off + c].double().reshape(n, h >> up, f, w >> up, f, c).sum((2, 4))
-            _assert_bitwise(f"{name}: backward part {i}", gxs[i], g.to(dt))
+            assert_bitwise(f"{name}: backward part {i}", gxs[i], g.to(dt))
         off += c
 
 
@@ -482,13 +382,13 @@ def test_upsample2x_vs_exact(name):
     code, dt, n, h, w, c = sp["dtype"], DT[sp["dtype"]], sp["n"], sp["h"], sp["w"], sp["c"]
     x = _ints(gen, n, h, w, c).to(dt)
     gy = _ints(gen, n, 2 * h, 2 * w, c).to(dt)
-    y, gx = _nan(n, 2 * h, 2 * w, c, dtype=dt), _nan(n, h, w, c, dtype=dt)
-    v = ",8" if c % 8 == 0 else ",1"
-    _traced(name, lambda: (_lib.check(lib.pcb_upsample2x_forward(x.data_ptr(), code, n, h, w, c, y.data_ptr(), st)),
-                           _lib.check(lib.pcb_upsample2x_backward(gy.data_ptr(), code, n, h, w, c, gx.data_ptr(), st))),
-            {("concat_fwd_kernel", v), ("concat_bwd_kernel", v)}, [(y, NAN), (gx, NAN)])
-    _assert_bitwise(f"{name}: forward", y, x.repeat_interleave(2, 1).repeat_interleave(2, 2))
-    _assert_bitwise(f"{name}: backward", gx, gy.double().reshape(n, h, 2, w, 2, c).sum((2, 4)).to(dt))
+    y, gx = nan(n, 2 * h, 2 * w, c, dtype=dt), nan(n, h, w, c, dtype=dt)
+    v = "8" if c % 8 == 0 else "1"
+    traced(name, lambda: (_lib.check(lib.pcb_upsample2x_forward(x.data_ptr(), code, n, h, w, c, y.data_ptr(), st)),
+                          _lib.check(lib.pcb_upsample2x_backward(gy.data_ptr(), code, n, h, w, c, gx.data_ptr(), st))),
+            _route(name, {("concat_fwd_kernel", v), ("concat_bwd_kernel", v)}), [(y, NAN), (gx, NAN)])
+    assert_bitwise(f"{name}: forward", y, x.repeat_interleave(2, 1).repeat_interleave(2, 2))
+    assert_bitwise(f"{name}: backward", gx, gy.double().reshape(n, h, 2, w, 2, c).sum((2, 4)).to(dt))
 
 
 # ------------------------------------------------------------------------------------------------ mask planes
@@ -501,17 +401,17 @@ def test_mask_planes_exact(name):
     if "up" not in sp:                                                  # planes from a dense NCHW mask
         m = _ints(gen, n, c, h, w, lo=-1, hi=1).float() * 0.5
         planes = torch.full((c, n, h, w), 77, dtype=torch.uint8, device="cuda")
-        _traced(name, lambda: _lib.check(lib.pcb_mask_planes_from_dense(m.data_ptr(), n, c, h, w, planes.data_ptr(), st)),
-                {("mask_from_dense_kernel", None)}, [(planes, 77)])
-        _assert_bitwise(f"{name}: planes", planes, (m != 0).to(torch.uint8).permute(1, 0, 2, 3))
+        traced(name, lambda: _lib.check(lib.pcb_mask_planes_from_dense(m.data_ptr(), n, c, h, w, planes.data_ptr(), st)),
+                _route(name, {("mask_from_dense_kernel", None)}), [(planes, 77)])
+        assert_bitwise(f"{name}: planes", planes, (m != 0).to(torch.uint8).permute(1, 0, 2, 3))
         return
     up, ctot, c0 = sp["up"], sp["ctot"], sp["c0"]
     plane = (torch.rand(n, h >> up, w >> up, generator=gen, device="cuda") > 0.3).to(torch.uint8)
-    dst = _nan(n, ctot, h, w)
-    _traced(name, lambda: _lib.check(lib.pcb_mask_plane_to_dense(plane.data_ptr(), n, h, w, up, dst.data_ptr(), ctot, c0, c, st)),
-            {("mask_to_dense_kernel", None)}, [(dst, NAN)])
+    dst = nan(n, ctot, h, w)
+    traced(name, lambda: _lib.check(lib.pcb_mask_plane_to_dense(plane.data_ptr(), n, h, w, up, dst.data_ptr(), ctot, c0, c, st)),
+            _route(name, {("mask_to_dense_kernel", None)}), [(dst, NAN)])
     full = plane.float().repeat_interleave(1 << up, 1).repeat_interleave(1 << up, 2)[:, None].expand(n, c, h, w)
-    _assert_bitwise(f"{name}: channels [c0, c0 + c)", dst[:, c0:c0 + c], full)
+    assert_bitwise(f"{name}: channels [c0, c0 + c)", dst[:, c0:c0 + c], full)
     rest = torch.cat([dst[:, :c0], dst[:, c0 + c:]], dim=1)
     assert bool(rest.isnan().all()), f"{name}: wrote outside its channels"
 
@@ -526,17 +426,18 @@ def test_l1_mean_vs_fp64(name):
     x = torch.randn(numel, generator=gen, device="cuda").to(dt)
     x[::7] = 0                                                          # sign(0) = 0
     gscale = float(torch.tensor(1.0 / numel, dtype=torch.float32))
-    loss, scratch, gx = _nan(1), torch.zeros(1, dtype=torch.float64, device="cuda") + 5, _nan(numel, dtype=dt)
-    _traced(name, lambda: (_lib.check(lib.pcb_l1_mean_forward(x.data_ptr(), code, numel, loss.data_ptr(), scratch.data_ptr(), st)),
-                           _lib.check(lib.pcb_l1_mean_backward(x.data_ptr(), code, numel, gscale, gx.data_ptr(), st))),
-            {("l1_sum_kernel", None), ("l1_finish_kernel", None), ("l1_bwd_kernel", None)}, [(loss, NAN), (scratch, 5.0), (gx, NAN)])
+    loss, scratch, gx = nan(1), torch.zeros(1, dtype=torch.float64, device="cuda") + 5, nan(numel, dtype=dt)
+    traced(name, lambda: (_lib.check(lib.pcb_l1_mean_forward(x.data_ptr(), code, numel, loss.data_ptr(), scratch.data_ptr(), st)),
+                          _lib.check(lib.pcb_l1_mean_backward(x.data_ptr(), code, numel, gscale, gx.data_ptr(), st))),
+            _route(name, {("l1_sum_kernel", None), ("l1_finish_kernel", None), ("l1_bwd_kernel", None)}),
+            [(loss, NAN), (scratch, 5.0), (gx, NAN)])
     a = x.double().abs()
     nsm = torch.cuda.get_device_properties(0).multi_processor_count
     grid = max(1, min(math.ceil(numel / (256 * 16)), 16 * nsm))
     L = math.ceil(numel / (grid * 256)) + 14
     ref = a.sum() / numel
-    _assert_within(f"{name}: loss", loss[0], ref, L * U * ref + U * ref)
-    _assert_bitwise(f"{name}: backward", gx, (torch.sign(x.double()) * gscale).float().to(dt))
+    assert_within(f"{name}: loss", loss[0], ref, L * U * ref + U * ref)
+    assert_bitwise(f"{name}: backward", gx, (torch.sign(x.double()) * gscale).float().to(dt))
 
 
 # ------------------------------------------------------------------------------------------------ SGD
@@ -552,9 +453,9 @@ def test_sgd_vs_torch_fp64(name):
     g = torch.randn(numel, generator=gen, device="cuda")
     buf = torch.randn(numel, generator=gen, device="cuda") if mom else None
     p0, b0 = p.clone(), (buf.clone() if buf is not None else None)
-    _traced(name, lambda: _lib.check(lib.pcb_sgd_step_scaled(p.data_ptr(), g.data_ptr(), None if buf is None else buf.data_ptr(), numel,
-                                                             lr, mom, wd, nest, first, gs, st)),
-            {("sgd_kernel", None)}, [(p, p0)] + ([(buf, b0)] if buf is not None else []))
+    traced(name, lambda: _lib.check(lib.pcb_sgd_step_scaled(p.data_ptr(), g.data_ptr(), None if buf is None else buf.data_ptr(), numel,
+                                                            lr, mom, wd, nest, first, gs, st)),
+            _route(name, {("sgd_kernel", None)}), [(p, p0)] + ([(buf, b0)] if buf is not None else []))
     # torch.optim.SGD in fp64 on the same values
     p64 = torch.nn.Parameter(p0.double())
     p64.grad = g.double() * gs
@@ -568,9 +469,9 @@ def test_sgd_vs_torch_fp64(name):
     if mom:
         b = d if first else mom * b0.double() + d
         e_b = e_d + (0 if first else 2 * U * (mom * b0.double().abs() + d.abs()))
-        _assert_within(f"{name}: momentum buffer", buf, opt.state[p64]["momentum_buffer"], e_b)
+        assert_within(f"{name}: momentum buffer", buf, opt.state[p64]["momentum_buffer"], e_b)
         dn = d + mom * b if nest else b
         e_dn = (e_d + mom * e_b + 2 * U * (d.abs() + mom * b.abs())) if nest else e_b
     else:
         dn, e_dn = d, e_d
-    _assert_within(f"{name}: parameters", p, p64.detach(), lr * e_dn + 2 * U * (P.abs() + lr * dn.abs()))
+    assert_within(f"{name}: parameters", p, p64.detach(), lr * e_dn + 2 * U * (P.abs() + lr * dn.abs()))
