@@ -7,7 +7,7 @@ shape-general kernels (conv_generic.cu).  Three sets of cases:
 
   * one per dense descriptor of tests/golden/conv_dispatch.json (the layers the workloads run), batch capped at 2 -- or the
     smallest batch above that whose routes (pcb_debug_conv_routes) equal those of the uncapped descriptor;
-  * hand cases for what production reaches rarely or never: gather row-halo groups, ragged M, two parts (one 2x-upsampled) on
+  * hand cases for what production reaches rarely or never: a stride-1 gather layer, ragged M, two parts (one 2x-upsampled) on
     a non-power-of-two grid, dilation; row-packed layers with cin 1 / 3 / 8 and kw 3 / 5 / 7; stems with holes, no_guard, cout
     32 / 40 and a grid that is not a whole number of tiles; RGB tails with 1 / 3 / 4 image channels, 32 / 64 upsampled channels
     and holes in both parts; small-Cout layers at 80 packed channels, ragged h and w, 1x1, an upsampled part; the stride-2 data
@@ -164,9 +164,9 @@ def _fixture_cases():
 
 P_ = _part
 HAND_CASES = {
-    # cp.async gather kernels: row-halo groups (stride 1, w a multiple of 8, not a power of two), ragged M (143 pixels), two parts
-    # with the first 2x-upsampled on a 24 x 40 grid, dilation 2; all with holes, so the gather weight gradient reads tap masks
-    "gather_halo_holes": _case(2, 24, 40, [P_(64, mask=True)], 64, route=("gather", "gather", "gather")),
+    # cp.async gather kernels: stride 1 on a 24 x 40 grid (w a multiple of 8, not a power of two), ragged M (143 pixels), two
+    # parts with the first 2x-upsampled on a 24 x 40 grid, dilation 2; all with holes, so the gather weight gradient reads tap masks
+    "gather_s1_w40_holes": _case(2, 24, 40, [P_(64, mask=True)], 64, route=("gather", "gather", "gather")),
     "gather_ragged_m_cout96": _case(1, 13, 11, [P_(64, mask=True)], 96, route=("gather", "gather", "gather")),
     "gather_two_parts_up": _case(2, 24, 40, [P_(64, 1, True), P_(32, mask=True)], 64, route=("gather", "gather", "gather")),
     "gather_dil2": _case(2, 20, 28, [P_(64, mask=True)], 64, dil=2, route=("gather", "gather", "gather")),

@@ -6,17 +6,18 @@ reference is a direct sum).  Two sets of cases:
     run: dw4 at dilations up to 29, dw3 at stride 2, the small GPU test cases), batch capped at 2;
   * hand cases for the paths production does not reach: holes on dw3 (one msum plane or c of them, a half-resolution hole
     plane, large values under the holes), strided channel views, awkward channel counts (8, 40, 296, 2048), dw4 segment,
-    x-tile and dilation-phase edges in both storage types, a "valid" 3x3 on dw3, and the first-generation kernels (k5, k7,
-    kh != kw, the stride-3 data gradient).
+    x-tile and dilation-phase edges in both storage types, a "valid" 3x3 on dw3, and the depthwise shapes the family leaves to
+    the shape-general kernels of conv_generic.cu (k5, k7, kh != kw, stride 3).
 
 Each case asserts the route it covers from the kernel names of a torch.profiler trace (kernel_harness.traced), then checks:
 
   * mask pass: msum and newmask equal the fp64 box sums exactly (times cin with same_holes); a plain convolution leaves both
     untouched;
   * forward, data gradient, weight gradient (zeroing and accumulating), all outputs prefilled with NaN and channels past c of
-    a strided view prefilled with a sentinel that must survive;
+    a strided view prefilled with a sentinel that must survive -- except in y on the generic route, whose channels past
+    rup(c, 8) are no outputs and may be zeroed (the header's contract; the generic forward zero-fills them);
   * the fused BatchNorm statistics and the eval-mode affine + activation epilogue where pcb_conv_fuses_bn_stats says the
-    kernel fuses them, and their refusal where it does not (first generation).
+    kernel fuses them, and their refusal where it does not (the generic route).
 
 Integer regime (every case).  x, w, dc are integers of magnitude <= 4 and the bias a multiple of 1/8, all exact in bf16.  Every
 partial sum stays below 2^24 (the largest is a weight gradient over 2 x 256 x 256 pixels: 2^17 * 16 = 2^21), so fp32
@@ -42,8 +43,8 @@ import torch
 import torch.nn.functional as F
 from torch.nn.grad import conv2d_input, conv2d_weight
 
-from kernel_harness import (HOLE_VALUE, act_ref, assert_bitwise, assert_within, conv_dispatch_cases, holes, nchw, sentinel_kept,
-                            strided, traced)
+from kernel_harness import (HOLE_VALUE, SENTINEL, act_ref, assert_bitwise, assert_within, conv_dispatch_cases, holes, nchw,
+                            sentinel_kept, strided, traced)
 from text_segmentation_image_inpainting_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -53,27 +54,27 @@ SLOPE = 0.2
 ACTS = (_lib.ACT_NONE, _lib.ACT_RELU, _lib.ACT_LEAKY, _lib.ACT_RELU6)
 DTYPES = {"bf16": (torch.bfloat16, _lib.PCB_BF16), "f32": (torch.float32, _lib.PCB_F32)}
 
-# the kernels of each generation, per direction (forward, data gradient, weight gradient)
+# the kernels of each route, per direction (forward, data gradient, weight gradient)
 KERNELS = {"dw4": ("dw4_s1_kernel", "dw4_s1_kernel", "dw4_s1_wgrad_kernel"),
            "dw3": ("dw3_fwd_kernel", "dw3_dgrad_kernel", "dw3_wgrad_kernel"),
-           "gen1": ("dw_fwd_kernel", "dw_dgrad_kernel", "dw_wgrad_kernel")}
+           "generic": ("generic_fwd_kernel", "generic_dgrad_kernel", "generic_wgrad_kernel")}
 
 
 def _case(n, h, w, c, k=3, s=1, pad=None, dil=1, dtype="bf16", holes=False, mask_up=0, same_holes=False, plain=None,
           cs=None, route=None):
-    """cs: channel strides (x, y, dc, dx), default c.  route: the generation of (forward, data gradient, weight gradient);
-    default: what the depthwise dispatch documents (dw4 for plain 3x3 stride 1 with padding == dilation, dw3 for other 3x3 --
-    first generation for a data gradient at a stride that is not a power of two -- and first generation otherwise)."""
+    """cs: channel strides (x, y, dc, dx), default c.  route: the kernels of (forward, data gradient, weight gradient);
+    default: what the depthwise dispatch documents (dw4 for plain 3x3 stride 1 with padding == dilation, dw3 for other 3x3 at
+    a power-of-two stride, the generic kernels otherwise)."""
     kh, kw = (k, k) if isinstance(k, int) else k
     ph, pw = (dil * (kh - 1) // 2, dil * (kw - 1) // 2) if pad is None else ((pad, pad) if isinstance(pad, int) else pad)
     plain = (not holes) if plain is None else plain
     if route is None:
-        if (kh, kw) != (3, 3):
-            route = ("gen1",) * 3
+        if (kh, kw) != (3, 3) or s & (s - 1):
+            route = ("generic",) * 3
         elif s == 1 and ph == pw == dil and plain and not holes:
             route = ("dw4",) * 3
         else:
-            route = ("dw3", "gen1" if s & (s - 1) else "dw3", "dw3")
+            route = ("dw3",) * 3
     return dict(n=n, h=h, w=w, c=c, kh=kh, kw=kw, s=s, ph=ph, pw=pw, dil=dil, dtype=dtype, holes=holes, mask_up=mask_up,
                 same_holes=same_holes, plain=plain, cs=tuple(cs) if cs else (c,) * 4, route=route)
 
@@ -109,7 +110,7 @@ HAND_CASES = {
     # strided channel views of x, y, dc and dx on every generation
     "dw4_strided_views": _case(2, 33, 45, 64, 3, 1, 2, 2, "bf16", cs=(80, 72, 96, 88)),
     "dw3_strided_views_holes_s2": _case(2, 26, 30, 48, 3, 2, 1, 1, "f32", holes=True, cs=(56, 64, 72, 80)),
-    "gen1_k5_strided_views": _case(1, 20, 22, 32, 5, 1, 2, 1, "bf16", holes=True, cs=(40, 48, 56, 64)),
+    "generic_k5_strided_views": _case(1, 20, 22, 32, 5, 1, 2, 1, "bf16", holes=True, cs=(40, 48, 56, 64)),
     # awkward channel counts: c 296 (37 vectors: dw3 falls back to 32-wide chunks, the last with 5; dw4 cq 2),
     # c 40 (dw3 cvb 5 x pl 51; dw4 cq 10 x xt 25, three x tiles, two row segments), c 8, c 2048 (the largest eligible)
     "dw3_c296_s2": _case(2, 30, 34, 296, 3, 2, 1, 1, "bf16"),
@@ -120,7 +121,7 @@ HAND_CASES = {
     "dw3_c8_holes_s2": _case(2, 21, 23, 8, 3, 2, 1, 1, "f32", holes=True),
     "dw4_c2048": _case(2, 10, 12, 2048, 3, 1, 2, 2, "bf16"),
     "dw3_c2048_holes_s2": _case(1, 9, 11, 2048, 3, 2, 1, 1, "bf16", holes=True, same_holes=True),
-    "gen1_k5_c2048": _case(1, 7, 9, 2048, 5, 1, 2, 1, "bf16"),
+    "generic_k5_c2048": _case(1, 7, 9, 2048, 5, 1, 2, 1, "bf16"),
     # dw4 edges: the fp32 template (3-row load queue) with three row segments (the last 6 rows) and a ragged x tile; phases
     # of unequal length with 4 phases per block; dilation >= h (phases of 0 or 1 rows); w < 256 / cq; h = 1; w = 1
     "dw4_f32_nseg3_ragged_x": _case(2, 70, 40, 64, 3, 1, 1, 1, "f32"),
@@ -134,13 +135,12 @@ HAND_CASES = {
     "dw4_f32_1x1": _case(2, 1, 1, 64, 3, 1, 1, 1, "f32"),
     # a "valid" 3x3 at stride 1 (padding != dilation) runs on dw3
     "dw3_valid_s1": _case(2, 20, 22, 64, 3, 1, 0, 1, "bf16"),
-    # first generation: weight gradient in passes of 9 taps with a partial last pass (25, 49 taps), kh != kw with
-    # pad_h != pad_w, and the stride-3 3x3 whose data gradient leaves dw3
-    "gen1_k5_holes": _case(2, 23, 29, 48, 5, 1, 2, 1, "bf16", holes=True),
-    "gen1_k7_s2_f32": _case(2, 30, 26, 24, 7, 2, 3, 1, "f32"),
-    "gen1_k3x5_p1x2_holes_same": _case(2, 19, 21, 32, (3, 5), 1, (1, 2), 1, "bf16", holes=True, same_holes=True),
-    "gen1_k5x3_p4x2_d2_f32": _case(2, 24, 20, 16, (5, 3), 1, (4, 2), 2, "f32"),
-    "s3_dgrad_gen1_holes": _case(2, 25, 28, 32, 3, 3, 1, 1, "bf16", holes=True),
+    # the generic kernels: 25 and 49 taps, kh != kw with pad_h != pad_w, and a 3x3 at stride 3
+    "generic_k5_holes": _case(2, 23, 29, 48, 5, 1, 2, 1, "bf16", holes=True),
+    "generic_k7_s2_f32": _case(2, 30, 26, 24, 7, 2, 3, 1, "f32"),
+    "generic_k3x5_p1x2_holes_same": _case(2, 19, 21, 32, (3, 5), 1, (1, 2), 1, "bf16", holes=True, same_holes=True),
+    "generic_k5x3_p4x2_d2_f32": _case(2, 24, 20, 16, (5, 3), 1, (4, 2), 2, "f32"),
+    "s3_generic_holes": _case(2, 25, 28, 32, 3, 3, 1, 1, "bf16", holes=True),
 }
 CASES = {**_fixture_cases(), **HAND_CASES}
 
@@ -235,7 +235,7 @@ def test_dwconv_vs_fp64(name):
     ycs, dcs, dxcs = sp["cs"][1:]
     assert lib.pcb_conv_uses_tensor_cores(cref) == 0 and lib.pcb_pconv_workspace(cref) == 0
     fuses = lib.pcb_conv_fuses_bn_stats(cref)
-    assert fuses == lib.pcb_conv_fuses_affine_act(cref) == int(sp["route"][0] != "gen1"), f"{name}: fused-epilogue query"
+    assert fuses == lib.pcb_conv_fuses_affine_act(cref) == int(sp["route"][0] != "generic"), f"{name}: fused-epilogue query"
 
     def ints(*shape):
         return torch.randint(-INT_RANGE, INT_RANGE + 1, shape, generator=dgen, device=dev).to(torch.float32)
@@ -264,8 +264,13 @@ def test_dwconv_vs_fp64(name):
 
     want = {KERNELS[r][i] for i, r in enumerate(sp["route"])}
 
+    def y_tail_kept(y):
+        """channels past c (a multiple of 8) keep the sentinel; the generic forward may zero them instead"""
+        past = y[..., c:]
+        return bool(((past == SENTINEL) | ((past == 0) & (sp["route"][0] == "generic"))).all())
+
     def check(records):
-        ran = {k for k, _ in records if k.startswith("dw")}
+        ran = {k for k, _ in records if k.startswith(("dw", "generic"))}
         assert ran == want, f"{name}: ran {sorted(ran)}, the case covers {sorted(want)}"
     traced(name, run, check, state)
 
@@ -287,7 +292,7 @@ def test_dwconv_vs_fp64(name):
         q = (S / torch.where(s == 0, torch.ones_like(s), s)).float().double()
         v = torch.where(s == 0, torch.zeros_like(S), q + b).float()
     assert_bitwise(f"{name}: forward", y[..., :c].permute(0, 3, 1, 2), v.to(dt))
-    assert sentinel_kept(y, c), f"{name}: forward wrote past c"
+    assert y_tail_kept(y), f"{name}: forward wrote past c"
 
     # data gradient: m * S, zero under the holes
     G = nchw(dc, c)
@@ -320,7 +325,7 @@ def test_dwconv_vs_fp64(name):
     store = 2.0 ** -8 if dt == torch.bfloat16 else 0.0
 
     def check_y(tag, y, v, e):
-        assert sentinel_kept(y, c), f"{name}: {tag} wrote past c"
+        assert y_tail_kept(y), f"{name}: {tag} wrote past c"
         assert_within(f"{name}: {tag}", nchw(y, c), v, e + store * (v.abs() + e))
 
     scale = torch.rand(c, generator=dgen, device=dev) + 0.5

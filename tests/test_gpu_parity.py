@@ -105,22 +105,14 @@ def test_bn_act_and_running_stats(c, dev):
             bn.eval(); ref.eval()
             assert relerr(ops.bn_act(xd.detach(), bn, act), act(ref(xq)) if act else ref(xq)) <= tol
             bn.train()
-            if c >= 256:                  # the two-launch path must agree with the one-launch path
-                ops.set_bn_small_kernel(False)
-                try:
-                    bn.zero_grad(set_to_none=True)
-                    x2 = xd.detach().clone().requires_grad_(True)
-                    ops.bn_act(x2, bn, act).backward(gy.to(dev).to(dtype))
-                    assert relerr(x2.grad, xd.grad) <= (1e-5 if dtype == F32 else 1e-2) and relerr(bn.weight.grad, ref.weight.grad) <= tol
-                finally:
-                    ops.set_bn_small_kernel(True)
 
 
 @pytest.mark.parametrize("shape", [(64, 128, 3, 1, 1, (2, 24, 20)), (64, 64, 3, 1, 1, (2, 8, 128)), (128, 256, 3, 2, 1, (2, 32, 32)),
                                    (192, 320, 1, 1, 0, (1, 16, 16))])
-def test_bn_statistics_fused_into_conv_epilogue(shape, dev):
+def test_bn_statistics_fused_into_conv_epilogue_vs_separate_pass(shape, dev):
     """PartialConv -> BatchNorm(train) -> LeakyReLU block: the per-channel sums accumulated in the tensor-core epilogue
-    (pcb_pconv_forward_bn) against the separate statistics pass (ops.set_fused_bn_stats(False)) and against the oracle."""
+    (pcb_pconv_forward_bn) against the separate statistics pass (the same weights through ops.partial_conv and then ops.bn_act
+    without a handoff) and against the oracle."""
     from gpu_cases import blob
     from oracle.detfill import det_fill_state_dict, det_tensor
     from text_segmentation_image_inpainting_b200 import ops
@@ -133,21 +125,22 @@ def test_bn_statistics_fused_into_conv_epilogue(shape, dev):
     gy = None
     res = {}
     for fused in (True, False):
-        ops.set_fused_bn_stats(fused)
-        try:
-            blk.load_state_dict(sd)
-            m = blk.to(dev).train()
-            m.zero_grad(set_to_none=True)
-            xd = x.to(dev).contiguous(memory_format=torch.channels_last).requires_grad_(True)
+        blk.load_state_dict(sd)
+        m = blk.to(dev).train()
+        m.zero_grad(set_to_none=True)
+        xd = x.to(dev).contiguous(memory_format=torch.channels_last).requires_grad_(True)
+        if fused:
             y, _ = m((xd, mask.to(dev)))
-            if gy is None:
-                gy = det_tensor("fbn.gy", tuple(y.shape)).to(BF)
-            y.backward(gy.to(dev))
-            torch.cuda.synchronize()
-            res[fused] = (y.detach().float().cpu(), xd.grad.float().cpu(), m[1].bn_act[0].running_mean.cpu().clone(),
-                          m[1].bn_act[0].running_var.cpu().clone(), m[1].bn_act[0].weight.grad.cpu().clone(), m[0].feature_conv.weight.grad.cpu().clone())
-        finally:
-            ops.set_fused_bn_stats(True)
+        else:
+            fc, bn_act = m[0].feature_conv, m[1].bn_act
+            y, _ = ops.partial_conv(xd, mask.to(dev), fc.weight, fc.bias, fc.stride, fc.padding, fc.dilation, fc.groups, same_holes=True)
+            y = ops.bn_act(y, bn_act[0], bn_act[1])
+        if gy is None:
+            gy = det_tensor("fbn.gy", tuple(y.shape)).to(BF)
+        y.backward(gy.to(dev))
+        torch.cuda.synchronize()
+        res[fused] = (y.detach().float().cpu(), xd.grad.float().cpu(), m[1].bn_act[0].running_mean.cpu().clone(),
+                      m[1].bn_act[0].running_var.cpu().clone(), m[1].bn_act[0].weight.grad.cpu().clone(), m[0].feature_conv.weight.grad.cpu().clone())
     assert _pipeline_clean()
     for a, b in zip(res[True], res[False]):
         assert relerr(a, b) <= 2e-2, relerr(a, b)

@@ -97,7 +97,7 @@ PCB_API int pcb_conv_weight_refresh(const pcb_conv *c, const float *w_master_krs
 static bool fuses_epilogue(const pcb_conv *c) {
     if (!c) return false;
     const Family f = family_of(c);
-    return (f == FAMILY_DW && pcb_dw_fuses_epilogue(c)) || (f == FAMILY_TC && pcb_tc_fuses_epilogue(c));
+    return f == FAMILY_DW || (f == FAMILY_TC && pcb_tc_fuses_epilogue(c));
 }
 
 // 1 when the forward kernel this problem dispatches to can accumulate the per-channel BatchNorm statistics of its output itself

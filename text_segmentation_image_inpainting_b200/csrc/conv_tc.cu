@@ -73,10 +73,9 @@ struct TcParams {
     int n, h, w, cin, cout, kh, kw, stride, pad_h, pad_w, dil, ho, wo;
     int m_total;              // GEMM M
     int nparts, no_guard, rowpack;
-    int hg;                   // row-halo mode: input pixels staged per group of 8 output pixels = 8 + (kw-1)*dil
-    int ring_a, ring_b;       // smem ring depths (A items / weight tiles)
-    int ktap;                 // K extent of one tap (sum of part kext); rowpack: 64 per kernel row
     int ncols;                // GEMM N extent covered by the grid (multiple of BLOCK_N)
+    int ring_a, ring_b;       // smem ring depths (A items / weight tiles): 8-byte aligned, the gather kernel loads them as a pair
+    int ktap;                 // K extent of one tap (sum of part kext); rowpack: 64 per kernel row
     TcPart parts[TC_MAX_PARTS];
     // fwd epilogue
     const float *bias; const float *msum; bf16 *y; int y_cstride;
@@ -397,31 +396,22 @@ template <int R> __device__ __forceinline__ void zero_acc(float (&a)[R]) {
 //   warp  12    B producer  : weight tiles by TMA (SWIZZLE_128B)
 // so the producers' per-tile latencies (mask-word loads, pipeline fill) of tile i+1 overlap the epilogue of tile i.
 //
-// Two A-operand layouts:
-//   HALO = false : per tap, a [128 pixel x 64 channel] tile in the 128B-swizzled K-major layout (any stride / dilation;
-//                  also the row-packed small-Cin mode: K block = kernel row, chunk = tap column).
-//   HALO = true  : stride-1 layers.  Per kernel ROW, each group of 8 consecutive output pixels stages its
-//                  8 + (kw-1)*dil input pixels once in the canonical NO-SWIZZLE K-major layout
-//                  addr(slot, chunk) = chunk*LBO + slot*16; the kw taps of the row are kw wgmma descriptors whose start
-//                  address is shifted by tap*dil slots (SBO = HG*16 between 8-row groups): kw x fewer gathers.
+// A operand: per tap, a [128 pixel x 64 channel] tile in the 128B-swizzled K-major layout (any stride / dilation; also the
+// row-packed small-Cin mode: K block = kernel row, chunk = tap column).
 // -------------------------------------------------------------------------------------------------
-constexpr int HALO_MAX_HG = 12;
 constexpr int PERSIST_THREADS = 4 * 32 + MMA_THREADS + 32;
 constexpr int MAX_RING = 8;
 
-template <int BLOCK_N, int MODE, bool HALO>
+template <int BLOCK_N, int MODE>
 __global__ void __launch_bounds__(PERSIST_THREADS, 1)
 pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUtensorMap tmap_w) {
     constexpr int B_STAGE_BYTES = BLOCK_N * 128;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = align1024(ptx::smem_u32(smem_raw));
     const int SA = P.ring_a, SB = P.ring_b;
-    const int HG = P.hg;
-    const uint32_t LBO = 16u * (16u * HG + 1u);                       // halo: byte distance between 8-channel chunks
-    const uint32_t A_STAGE = HALO ? ((8u * LBO + 127u) & ~127u) : static_cast<uint32_t>(A_STAGE_BYTES);
     const uint32_t sB = smem_base;
     const uint32_t sA = sB + SB * B_STAGE_BYTES;                      // stays 1024-aligned (B stages are multiples of 1024)
-    const uint32_t sBar = (sA + SA * A_STAGE + 15u) & ~15u;
+    const uint32_t sBar = (sA + SA * A_STAGE_BYTES + 15u) & ~15u;
     const uint32_t bar_full_a = sBar, bar_empty_a = sBar + 8 * MAX_RING;
     const uint32_t bar_full_b = sBar + 16 * MAX_RING, bar_empty_b = sBar + 24 * MAX_RING;
     const uint32_t s_stat_addr = sBar + 32 * MAX_RING;                                  // BatchNorm statistics slices
@@ -433,7 +423,6 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
     const int np = (MODE == 0) ? P.nparts : 1;
     const int n_tiles = P.ncols / BLOCK_N;
     const int num_tiles = ((P.m_total + BLOCK_M - 1) / BLOCK_M) * n_tiles;
-    const int nB = HALO ? P.kw : 1;                                   // weight tiles consumed per A item
 
     // dgrad: N tiles none of whose parts wants a gradient are skipped (same decision in every role)
     auto tile_active = [&](int n0) -> bool {
@@ -463,29 +452,18 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
         bool dead = false;
         // Tap-validity words of the NEXT tile are loaded while the current tile's items stream (software pipelining across
         // tiles): their global-load latency would otherwise stall all gathers at the start of every tile.
-        constexpr int NW = HALO ? HALO_MAX_HG : 8;
-        uint64_t wnext[TC_MAX_PARTS][NW];
+        uint64_t wnext[TC_MAX_PARTS][8];
         auto issue_mask_loads = [&](int tl) {
 #pragma unroll
             for (int p = 0; p < TC_MAX_PARTS; ++p)
 #pragma unroll
-                for (int i = 0; i < NW; ++i) wnext[p][i] = 0ull;
+                for (int i = 0; i < 8; ++i) wnext[p][i] = 0ull;
             if (MODE != 0 || tl >= num_tiles) return;
             const int tm0 = (tl / n_tiles) * BLOCK_M;
 #pragma unroll
-            for (int i = 0; i < NW; ++i) {
-                int idx;
-                if (HALO) {
-                    if (i >= HG) continue;
-                    const int S = r0 + 16 * i;
-                    const int g = S / HG, sl = S - g * HG;
-                    const int tcs = sl > 7 ? (sl - 7 + P.dil - 1) / P.dil : 0;
-                    idx = tm0 + g * 8 + (sl - tcs * P.dil);
-                    if (tm0 + g * 8 >= P.m_total) continue;
-                } else {
-                    idx = tm0 + r0 + 16 * i;
-                    if (idx >= P.m_total) continue;
-                }
+            for (int i = 0; i < 8; ++i) {
+                const int idx = tm0 + r0 + 16 * i;
+                if (idx >= P.m_total) continue;
 #pragma unroll
                 for (int p = 0; p < TC_MAX_PARTS; ++p)
                     if (p < P.nparts) wnext[p][i] = __ldg(P.parts[p].tapmask + idx);
@@ -494,184 +472,106 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
         issue_mask_loads(blockIdx.x);
         for (int tile = blockIdx.x; tile < num_tiles && !dead; tile += gridDim.x) {
             const int m0 = (tile / n_tiles) * BLOCK_M, n0 = (tile % n_tiles) * BLOCK_N;
-            uint64_t wcur[TC_MAX_PARTS][NW];
+            uint64_t wcur[TC_MAX_PARTS][8];
 #pragma unroll
             for (int p = 0; p < TC_MAX_PARTS; ++p)
 #pragma unroll
-                for (int i = 0; i < NW; ++i) wcur[p][i] = wnext[p][i];
+                for (int i = 0; i < 8; ++i) wcur[p][i] = wnext[p][i];
             issue_mask_loads(tile + gridDim.x);
             if (!tile_active(n0)) continue;
-            if (HALO) {
-                int ph[HALO_MAX_HG];                              // row coordinate of the slot at kernel row 0
-                int cterm[TC_MAX_PARTS][HALO_MAX_HG];             // image base + column*cstride + chunk*8 (element offset)
-                uint32_t vb[TC_MAX_PARTS][HALO_MAX_HG];           // bit tr = slot valid (bounds [+ hole]) for kernel row tr
+            const uint32_t sw = static_cast<uint32_t>((chunk ^ (r0 & 7)) << 4);   // (r & 7) == (r0 & 7) for all rows of a thread
+            int ph[8], pw[8];
+            int ibase[TC_MAX_PARTS][8];                 // element offset of the row's image inside each source (+ chunk)
+            bool prow[8];
+            const int ls = 31 - __clz(P.stride);        // dgrad: stride is a power of two on this path (host-checked)
 #pragma unroll
-                for (int i = 0; i < HALO_MAX_HG; ++i) {
-                    ph[i] = 0;
+            for (int i = 0; i < 8; ++i) {
+                const int m = m0 + r0 + 16 * i;
+                prow[i] = m < P.m_total;
+                const int mm = prow[i] ? m : 0;
+                const int nn = mm / plane, rem = mm - nn * plane;
+                const int hh = rem / pwid, ww = rem - hh * pwid;
+                if (MODE == 0) {
+                    ph[i] = hh * P.stride - P.pad_h; pw[i] = ww * P.stride - P.pad_w;
 #pragma unroll
-                    for (int p = 0; p < TC_MAX_PARTS; ++p) { vb[p][i] = 0; cterm[p][i] = 0; }
-                    if (i >= HG) continue;
-                    const int S = r0 + 16 * i;
-                    const int g = S / HG, sl = S - g * HG;
-                    const int m = m0 + g * 8;               // first pixel of the group (groups never straddle image rows)
-                    const bool ok = m < P.m_total;
-                    const int mm = ok ? m : 0;
-                    const int nn = mm / plane, rem = mm - nn * plane;
-                    const int hh = rem / pwid, ww = rem - hh * pwid;
-                    if (MODE == 0) {
-                        ph[i] = hh - P.pad_h;
-                        const int col = ww - P.pad_w + sl;
-                        // the (pixel j of the group, tap column tc) pair that looks at this slot: sl == j + tc*dil
-                        const int tcs = sl > 7 ? (sl - 7 + P.dil - 1) / P.dil : 0;
+                    for (int p = 0; p < TC_MAX_PARTS; ++p)
+                        ibase[p][i] = (p < P.nparts) ? nn * (P.h >> P.parts[p].xup) * (P.w >> P.parts[p].xup) * P.parts[p].cstride + chunk * 8 : 0;
+                } else {
+                    ph[i] = hh + P.pad_h; pw[i] = ww + P.pad_w;
+                    ibase[0][i] = nn * P.ho * P.wo * P.dc_cstride + chunk * 8;
 #pragma unroll
-                        for (int p = 0; p < TC_MAX_PARTS; ++p) {
-                            if (p >= P.nparts || !ok) continue;
-                            const TcPart &pt = P.parts[p];
-                            const uint64_t word = wcur[p][i];
-                            uint32_t bits = 0;
-                            for (int tr = 0; tr < P.kh; ++tr) bits |= static_cast<uint32_t>((word >> (tr * P.kw + tcs)) & 1ull) << tr;
-                            vb[p][i] = bits;
-                            const int colc = min(max(col, 0), P.w - 1) >> pt.xup;   // clamped: only dereferenced when valid
-                            cterm[p][i] = (nn * (P.h >> pt.xup) * (P.w >> pt.xup) + colc) * pt.cstride + chunk * 8;
-                        }
-                    } else {
-                        ph[i] = hh + P.pad_h;
-                        const int col = ww + P.pad_w - (P.kw - 1) * P.dil + sl;
-                        const bool cok = ok && col >= 0 && col < P.wo;
-                        uint32_t bits = 0;
-                        for (int tr = 0; tr < P.kh; ++tr) { const int hi = ph[i] - tr * P.dil; bits |= (cok && hi >= 0 && hi < P.ho ? 1u : 0u) << tr; }
-                        vb[0][i] = bits;
-                        cterm[0][i] = (nn * P.ho * P.wo + min(max(col, 0), P.wo - 1)) * P.dc_cstride + chunk * 8;
-                    }
+                    for (int p = 1; p < TC_MAX_PARTS; ++p) ibase[p][i] = 0;
                 }
+            }
+            uint64_t tmv[TC_MAX_PARTS][8];              // per-row tap-validity bits (bounds + holes), prefetched one tile ahead
+#pragma unroll
+            for (int p = 0; p < TC_MAX_PARTS; ++p)
+#pragma unroll
+                for (int i = 0; i < 8; ++i) tmv[p][i] = wcur[p][i];
+
+            auto push = [&](const bf16 *base, const int (&off)[8], const bool (&ok)[8]) -> bool {
+                const int s = it % SA;
+                if (!ptx::mbar_wait(bar_empty_a + 8 * s, ((it / SA) & 1) ^ 1, P.abort_flag, 101)) return false;
+                const uint32_t dst = sA + s * A_STAGE_BYTES + r0 * 128 + sw;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) ptx::cp_async_16(dst + i * (16 * 128), base + off[i], ok[i]);
+                ptx::cp_async_mbar_arrive(bar_full_a + 8 * s);
+                ptx::mbar_arrive(bar_full_a + 8 * s);
+                ++it;
+                return true;
+            };
+            if (MODE == 0 && P.rowpack) {
+                // small-Cin mode: K block = kernel row `tr`; chunk = tap column; the source pixel shifts with the chunk
+                const TcPart &pt = P.parts[0];
+                const int cs = pt.cstride, rowpitch = P.w * cs;
                 for (int tr = 0; tr < P.kh && !dead; ++tr) {
+                    int off[8];
+                    bool ok[8];
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const bool v = (chunk < P.kw) && ((tmv[0][i] >> (tr * P.kw + chunk)) & 1ull);
+                        off[i] = v ? (ibase[0][i] - chunk * 8) + (ph[i] + tr * P.dil) * rowpitch + (pw[i] + chunk * P.dil) * cs : 0;
+                        ok[i] = v;
+                    }
+                    if (!push(pt.x, off, ok)) dead = true;
+                }
+            } else {
+                for (int tap = 0; tap < taps && !dead; ++tap) {
+                    const int tr = tap / P.kw, tc = tap - tr * P.kw;
 #pragma unroll
                     for (int p = 0; p < TC_MAX_PARTS; ++p) {
                         if (p >= np || dead) break;
                         const TcPart &pt = P.parts[p];
                         const bf16 *src = (MODE == 0) ? pt.x : P.dc;
+                        const int cs = (MODE == 0) ? pt.cstride : P.dc_cstride;
                         const int xup = (MODE == 0) ? pt.xup : 0;
-                        const int hmax = ((MODE == 0) ? (P.h >> xup) : P.ho) - 1;
-                        const int rowpitch = (MODE == 0) ? (P.w >> xup) * pt.cstride : P.wo * P.dc_cstride;
-                        const int nb = ((MODE == 0) ? pt.kext : P.dc_kext) / BLOCK_K;
-                        const int c8 = (MODE == 0) ? pt.c8 : P.dc_c8;
-                        int rterm[HALO_MAX_HG];
-#pragma unroll
-                        for (int i = 0; i < HALO_MAX_HG; ++i) {
-                            const int hi = (MODE == 0) ? ((ph[i] + tr * P.dil) >> xup) : (ph[i] - tr * P.dil);
-                            rterm[i] = cterm[p][i] + min(max(hi, 0), hmax) * rowpitch;
-                        }
-                        for (int cb = 0; cb < nb; ++cb, ++it) {
-                            const int s = it % SA;
-                            if (!ptx::mbar_wait(bar_empty_a + 8 * s, ((it / SA) & 1) ^ 1, P.abort_flag, 111)) { dead = true; break; }
-                            const bool cv = cb * BLOCK_K + chunk * 8 < c8;
-                            const uint32_t dst0 = sA + s * A_STAGE + chunk * LBO + r0 * 16;
-                            const bf16 *srcb = src + cb * BLOCK_K;
-#pragma unroll
-                            for (int i = 0; i < HALO_MAX_HG; ++i) {
-                                if (i >= HG) break;
-                                ptx::cp_async_16(dst0 + i * 256, srcb + rterm[i], cv && ((vb[p][i] >> tr) & 1u));   // slot r0 + 16*i
-                            }
-                            ptx::cp_async_mbar_arrive(bar_full_a + 8 * s);
-                            ptx::mbar_arrive(bar_full_a + 8 * s);
-                        }
-                    }
-                }
-            } else {
-                const uint32_t sw = static_cast<uint32_t>((chunk ^ (r0 & 7)) << 4);   // (r & 7) == (r0 & 7) for all rows of a thread
-                int ph[8], pw[8];
-                int ibase[TC_MAX_PARTS][8];                 // element offset of the row's image inside each source (+ chunk)
-                bool prow[8];
-                const int ls = 31 - __clz(P.stride);        // dgrad: stride is a power of two on this path (host-checked)
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int m = m0 + r0 + 16 * i;
-                    prow[i] = m < P.m_total;
-                    const int mm = prow[i] ? m : 0;
-                    const int nn = mm / plane, rem = mm - nn * plane;
-                    const int hh = rem / pwid, ww = rem - hh * pwid;
-                    if (MODE == 0) {
-                        ph[i] = hh * P.stride - P.pad_h; pw[i] = ww * P.stride - P.pad_w;
-#pragma unroll
-                        for (int p = 0; p < TC_MAX_PARTS; ++p)
-                            ibase[p][i] = (p < P.nparts) ? nn * (P.h >> P.parts[p].xup) * (P.w >> P.parts[p].xup) * P.parts[p].cstride + chunk * 8 : 0;
-                    } else {
-                        ph[i] = hh + P.pad_h; pw[i] = ww + P.pad_w;
-                        ibase[0][i] = nn * P.ho * P.wo * P.dc_cstride + chunk * 8;
-#pragma unroll
-                        for (int p = 1; p < TC_MAX_PARTS; ++p) ibase[p][i] = 0;
-                    }
-                }
-                uint64_t tmv[TC_MAX_PARTS][8];              // per-row tap-validity bits (bounds + holes), prefetched one tile ahead
-#pragma unroll
-                for (int p = 0; p < TC_MAX_PARTS; ++p)
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) tmv[p][i] = wcur[p][i];
-
-                auto push = [&](const bf16 *base, const int (&off)[8], const bool (&ok)[8]) -> bool {
-                    const int s = it % SA;
-                    if (!ptx::mbar_wait(bar_empty_a + 8 * s, ((it / SA) & 1) ^ 1, P.abort_flag, 101)) return false;
-                    const uint32_t dst = sA + s * A_STAGE + r0 * 128 + sw;
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) ptx::cp_async_16(dst + i * (16 * 128), base + off[i], ok[i]);
-                    ptx::cp_async_mbar_arrive(bar_full_a + 8 * s);
-                    ptx::mbar_arrive(bar_full_a + 8 * s);
-                    ++it;
-                    return true;
-                };
-                if (MODE == 0 && P.rowpack) {
-                    // small-Cin mode: K block = kernel row `tr`; chunk = tap column; the source pixel shifts with the chunk
-                    const TcPart &pt = P.parts[0];
-                    const int cs = pt.cstride, rowpitch = P.w * cs;
-                    for (int tr = 0; tr < P.kh && !dead; ++tr) {
-                        int off[8];
-                        bool ok[8];
+                        const int rowpitch = ((MODE == 0) ? (P.w >> xup) : P.wo) * cs;
+                        int base[8];
+                        bool rv[8];
 #pragma unroll
                         for (int i = 0; i < 8; ++i) {
-                            const bool v = (chunk < P.kw) && ((tmv[0][i] >> (tr * P.kw + chunk)) & 1ull);
-                            off[i] = v ? (ibase[0][i] - chunk * 8) + (ph[i] + tr * P.dil) * rowpitch + (pw[i] + chunk * P.dil) * cs : 0;
-                            ok[i] = v;
+                            bool v;
+                            int hi, wi;
+                            if (MODE == 0) {
+                                v = (tmv[p][i] >> tap) & 1ull;                  // bounds + hole (0 for rows past m_total)
+                                hi = (ph[i] + tr * P.dil) >> xup; wi = (pw[i] + tc * P.dil) >> xup;
+                            } else {
+                                const int th = ph[i] - tr * P.dil, tw = pw[i] - tc * P.dil;
+                                hi = th >> ls; wi = tw >> ls;
+                                v = prow[i] && th >= 0 && tw >= 0 && ((th | tw) & (P.stride - 1)) == 0 && hi < P.ho && wi < P.wo;
+                            }
+                            base[i] = v ? ibase[p][i] + hi * rowpitch + wi * cs : 0;
+                            rv[i] = v;
                         }
-                        if (!push(pt.x, off, ok)) dead = true;
-                    }
-                } else {
-                    for (int tap = 0; tap < taps && !dead; ++tap) {
-                        const int tr = tap / P.kw, tc = tap - tr * P.kw;
+                        const int nb = ((MODE == 0) ? pt.kext : P.dc_kext) / BLOCK_K;
+                        const int c8 = (MODE == 0) ? pt.c8 : P.dc_c8;
+                        for (int cb = 0; cb < nb; ++cb) {
+                            const bool cv = cb * BLOCK_K + chunk * 8 < c8;       // channel padding of the part: zero-fill
+                            int off[8];
+                            bool ok[8];
 #pragma unroll
-                        for (int p = 0; p < TC_MAX_PARTS; ++p) {
-                            if (p >= np || dead) break;
-                            const TcPart &pt = P.parts[p];
-                            const bf16 *src = (MODE == 0) ? pt.x : P.dc;
-                            const int cs = (MODE == 0) ? pt.cstride : P.dc_cstride;
-                            const int xup = (MODE == 0) ? pt.xup : 0;
-                            const int rowpitch = ((MODE == 0) ? (P.w >> xup) : P.wo) * cs;
-                            int base[8];
-                            bool rv[8];
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                bool v;
-                                int hi, wi;
-                                if (MODE == 0) {
-                                    v = (tmv[p][i] >> tap) & 1ull;                  // bounds + hole (0 for rows past m_total)
-                                    hi = (ph[i] + tr * P.dil) >> xup; wi = (pw[i] + tc * P.dil) >> xup;
-                                } else {
-                                    const int th = ph[i] - tr * P.dil, tw = pw[i] - tc * P.dil;
-                                    hi = th >> ls; wi = tw >> ls;
-                                    v = prow[i] && th >= 0 && tw >= 0 && ((th | tw) & (P.stride - 1)) == 0 && hi < P.ho && wi < P.wo;
-                                }
-                                base[i] = v ? ibase[p][i] + hi * rowpitch + wi * cs : 0;
-                                rv[i] = v;
-                            }
-                            const int nb = ((MODE == 0) ? pt.kext : P.dc_kext) / BLOCK_K;
-                            const int c8 = (MODE == 0) ? pt.c8 : P.dc_c8;
-                            for (int cb = 0; cb < nb; ++cb) {
-                                const bool cv = cb * BLOCK_K + chunk * 8 < c8;       // channel padding of the part: zero-fill
-                                int off[8];
-                                bool ok[8];
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) { ok[i] = rv[i] && cv; off[i] = ok[i] ? base[i] + cb * BLOCK_K : 0; }
-                                if (!push(src, off, ok)) { dead = true; break; }
-                            }
+                            for (int i = 0; i < 8; ++i) { ok[i] = rv[i] && cv; off[i] = ok[i] ? base[i] + cb * BLOCK_K : 0; }
+                            if (!push(src, off, ok)) { dead = true; break; }
                         }
                     }
                 }
@@ -694,37 +594,17 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
             for (int tile = blockIdx.x; tile < num_tiles && !dead; tile += gridDim.x) {
                 const int n0 = (tile % n_tiles) * BLOCK_N;
                 if (!tile_active(n0)) continue;
-                if (HALO) {
-                    for (int tr = 0; tr < P.kh && !dead; ++tr)
-                        for (int p = 0; p < np && !dead; ++p) {
-                            const int nb = ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
-                            for (int cb = 0; cb < nb && !dead; ++cb)
-                                for (int tc = 0; tc < P.kw; ++tc) {
-                                    const int tap = tr * P.kw + tc;
-                                    const int kidx = (MODE == 0) ? tap * P.ktap + P.parts[p].koff + cb * BLOCK_K : tap * P.dc_kext + cb * BLOCK_K;
-                                    if (!load(kidx, n0)) { dead = true; break; }
-                                }
-                        }
-                } else {
-                    const int num_kb = (MODE == 0) ? (P.rowpack ? P.kh : taps * (P.ktap / BLOCK_K)) : taps * (P.dc_kext / BLOCK_K);
-                    for (int kb = 0; kb < num_kb; ++kb)
-                        if (!load(kb * BLOCK_K, n0)) { dead = true; break; }
-                }
+                const int num_kb = (MODE == 0) ? (P.rowpack ? P.kh : taps * (P.ktap / BLOCK_K)) : taps * (P.dc_kext / BLOCK_K);
+                for (int kb = 0; kb < num_kb; ++kb)
+                    if (!load(kb * BLOCK_K, n0)) { dead = true; break; }
             }
         }
     } else {
         // ================================ consumer warpgroups (warps 4-11) ================================
         const int e = warp - 4, g = e >> 2;
         const bool leader = (threadIdx.x & 127) == 0;
-        int num_a = 0;
-        if (HALO) {
-            for (int p = 0; p < np; ++p) num_a += ((MODE == 0) ? P.parts[p].kext : P.dc_kext) / BLOCK_K;
-            num_a *= P.kh;
-        } else {
-            num_a = (MODE == 0) ? (P.rowpack ? P.kh : taps * (P.ktap / BLOCK_K)) : taps * (P.dc_kext / BLOCK_K);
-        }
-        // this warpgroup's 64 rows: 8 groups of 8 rows further into the A stage
-        const uint32_t a_rows = HALO ? 8u * HG * 16u : 64u * 128u;
+        const int num_a = (MODE == 0) ? (P.rowpack ? P.kh : taps * (P.ktap / BLOCK_K)) : taps * (P.dc_kext / BLOCK_K);
+        const uint32_t a_rows = 64u * 128u;             // this warpgroup's 64 rows of 128 bytes further into the A stage
         float *s_stat = (MODE == 0 && P.bn_sums != nullptr)
                             ? reinterpret_cast<float *>(smem_raw + (s_stat_addr - ptx::smem_u32(smem_raw))) : nullptr;
         const EpiRole<BLOCK_N> R(e);
@@ -749,31 +629,24 @@ pconv_tc_persistent_kernel(const __grid_constant__ TcParams P, const __grid_cons
                 const int sa = ita % SA;
                 if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full_a + 8 * sa, (ita / SA) & 1, P.abort_flag, 104))) { dead = true; break; }
                 ptx::fence_proxy_async_smem();                   // cp.async (generic proxy) data -> wgmma (async proxy)
-                const int sb0 = itb % SB;
-                for (int tc = 0; tc < nB; ++tc, ++itb) {
-                    const int sb = itb % SB;
-                    if (!__all_sync(0xffffffffu, ptx::mbar_wait(bar_full_b + 8 * sb, (itb / SB) & 1, P.abort_flag, 105))) { dead = true; break; }
+                const int sb = itb % SB;
+                if (__all_sync(0xffffffffu, ptx::mbar_wait(bar_full_b + 8 * sb, (itb / SB) & 1, P.abort_flag, 105))) {
                     const uint64_t db = ptx::make_smem_desc(sB + sb * B_STAGE_BYTES, 16, 1024);
                     ptx::wgmma_fence();
-                    if (HALO) {
-                        const int shift = ((MODE == 0) ? tc : (P.kw - 1 - tc)) * P.dil;    // slots
-                        const uint32_t a0 = sA + sa * A_STAGE + g * a_rows + shift * 16;
+                    const uint64_t da = ptx::make_smem_desc(sA + sa * A_STAGE_BYTES + g * a_rows, 16, 1024);
 #pragma unroll
-                        for (int k = 0; k < BLOCK_K / 16; ++k)                              // 2 chunks (16 channels) per MMA
-                            ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, ptx::make_smem_desc_noswizzle(a0 + k * 2 * LBO, LBO, HG * 16), db + 2 * k);
-                    } else {
-                        const uint64_t da = ptx::make_smem_desc(sA + sa * A_STAGE + g * a_rows, 16, 1024);
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / 16; ++k)                              // +32 bytes per K=16 step inside the swizzle row
-                            ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + 2 * k, db + 2 * k);
-                    }
+                    for (int k = 0; k < BLOCK_K / 16; ++k)                                  // +32 bytes per K=16 step inside the swizzle row
+                        ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + 2 * k, db + 2 * k);
                     ptx::wgmma_commit();
+                    ++itb;
+                } else {
+                    dead = true;
                 }
-                // the A item and its weight tiles are released once this warpgroup's MMAs on them completed
+                // the A item and its weight tile are released once this warpgroup's MMAs on them completed
                 ptx::wgmma_wait<0>();
                 ptx::wgmma_fence_regs(acc);
                 if (leader) {
-                    for (int tc = 0; tc < nB; ++tc) ptx::mbar_arrive(bar_empty_b + 8 * ((sb0 + tc) % SB));
+                    ptx::mbar_arrive(bar_empty_b + 8 * sb);
                     ptx::mbar_arrive(bar_empty_a + 8 * sa);
                 }
             }
@@ -2250,31 +2123,22 @@ void base_params(TcParams &P, const pcb_conv *c, const Layout &L) {
     P.sub = 1; P.py = 0; P.px = 0; P.fh = c->h; P.fw = c->w;
 }
 
-// row-halo eligibility: stride 1, output rows made of whole groups of 8 pixels, halo small enough
-int halo_hg(const pcb_conv *c, bool rowpack) {
-    if (rowpack || c->stride != 1) return 0;
-    const int hg = 8 + (c->kw - 1) * c->dil;
-    if (c->kw < 2 || hg > HALO_MAX_HG || c->kh > 8) return 0;
-    if (c->wo % 8 != 0 || c->w % 8 != 0 || c->wo != c->w) return 0;
-    return hg;
-}
-
 // H100: 227 KB of shared memory per block.  The rings get what the epilogue staging tile, the statistics and the barriers leave.
 constexpr size_t MAX_SMEM = 227 * 1024;
 constexpr size_t RING_BUDGET = 208 * 1024;
 
-template <int BLOCK_N, int MODE, bool HALO>
+template <int BLOCK_N, int MODE>
 int launch_persistent(TcParams &P, const CUtensorMap &tm, cudaStream_t st) {
-    const size_t a_stage = HALO ? ((8 * 16 * (16 * P.hg + 1) + 127) / 128 * 128) : A_STAGE_BYTES;
+    const size_t a_stage = A_STAGE_BYTES;
     const size_t b_stage = BLOCK_N * 128;
     const size_t budget = RING_BUDGET - acc_stage_bytes(BLOCK_N);
     P.ring_b = 6;
-    P.ring_a = HALO ? 3 : 6;
+    P.ring_a = 6;
     while (P.ring_a * a_stage + P.ring_b * b_stage > budget && P.ring_b > 3) --P.ring_b;
     while (P.ring_a * a_stage + P.ring_b * b_stage > budget && P.ring_a > 2) --P.ring_a;
     const size_t smem = 1024 + P.ring_a * a_stage + P.ring_b * b_stage + 32 * MAX_RING + 16 + STAT_SMEM_BYTES + acc_stage_bytes(BLOCK_N);
     PCB_CHECK(smem <= MAX_SMEM, "tensor-core conv: %zu bytes of shared memory do not fit", smem);
-    auto kern = pconv_tc_persistent_kernel<BLOCK_N, MODE, HALO>;
+    auto kern = pconv_tc_persistent_kernel<BLOCK_N, MODE>;
     PCB_SMEM_OPT_IN(kern, MAX_SMEM);
     const int num_tiles = ((P.m_total + BLOCK_M - 1) / BLOCK_M) * (P.ncols / BLOCK_N);
     const int grid = std::min(num_tiles, pcb_num_sms());
@@ -2421,8 +2285,7 @@ int pick_bn(int cols, long long m_total, bool fwd, int sms) {
 
 template <int MODE>
 int launch_tc(TcParams &P, const CUtensorMap &tm, int bn, cudaStream_t st) {
-    if (P.hg) return (bn == 128) ? launch_persistent<128, MODE, true>(P, tm, st) : launch_persistent<64, MODE, true>(P, tm, st);
-    return (bn == 128) ? launch_persistent<128, MODE, false>(P, tm, st) : launch_persistent<64, MODE, false>(P, tm, st);
+    return (bn == 128) ? launch_persistent<128, MODE>(P, tm, st) : launch_persistent<64, MODE>(P, tm, st);
 }
 
 // internal streams for the four parity-class launches of low-resolution layers: one set per device AND per host thread (two
@@ -2623,7 +2486,6 @@ struct DirPlan {
     int box_w, box_h, box_n;           // M tile box of the TMA-fed kernels
     int bn;                            // N tile width
     bool halo;                         // TMA-fed row-halo tiles
-    int hg;                            // row-halo group of the cp.async gather kernels (0: none)
 };
 
 struct TcPlan {
@@ -2694,7 +2556,6 @@ TcPlan tc_plan(const pcb_conv *c) {
     } else {
         F.route = ROUTE_GATHER;
         F.bn = L.bn_f;
-        F.hg = halo_hg(c, L.rowpack);
         T.fwd_tapmask = true;
     }
 
@@ -2717,7 +2578,6 @@ TcPlan tc_plan(const pcb_conv *c) {
     } else {
         D.route = ROUTE_GATHER;
         D.bn = (L.ktap % 128 == 0) ? 128 : 64;
-        D.hg = halo_hg(c, false);
     }
 
     const bool wg_tma = tma_wgrad_ok(c, &bw, &bh, &bn);
@@ -2893,7 +2753,6 @@ int pcb_tc_forward_ws(const pcb_conv *c, const void *w_fwd, const float *bias, v
         P.wk_base = 0; P.wk_col = L.ktap; P.wk_row = c->kw * L.ktap;
         return launch_tma<0>(P, tm, ta[0], ta[1], F.bn, F.halo, st);
     }
-    P.hg = F.hg;
     return launch_tc<0>(P, tm, F.bn, st);
 }
 
@@ -2991,7 +2850,6 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
         }
         return 0;
     }
-    P.hg = D.hg;
     return launch_tc<1>(P, tm, D.bn, st);
 }
 

@@ -1,10 +1,11 @@
-// dwconv.cu -- depthwise k x k convolution (groups == channels), the HBM-bound half of the depthwise-separable
+// dwconv.cu -- depthwise 3x3 convolution (groups == channels) at a power-of-two stride, the HBM-bound half of the depthwise-separable
 // blocks: DSConvBlock (models/BaseModels.py:105-127), InvertedResidual / RFB branches (models/MobileNetV2.py:136-138,
 // models/common.py:136-143: dilation up to 29), and the depthwise PARTIAL convolutions of PartialInvertedResidual
 // (models/MobileNetV2.py:174-176).  NHWC, 8 channels (16 B of bf16 / 32 B of fp32) per thread, fp32 accumulation;
 // one read of x and one write of y per element is the roofline (weights are k*k*C, negligible).
 // It is an internal fast path of pcb_pconv_forward / backward_* (same semantics: optional hole mask with zero-fill,
-// mask-sum renormalisation, `plain` mode for ordinary convolutions).
+// mask-sum renormalisation, `plain` mode for ordinary convolutions); every other depthwise shape runs on the shape-general
+// kernels of conv_generic.cu.
 #include <stdlib.h>
 #include <string.h>
 
@@ -25,7 +26,7 @@ inline DwEp dw_ep(const pcb_ep *e) {
 }
 
 struct DwParams {
-    int n, h, w, c, kh, kw, stride, pad_h, pad_w, dil, ho, wo;
+    int n, h, w, c, stride, pad_h, pad_w, dil, ho, wo;
     int x_cstride, y_cstride;
     const uint8_t *mask;     // input hole plane [n, h>>mup, w>>mup] or null
     int mup;
@@ -40,150 +41,10 @@ __device__ __forceinline__ bool dw_mask(const DwParams &P, int nn, int hi, int w
     return P.mask[(static_cast<long long>(nn) * (P.h >> P.mup) + (hi >> P.mup)) * (P.w >> P.mup) + (wi >> P.mup)] != 0;
 }
 
-// w_t: [taps][c] (T), bias fp32 [c] or null
-template <typename T>
-__global__ void __launch_bounds__(256) dw_fwd_kernel(const DwParams P, const T *__restrict__ x, const T *__restrict__ w_t,
-                                                     const float *__restrict__ bias, T *__restrict__ y) {
-    const int cv = P.c >> 3;
-    const long long total = static_cast<long long>(P.n) * P.ho * P.wo;
-    const long long nvec = total * cv;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nvec; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const long long m = i / cv;
-        const int ch = static_cast<int>(i - m * cv) * 8;
-        const int ow = static_cast<int>(m % P.wo);
-        const long long t = m / P.wo;
-        const int oh = static_cast<int>(t % P.ho), nn = static_cast<int>(t / P.ho);
-        float acc[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-        for (int tr = 0; tr < P.kh; ++tr) {
-            const int hi = oh * P.stride - P.pad_h + tr * P.dil;
-            if (hi < 0 || hi >= P.h) continue;
-            for (int tc = 0; tc < P.kw; ++tc) {
-                const int wi = ow * P.stride - P.pad_w + tc * P.dil;
-                if (wi < 0 || wi >= P.w || !dw_mask(P, nn, hi, wi)) continue;
-                float xv[8], wv[8];
-                Vec8<T>::load(x + (static_cast<long long>(nn * P.h + hi) * P.w + wi) * P.x_cstride + ch, xv);
-                Vec8<T>::load(w_t + static_cast<long long>(tr * P.kw + tc) * P.c + ch, wv);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) acc[j] += xv[j] * wv[j];
-            }
-        }
-        float o[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float b = bias ? bias[ch + j] : 0.f;
-            if (!P.msum) { o[j] = acc[j] + b; continue; }                  // plain convolution
-            const float s = P.msum[(P.mg == 1 ? 0 : static_cast<long long>(ch + j) * total) + m];
-            if (P.no_guard) o[j] = acc[j] / s + b;
-            else o[j] = (s == 0.f) ? 0.f : acc[j] / s + b;
-        }
-        Vec8<T>::store(y + m * P.y_cstride + ch, o);
-    }
-}
-
-// dx[p][c] = mask(p) * sum_taps dc[(p + pad - tap*dil)/stride][c] * w[tap][c]
-template <typename T>
-__global__ void __launch_bounds__(256) dw_dgrad_kernel(const DwParams P, const T *__restrict__ dc, int dc_cstride, const T *__restrict__ w_t,
-                                                       T *__restrict__ dx, int dx_cstride) {
-    const int cv = P.c >> 3;
-    const long long total = static_cast<long long>(P.n) * P.h * P.w;
-    const long long nvec = total * cv;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nvec; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const long long m = i / cv;
-        const int ch = static_cast<int>(i - m * cv) * 8;
-        const int iw = static_cast<int>(m % P.w);
-        const long long t = m / P.w;
-        const int ih = static_cast<int>(t % P.h), nn = static_cast<int>(t / P.h);
-        float acc[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-        if (dw_mask(P, nn, ih, iw)) {
-            for (int tr = 0; tr < P.kh; ++tr) {
-                const int th = ih + P.pad_h - tr * P.dil;
-                if (th < 0) continue;
-                const int oh = th / P.stride;
-                if (oh * P.stride != th || oh >= P.ho) continue;
-                for (int tc = 0; tc < P.kw; ++tc) {
-                    const int tw = iw + P.pad_w - tc * P.dil;
-                    if (tw < 0) continue;
-                    const int ow = tw / P.stride;
-                    if (ow * P.stride != tw || ow >= P.wo) continue;
-                    float dv[8], wv[8];
-                    Vec8<T>::load(dc + (static_cast<long long>(nn * P.ho + oh) * P.wo + ow) * dc_cstride + ch, dv);
-                    Vec8<T>::load(w_t + static_cast<long long>(tr * P.kw + tc) * P.c + ch, wv);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) acc[j] += dv[j] * wv[j];
-                }
-            }
-        }
-        Vec8<T>::store(dx + m * dx_cstride + ch, acc);
-    }
-}
-
-// dw[c][tap] += sum_pixels dc[p][c] * (x*m)[p@tap][c];  TP taps per pass kept in registers
-template <typename T, int TP>
-__global__ void __launch_bounds__(256) dw_wgrad_kernel(const DwParams P, const T *__restrict__ dc, int dc_cstride, const T *__restrict__ x,
-                                                       float *__restrict__ dw, int tap0) {
-    __shared__ float s_red[256][8];
-    const int cv = P.c >> 3, rpb = 256 / cv;
-    const int r = threadIdx.x / cv, v = threadIdx.x - r * cv;
-    const int taps = P.kh * P.kw;
-    const long long total = static_cast<long long>(P.n) * P.ho * P.wo;
-    float acc[TP][8];
-#pragma unroll
-    for (int tp = 0; tp < TP; ++tp)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[tp][j] = 0.f;
-    if (r < rpb) {
-        for (long long m = static_cast<long long>(blockIdx.x) * rpb + r; m < total; m += static_cast<long long>(gridDim.x) * rpb) {
-            const int ow = static_cast<int>(m % P.wo);
-            const long long t = m / P.wo;
-            const int oh = static_cast<int>(t % P.ho), nn = static_cast<int>(t / P.ho);
-            float dv[8];
-            Vec8<T>::load(dc + m * dc_cstride + v * 8, dv);
-#pragma unroll
-            for (int tp = 0; tp < TP; ++tp) {
-                const int tap = tap0 + tp;
-                if (tap >= taps) continue;
-                const int tr = tap / P.kw, tc = tap - tr * P.kw;
-                const int hi = oh * P.stride - P.pad_h + tr * P.dil, wi = ow * P.stride - P.pad_w + tc * P.dil;
-                if (hi < 0 || hi >= P.h || wi < 0 || wi >= P.w || !dw_mask(P, nn, hi, wi)) continue;
-                float xv[8];
-                Vec8<T>::load(x + (static_cast<long long>(nn * P.h + hi) * P.w + wi) * P.x_cstride + v * 8, xv);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) acc[tp][j] += dv[j] * xv[j];
-            }
-        }
-    }
-#pragma unroll
-    for (int tp = 0; tp < TP; ++tp) {
-        const int tap = tap0 + tp;
-        if (tap >= taps) continue;          // uniform across the block
-        __syncthreads();
-        if (r < rpb) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) s_red[threadIdx.x][j] = acc[tp][j];
-        }
-        __syncthreads();
-        if (r == 0 && v < cv) {
-            float tot[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) tot[j] = 0.f;
-            for (int rr = 0; rr < rpb; ++rr)
-#pragma unroll
-                for (int j = 0; j < 8; ++j) tot[j] += s_red[rr * cv + v][j];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) atomicAdd(dw + static_cast<long long>(v * 8 + j) * taps + tap, tot[j]);
-        }
-    }
-}
-
-
 // =================================================================================================================
-// 3x3 depthwise kernels, second generation (any stride / dilation).  The first-generation kernels above spend most of their
-// instructions on 64-bit index divisions per element and reload the nine weight vectors for every output: they are
-// issue-bound, not bandwidth-bound.  Here
+// 3x3 depthwise kernels, second generation (any power-of-two stride / dilation).  A thread per output element spends most of
+// its instructions on 64-bit index divisions and reloads the nine weight vectors for every output: it is issue-bound, not
+// bandwidth-bound.  Here
 //   * a block owns a chunk of `cvb` channel vectors (8 channels each) x PL pixel lanes; a thread keeps ONE channel vector for
 //     its whole life, so the nine weight vectors (fwd / dgrad) or the nine gradient accumulators (wgrad) live in registers,
 //   * rows are walked by blockIdx.y in groups, pixels of a row by the PL lanes: all index math is 32-bit adds,
@@ -298,7 +159,7 @@ __global__ void __launch_bounds__(256) dw3_fwd_kernel(const DwParams P, const T 
     }
 }
 
-// dx[p][c] = mask(p) * sum_taps dc[(p + pad - tap*dil) / stride][c] * w[tap][c]   (stride is a power of two here)
+// dx[p][c] = mask(p) * sum_taps dc[(p + pad - tap*dil) / stride][c] * w[tap][c]   (stride is a power of two)
 template <typename T, bool PLAIN>
 __global__ void __launch_bounds__(256) dw3_dgrad_kernel(const DwParams P, const T *__restrict__ dc, int dc_cstride, const T *__restrict__ w_t,
                                                         T *__restrict__ dx, int dx_cstride, int cvb, int pl, int sshift) {
@@ -728,15 +589,13 @@ __global__ void __launch_bounds__(256, 2) dw4_s1_wgrad_kernel(const T *__restric
     }
 }
 
-// the kernel generation a direction takes: dw4 (plain 3x3 stride 1, pad == dil; the data gradient is the same convolution with
-// flipped taps), dw3 (any other 3x3; its data gradient walks the input grid with shifts, so power-of-two strides only), or
-// the first generation (every other shape)
-enum DwRoute { DW_GEN1, DW3, DW4 };
+// the kernel generation a problem takes in all three directions: dw4 (plain stride 1, pad == dil; the data gradient is the
+// same convolution with flipped taps) or dw3 (every other 3x3 at a power-of-two stride: pcb_dw_eligible)
+enum DwRoute { DW3, DW4 };
 
-DwRoute dw_route(const pcb_conv *c, bool dgrad) {
-    if (c->kh != 3 || c->kw != 3) return DW_GEN1;
+DwRoute dw_route(const pcb_conv *c) {
     if (c->stride == 1 && c->pad_h == c->dil && c->pad_w == c->dil && c->plain && c->parts[0].mask == nullptr && c->cin % 4 == 0) return DW4;
-    return (dgrad && (c->stride & (c->stride - 1))) ? DW_GEN1 : DW3;
+    return DW3;
 }
 
 template <typename T>
@@ -750,7 +609,7 @@ __global__ void dw_weight_transpose_kernel(const float *__restrict__ wm, int c, 
 
 void fill(DwParams &P, const pcb_conv *c) {
     memset(&P, 0, sizeof(P));
-    P.n = c->n; P.h = c->h; P.w = c->w; P.c = c->cin; P.kh = c->kh; P.kw = c->kw; P.stride = c->stride; P.pad_h = c->pad_h;
+    P.n = c->n; P.h = c->h; P.w = c->w; P.c = c->cin; P.stride = c->stride; P.pad_h = c->pad_h;
     P.pad_w = c->pad_w; P.dil = c->dil; P.ho = c->ho; P.wo = c->wo; P.x_cstride = c->parts[0].x_cstride;
     P.mask = c->parts[0].mask; P.mup = c->parts[0].mask_up; P.no_guard = c->no_guard;
     P.mg = (c->groups > 1 && !c->same_holes) ? c->groups : 1;
@@ -766,6 +625,7 @@ inline int dw_grid(long long items) {
 
 bool pcb_dw_eligible(const pcb_conv *c) {
     if (!(c->groups == c->cin && c->cin == c->cout && c->groups > 1 && c->nparts == 1)) return false;
+    if (c->kh != 3 || c->kw != 3 || (c->stride & (c->stride - 1))) return false;
     const pcb_part &pt = c->parts[0];
     if (c->cin % 8 != 0 || c->cin > 2048 || pt.x_cstride % 8 != 0 || pt.x_up != 0) return false;
     const uintptr_t align = (c->dtype == PCB_BF16) ? 15 : 31;
@@ -782,21 +642,14 @@ int pcb_dw_weight_prepare(const pcb_conv *c, const float *w_master, void *w_t, c
     return 0;
 }
 
-// the 3x3 kernels (dw3_fwd_kernel, dw4_s1_kernel) can accumulate the BatchNorm statistics of their output / apply an eval-mode
-// BatchNorm + activation before they store
-bool pcb_dw_fuses_epilogue(const pcb_conv *c) { return dw_route(c, false) != DW_GEN1; }
-
 int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *y, int y_cstride, const float *msum, double *bn_sums,
                    const pcb_ep *ep, cudaStream_t st) {
-    const DwRoute route = dw_route(c, false);
-    PCB_CHECK(bn_sums == nullptr || route != DW_GEN1, "depthwise forward: fused BatchNorm statistics need the 3x3 kernels");
-    PCB_CHECK(ep == nullptr || route != DW_GEN1, "depthwise forward: fused BatchNorm + activation needs the 3x3 kernels");
     DwParams P;
     fill(P, c);
     P.ep = dw_ep(ep);
     P.y_cstride = y_cstride;
     P.msum = msum;       // plain mode: mask_sums wrote 1.0 everywhere, so the same epilogue applies
-    if (route == DW4) {
+    if (dw_route(c) == DW4) {
         const Dw4Geom g = dw4_geom(c->cin, c->w, c->h, c->dil);
         const dim3 grid(g.chunks, g.xtiles, c->n * g.pgroups * g.nseg);
 #define PCB_DW4_FWD(TT, EP_) dw4_s1_kernel<TT, false, EP_><<<grid, 256, 0, st>>>(static_cast<const TT *>(c->parts[0].x), c->parts[0].x_cstride, static_cast<const TT *>(w_t), bias, static_cast<TT *>(y), y_cstride, bn_sums, P.ep, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb)
@@ -806,25 +659,18 @@ int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *
         PCB_LAUNCH_CHECK();
         return 0;
     }
-    if (route == DW3) {
-        const Dw3Geom g = dw3_geom(c->cin);
-        const dim3 grid(g.chunks, (c->n * c->ho + DW3_ROWS - 1) / DW3_ROWS);
-        const bool plain = c->plain && c->parts[0].mask == nullptr;
+    const Dw3Geom g = dw3_geom(c->cin);
+    const dim3 grid(g.chunks, (c->n * c->ho + DW3_ROWS - 1) / DW3_ROWS);
+    const bool plain = c->plain && c->parts[0].mask == nullptr;
 #define PCB_DW3_FWD(TT, PL_, EP_) dw3_fwd_kernel<TT, PL_, EP_><<<grid, 256, 0, st>>>(P, static_cast<const TT *>(c->parts[0].x), static_cast<const TT *>(w_t), bias, static_cast<TT *>(y), g.cvb, g.pl, bn_sums)
-        if (ep) {
-            if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_FWD(bf16, true, true); else PCB_DW3_FWD(bf16, false, true); }
-            else { if (plain) PCB_DW3_FWD(float, true, true); else PCB_DW3_FWD(float, false, true); }
-        } else {
-            if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_FWD(bf16, true, false); else PCB_DW3_FWD(bf16, false, false); }
-            else { if (plain) PCB_DW3_FWD(float, true, false); else PCB_DW3_FWD(float, false, false); }
-        }
-#undef PCB_DW3_FWD
-        PCB_LAUNCH_CHECK();
-        return 0;
+    if (ep) {
+        if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_FWD(bf16, true, true); else PCB_DW3_FWD(bf16, false, true); }
+        else { if (plain) PCB_DW3_FWD(float, true, true); else PCB_DW3_FWD(float, false, true); }
+    } else {
+        if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_FWD(bf16, true, false); else PCB_DW3_FWD(bf16, false, false); }
+        else { if (plain) PCB_DW3_FWD(float, true, false); else PCB_DW3_FWD(float, false, false); }
     }
-    const long long nvec = static_cast<long long>(c->n) * c->ho * c->wo * (c->cin / 8);
-    if (c->dtype == PCB_BF16) dw_fwd_kernel<bf16><<<dw_grid(nvec), 256, 0, st>>>(P, static_cast<const bf16 *>(c->parts[0].x), static_cast<const bf16 *>(w_t), bias, static_cast<bf16 *>(y));
-    else dw_fwd_kernel<float><<<dw_grid(nvec), 256, 0, st>>>(P, static_cast<const float *>(c->parts[0].x), static_cast<const float *>(w_t), bias, static_cast<float *>(y));
+#undef PCB_DW3_FWD
     PCB_LAUNCH_CHECK();
     return 0;
 }
@@ -832,8 +678,7 @@ int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *
 int pcb_dw_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_t, void *dx, int dx_cstride, cudaStream_t st) {
     DwParams P;
     fill(P, c);
-    const DwRoute route = dw_route(c, true);
-    if (route == DW4) {
+    if (dw_route(c) == DW4) {
         const Dw4Geom g = dw4_geom(c->cin, c->w, c->h, c->dil);
         const dim3 grid(g.chunks, g.xtiles, c->n * g.pgroups * g.nseg);
         if (c->dtype == PCB_BF16) dw4_s1_kernel<bf16, true, false><<<grid, 256, 0, st>>>(static_cast<const bf16 *>(dc), dc_cstride, static_cast<const bf16 *>(w_t), nullptr, static_cast<bf16 *>(dx), dx_cstride, nullptr, P.ep, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
@@ -841,22 +686,15 @@ int pcb_dw_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
         PCB_LAUNCH_CHECK();
         return 0;
     }
-    if (route == DW3) {
-        const Dw3Geom g = dw3_geom(c->cin);
-        const dim3 grid(g.chunks, (c->n * c->h + DW3_ROWS - 1) / DW3_ROWS);
-        const bool plain = c->plain && c->parts[0].mask == nullptr;
-        int sshift = 0;
-        while ((1 << sshift) < c->stride) ++sshift;
+    const Dw3Geom g = dw3_geom(c->cin);
+    const dim3 grid(g.chunks, (c->n * c->h + DW3_ROWS - 1) / DW3_ROWS);
+    const bool plain = c->plain && c->parts[0].mask == nullptr;
+    int sshift = 0;
+    while ((1 << sshift) < c->stride) ++sshift;
 #define PCB_DW3_DG(TT, PL_) dw3_dgrad_kernel<TT, PL_><<<grid, 256, 0, st>>>(P, static_cast<const TT *>(dc), dc_cstride, static_cast<const TT *>(w_t), static_cast<TT *>(dx), dx_cstride, g.cvb, g.pl, sshift)
-        if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_DG(bf16, true); else PCB_DW3_DG(bf16, false); }
-        else { if (plain) PCB_DW3_DG(float, true); else PCB_DW3_DG(float, false); }
+    if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_DG(bf16, true); else PCB_DW3_DG(bf16, false); }
+    else { if (plain) PCB_DW3_DG(float, true); else PCB_DW3_DG(float, false); }
 #undef PCB_DW3_DG
-        PCB_LAUNCH_CHECK();
-        return 0;
-    }
-    const long long nvec = static_cast<long long>(c->n) * c->h * c->w * (c->cin / 8);
-    if (c->dtype == PCB_BF16) dw_dgrad_kernel<bf16><<<dw_grid(nvec), 256, 0, st>>>(P, static_cast<const bf16 *>(dc), dc_cstride, static_cast<const bf16 *>(w_t), static_cast<bf16 *>(dx), dx_cstride);
-    else dw_dgrad_kernel<float><<<dw_grid(nvec), 256, 0, st>>>(P, static_cast<const float *>(dc), dc_cstride, static_cast<const float *>(w_t), static_cast<float *>(dx), dx_cstride);
     PCB_LAUNCH_CHECK();
     return 0;
 }
@@ -866,8 +704,7 @@ int pcb_dw_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, b
     fill(P, c);
     const int taps = c->kh * c->kw;
     if (zero_dw) PCB_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * c->cin * taps, st));
-    const DwRoute route = dw_route(c, false);
-    if (route == DW4) {
+    if (dw_route(c) == DW4) {
         const Dw4Geom g = dw4_geom(c->cin, c->w, c->h, c->dil);
         const dim3 grid(g.chunks, g.xtiles, c->n * g.pgroups * g.nseg);
         if (c->dtype == PCB_BF16) dw4_s1_wgrad_kernel<bf16><<<grid, 256, 0, st>>>(static_cast<const bf16 *>(c->parts[0].x), c->parts[0].x_cstride, static_cast<const bf16 *>(dc), dc_cstride, dw, c->n, c->h, c->w, c->cin, c->dil, g.cq, g.xt, g.nseg, g.rseg, g.ppb);
@@ -875,31 +712,18 @@ int pcb_dw_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, b
         PCB_LAUNCH_CHECK();
         return 0;
     }
-    if (route == DW3) {
-        const Dw3Geom g = dw3_geom(c->cin);
-        // about two resident waves of blocks; every block ends with cvb * 72 atomics
-        const int rows_total = c->n * c->ho;
-        int row_groups = std::max(1, std::min(rows_total, (4 * pcb_num_sms() + g.chunks - 1) / g.chunks));
-        const int rpbk = (rows_total + row_groups - 1) / row_groups;
-        row_groups = (rows_total + rpbk - 1) / rpbk;
-        const dim3 grid(g.chunks, row_groups);
-        const bool plain = c->plain && c->parts[0].mask == nullptr;
+    const Dw3Geom g = dw3_geom(c->cin);
+    // about two resident waves of blocks; every block ends with cvb * 72 atomics
+    const int rows_total = c->n * c->ho;
+    int row_groups = std::max(1, std::min(rows_total, (4 * pcb_num_sms() + g.chunks - 1) / g.chunks));
+    const int rpbk = (rows_total + row_groups - 1) / row_groups;
+    row_groups = (rows_total + rpbk - 1) / rpbk;
+    const dim3 grid(g.chunks, row_groups);
+    const bool plain = c->plain && c->parts[0].mask == nullptr;
 #define PCB_DW3_WG(TT, PL_) dw3_wgrad_kernel<TT, PL_><<<grid, 256, 0, st>>>(P, static_cast<const TT *>(dc), dc_cstride, static_cast<const TT *>(c->parts[0].x), dw, g.cvb, g.pl, rpbk)
-        if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_WG(bf16, true); else PCB_DW3_WG(bf16, false); }
-        else { if (plain) PCB_DW3_WG(float, true); else PCB_DW3_WG(float, false); }
+    if (c->dtype == PCB_BF16) { if (plain) PCB_DW3_WG(bf16, true); else PCB_DW3_WG(bf16, false); }
+    else { if (plain) PCB_DW3_WG(float, true); else PCB_DW3_WG(float, false); }
 #undef PCB_DW3_WG
-        PCB_LAUNCH_CHECK();
-        return 0;
-    }
-    const long long total = static_cast<long long>(c->n) * c->ho * c->wo;
-    const int rpb = 256 / (c->cin / 8);
-    long long blocks = (total + rpb * 16 - 1) / (rpb * 16);
-    const int grid = static_cast<int>(std::max<long long>(1, std::min<long long>(blocks, 8ll * pcb_num_sms())));
-    constexpr int TP = 9;
-    for (int tap0 = 0; tap0 < taps; tap0 += TP) {
-        if (c->dtype == PCB_BF16) dw_wgrad_kernel<bf16, TP><<<grid, 256, 0, st>>>(P, static_cast<const bf16 *>(dc), dc_cstride, static_cast<const bf16 *>(c->parts[0].x), dw, tap0);
-        else dw_wgrad_kernel<float, TP><<<grid, 256, 0, st>>>(P, static_cast<const float *>(dc), dc_cstride, static_cast<const float *>(c->parts[0].x), dw, tap0);
-        PCB_LAUNCH_CHECK();
-    }
+    PCB_LAUNCH_CHECK();
     return 0;
 }

@@ -204,11 +204,10 @@ int pcb_stem_forward(const pcb_conv *c, const StemPlan &K, const void *w_fwd_ext
                      const float *msum, void *workspace, double *bn_sums, const pcb_ep *ep, cudaStream_t st);
 int pcb_stem_wgrad(const pcb_conv *c, const StemPlan &K, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw,
                    cudaStream_t st);
-// depthwise fast path (dwconv.cu)
+// depthwise fast path (dwconv.cu): 3x3 at a power-of-two stride
 bool pcb_dw_eligible(const pcb_conv *c);
 int pcb_dw_weight_prepare(const pcb_conv *c, const float *w_master, void *w_t, cudaStream_t st);
 int pcb_dw_forward(const pcb_conv *c, const void *w_t, const float *bias, void *y, int y_cstride, const float *msum, double *bn_sums,
                    const pcb_ep *ep, cudaStream_t st);
-bool pcb_dw_fuses_epilogue(const pcb_conv *c);
 int pcb_dw_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *w_t, void *dx, int dx_cstride, cudaStream_t st);
 int pcb_dw_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, bool zero_dw, cudaStream_t st);

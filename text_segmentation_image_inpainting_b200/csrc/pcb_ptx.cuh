@@ -168,14 +168,5 @@ __host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, 
     d |= 1ull << 62;     // SWIZZLE_128B
     return d;
 }
-// Same, no swizzle ("interleave"): core matrices are 8 rows x 16 bytes stored contiguously (128 B).
-//   K-major : LBO = byte distance between the two 8-element K chunks of one MMA, SBO = distance between 8-row groups.
-__host__ __device__ __forceinline__ uint64_t make_smem_desc_noswizzle(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    return d;
-}
 
 }  // namespace ptx

@@ -90,7 +90,7 @@ class BaseModule(nn.Module):
 class B200Conv2d(nn.Conv2d):
     """An ``nn.Conv2d`` (isinstance / out_channels / state_dict identical -- SURVEY 8b "attribute conventions")
     whose forward runs on libpconv_b200: dense and 1x1 convolutions on the wgmma implicit-GEMM kernel,
-    depthwise ones on the vectorised HBM-bound kernel, anything else on the shape-general kernel."""
+    depthwise 3x3 ones at a power-of-two stride on the vectorised HBM-bound kernels, anything else on the shape-general kernel."""
 
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)

@@ -483,7 +483,7 @@ class PartialConvFn(torch.autograd.Function):
         b32 = bias.detach().float().contiguous() if bias is not None else None
         # BatchNorm statistics of y in the convolution epilogue when the consumer announced itself (RenormHandoff.want_stats)
         bn_sums = None
-        if handoff is not None and handoff.want_stats and _FUSED_BN_STATS and lib.pcb_conv_fuses_bn_stats(ctypes.byref(c)) \
+        if handoff is not None and handoff.want_stats and lib.pcb_conv_fuses_bn_stats(ctypes.byref(c)) \
                 and nhwc_layout(y) == geom.cout:
             bn_sums = zeros_f64(2 * geom.cout, dev)
             handoff.bn_sums = bn_sums
@@ -563,7 +563,7 @@ class PartialConvFn(torch.autograd.Function):
             # weight and data gradient only share their input dc: run the weight gradient on a side stream so that the two
             # kernels of a low-resolution layer (far fewer tiles than SMs each) fill the GPU together.  Buffers are
             # allocated on the main stream before the fork and the streams re-join before this function returns.
-            if _OVERLAP_WGRAD and (any(need) or sink is not None) and _PROFILE is None:
+            if (any(need) or sink is not None) and _PROFILE is None:
                 side = _side_stream(dev)
                 side.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(side):
@@ -710,7 +710,6 @@ def prefetch_weights(caches):
             cache["key"], cache["ready"] = key, ev
 
 
-_OVERLAP_WGRAD = True
 _MASK_CHAIN_STREAM = False
 _LAST_MASK_EVENT = None
 _SIDE_STREAMS = {}
@@ -777,11 +776,6 @@ def join_mask_streams():
     _DEFERRED.clear()
 
 
-def set_overlap_wgrad(enabled: bool):
-    global _OVERLAP_WGRAD
-    _OVERLAP_WGRAD = bool(enabled)
-
-
 def _side_stream(dev):
     key = (dev.type, dev.index if dev.index is not None else torch.cuda.current_device())
     if key not in _SIDE_STREAMS:
@@ -799,14 +793,6 @@ class RenormHandoff:
         # want_stats: the consumer is a training-mode BatchNorm -> the convolution accumulates the per-channel sum / sum of
         # squares of its output in its epilogue (`bn_sums`, [2][cout] doubles) and the statistics pass over y disappears
         self.want_stats, self.bn_sums = bool(want_stats), None
-
-
-_FUSED_BN_STATS = True
-
-
-def set_fused_bn_stats(enabled: bool):
-    global _FUSED_BN_STATS
-    _FUSED_BN_STATS = bool(enabled)
 
 
 def partial_conv(x, mask, weight, bias, stride, padding, dilation, groups, same_holes=False, no_guard=False, cache=None,
@@ -911,14 +897,6 @@ def _vec_bn(c):
     return c % 8 == 0 and c <= 2048
 
 
-_BN_SMALL = True
-
-
-def set_bn_small_kernel(enabled: bool):
-    global _BN_SMALL
-    _BN_SMALL = bool(enabled)
-
-
 class BNActFn(torch.autograd.Function):
     """y = act(BN(x)) [+ residual]; BN optional (gamma None => plain activation).
 
@@ -1000,7 +978,7 @@ class BNActFn(torch.autograd.Function):
                     sinks.append(sk); outs.append(sk.view)
                 else:
                     sinks.append(None); outs.append(torch.empty((c,), dtype=torch.float32, device=dev))
-            small = _vec_bn(c) and _BN_SMALL and count <= 16384 and c >= 256 and scale.data_ptr() + 4 * c == shift.data_ptr() \
+            small = _vec_bn(c) and count <= 16384 and c >= 256 and scale.data_ptr() + 4 * c == shift.data_ptr() \
                 and shift.data_ptr() + 4 * c == mean.data_ptr() and mean.data_ptr() + 4 * c == invstd.data_ptr()
             if small:
                 # the bottom of the U: one launch does reduction + apply + parameter gradients (scale|shift|mean|invstd are the
