@@ -1,7 +1,7 @@
 """The inpainting loss on the GPU (text_segmentation_image_inpainting_b200/loss.py, csrc/inpaint_loss.cu): fp32 mode against the
-reference's goldens, bf16 mode against the emulating oracle, the max-pool tie and NaN rules, the Gram products against fp64,
-exact features away from holes, conv1_1's kernel-to-row data gradient against the generic kernel, the ReLU backward in the
-data-gradient epilogue, and the training step: graph replay against eager, SGD against the oracle, two ranks."""
+reference's goldens, bf16 mode against the emulating oracle, the Gram products against fp64, exact features away from holes,
+the ReLU backward in the data-gradient epilogue, and the training step: graph replay against eager, SGD against the oracle,
+two ranks.  The kernels of inpaint_loss.cu one by one: test_gpu_inpaint_loss_kernels.py."""
 import numpy as np
 import pytest
 import torch
@@ -113,33 +113,6 @@ def test_features_away_from_holes_are_exact():
     assert float(df[:n].float().abs().sum()) > 0
 
 
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
-def test_image_layer_dgrad_kernel_to_row_matches_generic(dtype):
-    """conv1_1's data gradient (64 -> 3) in kernel-to-row form against the generic data-gradient kernel."""
-    import ctypes
-
-    from text_segmentation_image_inpainting_b200 import _lib, ops
-    from text_segmentation_image_inpainting_b200.loss import _Vgg
-    crit = _criterion(0)
-    vgg = _Vgg(crit.feature_encoder.encoder, 1)
-    conv = crit.feature_encoder.encoder.stage_convs(0)[0]
-    torch.manual_seed(3)
-    m, h, w = 2, 64, 96
-    x = ops.padded_empty(m, 3, h, w, dtype, torch.device("cuda"))
-    dc = torch.randn(m, 64, h, w, device="cuda").to(dtype).contiguous(memory_format=CL)
-    got = vgg.dgrad(conv, x, None, dc)
-    lib = _lib.load()
-    geom = vgg._geom(x, conv)
-    c = geom.struct([x], force_generic=True)
-    ref = ops.padded_empty(m, 3, h, w, dtype, torch.device("cuda"))
-    wk = conv.weight.detach().float().contiguous(memory_format=CL).to(dtype)
-    _lib.check(lib.pcb_pconv_backward_data(ctypes.byref(c), dc.data_ptr(), 64, wk.data_ptr(), None, (ctypes.c_void_p * 1)(ref.data_ptr()),
-                                           (ctypes.c_int32 * 1)(8), None))
-    torch.cuda.synchronize()
-    tol = 1e-2 if dtype == torch.bfloat16 else 1e-5                  # bf16: Z is rounded once before the tap sum
-    assert _rel(got.float(), ref.float().cpu()) <= tol
-
-
 def test_dgrad_relu_epilogue_matches_separate_pass():
     """The ReLU backward applied in the TMA-fed data-gradient epilogue equals the data gradient followed by the separate
     activation-backward pass, bit for bit (a select on the same bf16 values)."""
@@ -165,33 +138,6 @@ def test_dgrad_relu_epilogue_matches_separate_pass():
     torch.cuda.synchronize()
     assert torch.equal(fused, sep)
     assert int((fused == 0).sum()) > int((plain == 0).sum())
-
-
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
-def test_maxpool_ties_first_maximum_and_nan(dtype):
-    from text_segmentation_image_inpainting_b200 import _lib
-    lib = _lib.load()
-    torch.manual_seed(0)
-    x = torch.randint(-2, 3, (2, 16, 8, 12)).float()                 # many ties, negatives and zeros
-    x[0, 3, 2, 5] = float("nan")
-    x = x.to(dtype)
-    gy = torch.randn(2, 16, 4, 6).to(dtype)
-    xd = x.cuda().contiguous(memory_format=CL)
-    y = torch.empty((2, 16, 4, 6), dtype=dtype, device="cuda", memory_format=CL)
-    gx = torch.empty_like(xd)
-    code = 1 if dtype == torch.bfloat16 else 0
-    gyd = gy.cuda().contiguous(memory_format=CL)
-    _lib.check(lib.pcb_maxpool2x2_forward(xd.data_ptr(), y.data_ptr(), code, 2, 8, 12, 16, None))
-    xr = x.float().requires_grad_(True)
-    yr = F.max_pool2d(xr, 2, 2)
-    yr.backward(gy.float())
-    for relu in (0, 1):
-        _lib.check(lib.pcb_maxpool2x2_backward(gyd.data_ptr(), xd.data_ptr(), gx.data_ptr(), code, 2, 8, 12, 16, relu, None))
-        torch.cuda.synchronize()
-        ref = xr.grad if not relu else torch.where(x.float() <= 0, torch.zeros_like(xr.grad), xr.grad)
-        assert torch.equal(gx.float().cpu(), ref)
-    assert torch.allclose(y.float().cpu(), yr.detach(), rtol=0, atol=0, equal_nan=True)
-    assert torch.isnan(y.float().cpu()[0, 3, 1, 2])
 
 
 def test_gram_matches_fp64():
