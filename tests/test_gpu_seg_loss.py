@@ -1,6 +1,9 @@
-"""The segmentation losses on the GPU (csrc/seg_loss.cu, loss.BinaryFocalLoss, loss.SoftBootstrapCrossEntropy) against the
-fp64 oracle (oracle/seg_loss.py): fp32 and bf16 logits, dense and the channel-padded view the networks return; the bootstrap
-indicator against torch's CPU sigmoid for every bf16 value and a dense fp32 sweep; determinism; graph replay."""
+"""The segmentation losses as modules (loss.BinaryFocalLoss, loss.SoftBootstrapCrossEntropy): every constructor's reduction
+option, output value and shape, and gradient against direct kernel calls and the fp64 oracle (oracle/seg_loss.py), fp32 and
+bf16 logits, dense and the channel-padded view the networks return; the bootstrap indicator against torch's CPU sigmoid for
+every bf16 value and a dense fp32 sweep; determinism; graph replay; the Xception output view fed in place.  The kernels
+themselves, element by element against the fp64 oracle at every dtype, layout, reduction and call-site geometry, are
+tests/test_gpu_seg_loss_kernels.py."""
 import numpy as np
 import pytest
 import torch
@@ -31,14 +34,6 @@ def _inputs(seed, shape=(3, 1, 40, 56), hard=False):
     return x, t
 
 
-def _oracle(kind, x32, t, kw, gout):
-    if kind == "focal":
-        loss, grad = OL.focal(x32.numpy().ravel(), t.numpy().ravel(), **kw)
-    else:
-        loss, grad = OL.bootstrap(x32.numpy().ravel(), t.numpy().ravel(), x32=x32.numpy().ravel(), **kw)
-    return loss, grad * gout
-
-
 def _grad_scale(kind, x, t, kw, gout):
     """Per element, the size of what the fp32 gradient sums: w f (gamma |s| sig(xs) bce + sig(x) + |t|) |gout| / N."""
     x, t = x.numpy().astype(np.float64).ravel(), t.numpy().astype(np.float64).ravel()
@@ -53,6 +48,14 @@ def _grad_scale(kind, x, t, kw, gout):
     return w * (OL.sigmoid(x) + np.abs(t) + 0.05) * np.abs(gout) / n
 
 
+def _oracle(kind, x32, t, kw, gout):
+    if kind == "focal":
+        loss, grad = OL.focal(x32.numpy().ravel(), t.numpy().ravel(), **kw)
+    else:
+        loss, grad = OL.bootstrap(x32.numpy().ravel(), t.numpy().ravel(), x32=x32.numpy().ravel(), **kw)
+    return loss, grad * gout
+
+
 CASES = [("focal", {"gamma": 0}), ("focal", {"gamma": 2}), ("bootstrap", {"reduction": "mean"}), ("bootstrap", {"reduction": "sum"}),
          ("bootstrap", {"reduction": "none"})]
 
@@ -65,11 +68,44 @@ def _module(kind, kw):
     return SoftBootstrapCrossEntropy(size_average=red != "sum", reduce=red != "none")
 
 
+def _direct(kind, kw, x, t, gout=None, dx=None):
+    """the kernels called directly through the C ABI with the loss, reduction and fp32 coefficients the case names (not the
+    module's): the forward output (gout None), else the backward into dx"""
+    import ctypes
+
+    from text_segmentation_image_inpainting_b200 import _lib
+    lib = _lib.load()
+    n, _, h, w = x.shape
+    loss = _lib.SEG_FOCAL if kind == "focal" else _lib.SEG_BOOTSTRAP
+    red = {"mean": _lib.SEG_MEAN, "sum": _lib.SEG_SUM, "none": _lib.SEG_NONE}[kw.get("reduction", "mean")]
+    coefs = (float(kw["gamma"]), 0.0, 1.0, 2.0) if kind == "focal" else (0.95, 1 - 0.95, 1.0, 2.0)
+    code = _lib.PCB_BF16 if x.dtype == torch.bfloat16 else _lib.PCB_F32
+    xs = (ctypes.c_longlong * 4)(*x.stride())
+    st = torch.cuda.current_stream().cuda_stream
+    if gout is None:
+        out = torch.full((n * h * w, 1) if red == _lib.SEG_NONE else (), float("nan"), device="cuda")
+        partials = torch.empty(lib.pcb_seg_loss_partials(n * h * w), dtype=torch.float64, device="cuda")
+        counter = torch.zeros(1, dtype=torch.int32, device="cuda")
+        _lib.check(lib.pcb_seg_loss_forward(x.data_ptr(), code, xs, t.data_ptr(), n, h, w, loss, red, *coefs, partials.data_ptr(),
+                                            counter.data_ptr(), out.data_ptr(), st))
+        return out
+    _lib.check(lib.pcb_seg_loss_backward(x.data_ptr(), code, xs, t.data_ptr(), n, h, w, loss, red, *coefs, gout.data_ptr(), dx.data_ptr(),
+                                         (ctypes.c_longlong * 4)(*dx.stride()), st))
+    return dx
+
+
 @pytest.mark.parametrize("layout", ["dense", "padded"])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("case", range(len(CASES)))
 @pytest.mark.parametrize("hard", [False, True])
 def test_loss_and_gradient_against_the_fp64_oracle(case, dtype, layout, hard):
+    """The modules with each reduction option (BinaryFocalLoss(gamma=0 / 2); SoftBootstrapCrossEntropy() mean,
+    size_average=False sum, reduce=False none), a scalar upstream gradient of 0.75 or a per-element one.  The output has the
+    reduction's shape ((n*h*w, 1) for none, () otherwise) and equals, bit for bit, the forward kernel called directly with
+    the case's loss and reduction codes, so a module that maps its options to the wrong code fails.  The gradient equals
+    fl32(g * gs) of the raw per-element gradient g (an fp32 call with gs = 1: focal mean with gout = count, bootstrap sum with
+    gout = 1), gs = fl32(fl64(gout) / count) for mean, gout for sum and gout_e for none, stored in the logits' dtype.  Both
+    are also within the stated tolerances of the fp64 oracle."""
     kind, kw = CASES[case]
     x, t = _inputs(case + 10 * hard, hard=hard)
     xd = x.to(dtype)
@@ -78,24 +114,40 @@ def test_loss_and_gradient_against_the_fp64_oracle(case, dtype, layout, hard):
     crit = _module(kind, kw)
     raw = []
     xin.register_hook(lambda g: raw.append(g))              # the gradient as the kernel wrote it, before accumulation
-    loss = crit(xin, t.cuda())
+    td = t.cuda()
+    loss = crit(xin, td)
     n = x.numel()
-    gout = torch.rand(n, 1) + 0.5 if kw.get("reduction") == "none" else torch.tensor(0.75)
+    none = kw.get("reduction") == "none"
+    gout = torch.rand(n, 1) + 0.5 if none else torch.tensor(0.75)
     loss.backward(gout.cuda())
     torch.cuda.synchronize()
-    ref_loss, ref_grad = _oracle(kind, x32, t, kw, gout.numpy().ravel() if kw.get("reduction") == "none" else float(gout))
+    ref_loss, ref_grad = _oracle(kind, x32, t, kw, gout.numpy().ravel() if none else float(gout))
     got = loss.detach().cpu().double().numpy()
-    if kw.get("reduction") == "none":
+    if none:
         assert got.shape == (n, 1)
         scale = 2 * (np.abs(x32.double().numpy().ravel()) + 1)         # w (|x| + log 2) bounds what each element sums
         assert np.all(np.abs(got.ravel() - ref_loss) <= 8 * EPS32 * scale)
     else:
         assert got.shape == ()
         assert abs(float(got) - ref_loss) <= 1e-6 * abs(ref_loss), (float(got), ref_loss)
+    direct = _direct(kind, kw, xin.detach(), td)
+    torch.cuda.synchronize()
+    assert direct.shape == loss.shape and torch.equal(loss.detach(), direct), "the module's output is not the kernel's for its reduction"
     g = raw[0]
     assert g.dtype == dtype and g.shape == xin.shape and g.stride() == xin.stride()
+    # exactly one fp32 multiply of the raw per-element gradient
+    raw_kw = dict(kw, reduction="mean" if kind == "focal" else "sum")
+    g_raw = _direct(kind, raw_kw, x32.cuda(), td, torch.tensor([float(n) if kind == "focal" else 1.0], device="cuda"),
+                    torch.full(tuple(x.shape), float("nan"), device="cuda"))
+    torch.cuda.synchronize()
+    if none:
+        gs = gout.cuda().view(x.shape).double()
+    else:
+        gs = float(np.float32(0.75 / n)) if kw.get("reduction", "mean") == "mean" else 0.75     # fl32(fl64(0.75) / count)
+    want = (g_raw.double() * gs).float().to(dtype)
+    assert torch.equal(g, want), f"{int((g != want).sum())} gradient elements are not fl32(g * gs)"
     g = g.float().cpu().double().numpy().ravel()
-    bound = 64 * EPS32 * _grad_scale(kind, x32, t, kw, gout.numpy().ravel() if kw.get("reduction") == "none" else float(gout))
+    bound = 64 * EPS32 * _grad_scale(kind, x32, t, kw, gout.numpy().ravel() if none else float(gout))
     if dtype == torch.bfloat16:                            # one rounding of the stored gradient
         bound = bound * (1 + 2.0 ** -8) + 2.0 ** -8 * np.abs(ref_grad)
     assert np.all(np.abs(g - ref_grad) <= bound), float(np.max(np.abs(g - ref_grad) / np.maximum(bound, 1e-300)))

@@ -82,6 +82,12 @@ template <typename T> __device__ __forceinline__ T from_f32(float v);
 template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
 template <> __device__ __forceinline__ bf16 from_f32<bf16>(float v) { return __float2bfloat16_rn(v); }
 
+// torch's CPU float32 sigmoid(x) > 0.5 holds exactly for x > 1.5 * 2^-24: below it 1 + exp(-x) rounds to 2.  Device expf is
+// only within 2 ulp, and 1 / (1 + expf(-x)) > 0.5f also holds for some x in [1.38 * 2^-24, 1.5 * 2^-24), so the kernels that
+// threshold sigmoid at 0.5 (the bootstrap loss, the text-mask post-processing) compare x with this constant instead.
+constexpr float PCB_SIGMOID_HALF_THRESHOLD = 8.940696716308594e-08f;
+__device__ __forceinline__ bool sigmoid_above_half(float x) { return x > PCB_SIGMOID_HALF_THRESHOLD; }
+
 __device__ __forceinline__ float apply_act(float z, int act, float slope) {
     if (act == PCB_ACT_RELU) return z > 0.f ? z : 0.f;
     if (act == PCB_ACT_LEAKY) return z > 0.f ? z : z * slope;

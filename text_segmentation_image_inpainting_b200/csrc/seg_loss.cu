@@ -18,8 +18,6 @@ namespace {
 constexpr int TPB = 256;
 constexpr int EPT = 8;                   // elements per thread and block pass
 constexpr int MAX_BLOCKS = 1024;
-// torch's CPU float32 sigmoid(x) > 0.5 holds exactly for x > 1.5 * 2^-24: below it 1 + exp(-x) rounds to 2
-constexpr float BOOT_THRESHOLD = 8.940696716308594e-08f;
 
 struct Args {
     const void *x;
@@ -69,7 +67,7 @@ __device__ __forceinline__ float element(const Args &a, float x, float t, float 
         if (g) *g = w * f * (-a.p0 * s * sigmoidf_stable(x * s) * b + sigmoidf_stable(x) - t);
         return f * w * b;
     }
-    const float tb = a.p0 * t + (x > BOOT_THRESHOLD ? a.omb : 0.f);
+    const float tb = a.p0 * t + (sigmoid_above_half(x) ? a.omb : 0.f);
     if (g) *g = w * (sigmoidf_stable(x) - tb);
     return w * bce(x, tb);
 }

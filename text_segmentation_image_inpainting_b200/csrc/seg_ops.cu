@@ -338,7 +338,7 @@ __device__ __forceinline__ bool post_pooled(const T *__restrict__ x, int cstride
             const int xx = ix + dx;
             if (xx < 0 || xx >= w) continue;
             const float v = to_f32(x[(static_cast<long long>(nn * h + yy) * w + xx) * cstride]);
-            if (1.0f / (1.0f + expf(-v)) > 0.5f) return true;      // the demo's sigmoid threshold, accurate expf
+            if (sigmoid_above_half(v)) return true;                 // the demo's sigmoid(x) > 0.5, exactly as torch's CPU float32
         }
     }
     return false;
