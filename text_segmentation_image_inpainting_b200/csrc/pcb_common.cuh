@@ -168,6 +168,8 @@ int pcb_tc_dgrad(const pcb_conv *c, const void *dc, int dc_cstride, const void *
 bool pcb_tc_dgrad_fuses_relu(const pcb_conv *c);
 int pcb_tc_wgrad(const pcb_conv *c, const void *dc, int dc_cstride, float *dw, void *workspace, bool zero_dw, cudaStream_t st);
 int pcb_tc_read_abort_flag(int *value);
+// the current device's abort flag of the bounded mbarrier waits (null: allocation failed)
+int *pcb_tc_abort_flag();
 // the plan's route of the forward, data gradient and weight gradient as PCB_ROUTE_* codes (pcb_debug_conv_routes)
 void pcb_tc_routes(const pcb_conv *c, int32_t routes[3]);
 // layers with <= 8 output channels (conv_smallco.cu); weights are read from the tensor-core operand layouts
@@ -199,9 +201,8 @@ int pcb_k2r_wgrad(const pcb_conv *c, const K2rPlan &K, const void *dc, int dc_cs
 // 7x7 stride-2 image stems as a 4x4 convolution over the space-to-depth image (conv_stem.cu)
 struct StemPlan {
     bool ok;
-    pcb_conv sub;                  // the 4x4 problem over the space-to-depth image
-    size_t sub_fe;                 // bf16 elements of the sub-problem's forward operand (rounded to 64)
-    size_t fwd_extra;              // + fp32 staging of the re-indexed master weights
+    int sc;                        // channels per space-to-depth cell: 16 for images of <= 4 channels, else 32
+    size_t fwd_extra;              // bf16 elements of the stem's forward weights [rup(cout, 64)][16 sc]
     size_t workspace;
 };
 StemPlan pcb_stem_plan(const pcb_conv *c);

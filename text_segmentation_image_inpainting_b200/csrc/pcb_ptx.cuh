@@ -64,6 +64,11 @@ __device__ __forceinline__ void cp_async_16(uint32_t dst, const void *src, bool 
     const uint32_t sz = valid ? 16u : 0u;   // src-size 0 => 16 zero bytes are written
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
 }
+// the same through L1 (.ca): for gathers that read each source line several times within one stage
+__device__ __forceinline__ void cp_async_16_ca(uint32_t dst, const void *src, bool valid) {
+    const uint32_t sz = valid ? 16u : 0u;
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
