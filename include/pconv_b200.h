@@ -410,6 +410,19 @@ int pcb_sgd_step(float *param, const float *grad, float *momentum_buf, long long
    arenas and folds the 1/world of the mean in here instead of a separate pass over the arena. */
 int pcb_sgd_step_scaled(float *param, const float *grad, float *momentum_buf, long long numel, float lr, float momentum,
                         float weight_decay, int nesterov, int first_step, float grad_scale, pcb_stream_t stream);
+/* the same update with the learning rate read from device memory (`lr`: one fp32, e.g. written by pcb_lr_cyclic earlier in the
+   stream), so a captured graph follows a schedule.  No first-step flag: the momentum buffer is always read (zero-initialise it;
+   momentum * 0 + d == d), so a buffer restored from a checkpoint is never discarded. */
+int pcb_sgd_step_dev(float *param, const float *grad, float *momentum_buf, long long numel, const float *lr, float momentum,
+                     float weight_decay, int nesterov, float grad_scale, pcb_stream_t stream);
+/* cyclical learning rate (the reference's CyclicLR, models/utils/cls.py): one thread reads the iteration counter (device int64),
+   writes that iteration's rate to `lr` (device fp32, for pcb_sgd_step_dev) and `lr64` (device fp64) and increments the counter.
+   Evaluated in fp64 in the reference's operation order, each operation rounded once: triangular and triangular2 rates are
+   bit-identical to the reference's; exp_range uses CUDA's pow for gamma^iteration.  step_size > 0 (iterations per half
+   cycle). */
+enum { PCB_CLR_TRIANGULAR = 0, PCB_CLR_TRIANGULAR2 = 1, PCB_CLR_EXP_RANGE = 2 };
+int pcb_lr_cyclic(long long *iteration, double base_lr, double max_lr, double step_size, int mode, double gamma, float *lr,
+                  double *lr64, pcb_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -13,6 +13,7 @@ ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_RELU6 = 0, 1, 2, 3
 MAX_PARTS = 8
 SEG_FOCAL, SEG_BOOTSTRAP = 0, 1
 SEG_NONE, SEG_MEAN, SEG_SUM = 0, 1, 2
+CLR_TRIANGULAR, CLR_TRIANGULAR2, CLR_EXP_RANGE = 0, 1, 2
 # PCB_ROUTE_* of pcb_debug_conv_routes, by code
 ROUTES = ("none", "generic", "depthwise", "stem", "k2r", "smallco", "tma", "tma_s2", "gather")
 
@@ -121,6 +122,9 @@ _SIGS = {
     "pcb_l1_mean_backward": (c_int, [c_void_p, c_int, c_ll, c_float, c_void_p, c_void_p]),
     "pcb_sgd_step": (c_int, [c_void_p, c_void_p, c_void_p, c_ll, c_float, c_float, c_float, c_int, c_int, c_void_p]),
     "pcb_sgd_step_scaled": (c_int, [c_void_p, c_void_p, c_void_p, c_ll, c_float, c_float, c_float, c_int, c_int, c_float, c_void_p]),
+    "pcb_sgd_step_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_float, c_float, c_int, c_float, c_void_p]),
+    "pcb_lr_cyclic": (c_int, [c_void_p, ctypes.c_double, ctypes.c_double, ctypes.c_double, c_int, ctypes.c_double, c_void_p, c_void_p,
+                              c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGS)

@@ -691,8 +691,12 @@ __global__ void l1_bwd_kernel(const T *__restrict__ x, long long numel, float gs
     }
 }
 
-__global__ void sgd_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ buf, long long numel, float lr, float mom,
-                           float wd, int nesterov, int first, float gscale) {
+// kDevLr: the learning rate is read from device memory (lr_dev, written by lr_cyclic_kernel earlier in the same stream), so a
+// captured graph follows the schedule; otherwise it is the launch argument lr.  One body: both entry points round alike.
+template <bool kDevLr>
+__global__ void sgd_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ buf, long long numel, float lr,
+                           const float *__restrict__ lr_dev, float mom, float wd, int nesterov, int first, float gscale) {
+    if (kDevLr) lr = *lr_dev;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < numel; i += static_cast<long long>(gridDim.x) * blockDim.x) {
         float d = g[i] * gscale + wd * p[i];
         if (mom != 0.f) {
@@ -702,6 +706,32 @@ __global__ void sgd_kernel(float *__restrict__ p, const float *__restrict__ g, f
         }
         p[i] -= lr * d;
     }
+}
+
+// The reference's CyclicLR.get_lr() (models/utils/cls.py:143-157) at iteration *it, then ++*it.  fp64, operation for operation in
+// numpy's order, each rounded once (the _rn intrinsics are never contracted into FMAs), so the rate rounds like the reference's:
+//   cycle = floor(1 + it / (2 step)),  x = |it / step - 2 cycle + 1|,  h = (max - base) max(0, 1 - x),  lr = base + h scale
+// scale: 1 (triangular); 1 / 2^(cycle - 1) (triangular2), exact, and 0 where numpy's 2.0 ** (cycle - 1) overflows to inf;
+// gamma^it (exp_range), CUDA's pow (within 2 ulp of the correctly rounded power).
+__global__ void lr_cyclic_kernel(long long *it, double base_lr, double max_lr, double step, int mode, double gamma, float *lr32,
+                                 double *lr64) {
+    const long long i = *it;
+    const double t = static_cast<double>(i);
+    const double cycle = floor(__dadd_rn(1.0, __ddiv_rn(t, __dmul_rn(2.0, step))));
+    const double x = fabs(__dadd_rn(__dsub_rn(__ddiv_rn(t, step), __dmul_rn(2.0, cycle)), 1.0));
+    const double rise = __dsub_rn(1.0, x);
+    const double height = __dmul_rn(__dsub_rn(max_lr, base_lr), rise > 0.0 ? rise : 0.0);
+    double scale = 1.0;
+    if (mode == PCB_CLR_TRIANGULAR2) {
+        const double e = __dsub_rn(cycle, 1.0);
+        scale = e > 1023.0 ? 0.0 : scalbn(1.0, -static_cast<int>(e));
+    } else if (mode == PCB_CLR_EXP_RANGE) {
+        scale = pow(gamma, t);
+    }
+    const double lr = __dadd_rn(base_lr, __dmul_rn(height, scale));
+    *lr64 = lr;
+    *lr32 = __double2float_rn(lr);
+    *it = i + 1;
 }
 
 }  // namespace
@@ -1031,7 +1061,27 @@ extern "C" __attribute__((visibility("default"))) int pcb_l1_mean_backward(const
 extern "C" __attribute__((visibility("default"))) int pcb_sgd_step_scaled(float *param, const float *grad, float *momentum_buf, long long numel, float lr, float momentum,
                             float weight_decay, int nesterov, int first_step, float grad_scale, pcb_stream_t stream) {
     PCB_CHECK(param && grad && numel > 0 && (momentum == 0.f || momentum_buf), "pcb_sgd_step: bad arguments");
-    sgd_kernel<<<ew_grid(numel, EW_THREADS * 8), EW_THREADS, 0, ST>>>(param, grad, momentum_buf, numel, lr, momentum, weight_decay, nesterov, first_step, grad_scale);
+    sgd_kernel<false><<<ew_grid(numel, EW_THREADS * 8), EW_THREADS, 0, ST>>>(param, grad, momentum_buf, numel, lr, nullptr, momentum, weight_decay,
+                                                                          nesterov, first_step, grad_scale);
+    PCB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" __attribute__((visibility("default"))) int pcb_sgd_step_dev(float *param, const float *grad, float *momentum_buf, long long numel, const float *lr,
+                                                                       float momentum, float weight_decay, int nesterov, float grad_scale,
+                                                                       pcb_stream_t stream) {
+    PCB_CHECK(param && grad && lr && numel > 0 && (momentum == 0.f || momentum_buf), "pcb_sgd_step_dev: bad arguments");
+    sgd_kernel<true><<<ew_grid(numel, EW_THREADS * 8), EW_THREADS, 0, ST>>>(param, grad, momentum_buf, numel, 0.f, lr, momentum, weight_decay, nesterov,
+                                                                         0, grad_scale);
+    PCB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" __attribute__((visibility("default"))) int pcb_lr_cyclic(long long *iteration, double base_lr, double max_lr, double step_size, int mode,
+                                                                    double gamma, float *lr, double *lr64, pcb_stream_t stream) {
+    PCB_CHECK(iteration && lr && lr64 && step_size > 0.0 && mode >= PCB_CLR_TRIANGULAR && mode <= PCB_CLR_EXP_RANGE,
+              "pcb_lr_cyclic: bad arguments");
+    lr_cyclic_kernel<<<1, 1, 0, ST>>>(iteration, base_lr, max_lr, step_size, mode, gamma, lr, lr64);
     PCB_LAUNCH_CHECK();
     return 0;
 }

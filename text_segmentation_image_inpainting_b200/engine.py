@@ -5,12 +5,16 @@ into the convolution epilogues.
 
 The reference has no train script (SURVEY 3): its recipe is prose -- SGD + Nesterov momentum, weight decay,
 cyclic LR (checkpoints/ReadME.md:4).  One step here = forward + loss + backward (+ all-reduce) + SGD update,
-the unit BASELINE.json's images/sec is quoted on.
+the unit BASELINE.json's images/sec is quoted on.  `TrainStep(..., lr_schedule=CyclicLR(...))` runs the recipe's schedule on
+the device, inside the captured step; `TrainStep.state_dict()` / `load_state_dict()` save and resume a run.
 """
 from __future__ import annotations
 
 import ctypes
+import math
+import numbers
 import os
+from collections import OrderedDict
 from typing import List, Optional
 
 import torch
@@ -69,13 +73,77 @@ class FlatParams:
                 self.sink_of[i] = p._pcb_grad_sink
 
 
+class CyclicLR:
+    """The reference's cyclical learning rate (models/utils/cls.py, `CyclicLR`) as a TrainStep schedule: the same arguments and
+    defaults, without the optimizer.  The rate is computed on the device at every update (ops.lr_cyclic), so a captured step
+    follows it.  Modes: "triangular", "triangular2" (amplitude halved every cycle), "exp_range" (amplitude times
+    gamma ** iteration).  A custom `scale_fn` cannot run on the device and is refused.
+
+    `last_batch_iteration=k` resumes as the reference documents: the first update runs iteration k + 1."""
+
+    MODES = {"triangular": _lib.CLR_TRIANGULAR, "triangular2": _lib.CLR_TRIANGULAR2, "exp_range": _lib.CLR_EXP_RANGE}
+
+    def __init__(self, base_lr=1e-3, max_lr=6e-3, step_size=2000, mode="triangular", gamma=1.0, scale_fn=None,
+                 scale_mode="cycle", last_batch_iteration=-1):
+        if scale_fn is not None:
+            raise ValueError("CyclicLR: a custom scale_fn cannot run on the device; use mode='triangular', 'triangular2' or "
+                             "'exp_range'")
+        if mode not in self.MODES:
+            raise ValueError(f"CyclicLR: mode must be one of {sorted(self.MODES)}, got {mode!r}")
+        for name, v in (("base_lr", base_lr), ("max_lr", max_lr), ("step_size", step_size), ("gamma", gamma)):
+            if not isinstance(v, numbers.Real) or isinstance(v, bool) or not math.isfinite(v):
+                raise ValueError(f"CyclicLR: {name} must be a finite real number (one parameter group), got {v!r}")
+        if step_size <= 0:
+            raise ValueError(f"CyclicLR: step_size must be positive, got {step_size!r}")
+        if not isinstance(last_batch_iteration, numbers.Integral) or isinstance(last_batch_iteration, bool) or last_batch_iteration < -1:
+            raise ValueError(f"CyclicLR: last_batch_iteration must be an integer >= -1, got {last_batch_iteration!r}")
+        self.base_lr, self.max_lr, self.step_size = float(base_lr), float(max_lr), step_size
+        self.mode, self.gamma, self.last_batch_iteration = mode, float(gamma), int(last_batch_iteration)
+
+    def rate(self, iteration: int) -> float:
+        """The rate of `iteration` on the host, in the reference's fp64 order (the device computes the same)."""
+        step = float(self.step_size)
+        cycle = math.floor(1 + iteration / (2 * step))
+        x = abs(iteration / step - 2 * cycle + 1)
+        height = (self.max_lr - self.base_lr) * max(0.0, 1 - x)
+        if self.mode == "triangular2":
+            scale = 0.0 if cycle - 1 > 1023 else 1 / (2.0 ** (cycle - 1))
+        elif self.mode == "exp_range":
+            scale = self.gamma ** iteration
+        else:
+            scale = 1.0
+        return self.base_lr + height * scale
+
+
 class TrainStep:
+    """One training step: forward, loss, backward, (data parallel: gradient all-reduce,) SGD with momentum, Nesterov and weight
+    decay, captured in one CUDA graph by `warmup_and_capture()`.
+
+    Learning rate: the constant `lr`, or with `lr_schedule=CyclicLR(...)` a rate computed on the device before every update
+    (the counter and the rate live in device memory, so each graph replay advances the schedule; `lr` is then unused and
+    assigning it raises).  Every update counts, the eager warm-up updates of `warmup_and_capture()` included.
+    `iteration` is the schedule iteration the next update runs, `last_lr` the rate of the last one (device fp64 scalar).
+
+    Checkpoints: `state_dict()` / `load_state_dict()` save and restore the parameters, module buffers, momentum, schedule counter
+    and the batcher's generator; see there."""
+
     def __init__(self, net: torch.nn.Module, compute_dtype=torch.bfloat16, lr=2e-4, momentum=0.9, weight_decay=1e-4,
-                 nesterov=True, process_group=None, use_graph=True, bucket_mb=32, overlap_allreduce=None):
+                 nesterov=True, process_group=None, use_graph=True, bucket_mb=32, overlap_allreduce=None,
+                 lr_schedule: Optional[CyclicLR] = None):
         self.net = net.train()
         self.dtype = compute_dtype
-        self.lr, self.momentum, self.wd, self.nesterov = lr, momentum, weight_decay, nesterov
+        if lr_schedule is not None and not isinstance(lr_schedule, CyclicLR):
+            raise TypeError("lr_schedule must be an engine.CyclicLR")
+        self.lr_schedule = lr_schedule
+        self._lr, self.momentum, self.wd, self.nesterov = lr, momentum, weight_decay, nesterov
         self.flat = FlatParams(net)
+        if lr_schedule is not None:
+            dev = self.flat.flat_p.device
+            start = lr_schedule.last_batch_iteration + 1
+            self._lr_iter = torch.tensor([start], dtype=torch.int64, device=dev)
+            self._lr32 = torch.zeros(1, dtype=torch.float32, device=dev)
+            # before the first update: the rate that update will use, as the reference's CyclicLR sets it at construction
+            self._lr64 = torch.tensor(lr_schedule.rate(start), dtype=torch.float64, device=dev)
         self._wcaches = [m._wcache for m in net.modules() if isinstance(getattr(m, "_wcache", None), dict)]
         self.pg = process_group
         self.world = torch.distributed.get_world_size(process_group) if process_group is not None else 1
@@ -101,14 +169,43 @@ class TrainStep:
         if self.pg is not None:
             self._sync_replicas()
 
-    def _sync_replicas(self):
-        """Data parallel start-up: every rank adopts rank 0's parameters and module buffers (BatchNorm running statistics,
-        `num_batches_tracked`), like torch DDP does, so replicas built from different seeds or checkpoints cannot silently
-        diverge.  BatchNorm batch statistics stay rank-local afterwards (the reference has no SyncBN); running statistics
-        therefore drift per rank during training and rank 0's are the ones to checkpoint."""
+    @property
+    def lr(self):
+        return self._lr
+
+    @lr.setter
+    def lr(self, value):
+        if self.lr_schedule is not None:
+            raise AttributeError("this TrainStep follows its lr_schedule: the rate is computed on the device at every update")
+        self._lr = value
+
+    @property
+    def iteration(self) -> Optional[int]:
+        """The schedule iteration the next update runs (the reference's `last_batch_iteration + 1`); None without a schedule.
+        Reading it synchronises with the device."""
+        return int(self._lr_iter.item()) if self.lr_schedule is not None else None
+
+    @property
+    def last_lr(self) -> Optional[torch.Tensor]:
+        """The rate of the last update as a device fp64 scalar, overwritten by the next update (reading it does not
+        synchronise); before the first update, the rate that update will use.  None without a schedule."""
+        return self._lr64 if self.lr_schedule is not None else None
+
+    def _sync_replicas(self, momentum=False):
+        """Data parallel start-up and resume: every rank adopts rank 0's parameters, schedule counter and module buffers
+        (BatchNorm running statistics, `num_batches_tracked`), like torch DDP does, so replicas built from different seeds or
+        checkpoints cannot silently diverge; every rank then computes the same rate from the same counter.  `momentum`: the
+        momentum arena too (after a load; at construction it is zeros on every rank).  BatchNorm batch statistics stay
+        rank-local afterwards (the reference has no SyncBN); running statistics therefore drift per rank during training and
+        rank 0's are the ones to checkpoint."""
         dist = torch.distributed
         src = dist.get_global_rank(self.pg, 0)
         dist.broadcast(self.flat.flat_p, src=src, group=self.pg)
+        if momentum:
+            dist.broadcast(self.flat.flat_m, src=src, group=self.pg)
+        if self.lr_schedule is not None:
+            dist.broadcast(self._lr_iter, src=src, group=self.pg)
+            dist.broadcast(self._lr64, src=src, group=self.pg)
         for b in self.net.buffers():
             dist.broadcast(b, src=src, group=self.pg)
         ops.bump_weight_epoch()
@@ -240,8 +337,14 @@ class TrainStep:
         return ops.l1_mean(self.net((xin, hm)))
 
     def _update(self, first_step: bool):
-        ops.sgd_step(self.flat.flat_p, self.flat.flat_g, self.flat.flat_m, self.lr, self.momentum, self.wd, self.nesterov,
-                     first_step, grad_scale=self.grad_scale)
+        if self.lr_schedule is None:
+            ops.sgd_step(self.flat.flat_p, self.flat.flat_g, self.flat.flat_m, self.lr, self.momentum, self.wd, self.nesterov,
+                         first_step, grad_scale=self.grad_scale)
+            return
+        s = self.lr_schedule
+        ops.lr_cyclic(self._lr_iter, self._lr32, self._lr64, s.base_lr, s.max_lr, s.step_size, CyclicLR.MODES[s.mode], s.gamma)
+        ops.sgd_step_dev(self.flat.flat_p, self.flat.flat_g, self.flat.flat_m, self._lr32, self.momentum, self.wd, self.nesterov,
+                         grad_scale=self.grad_scale)
 
     def _step(self, x, mask, first_step: bool, overlap=None):
         overlap = self.overlap if overlap is None else overlap
@@ -321,6 +424,123 @@ class TrainStep:
         self.first = False
         return loss
 
+    # -- checkpoints ----------------------------------------------------------------------------------
+    def _arena_views(self, arena):
+        """Per trainable parameter (FlatParams order), its slice of `arena` with the parameter's logical shape."""
+        return [_flat_view(arena, o, p.data) for p, o in zip(self.flat.params, self.flat.offsets)]
+
+    def state_dict(self) -> dict:
+        """The training state as CPU tensors (for torch.save; loads on any machine):
+
+          * "model": `net.state_dict()` -- the reference's keys, BatchNorm buffers included;
+          * "optimizer": in torch.optim.SGD's state_dict format over the trainable parameters (FlatParams order:
+            `[p for p in net.parameters() if p.requires_grad]`), each momentum buffer in its parameter's logical shape;
+            `param_groups[0]["lr"]` is the current rate (`last_lr` with a schedule);
+          * "last_batch_iteration" (with a schedule): the value that continues the reference's CyclicLR;
+          * "batcher_rng" (steps fed by a GPU batcher): the batcher's device generator state.
+
+        Data parallel: save rank 0's (its BatchNorm running statistics are the ones that count, see _sync_replicas)."""
+        def cpu(t):
+            return t.detach().to("cpu", copy=True)
+        sched = self.lr_schedule is not None
+        group = {"lr": float(self._lr64) if sched else float(self.lr), "momentum": self.momentum, "dampening": 0,
+                 "weight_decay": self.wd, "nesterov": bool(self.nesterov), "maximize": False, "foreach": None,
+                 "differentiable": False, "fused": None, "params": list(range(len(self.flat.params)))}
+        state = {}
+        if self.momentum != 0:
+            state = {i: {"momentum_buffer": cpu(m)} for i, m in enumerate(self._arena_views(self.flat.flat_m))}
+        sd = {"model": OrderedDict((k, cpu(v)) for k, v in self.net.state_dict().items()),
+              "optimizer": {"state": state, "param_groups": [group]}}
+        if sched:
+            sd["last_batch_iteration"] = self.iteration - 1
+        batcher = getattr(self, "batcher", None)
+        if batcher is not None:
+            sd["batcher_rng"] = cpu(batcher.rng)
+        return sd
+
+    def _momentum_buffers(self, opt) -> list:
+        """The momentum buffer of every trainable parameter (None: zeros) from a torch.optim.SGD-format state dict, whose one
+        parameter group lists either the trainable parameters or all of `net.parameters()` (frozen ones carry no state)."""
+        groups = opt.get("param_groups")
+        if not isinstance(groups, (list, tuple)) or len(groups) != 1:
+            raise ValueError("load_state_dict: the optimizer state must have exactly one parameter group")
+        g = groups[0]
+        for key, have, want in (("momentum", float(g.get("momentum", 0.0)), float(self.momentum)),
+                                ("nesterov", bool(g.get("nesterov", False)), bool(self.nesterov)),
+                                ("dampening", float(g.get("dampening", 0.0)), 0.0),
+                                ("maximize", bool(g.get("maximize", False)), False)):
+            if have != want:
+                raise ValueError(f"load_state_dict: the checkpoint's {key} is {have}, this step's {want}: its momentum buffers "
+                                 "would mean something else")
+        params = self.flat.params
+        every = list(self.net.parameters())
+        ids = list(g.get("params", []))
+        if len(ids) == len(params):
+            order = params
+        elif len(ids) == len(every):
+            order = every
+        else:
+            raise ValueError(f"load_state_dict: the optimizer state lists {len(ids)} parameters; this network has {len(params)} "
+                             f"trainable of {len(every)}")
+        pos = {id(p): i for i, p in enumerate(params)}
+        state = opt.get("state", {})
+        bufs = [None] * len(params)
+        for j, (pid, p) in enumerate(zip(ids, order)):
+            buf = state.get(pid, {}).get("momentum_buffer")
+            if buf is None:
+                continue
+            if id(p) not in pos:
+                raise ValueError(f"load_state_dict: optimizer parameter {j} is frozen here but carries a momentum buffer")
+            if tuple(buf.shape) != tuple(p.shape):
+                raise ValueError(f"load_state_dict: optimizer parameter {j}: momentum buffer of shape {tuple(buf.shape)}, "
+                                 f"parameter of shape {tuple(p.shape)}")
+            bufs[pos[id(p)]] = buf
+        return bufs
+
+    def load_state_dict(self, state_dict: dict):
+        """Restore a `state_dict()` (or a checkpoint of the reference modules: their state_dict as "model" and a
+        torch.optim.SGD state_dict as "optimizer") IN PLACE: parameters and momentum into their arenas, module buffers
+        (`num_batches_tracked` included), the schedule counter (from "last_batch_iteration"; without it, the schedule's own
+        start) and the batcher's generator (when saved).  A missing momentum buffer means zeros.  The captured graph keeps
+        replaying, now from the loaded state: capture first, then load (the warm-up of `warmup_and_capture()` takes real
+        updates, which the load overwrites).
+
+        The learning rate and weight decay stay this step's own; a momentum, nesterov, dampening or maximize that differs
+        from it, or a parameter count or shape mismatch, raises ValueError before anything is written.  Data parallel: rank
+        0's loaded state is then broadcast to every rank."""
+        if "model" not in state_dict or "optimizer" not in state_dict:
+            raise ValueError("load_state_dict: needs 'model' and 'optimizer' entries (net.load_state_dict loads weights alone)")
+        model = state_dict["model"]
+        own = self.net.state_dict()
+        if set(model) != set(own):
+            missing, extra = sorted(set(own) - set(model)), sorted(set(model) - set(own))
+            raise ValueError(f"load_state_dict: model keys differ: missing {missing[:5]}, unexpected {extra[:5]}")
+        for k, v in own.items():
+            if tuple(model[k].shape) != tuple(v.shape):
+                raise ValueError(f"load_state_dict: {k} has shape {tuple(model[k].shape)}, the network's {tuple(v.shape)}")
+        bufs = self._momentum_buffers(state_dict["optimizer"])
+        it = None
+        if self.lr_schedule is not None:
+            it = int(state_dict.get("last_batch_iteration", self.lr_schedule.last_batch_iteration)) + 1
+            if it < 0:
+                raise ValueError("load_state_dict: last_batch_iteration must be >= -1")
+        batcher, rng = getattr(self, "batcher", None), state_dict.get("batcher_rng")
+        if batcher is not None and rng is not None and tuple(rng.shape) != tuple(batcher.rng.shape):
+            raise ValueError(f"load_state_dict: batcher_rng has shape {tuple(rng.shape)}, expected {tuple(batcher.rng.shape)}")
+        with torch.no_grad():
+            for k, v in own.items():
+                v.copy_(model[k])
+            for view, buf in zip(self._arena_views(self.flat.flat_m), bufs):
+                view.zero_() if buf is None else view.copy_(buf)
+            if it is not None:
+                self._lr_iter.fill_(it)
+                self._lr64.fill_(self.lr_schedule.rate(it))
+            if batcher is not None and rng is not None:
+                batcher.rng.copy_(rng)
+        self.first = False          # the constant-rate path must read the restored momentum on its next update
+        ops.bump_weight_epoch()
+        if self.pg is not None:
+            self._sync_replicas(momentum=True)
 
     def close(self):
         """Destroy the captured graphs (the step falls back to eager mode).  REQUIRED before

@@ -1153,6 +1153,31 @@ def sgd_step(param, grad, buf, lr, momentum=0.0, weight_decay=0.0, nesterov=Fals
     bump_weight_epoch()
 
 
+def sgd_step_dev(param, grad, buf, lr, momentum=0.0, weight_decay=0.0, nesterov=False, grad_scale=1.0):
+    """sgd_step with the learning rate read on the device from `lr` (fp32, one element) and no first-step flag: `buf` is always
+    read, so it must start zeroed (momentum * 0 + d == d) and a restored buffer is never discarded."""
+    lib = _lib.load()
+    if not param.is_cuda or not (param.is_contiguous() or param.is_contiguous(memory_format=CL)) or param.stride() != grad.stride():
+        raise _lib.PcbError("sgd_step_dev: param and grad must be dense CUDA tensors with identical strides")
+    if lr.dtype != torch.float32 or lr.numel() != 1 or lr.device != param.device:
+        raise _lib.PcbError("sgd_step_dev: lr must be one fp32 element on the parameters' device")
+    _lib.check(lib.pcb_sgd_step_dev(param.data_ptr(), grad.data_ptr(), _ptr(buf), param.numel(), lr.data_ptr(), float(momentum),
+                                    float(weight_decay), int(nesterov), float(grad_scale), _stream()))
+    bump_weight_epoch()
+
+
+def lr_cyclic(iteration, lr, lr64, base_lr, max_lr, step_size, mode, gamma=1.0):
+    """The cyclical learning rate of device iteration counter `iteration` (int64, one element) into `lr` (fp32) and `lr64`
+    (fp64), then iteration += 1 -- all on the device, so a captured graph advances the schedule on every replay.  `mode`:
+    _lib.CLR_TRIANGULAR, CLR_TRIANGULAR2 or CLR_EXP_RANGE."""
+    lib = _lib.load()
+    if iteration.dtype != torch.int64 or lr.dtype != torch.float32 or lr64.dtype != torch.float64 or \
+            not (iteration.device == lr.device == lr64.device) or not iteration.is_cuda:
+        raise _lib.PcbError("lr_cyclic: iteration (int64), lr (fp32) and lr64 (fp64) must be CUDA tensors on one device")
+    _lib.check(lib.pcb_lr_cyclic(iteration.data_ptr(), float(base_lr), float(max_lr), float(step_size), int(mode), float(gamma),
+                                 lr.data_ptr(), lr64.data_ptr(), _stream()))
+
+
 # ------------------------------------------------------------------------------------------------
 # dense (non-partial) building blocks of the segmentation networks
 # ------------------------------------------------------------------------------------------------
