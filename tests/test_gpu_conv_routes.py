@@ -87,6 +87,12 @@ DTYPES = {"bf16": (torch.bfloat16, _lib.PCB_BF16), "f32": (torch.float32, _lib.P
 TC_ROUTES = {"stem", "k2r", "smallco", "tma", "tma_s2", "gather"}
 
 
+def accumulation_bound(nz, mag, rounds_bf16_intermediate):
+    """the Gaussian-regime bound of one convolution direction (module docstring): n nonzero products added in any order with
+    one-ulp fp32 additions, n 2^-22 M, plus 2^-8 M where the route rounds an intermediate sum to bf16"""
+    return nz * 2.0 ** -22 * mag + (2.0 ** -8 * mag if rounds_bf16_intermediate else 0.0)
+
+
 def _rup8(v):
     return (v + 7) // 8 * 8
 
@@ -651,7 +657,7 @@ def test_conv_route_vs_fp64(name):
     b = bias.double()[None, :, None, None]
     acc = P.conv_ref(P.XM, P.W)
     mag = P.conv_ref(P.XM.abs(), P.W.abs())
-    e_acc = P.nz_fwd * 2.0 ** -22 * mag + (2.0 ** -8 * mag if route[0] == "k2r" else 0.0)
+    e_acc = accumulation_bound(P.nz_fwd, mag, route[0] == "k2r")
     v_ref = torch.where(empty, torch.zeros_like(acc), acc / safe + b)
     e_ref = torch.where(empty, torch.zeros_like(acc), e_acc / safe + 2.0 ** -22 * (acc.abs() / safe + v_ref.abs()))
     del acc, mag, e_acc
@@ -719,11 +725,11 @@ def test_conv_route_vs_fp64(name):
     rounds_d = route[1] == "k2r" or (route[1] != "none" and at_src)
     gref = P.dgrad_ref(G, P.W) * P.M
     gmag = P.dgrad_ref(G.abs(), P.W.abs()) * P.M
-    gerr = P.nz_dg * 2.0 ** -22 * gmag + (2.0 ** -8 * gmag if rounds_d else 0.0)
+    gerr = accumulation_bound(P.nz_dg, gmag, rounds_d)
     refs, errs = P.dx_parts(gref, at_src), P.dx_parts(gerr, at_src)
     check_dx("Gaussian data gradient", dxs, refs, [e + store * (r.abs() + e) for r, e in zip(refs, errs)])
     del gref, gmag, gerr
     wref = P.wgrad_ref(P.XM, G)
     wmag = P.wgrad_ref(P.XM.abs(), G.abs())
-    werr = P.nz_wg * 2.0 ** -22 * wmag + (2.0 ** -8 * wmag if route[2] == "k2r" else 0.0)
+    werr = accumulation_bound(P.nz_wg, wmag, route[2] == "k2r")
     assert_within(f"{name}: Gaussian weight gradient", dw.double(), wref.permute(0, 2, 3, 1), werr.permute(0, 2, 3, 1))
