@@ -303,6 +303,29 @@ int pcb_inpaint_sample(const pcb_inpaint_src *srcs, int n, int out, int strokes,
 int pcb_inpaint_prepare(const pcb_inpaint_src *srcs, const pcb_inpaint_params *params, int n, int cap_h, int cap_w, int out,
                         int strokes, uint8_t *tmp, void *corrupted, int dtype, uint8_t *mask_plane, float *clean, pcb_stream_t stream);
 
+/* ---- inpainting data from raw/clean page pairs (TestDataset.process_images + get_mask, Dataloader.py:201-222) -------------
+ * One decoded pair per image: the raw page and its text-cleaned copy, RGB uint8 [h][stride] each (3 bytes per pixel), the same
+ * size (the crop box is drawn on raw and applied to both).  32 bytes with the layout of pcb_inpaint_src. */
+typedef struct {
+    const uint8_t *raw;
+    const uint8_t *clean;
+    int32_t h, w, raw_stride, clean_stride;
+} pcb_inpaint_pair_src;
+/* pcb_inpaint_validate for a staged pair batch; explicit parameters must also have gray == 0 (no RandomGrayscale). */
+int pcb_inpaint_pair_validate(const pcb_inpaint_pair_src *h_srcs, const pcb_inpaint_params *h_params, int n, int cap_n, int cap_h,
+                              int cap_w, int out);
+/* pcb_inpaint_sample's draws for pair sources: the same Philox slots, so the same crop boxes and strokes for the same seed,
+ * counter and sizes, with the grayscale flag always 0. */
+int pcb_inpaint_pair_sample(const pcb_inpaint_pair_src *srcs, int n, int out, int strokes, uint64_t *rng, pcb_inpaint_params *params,
+                            pcb_stream_t stream);
+/* TestDataset.process_images for a batch, two launches: Pillow-exact bicubic crop + resize of raw and clean, Image.convert("L")
+ * of both, |L_raw - L_clean| (ImageChops.difference), the strokes drawn at 255 on the difference (if `strokes`), > 0.4 * 255,
+ * cv2.dilate(10x10), ToTensor and clean * (1 - mask).  tmp: uint8 [n][cap_h][out][8] scratch (raw RGB0 | clean RGB0: twice
+ * pcb_inpaint_prepare's, 134 MB at n = 8, cap_h = 4096, out = 512).  Outputs as pcb_inpaint_prepare's; grids depend on n,
+ * cap_h and out only. */
+int pcb_inpaint_pair_prepare(const pcb_inpaint_pair_src *srcs, const pcb_inpaint_params *params, int n, int cap_h, int cap_w, int out,
+                             int strokes, uint8_t *tmp, void *corrupted, int dtype, uint8_t *mask_plane, float *clean, pcb_stream_t stream);
+
 /* ---- segmentation training data (TextSegmentationData.process_images, Dataloader.py:66-74) -------------------------------
  * One decoded source per image: the gray (`L`) page uint8 [h][page_stride] and its text mask uint8 [h][mask_stride]. */
 typedef struct {

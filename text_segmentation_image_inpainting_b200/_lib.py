@@ -93,6 +93,10 @@ _SIGS = {
     "pcb_inpaint_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_inpaint_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                     c_void_p]),
+    "pcb_inpaint_pair_validate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int]),
+    "pcb_inpaint_pair_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "pcb_inpaint_pair_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                         c_void_p, c_void_p]),
     "pcb_seg_validate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int]),
     "pcb_seg_sample": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_seg_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,

@@ -1,6 +1,8 @@
 """Training batches prepared on the GPU from decoded source bytes: the reference's `process_images` for a whole batch.
 
   * `InpaintBatcher`: `ImageInpaintingData.process_images` (Dataloader.py:110-162), csrc/inpaint_data.cu.
+  * `InpaintPairBatcher`: `TestDataset.process_images` (Dataloader.py:165-222), the masks derived from raw/clean page pairs,
+    csrc/inpaint_data.cu.
   * `SegBatcher`: `TextSegmentationData.process_images` (Dataloader.py:66-74), csrc/seg_data.cu.
 
 Both share the host side (`_SourceStager`): the host decodes files and calls `stage(samples)`, which copies the uint8 bytes
@@ -10,7 +12,7 @@ fixed addresses, so the training steps of engine.py capture the whole thing in t
 within the capacity replays without recapture.  Source bytes are double buffered: the upload of the next batch overlaps the
 current step.
 
-InpaintBatcher returns the reference's triplet, batched, in the layouts the training step consumes:
+InpaintBatcher and InpaintPairBatcher return the reference's triplet, batched, in the layouts the training step consumes:
 
   * corrupted: `[n, 3, s, s]` view of an 8-channel-padded NHWC buffer in the compute dtype (TrainStep._prepare's layout),
   * mask:      `HoleMask` over one uint8 plane `[n, s, s]` (1 = valid), 3 channels,
@@ -94,7 +96,7 @@ class _SourceStager:
         for i, (a, b) in enumerate(samples):
             a, b = np.asarray(a), np.asarray(b)
             self._check_sample(i, a, b)
-            h, w = b.shape
+            h, w = b.shape[:2]
             if h > self.cap_h or w > self.cap_w:
                 raise ValueError(f"sample {i} is {h}x{w}, capacity {self.cap_h}x{self.cap_w}")
             na, nb = h * w * ca, h * w * cb
@@ -136,6 +138,9 @@ class InpaintBatcher(_SourceStager):
     `image_size`).  `add_random_masks` draws random_masks' strokes; `seed` seeds the device generator.  `stage(samples)` takes
     `batch` pairs (RGB uint8 [h, w, 3], text mask uint8 [h, w])."""
 
+    _sample, _prepare = "pcb_inpaint_sample", "pcb_inpaint_prepare"
+    _TMP_PIXEL_BYTES = 4            # the horizontal pass's intermediate (pcb_inpaint_prepare's tmp)
+
     def __init__(self, batch: int, max_hw: Tuple[int, int], image_size: int = 512, add_random_masks: bool = True, seed: int = 0,
                  compute_dtype=torch.bfloat16, device=None):
         if compute_dtype not in (torch.bfloat16, torch.float32):
@@ -151,7 +156,7 @@ class InpaintBatcher(_SourceStager):
         dev, n, s = self.device, self.batch, self.size
         self._init_staging(seed)
         self.params = torch.zeros((n, PARAM_INTS), dtype=torch.int32, device=dev)
-        self._tmp = torch.empty(n * self.cap_h * s * 4, dtype=torch.uint8, device=dev)
+        self._tmp = torch.empty(n * self.cap_h * s * self._TMP_PIXEL_BYTES, dtype=torch.uint8, device=dev)
         self._xbuf = torch.empty((n, 8, s, s), dtype=compute_dtype, device=dev, memory_format=torch.channels_last).zero_()
         self.corrupted = self._xbuf[:, :3]
         self.plane = torch.zeros((n, s, s), dtype=torch.uint8, device=dev)
@@ -173,26 +178,50 @@ class InpaintBatcher(_SourceStager):
             self.activate()
         lib, st = _lib.load(), _stream()
         if params is None:
-            _lib.check(lib.pcb_inpaint_sample(self.table.data_ptr(), self.batch, self.size, int(self.strokes), self.rng.data_ptr(),
-                                              self.params.data_ptr(), st))
+            _lib.check(getattr(lib, self._sample)(self.table.data_ptr(), self.batch, self.size, int(self.strokes), self.rng.data_ptr(),
+                                                  self.params.data_ptr(), st))
         else:
             if capturing:
                 raise RuntimeError("explicit parameters cannot be captured; prepare(params) runs eagerly")
             p = np.ascontiguousarray(params, dtype=np.int32)
             if p.shape != (self.batch, PARAM_INTS):
                 raise ValueError(f"params must be int32 [{self.batch}, {PARAM_INTS}]")
-            _lib.check(lib.pcb_inpaint_validate(self._host_table.ctypes.data, p.ctypes.data, self.batch, self.batch, self.cap_h,
-                                                self.cap_w, self.size))
+            _lib.check(getattr(lib, self._validate)(self._host_table.ctypes.data, p.ctypes.data, self.batch, self.batch, self.cap_h,
+                                                    self.cap_w, self.size))
             self.params.copy_(torch.from_numpy(p))
-        _lib.check(lib.pcb_inpaint_prepare(self.table.data_ptr(), self.params.data_ptr(), self.batch, self.cap_h, self.cap_w, self.size,
-                                           int(self.strokes), self._tmp.data_ptr(), self._xbuf.data_ptr(),
-                                           _lib.PCB_BF16 if self.dtype == torch.bfloat16 else _lib.PCB_F32, self.plane.data_ptr(),
-                                           self.clean.data_ptr(), st))
+        _lib.check(getattr(lib, self._prepare)(self.table.data_ptr(), self.params.data_ptr(), self.batch, self.cap_h, self.cap_w,
+                                               self.size, int(self.strokes), self._tmp.data_ptr(), self._xbuf.data_ptr(),
+                                               _lib.PCB_BF16 if self.dtype == torch.bfloat16 else _lib.PCB_F32, self.plane.data_ptr(),
+                                               self.clean.data_ptr(), st))
         if not capturing:
             self.release()
         # a new view object per call: the layers tag an input plane with the event that made it ready (ops._pconv_launch), and
         # this plane is rewritten in place by every call
         return self.corrupted, HoleMask.from_plane(self.plane.view(self.plane.shape), 3), self.clean
+
+
+class InpaintPairBatcher(InpaintBatcher):
+    """GPU `TestDataset.process_images` (Dataloader.py:201-222): inpainting batches from raw/clean page pairs, the mask being
+    where the two differ.  Both pages are cropped and resized with the one box drawn on raw; their `L` conversions are
+    subtracted (ImageChops.difference), the strokes (`add_random_masks`) are drawn at 255 on the difference, and the result is
+    thresholded at 0.4 * 255 and dilated 10x10.  There is no grayscale draw.  `prepare()` returns the same triplet as
+    InpaintBatcher (`params` rows must have the grayscale flag 0), so the training steps and engine.InpaintEvalStep take
+    either batcher.  The device draws the same crop boxes and strokes as an InpaintBatcher with the same seed and counter.
+
+    `stage(samples)` takes `batch` pairs (raw RGB uint8 [h, w, 3], clean RGB uint8 [h, w, 3]) of equal size.  Decoding and
+    pairing the files stay with the caller.  Note that `TestDataset.__getitem__` globs `clean/*` and derives the raw path
+    with `re.sub("raw", "clean", ...)`, which leaves a path without "raw" in it unchanged, so the reference as written often
+    pairs a file with itself (an empty mask).  This batcher takes whatever pair the caller decoded."""
+
+    _channels = (3, 3)
+    _validate = "pcb_inpaint_pair_validate"
+    _sample, _prepare = "pcb_inpaint_pair_sample", "pcb_inpaint_pair_prepare"
+    _TMP_PIXEL_BYTES = 8            # raw RGB0 | clean RGB0
+
+    def _check_sample(self, i, raw, clean):
+        if raw.dtype != np.uint8 or clean.dtype != np.uint8 or raw.ndim != 3 or raw.shape[2] != 3 or clean.shape != raw.shape:
+            raise ValueError(f"sample {i}: expected a uint8 RGB [h, w, 3] raw page and a clean page of the same shape and dtype, got "
+                             f"{raw.shape} {raw.dtype} / {clean.shape} {clean.dtype}")
 
 
 def seg_params(rows) -> np.ndarray:

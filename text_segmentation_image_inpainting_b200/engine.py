@@ -1,7 +1,8 @@
 """Training-step engine for the partial-conv U-Nets: flat fp32 parameter / gradient arenas, one fused SGD
 launch, optional data-parallel gradient all-reduce (NCCL over NVLink) and whole-step CUDA-graph capture.
 Inference engines (InferStep, SegInferStep): graph-captured eval-mode forward with the BatchNorm + activation passes fused
-into the convolution epilogues.
+into the convolution epilogues.  InpaintEvalStep: held-out evaluation of an inpainting U-Net on a GPU batcher, loss included,
+in one graph that coexists with a captured training step on the same network.
 
 The reference has no train script (SURVEY 3): its recipe is prose -- SGD + Nesterov momentum, weight decay,
 cyclic LR (checkpoints/ReadME.md:4).  One step here = forward + loss + backward (+ all-reduce) + SGD update,
@@ -10,6 +11,7 @@ the device, inside the captured step; `TrainStep.state_dict()` / `load_state_dic
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import math
 import numbers
@@ -419,6 +421,7 @@ class TrainStep:
             if self.graph_update is not None:
                 self._allreduce()
                 self.graph_update.replay()
+            ops.bump_weight_epoch()             # the replay updated the parameters and running statistics in place
             return self.static_loss
         loss = self._step(x, mask, self.first)
         self.first = False
@@ -585,6 +588,7 @@ class _BatcherStep:
         if self.graph_update is not None:
             self._allreduce()
             self.graph_update.replay()
+        ops.bump_weight_epoch()                 # the replay updated the parameters and running statistics in place
         return self.static_loss
 
 
@@ -803,3 +807,95 @@ class SegInferStep(InferStep):
 
     def _inputs(self, x):
         return (x,)
+
+
+class InpaintEvalStep(InferStep):
+    """Held-out evaluation of an inpainting U-Net in one CUDA graph: `batcher.prepare()` (data.InpaintBatcher or
+    data.InpaintPairBatcher: the device draws the crops and strokes), the eval-mode forward with InferStep's fused BatchNorm +
+    activation epilogues and mask-chain stream, and, with an `extractor` (loss.VggExtractor), the reference's InpaintingLoss
+    forward without a backward.  Per batch the host decodes, calls ``batcher.stage(samples)`` and ``run()``.
+
+    ``run()`` returns the output as a static fp32 NCHW buffer that the next call overwrites; `last_loss` (device fp32 scalar) and
+    `last_terms` (device fp32 [5]: valid, hole, tv, perceptual, style, unweighted) hold the loss of that batch (None without an
+    extractor).  ``batcher.reseed(seed)`` before a validation pass makes every pass draw the same crops and strokes;
+    `warmup_and_capture()` leaves the generator where it found it.
+
+    Sharing the network with a (captured) TrainStep: run() evaluates the parameters and BatchNorm running statistics as they are
+    at the call.  Every TrainStep step bumps the weight epoch, and the first run() after a change rewrites this step's operand
+    buffers and BatchNorm coefficients once (InferStep's refresh).  The forward runs on operand caches of its own, swapped in for
+    the call, so it never writes a buffer that the training graph reads, and it keeps every buffer its graph captured alive.
+    run() leaves `net.training` as it found it.  Give it a batcher of its own: the training step's batcher buffers are the
+    training graph's inputs."""
+
+    _CACHES = ("_wcache", "_pcb_k2r_cache")        # per-module operand caches (ops.prepare_weight, loss._Vgg)
+
+    def __init__(self, net: torch.nn.Module, batcher, extractor=None, feature_range=3, compute_dtype=None):
+        if compute_dtype is not None and compute_dtype != batcher.dtype:
+            raise ValueError(f"compute_dtype {compute_dtype} differs from the batcher's {batcher.dtype}")
+        training = net.training
+        super().__init__(net, compute_dtype=batcher.dtype)
+        net.train(training)
+        self.batcher = batcher
+        self.criterion = None
+        mods = list(net.modules())
+        if extractor is not None:
+            from .loss import InpaintingLoss
+            self.criterion = InpaintingLoss(extractor, feature_range)
+            mods += list(extractor.modules())
+        self._cached_modules = [m for m in mods if isinstance(getattr(m, "_wcache", None), dict)]
+        self._own = {}
+        self.last_loss = None
+
+    @property
+    def last_terms(self):
+        return self.criterion.last_terms if self.criterion is not None else None
+
+    @contextlib.contextmanager
+    def _own_state(self):
+        """Eval mode and this step's own operand caches for the duration of a call; the modules' own are restored after."""
+        training = self.net.training
+        saved = []
+        for m in self._cached_modules:
+            for name in self._CACHES:
+                saved.append((m, name, m.__dict__.get(name)))
+                m.__dict__[name] = self._own.setdefault((id(m), name), {})
+        self.net.eval()
+        try:
+            yield
+        finally:
+            self.net.train(training)
+            for m, name, cache in saved:
+                if cache is None:
+                    m.__dict__.pop(name, None)
+                else:
+                    m.__dict__[name] = cache
+
+    def _forward(self):
+        xin, hm, clean = self.batcher.prepare()
+        out = self.net((xin, hm))
+        if self.criterion is not None:
+            loss = self.criterion(clean, hm, out, clean)
+            if self.last_loss is None:
+                self.last_loss = torch.zeros((), dtype=torch.float32, device=loss.device)
+            self.last_loss.copy_(loss)
+        return out
+
+    def _key(self):
+        return ()
+
+    def _inputs(self):
+        return ()
+
+    def warmup_and_capture(self):
+        """Run the eager warm-up and capture the graph on the staged batch (the first run() does this when not called)."""
+        rng = self.batcher.rng.clone()
+        self.run()
+        self.batcher.rng.copy_(rng)
+
+    def run(self) -> torch.Tensor:
+        """Evaluate the staged batch.  Returns the static fp32 NCHW output."""
+        self.batcher.activate()
+        with self._own_state():
+            out = super().run()
+        self.batcher.release()
+        return out
