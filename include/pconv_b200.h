@@ -422,6 +422,19 @@ int pcb_seg_loss_backward(const void *x, int dtype, const long long *x_strides, 
                           int reduction, float p0, float one_minus_beta, float background_weight, float words_weight, const float *gout,
                           void *dx, const long long *dx_strides, pcb_stream_t stream);
 
+/* ---- pixel average precision of segmentation logits (metrics.PixelAveragePrecision) ---------------------------------------
+ * update: x, x_strides, target, n, h, w as for the losses above.  Each pixel's score is its logit rounded to bf16 (fp32 to
+ * nearest-even, -0 as +0); hist (device int64 [2][65536]: pixels, positives) gains one count per pixel at the score's
+ * order-preserving key (negative bf16 bits b: ~b & 0xffff, others: b | 0x8000), in row 1 when target > 0.5.  counts (device
+ * int64 [5]) gains tp, fp, fn, tn at the threshold sigmoid(x) > 0.5 of the unrounded logit, and nan: NaN logits, which count
+ * nowhere else.  Integer sums only: the result is independent of the launch grid and the order of its atomics.  No host
+ * synchronisation, no workspace (capturable).  At most 2^40 pixels per call.
+ * finalize: out (device fp64 [1]) = sklearn's average_precision_score over the histogram, 0 without positives, NaN when
+ * counts[4] > 0; one CTA in a fixed order, so repeated calls agree bit for bit. */
+int pcb_seg_score_update(const void *x, int dtype, const long long *x_strides, const float *target, int n, int h, int w,
+                         long long *hist, long long *counts, pcb_stream_t stream);
+int pcb_seg_score_finalize(const long long *hist, const long long *counts, double *out, pcb_stream_t stream);
+
 /* ---- loss / optimiser used by the benchmark step (SURVEY 8d: loss = out.abs().mean()) ------ */
 int pcb_l1_mean_forward(const void *x, int dtype, long long numel, float *loss /* device scalar, overwritten */,
                         double *scratch /* device, 1 double */, pcb_stream_t stream);

@@ -106,6 +106,8 @@ _SIGS = {
                                      c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcb_seg_loss_backward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
                                       c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcb_seg_score_update": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "pcb_seg_score_finalize": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcb_inpaint_loss_pixel_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                                c_int, c_void_p, c_void_p]),
     "pcb_inpaint_loss_pixel_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,

@@ -2,7 +2,8 @@
 launch, optional data-parallel gradient all-reduce (NCCL over NVLink) and whole-step CUDA-graph capture.
 Inference engines (InferStep, SegInferStep): graph-captured eval-mode forward with the BatchNorm + activation passes fused
 into the convolution epilogues.  InpaintEvalStep: held-out evaluation of an inpainting U-Net on a GPU batcher, loss included,
-in one graph that coexists with a captured training step on the same network.
+in one graph that coexists with a captured training step on the same network; SegEvalStep: the same for a segmentation network,
+with its loss and the pixel average precision (metrics.PixelAveragePrecision) in the graph.
 
 The reference has no train script (SURVEY 3): its recipe is prose -- SGD + Nesterov momentum, weight decay,
 cyclic LR (checkpoints/ReadME.md:4).  One step here = forward + loss + backward (+ all-reduce) + SGD update,
@@ -12,6 +13,7 @@ the device, inside the captured step; `TrainStep.state_dict()` / `load_state_dic
 from __future__ import annotations
 
 import contextlib
+import copy
 import ctypes
 import math
 import numbers
@@ -809,16 +811,12 @@ class SegInferStep(InferStep):
         return (x,)
 
 
-class InpaintEvalStep(InferStep):
-    """Held-out evaluation of an inpainting U-Net in one CUDA graph: `batcher.prepare()` (data.InpaintBatcher or
-    data.InpaintPairBatcher: the device draws the crops and strokes), the eval-mode forward with InferStep's fused BatchNorm +
-    activation epilogues and mask-chain stream, and, with an `extractor` (loss.VggExtractor), the reference's InpaintingLoss
-    forward without a backward.  Per batch the host decodes, calls ``batcher.stage(samples)`` and ``run()``.
-
-    ``run()`` returns the output as a static fp32 NCHW buffer that the next call overwrites; `last_loss` (device fp32 scalar) and
-    `last_terms` (device fp32 [5]: valid, hole, tv, perceptual, style, unweighted) hold the loss of that batch (None without an
-    extractor).  ``batcher.reseed(seed)`` before a validation pass makes every pass draw the same crops and strokes;
-    `warmup_and_capture()` leaves the generator where it found it.
+class _BatcherEvalStep(InferStep):
+    """Held-out evaluation on a GPU batcher in one CUDA graph: `batcher.prepare()`, the eval-mode forward with InferStep's fused
+    BatchNorm + activation epilogues and whatever the subclass's `_forward` adds, captured on the first call.  Per batch the host
+    decodes, calls ``batcher.stage(samples)`` and ``run()``, which returns the network output as a static fp32 NCHW buffer that
+    the next call overwrites.  ``batcher.reseed(seed)`` before a validation pass makes every pass draw the same crops;
+    `warmup_and_capture()` leaves the generator (and the tensors `_kept_by_warmup` names) where it found them.
 
     Sharing the network with a (captured) TrainStep: run() evaluates the parameters and BatchNorm running statistics as they are
     at the call.  Every TrainStep step bumps the weight epoch, and the first run() after a change rewrites this step's operand
@@ -829,26 +827,17 @@ class InpaintEvalStep(InferStep):
 
     _CACHES = ("_wcache", "_pcb_k2r_cache")        # per-module operand caches (ops.prepare_weight, loss._Vgg)
 
-    def __init__(self, net: torch.nn.Module, batcher, extractor=None, feature_range=3, compute_dtype=None):
+    def __init__(self, net: torch.nn.Module, batcher, compute_dtype=None, extra_modules=()):
         if compute_dtype is not None and compute_dtype != batcher.dtype:
             raise ValueError(f"compute_dtype {compute_dtype} differs from the batcher's {batcher.dtype}")
         training = net.training
         super().__init__(net, compute_dtype=batcher.dtype)
         net.train(training)
         self.batcher = batcher
-        self.criterion = None
-        mods = list(net.modules())
-        if extractor is not None:
-            from .loss import InpaintingLoss
-            self.criterion = InpaintingLoss(extractor, feature_range)
-            mods += list(extractor.modules())
+        mods = list(net.modules()) + [m for e in extra_modules for m in e.modules()]
         self._cached_modules = [m for m in mods if isinstance(getattr(m, "_wcache", None), dict)]
         self._own = {}
         self.last_loss = None
-
-    @property
-    def last_terms(self):
-        return self.criterion.last_terms if self.criterion is not None else None
 
     @contextlib.contextmanager
     def _own_state(self):
@@ -870,15 +859,10 @@ class InpaintEvalStep(InferStep):
                 else:
                     m.__dict__[name] = cache
 
-    def _forward(self):
-        xin, hm, clean = self.batcher.prepare()
-        out = self.net((xin, hm))
-        if self.criterion is not None:
-            loss = self.criterion(clean, hm, out, clean)
-            if self.last_loss is None:
-                self.last_loss = torch.zeros((), dtype=torch.float32, device=loss.device)
-            self.last_loss.copy_(loss)
-        return out
+    def _keep_loss(self, loss):
+        if self.last_loss is None:
+            self.last_loss = torch.zeros((), dtype=torch.float32, device=loss.device)
+        self.last_loss.copy_(loss)
 
     def _key(self):
         return ()
@@ -886,16 +870,100 @@ class InpaintEvalStep(InferStep):
     def _inputs(self):
         return ()
 
+    def _kept_by_warmup(self):
+        """The device state the warm-up's eager forwards advance and `warmup_and_capture()` restores."""
+        return [self.batcher.rng]
+
     def warmup_and_capture(self):
         """Run the eager warm-up and capture the graph on the staged batch (the first run() does this when not called)."""
-        rng = self.batcher.rng.clone()
-        self.run()
-        self.batcher.rng.copy_(rng)
+        kept = self._kept_by_warmup()
+        saved = [t.clone() for t in kept]
+        self._run()
+        for t, v in zip(kept, saved):
+            t.copy_(v)
 
-    def run(self) -> torch.Tensor:
-        """Evaluate the staged batch.  Returns the static fp32 NCHW output."""
+    def _run(self) -> torch.Tensor:
         self.batcher.activate()
         with self._own_state():
             out = super().run()
         self.batcher.release()
         return out
+
+    def run(self) -> torch.Tensor:
+        """Evaluate the staged batch.  Returns the static fp32 NCHW output."""
+        return self._run()
+
+
+class InpaintEvalStep(_BatcherEvalStep):
+    """Held-out evaluation of an inpainting U-Net in one CUDA graph (see _BatcherEvalStep): `batcher.prepare()`
+    (data.InpaintBatcher or data.InpaintPairBatcher: the device draws the crops and strokes), the eval-mode forward with
+    InferStep's fused BatchNorm + activation epilogues and mask-chain stream, and, with an `extractor` (loss.VggExtractor), the
+    reference's InpaintingLoss forward without a backward.
+
+    ``run()`` returns the output as a static fp32 NCHW buffer that the next call overwrites; `last_loss` (device fp32 scalar) and
+    `last_terms` (device fp32 [5]: valid, hole, tv, perceptual, style, unweighted) hold the loss of that batch (None without an
+    extractor).  ``batcher.reseed(seed)`` before a validation pass makes every pass draw the same crops and strokes."""
+
+    def __init__(self, net: torch.nn.Module, batcher, extractor=None, feature_range=3, compute_dtype=None):
+        super().__init__(net, batcher, compute_dtype=compute_dtype, extra_modules=() if extractor is None else (extractor,))
+        self.criterion = None
+        if extractor is not None:
+            from .loss import InpaintingLoss
+            self.criterion = InpaintingLoss(extractor, feature_range)
+
+    @property
+    def last_terms(self):
+        return self.criterion.last_terms if self.criterion is not None else None
+
+    def _forward(self):
+        xin, hm, clean = self.batcher.prepare()
+        out = self.net((xin, hm))
+        if self.criterion is not None:
+            self._keep_loss(self.criterion(clean, hm, out, clean))
+        return out
+
+
+class SegEvalStep(_BatcherEvalStep):
+    """Held-out evaluation of a segmentation network (TextSegament, XceptionTextSegment) in one CUDA graph (see
+    _BatcherEvalStep): `batcher.prepare()` (data.SegBatcher), the eval-mode forward with the fused BatchNorm + activation
+    epilogues, the optional loss forward (`criterion`: loss.BinaryFocalLoss or loss.SoftBootstrapCrossEntropy with a reduced
+    output; `last_loss` is its device fp32 scalar) and `score.update(logits, target)` (metrics.PixelAveragePrecision), which
+    reads the logits in place as the network returns them.
+
+    ``run()`` returns the logits [n, 1, h, w] as a static fp32 NCHW buffer that the next call overwrites.  A validation pass:
+    ``reset()`` (and ``batcher.reseed(seed)`` to repeat the draws), then per batch ``batcher.stage(samples)`` and ``run()``,
+    then ``score.average_precision()`` and ``score.counts``.  The capture's eager warm-up leaves the score as it found it, and a
+    first run() without `warmup_and_capture()` captures first, so every run() counts its batch exactly once.
+
+    The criterion is copied: the evaluation graph reduces its loss through a workspace of its own, never the one a training
+    step captured."""
+
+    def __init__(self, net: torch.nn.Module, batcher, criterion=None, compute_dtype=None):
+        super().__init__(net, batcher, compute_dtype=compute_dtype)
+        from .metrics import PixelAveragePrecision
+        self.criterion = None
+        if criterion is not None:
+            self.criterion = copy.copy(criterion)
+            self.criterion.__dict__.pop("_pcb_ws", None)
+        self.score = PixelAveragePrecision(batcher.device)
+
+    def reset(self):
+        """Start a pass: zero the score."""
+        self.score.reset()
+
+    def _kept_by_warmup(self):
+        return [self.batcher.rng, self.score.hist, self.score.counts_tensor]
+
+    def _forward(self):
+        x, target = self.batcher.prepare()
+        out = self.net(x)
+        if self.criterion is not None:
+            self._keep_loss(self.criterion(out, target))
+        self.score.update(out, target)
+        return out
+
+    def run(self) -> torch.Tensor:
+        """Evaluate the staged batch and add it to the score.  Returns the static fp32 NCHW logits."""
+        if not self._graphs:
+            self.warmup_and_capture()
+        return self._run()
