@@ -14,7 +14,6 @@ from __future__ import annotations
 
 import contextlib
 import copy
-import ctypes
 import math
 import numbers
 import os
@@ -148,7 +147,7 @@ class TrainStep:
             self._lr32 = torch.zeros(1, dtype=torch.float32, device=dev)
             # before the first update: the rate that update will use, as the reference's CyclicLR sets it at construction
             self._lr64 = torch.tensor(lr_schedule.rate(start), dtype=torch.float64, device=dev)
-        self._wcaches = [m._wcache for m in net.modules() if isinstance(getattr(m, "_wcache", None), dict)]
+        self._caches = [c for _, _, c in ops.operand_caches(net)]
         self.pg = process_group
         self.world = torch.distributed.get_world_size(process_group) if process_group is not None else 1
         # data parallel: ranks exchange the SUM of their gradient arenas; the 1/world of the mean is folded into the optimiser
@@ -323,7 +322,7 @@ class TrainStep:
         ops.set_mask_chain_stream(True)
         self._arm_overlap(overlap)
         try:
-            ops.prefetch_weights(self._wcaches)        # operand re-layout of all layers runs ahead on its own stream
+            ops.prefetch_weights(self._caches)         # operand re-layout of all layers runs ahead on its own stream
             loss = self._forward_loss(x, mask)
             loss.backward()
         finally:
@@ -405,11 +404,11 @@ class TrainStep:
             with torch.cuda.graph(self.graph_update):
                 self._update(False)
         self.graph = graph
-        # The captured kernels hold raw pointers to the per-layer operand buffers (the `_wcache` entries): keep them alive for as
-        # long as the graph exists.  An eager forward after capture (validation) misses the cache -- the optimiser bumps the
-        # weight epoch -- and, with the in-place refresh off, replaces `cache["val"]` with new buffers; without this list the
-        # old ones would be freed under the graph.  (Each replay refreshes the captured buffers itself.)
-        self._captured_operands = [c.get("val") for c in self._wcaches]
+        # The captured kernels hold raw pointers to the per-layer operand buffers (ops.Operands): keep them alive for as long
+        # as the graph exists.  An eager forward after capture (validation) misses the cache -- the optimiser bumps the
+        # weight epoch -- and, with the in-place refresh off, replaces the cache's record with new buffers; without this list
+        # the old ones would be freed under the graph.  (Each replay refreshes the captured buffers itself.)
+        self._captured_operands = [c.current for c in self._caches if c.current is not None]
         torch.cuda.synchronize()
 
     def step(self, x: torch.Tensor, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -623,12 +622,7 @@ class InpaintLossTrainStep(InpaintTrainStep):
         from .loss import InpaintingLoss
         super().__init__(net, batcher, **kwargs)
         self.criterion = InpaintingLoss(extractor, feature_range)
-        self._frozen_caches = [m.__dict__ for m in extractor.modules() if isinstance(getattr(m, "_wcache", None), dict)]
-
-    def warmup_and_capture(self, eager_warmup=2):
-        super().warmup_and_capture(eager_warmup=eager_warmup)
-        if self._captured_operands is not None:
-            self._captured_operands += [(d["_wcache"].get("val"), d.get("_pcb_k2r_cache", {}).get("val")) for d in self._frozen_caches]
+        self._caches += [c for _, _, c in ops.operand_caches(extractor)]     # frozen: pinned with the graph, never prefetched
 
     @property
     def last_terms(self):
@@ -680,7 +674,7 @@ class InferStep:
     (BatchNorm/activation passes applied in a convolution epilogue / still run on their own).
 
     Weights: a change of the weight epoch since capture (``load_state_dict`` and the initialisers bump it) makes the next run()
-    rewrite the captured operand buffers in place (pcb_conv_weight_refresh) and the BatchNorm coefficients before it replays;
+    rewrite the captured operand buffers in place (ops.OperandCache.refresh) and the BatchNorm coefficients before it replays;
     call refresh() after a mutation that does not bump the epoch."""
 
     def __init__(self, net: torch.nn.Module, compute_dtype=torch.bfloat16):
@@ -688,7 +682,7 @@ class InferStep:
         self.dtype = compute_dtype
         self._bns = [m for m in net.modules() if isinstance(m, torch.nn.BatchNorm2d)]
         self._graphs = {}
-        self._captured_operands = []          # (cache, operand buffers, geometry, weight) of every captured convolution
+        self._captured_operands = []          # (cache, ops.Operands) of every captured convolution
         self._epoch = None
         self.launches_per_run = 0
         self.fused_sites = self.unfused_sites = 0
@@ -750,10 +744,7 @@ class InferStep:
             static_out.copy_(self._run_forward(*static_in))
         self._check_markers()
         # the captured kernels hold raw pointers to the operand buffers current at capture: keep them (and what rewrites them)
-        for m in self.net.modules():
-            cache = getattr(m, "_wcache", None)
-            if isinstance(cache, dict) and cache.get("val") is not None:
-                self._captured_operands.append((cache, cache["val"], cache["geom"], cache["weight"]))
+        self._captured_operands += [(c, c.current) for _, _, c in ops.operand_caches(self.net) if c.current is not None]
         torch.cuda.synchronize()
         return graph, static_in, static_out
 
@@ -763,15 +754,8 @@ class InferStep:
         self._refresh()
 
     def _refresh(self):
-        lib = _lib.load()
-        for cache, val, geom, weight in self._captured_operands:
-            w_fwd, w_dg = val
-            wm = weight.detach().float().contiguous(memory_format=CL)
-            _lib.check(lib.pcb_conv_weight_refresh(ctypes.byref(geom.struct(None)), wm.data_ptr(), w_fwd.data_ptr(), ops._ptr(w_dg),
-                                                   ops._stream()))
-            if cache.get("val") is val:       # eager calls find the refreshed buffers current
-                cache["key"] = (weight.data_ptr(), weight._version, str(weight.device), ops._WEIGHT_EPOCH, geom.signature)
-                cache["ready"] = None
+        for cache, rec in self._captured_operands:
+            cache.refresh(rec)
         self._refresh_coefficients()
         self._epoch = ops._WEIGHT_EPOCH
 
@@ -825,8 +809,6 @@ class _BatcherEvalStep(InferStep):
     run() leaves `net.training` as it found it.  Give it a batcher of its own: the training step's batcher buffers are the
     training graph's inputs."""
 
-    _CACHES = ("_wcache", "_pcb_k2r_cache")        # per-module operand caches (ops.prepare_weight, loss._Vgg)
-
     def __init__(self, net: torch.nn.Module, batcher, compute_dtype=None, extra_modules=()):
         if compute_dtype is not None and compute_dtype != batcher.dtype:
             raise ValueError(f"compute_dtype {compute_dtype} differs from the batcher's {batcher.dtype}")
@@ -834,30 +816,23 @@ class _BatcherEvalStep(InferStep):
         super().__init__(net, compute_dtype=batcher.dtype)
         net.train(training)
         self.batcher = batcher
-        mods = list(net.modules()) + [m for e in extra_modules for m in e.modules()]
-        self._cached_modules = [m for m in mods if isinstance(getattr(m, "_wcache", None), dict)]
-        self._own = {}
+        self._own = [(m, name, ops.OperandCache(c.frozen, c.derive)) for m, name, c in ops.operand_caches(net, *extra_modules)]
         self.last_loss = None
 
     @contextlib.contextmanager
     def _own_state(self):
         """Eval mode and this step's own operand caches for the duration of a call; the modules' own are restored after."""
         training = self.net.training
-        saved = []
-        for m in self._cached_modules:
-            for name in self._CACHES:
-                saved.append((m, name, m.__dict__.get(name)))
-                m.__dict__[name] = self._own.setdefault((id(m), name), {})
+        saved = [(m, name, vars(m)[name]) for m, name, _ in self._own]
+        for m, name, own in self._own:
+            vars(m)[name] = own
         self.net.eval()
         try:
             yield
         finally:
             self.net.train(training)
             for m, name, cache in saved:
-                if cache is None:
-                    m.__dict__.pop(name, None)
-                else:
-                    m.__dict__[name] = cache
+                vars(m)[name] = cache
 
     def _keep_loss(self, loss):
         if self.last_loss is None:

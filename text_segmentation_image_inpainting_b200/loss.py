@@ -21,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib, ops
-from ._lib import ACT_RELU, PCB_BF16
+from ._lib import ACT_RELU
 from .masks import HoleMask
 
 CL = torch.channels_last
@@ -92,7 +92,8 @@ class VggExtractor(nn.Module):
             p.requires_grad = False
         for m in self.modules():
             if isinstance(m, nn.Conv2d):
-                m._wcache = {}                 # compute-dtype operand buffers (_Vgg.operands)
+                m._wcache = ops.OperandCache(frozen=True)                             # _Vgg.conv_relu, _Vgg.dgrad
+                m._k2r_cache = ops.OperandCache(frozen=True, derive=_k2r_image_weight)   # _Vgg.dgrad_image
 
     def stage_convs(self, s) -> List[nn.Conv2d]:
         return [m for m in self.features[s] if isinstance(m, nn.Conv2d)]
@@ -121,6 +122,14 @@ class FeatureExtractor(nn.Module):
         return _Vgg(self.encoder, self.feature_range).forward(_as_vgg_input(x))[1]
 
 
+def _k2r_image_weight(weight):
+    """The fp32 master of conv1_1's kernel-to-row data gradient: W'[tap·3 + ci][co], 27 of 32 rows (pcb_k2r_image_weight)."""
+    cout = weight.shape[0]
+    wz = torch.empty((32, cout), dtype=torch.float32, device=weight.device)
+    _lib.check(_lib.load().pcb_k2r_image_weight(weight.detach().float().contiguous().data_ptr(), cout, wz.data_ptr(), _stream()))
+    return wz
+
+
 def _as_vgg_input(img):
     """[n, 3, h, w] image -> [n, 3, h, w] view of an 8-channel-padded NHWC buffer in its dtype."""
     img = ops.as_feature_padded(img)
@@ -142,25 +151,8 @@ class _Vgg:
         return ops.ConvGeom([x], [0], conv.out_channels, 3, 1, 1, 1, 1, False, False, [(None, conv.in_channels, 0)], plain=True)
 
     def operands(self, conv, geom):
-        """Compute-dtype operand buffers of a frozen VGG weight, cached on the module and keyed on the weight itself (pointer,
-        version) rather than the training engine's weight epoch: they are laid out again only when the weight changes."""
-        w = conv.weight
-        key = (w.data_ptr(), w._version, str(w.device), geom.signature)
-        cache = conv._wcache
-        if cache.get("key") != key:
-            if torch.cuda.is_current_stream_capturing():
-                raise _lib.PcbError("VGG operands are stale inside a graph capture: run the loss once before capturing")
-            lib = self.lib
-            c = geom.struct(None)
-            fe, de = ctypes.c_size_t(0), ctypes.c_size_t(0)
-            lib.pcb_conv_weight_layout(ctypes.byref(c), ctypes.byref(fe), ctypes.byref(de))
-            tdt = torch.bfloat16 if geom.dtype == PCB_BF16 else torch.float32
-            w_fwd = torch.empty((fe.value,), dtype=tdt, device=w.device)
-            w_dg = torch.empty((de.value,), dtype=tdt, device=w.device) if de.value else None
-            wm = w.detach().float().contiguous(memory_format=CL)
-            _lib.check(lib.pcb_conv_weight_prepare(ctypes.byref(c), wm.data_ptr(), w_fwd.data_ptr(), ops._ptr(w_dg), _stream()))
-            cache["key"], cache["val"] = key, (w_fwd, w_dg)
-        return cache["val"]
+        """The operands of a frozen VGG weight (its frozen OperandCache: laid out again only when the weight changes)."""
+        return conv._wcache.get(conv.weight, geom)
 
     def conv_relu(self, conv, x):
         """relu(conv(x) + b), the ReLU in the forward epilogue when the kernel applies one, else in a second pass."""
@@ -173,11 +165,11 @@ class _Vgg:
         ws = ops._workspace(lib, c, dev)
         b32 = conv.bias.detach().float().contiguous()
         if lib.pcb_conv_fuses_affine_act(ctypes.byref(c)):
-            _lib.check(lib.pcb_pconv_forward_affine_act(ctypes.byref(c), wprep[0].data_ptr(), b32.data_ptr(), y.data_ptr(), geom.cout,
+            _lib.check(lib.pcb_pconv_forward_affine_act(ctypes.byref(c), wprep.w_fwd.data_ptr(), b32.data_ptr(), y.data_ptr(), geom.cout,
                                                         dummy.data_ptr(), dummy.data_ptr(), ws.data_ptr(), 0, None, None, ACT_RELU, 0.0,
                                                         _stream()))
         else:
-            _lib.check(lib.pcb_pconv_forward(ctypes.byref(c), wprep[0].data_ptr(), b32.data_ptr(), y.data_ptr(), geom.cout,
+            _lib.check(lib.pcb_pconv_forward(ctypes.byref(c), wprep.w_fwd.data_ptr(), b32.data_ptr(), y.data_ptr(), geom.cout,
                                              dummy.data_ptr(), dummy.data_ptr(), ws.data_ptr(), _stream()))
             _lib.check(lib.pcb_bn_act_forward(y.data_ptr(), geom.dtype, geom.n * geom.ho * geom.wo, geom.cout, None, None, ACT_RELU, 0.0,
                                               None, y.data_ptr(), _stream()))
@@ -232,22 +224,7 @@ class _Vgg:
         m, _, h, w = xs.shape
         cout = conv.out_channels
         geom = ops.ConvGeom([dc], [0], 32, 1, 1, 0, 1, 1, False, False, [(None, cout, 0)], plain=True)
-        wt = conv.weight
-        key = (wt.data_ptr(), wt._version, str(dev), geom.signature)
-        cache = conv.__dict__.setdefault("_pcb_k2r_cache", {})
-        if cache.get("key") != key:
-            if torch.cuda.is_current_stream_capturing():
-                raise _lib.PcbError("VGG operands are stale inside a graph capture: run the loss once before capturing")
-            wz = torch.empty((32, cout), dtype=torch.float32, device=dev)
-            _lib.check(lib.pcb_k2r_image_weight(wt.detach().float().contiguous().data_ptr(), cout, wz.data_ptr(), _stream()))
-            s0 = geom.struct(None)
-            fe, de = ctypes.c_size_t(0), ctypes.c_size_t(0)
-            lib.pcb_conv_weight_layout(ctypes.byref(s0), ctypes.byref(fe), ctypes.byref(de))
-            w_fwd = torch.empty((fe.value,), dtype=dt, device=dev)
-            w_dg = torch.empty((de.value,), dtype=dt, device=dev) if de.value else None
-            _lib.check(lib.pcb_conv_weight_prepare(ctypes.byref(s0), wz.data_ptr(), w_fwd.data_ptr(), ops._ptr(w_dg), _stream()))
-            cache["key"], cache["val"] = key, (w_fwd, w_dg)
-        w_fwd = cache["val"][0]
+        w_fwd = conv._k2r_cache.get(conv.weight, geom).w_fwd
         c = geom.struct([dc])
         z = torch.empty((m, 32, h, w), dtype=dt, device=dev, memory_format=CL)
         dummy = torch.empty((16,), dtype=torch.uint8, device=dev)
@@ -289,17 +266,15 @@ class _Gram:
         """out[i] = F_i t[i]^T for the leading t.shape[0] images (t: fp32 [m][c][c], symmetric)."""
         lib, c, m = self.lib, self.c, t.shape[0]
         s0 = self.geom.struct([f[:1]])
-        fe, de = ctypes.c_size_t(0), ctypes.c_size_t(0)
-        lib.pcb_conv_weight_layout(ctypes.byref(s0), ctypes.byref(fe), ctypes.byref(de))
-        w = torch.empty((m, fe.value), dtype=f.dtype, device=f.device)
-        wd = torch.empty((max(de.value, 1),), dtype=f.dtype, device=f.device)
+        fe, de = ops.Operands.sizes(s0)
+        w = torch.empty((m, fe), dtype=f.dtype, device=f.device)
+        wd = torch.empty((de,), dtype=f.dtype, device=f.device) if de else None
         out = torch.empty((m, c, f.shape[2], f.shape[3]), dtype=f.dtype, device=f.device, memory_format=CL)
         dummy = torch.empty((16,), dtype=torch.uint8, device=f.device)
         ws = ops._workspace(lib, s0, f.device)
         for i in range(m):
             s = self.geom.struct([f[i:i + 1]])
-            _lib.check(lib.pcb_conv_weight_prepare(ctypes.byref(s), t[i].data_ptr(), w[i].data_ptr(), wd.data_ptr() if de.value else None,
-                                                   _stream()))
+            ops.Operands.lay_out(s, t[i], w[i], wd)
             _lib.check(lib.pcb_pconv_forward(ctypes.byref(s), w[i].data_ptr(), None, out[i:i + 1].data_ptr(), c, dummy.data_ptr(),
                                              dummy.data_ptr(), ws.data_ptr(), _stream()))
         return out

@@ -93,11 +93,12 @@ class B200Conv2d(nn.Conv2d):
     depthwise 3x3 ones at a power-of-two stride on the vectorised HBM-bound kernels, anything else on the shape-general kernel."""
 
     def __init__(self, *args, **kwargs):
+        from .. import ops
         super().__init__(*args, **kwargs)
         if self.padding_mode != "zeros" or isinstance(self.padding, str):
             raise NotImplementedError("only explicit zero padding")
         self.weight.data = self.weight.data.contiguous(memory_format=torch.channels_last)
-        self._wcache = {}
+        self._wcache = ops.OperandCache()
 
     def forward(self, x):
         from .. import ops

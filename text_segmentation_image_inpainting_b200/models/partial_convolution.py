@@ -40,7 +40,7 @@ class PartialConv(BaseModule):
         nn.init.constant_(self.mask_conv.weight, 1.0)
         for p in self.mask_conv.parameters():
             p.requires_grad = False
-        self._wcache = {}
+        self._wcache = ops.OperandCache()
 
     def _conv(self, x, mask, no_guard=False, handoff=None, epilogue=None):
         fc = self.feature_conv
@@ -61,7 +61,7 @@ class PartialConv1x1(BaseModule):
         self.feature_conv = nn.Conv2d(in_channels, out_channels, kernel_size, stride, padding, dilation, groups, bias)
         nn.init.kaiming_normal_(self.feature_conv.weight)
         _channels_last_(self.feature_conv)
-        self._wcache = {}
+        self._wcache = ops.OperandCache()
 
     def forward(self, args):
         x, mask = args

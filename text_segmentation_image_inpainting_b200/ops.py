@@ -461,7 +461,7 @@ def _partial_conv_fused_eval(geom: ConvGeom, wprep, bias, xs, epi: EvalEpilogue)
     else:
         y = torch.empty((geom.n, geom.cout, geom.ho, geom.wo), dtype=xs[0].dtype, device=dev, memory_format=CL)
     b32 = bias.detach().float().contiguous() if bias is not None else None
-    msum, newmask = _pconv_launch(lib, geom, c, wprep[0], b32, y, None, epi)
+    msum, newmask = _pconv_launch(lib, geom, c, wprep.w_fwd, b32, y, None, epi)
     epi.fused = True
     EPILOGUE_SITES["fused"] += 1
     return y, msum, newmask
@@ -635,59 +635,114 @@ _INPLACE_WEIGHT_REFRESH = False
 
 
 def set_inplace_weight_refresh(enabled: bool):
-    """Training engines that update the masters once per step (after every backward of that step has run) may let
-    `prepare_weight` rewrite the cached operand buffers in place instead of allocating + zero-filling new ones each step.
+    """Training engines that update the masters once per step (after every backward of that step has run) may let an
+    `OperandCache` rewrite its operand buffers in place instead of allocating + zero-filling new ones each step.
     Off by default: a backward that runs after a later weight update would otherwise read the new weights."""
     global _INPLACE_WEIGHT_REFRESH
     _INPLACE_WEIGHT_REFRESH = bool(enabled)
 
 
-def prepare_weight(weight: torch.Tensor, geom: ConvGeom, cache: dict):
-    """fp32 master weight (OIHW logical, KRSC physical) -> the operand buffers the kernels want
-    (pcb_conv_weight_layout / pcb_conv_weight_prepare), cached per parameter version and problem signature."""
-    key = (weight.data_ptr(), weight._version, str(weight.device), _WEIGHT_EPOCH, geom.signature)
-    if cache.get("key") == key:
-        ev = cache.get("ready")
-        if ev is not None:                                # refreshed ahead of time on the prefetch stream (prefetch_weights)
-            torch.cuda.current_stream().wait_event(ev)
-            cache["ready"] = None
-        return cache["val"]
-    lib = _lib.load()
-    wm = weight.detach()
-    if wm.dtype != torch.float32:
-        wm = wm.float()
-    wm = wm.contiguous(memory_format=CL)          # physical [cout][kh][kw][cig]
-    c = geom.struct(None)
-    fe, de = ctypes.c_size_t(0), ctypes.c_size_t(0)
-    lib.pcb_conv_weight_layout(ctypes.byref(c), ctypes.byref(fe), ctypes.byref(de))
-    tdt = torch.bfloat16 if geom.dtype == PCB_BF16 else torch.float32
-    old = cache.get("val")
-    if _INPLACE_WEIGHT_REFRESH and old is not None and cache.get("sig") == (geom.signature, str(wm.device), fe.value, de.value):
-        w_fwd, w_dg = old
-        _lib.check(lib.pcb_conv_weight_refresh(ctypes.byref(c), wm.data_ptr(), w_fwd.data_ptr(), _ptr(w_dg), _stream()))
-    else:
-        w_fwd = torch.empty((fe.value,), dtype=tdt, device=wm.device)
-        w_dg = torch.empty((de.value,), dtype=tdt, device=wm.device) if de.value else None
-        _lib.check(lib.pcb_conv_weight_prepare(ctypes.byref(c), wm.data_ptr(), w_fwd.data_ptr(), _ptr(w_dg), _stream()))
-    cache["sig"] = (geom.signature, str(wm.device), fe.value, de.value)
-    cache["key"], cache["val"] = key, (w_fwd, w_dg)
-    cache["ready"] = None
-    cache["geom"], cache["weight"] = geom, weight         # remembered for prefetch_weights()
-    return cache["val"]
+def _operand_key(weight: torch.Tensor, geom: ConvGeom, frozen: bool):
+    """What operands laid out from `weight` for `geom` stay valid for: the weight's storage, version and device, the problem
+    signature and, unless frozen, the weight epoch (updates through raw pointers do not bump the version)."""
+    return (weight.data_ptr(), weight._version, str(weight.device), None if frozen else _WEIGHT_EPOCH, geom.signature)
+
+
+class Operands:
+    """One convolution weight as the compute-dtype operand buffers the kernels read for the problem `geom`: `w_fwd`, and `w_dg`
+    (None when the problem has none); unpacks as the pair ``w_fwd, w_dg``.  The fp32 master laid out is `derive(weight)`, by
+    default the weight itself (physically [cout][kh][kw][cin/groups])."""
+
+    def __init__(self, weight: torch.Tensor, geom: ConvGeom, derive=None):
+        self.weight, self.geom, self.derive = weight, geom, derive
+        wm, c = self.master(), geom.struct(None)
+        fe, de = self.sizes(c)
+        tdt = torch.bfloat16 if geom.dtype == PCB_BF16 else torch.float32
+        self.w_fwd = torch.empty((fe,), dtype=tdt, device=wm.device)
+        self.w_dg = torch.empty((de,), dtype=tdt, device=wm.device) if de else None
+        self.lay_out(c, wm, self.w_fwd, self.w_dg)
+
+    @staticmethod
+    def sizes(c: Conv) -> Tuple[int, int]:
+        """Element counts of the forward and data-gradient operand buffers of problem `c` (0: none)."""
+        fe, de = ctypes.c_size_t(0), ctypes.c_size_t(0)
+        _lib.load().pcb_conv_weight_layout(ctypes.byref(c), ctypes.byref(fe), ctypes.byref(de))
+        return fe.value, de.value
+
+    @staticmethod
+    def lay_out(c: Conv, master: torch.Tensor, w_fwd, w_dg, refresh=False):
+        """Lay `master` out into the buffers of problem `c` on the current stream; `refresh`: buffers a prepare already filled."""
+        lib = _lib.load()
+        fn = lib.pcb_conv_weight_refresh if refresh else lib.pcb_conv_weight_prepare
+        _lib.check(fn(ctypes.byref(c), master.data_ptr(), w_fwd.data_ptr(), _ptr(w_dg), _stream()))
+
+    def __iter__(self):
+        return iter((self.w_fwd, self.w_dg))
+
+    def master(self) -> torch.Tensor:
+        return self.derive(self.weight) if self.derive is not None else self.weight.detach().float().contiguous(memory_format=CL)
+
+    def refresh(self):
+        """Rewrite the buffers in place from the weight's current values, on the current stream."""
+        self.lay_out(self.geom.struct(None), self.master(), self.w_fwd, self.w_dg, refresh=True)
+
+
+class OperandCache:
+    """A module's operands of one convolution weight, kept from one call to the next.  `get(weight, geom)` returns the current
+    record while its key (`_operand_key`) matches, else the current record rewritten in place when set_inplace_weight_refresh()
+    is on and the layout is unchanged, else a new record: the buffers of a record a captured graph keeps are never freed.
+
+    `frozen` (weights no optimiser updates, the VGG loss): the key leaves out the weight epoch, so the operands are laid out again
+    only when the weight itself changes, never in place and never inside a graph capture.  `derive`: see Operands."""
+
+    def __init__(self, frozen=False, derive=None):
+        self.frozen, self.derive = frozen, derive
+        self.current: Optional[Operands] = None
+        self.key, self.ready = None, None       # ready: event of a prefetch_weights() refresh not yet waited on
+
+    def get(self, weight: torch.Tensor, geom: ConvGeom) -> Operands:
+        key = _operand_key(weight, geom, self.frozen)
+        rec = self.current
+        if key == self.key:
+            if self.ready is not None:
+                torch.cuda.current_stream().wait_event(self.ready)
+                self.ready = None
+            return rec
+        if self.frozen and torch.cuda.is_current_stream_capturing():
+            raise _lib.PcbError("VGG operands are stale inside a graph capture: run the loss once before capturing")
+        if (_INPLACE_WEIGHT_REFRESH and not self.frozen and rec is not None and rec.geom.signature == geom.signature
+                and rec.w_fwd.device == weight.device
+                and Operands.sizes(geom.struct(None)) == (rec.w_fwd.numel(), rec.w_dg.numel() if rec.w_dg is not None else 0)):
+            rec.weight, rec.geom = weight, geom
+            rec.refresh()
+        else:
+            rec = Operands(weight, geom, self.derive)
+        self.current, self.key, self.ready = rec, key, None
+        return rec
+
+    def refresh(self, rec: Operands):
+        """Rewrite `rec`, a record this cache handed out, in place on the current stream; the next get() hits if it is current."""
+        rec.refresh()
+        if rec is self.current:
+            self.key, self.ready = _operand_key(rec.weight, rec.geom, self.frozen), None
+
+
+def operand_caches(*roots: torch.nn.Module):
+    """(module, attribute name, cache) of every OperandCache that a module of these module trees holds."""
+    return [(m, name, c) for r in roots for m in r.modules() for name, c in vars(m).items() if isinstance(c, OperandCache)]
 
 
 _PREFETCH_STREAMS = {}
 
 
 def prefetch_weights(caches):
-    """Re-lay-out the convolution weights behind `caches` (the per-module operand caches) on a prefetch stream, ahead of the layers' forward calls (training
-    engines call this right after the optimiser step / epoch bump; requires the in-place refresh mode).  Each layer's
-    forward then only waits on its own event, so the re-layout of layer k overlaps the forward of the layers before it."""
-    caches = [c for c in caches if c.get("val") is not None and c.get("weight") is not None]
+    """Re-lay-out the weights behind `caches` (OperandCache; frozen and empty ones are skipped) on a prefetch stream, ahead of the
+    layers' forward calls (training engines call this right after the optimiser step / epoch bump; requires the in-place refresh
+    mode).  Each layer's forward then only waits on its own event, so the re-layout of layer k overlaps the layers before it."""
+    caches = [c for c in caches if c.current is not None and not c.frozen]
     if not _INPLACE_WEIGHT_REFRESH or not caches:
         return
-    lib = _lib.load()
-    dev = caches[0]["weight"].device
+    dev = caches[0].current.weight.device
     key_dev = (dev.type, dev.index if dev.index is not None else torch.cuda.current_device())
     if key_dev not in _PREFETCH_STREAMS:
         _PREFETCH_STREAMS[key_dev] = torch.cuda.Stream(device=dev)
@@ -695,19 +750,12 @@ def prefetch_weights(caches):
     ps.wait_stream(torch.cuda.current_stream())           # after the optimiser step, and after every reader of the old buffers
     with torch.cuda.stream(ps):
         for cache in caches:
-            weight, geom = cache["weight"], cache["geom"]
-            if weight.device != dev or weight.dtype != torch.float32:
+            rec = cache.current
+            if rec.weight.device != dev or rec.weight.dtype != torch.float32 or cache.key == _operand_key(rec.weight, rec.geom, False):
                 continue
-            key = (weight.data_ptr(), weight._version, str(weight.device), _WEIGHT_EPOCH, geom.signature)
-            if cache.get("key") == key:
-                continue
-            wm = weight.detach().contiguous(memory_format=CL)
-            c = geom.struct(None)
-            w_fwd, w_dg = cache["val"]
-            _lib.check(lib.pcb_conv_weight_refresh(ctypes.byref(c), wm.data_ptr(), w_fwd.data_ptr(), _ptr(w_dg), _stream()))
-            ev = torch.cuda.Event()
-            ev.record()
-            cache["key"], cache["ready"] = key, ev
+            cache.refresh(rec)
+            cache.ready = torch.cuda.Event()
+            cache.ready.record()
 
 
 _MASK_CHAIN_STREAM = False
@@ -826,7 +874,7 @@ def partial_conv(x, mask, weight, bias, stride, padding, dilation, groups, same_
         geom = ConvGeom(xs, ups, cout, tuple(weight.shape[2:]), stride, padding, dilation, groups, same_holes, no_guard, parts, plain=plain)
     except TooManyParts:
         return _partial_conv_dense_masks(x, hm, weight, bias, stride, padding, dilation, groups, same_holes, no_guard, cache)
-    wprep = prepare_weight(weight, geom, cache if cache is not None else {})
+    wprep = (cache if cache is not None else OperandCache()).get(weight, geom)
     out = _partial_conv_fused_eval(geom, wprep, bias, xs, epilogue) if epilogue is not None else None
     y, msum, newmask = out if out is not None else PartialConvFn.apply(geom, wprep, weight, bias, handoff, *xs)
     planes = [newmask[g] for g in range(geom.mg)]
