@@ -270,6 +270,26 @@ int pcb_scse_backward(const void *gy, const void *x, const float *cse, const flo
 int pcb_seg_mask_postprocess(const void *logits, int dtype, int n, int h, int w, int cstride, int h_valid, int w_valid, int oh,
                              int ow, uint8_t *out, pcb_stream_t stream);
 
+/* ---- text removal (engine.TextRemovalStep): the glue between segmentation, mask and inpainting ---------------------------
+ * `page`: fp32 NCHW [n, 3, h, w], contiguous, device memory.
+ *
+ * The segmentation input (EvaluateSet, Dataloader.py:271-273, 296-303): per pixel of the [hs, ws] grid (hs >= h, ws >= w),
+ * (page - mean) / std in fp32 (sub, then div, each rounded; `norm`: HOST pointer to mean[3], std[3], or NULL to skip it),
+ * rounded once to `dtype`, zero outside the page.  out: [n, hs, ws, 8] NHWC (channels 3..7 zero), every element written. */
+int pcb_removal_seg_input(const float *page, int n, int h, int w, const float *norm, int hs, int ws, void *out, int dtype,
+                          pcb_stream_t stream);
+/* The U-Net's input from the demo's text mask (uint8 [n, h, w], nonzero = text): the mask as a {0, 255} image, > 0.4 * 255,
+ * cv2.dilate with a 10x10 kernel (anchor 5: rows and columns -5 .. +4, pixels outside the page ignored) (Dataloader.py:120-121),
+ * then on the [hu, wu] grid (hu >= h, wu >= w): valid uint8 [n, hu, wu] = 1 - hole and corrupted [n, hu, wu, 8] NHWC in
+ * `dtype` = page * valid in fp32 rounded once (:128-131; channels 3..7 zero).  Outside the page: valid 0, corrupted 0. */
+int pcb_removal_holes(const uint8_t *text_mask, const float *page, int n, int h, int w, int hu, int wu, uint8_t *valid,
+                      void *corrupted, int dtype, pcb_stream_t stream);
+/* The composite (loss.py:196, comp_img) cropped to the page: out fp32 NCHW [n, 3, h, w] = valid ? page : fill, where `fill` is
+ * the U-Net output on the [hu, wu] grid, NHWC with pixel stride `cstride` (channels 0..2 read) in `dtype`, and `valid` the
+ * plane pcb_removal_holes wrote. */
+int pcb_removal_composite(const void *fill, int dtype, int cstride, const float *page, const uint8_t *valid, int n, int h, int w,
+                          int hu, int wu, float *out, pcb_stream_t stream);
+
 /* ---- inpainting training data (ImageInpaintingData.process_images, Dataloader.py:110-162) -------------------------------
  * One decoded source per image: RGB uint8 [h][rgb_stride] (3 bytes per pixel) and the text mask uint8 [h][mask_stride]. */
 typedef struct {

@@ -12,6 +12,7 @@
 //      (separable max in shared memory), grayscale, /255, x mask and the three stores.
 // Grids are sized from the batcher's capacity (largest source), so one captured graph serves any mix of source sizes.
 // The resampler follows Pillow's fixed-point 8-bit path bit for bit (pil_data.cuh, shared with seg_data.cu).
+#include "pcb_dilate.cuh"
 #include "pil_data.cuh"
 
 #define ST static_cast<cudaStream_t>(stream)
@@ -27,7 +28,7 @@ using pil::pil_coeffs;
 constexpr int HX = 128;       // horizontal pass: output columns per block (one per thread)
 constexpr int HROWS = 16;     // horizontal pass: box rows per block
 constexpr int T = 32;         // fused kernel: output tile edge
-constexpr int HT = T + 9;     // tile + dilation halo (5 rows / columns before, 4 after: cv2's anchor of a 10x10 kernel)
+constexpr int HT = dil::Tile<T>::HT;   // tile + dilation halo (5 rows / columns before, 4 after: cv2's anchor of a 10x10 kernel)
 
 // What the kernels need to know about a source kind: its descriptor, the intermediate pixel, the horizontal pass of one box row
 // at one output column (taps k[0], k[HX], ...), and the vertical pass of one output pixel (taps k[0], k[1], ...; rows `step`
@@ -199,8 +200,7 @@ __global__ void __launch_bounds__(256) inpaint_fused_kernel(const typename K::Sr
                                                             TO *__restrict__ corrupted, uint8_t *__restrict__ plane, float *__restrict__ clean) {
     __shared__ int vk[HT * KMAX];
     __shared__ int vmin[HT], vcnt[HT];
-    __shared__ uint8_t hole[HT][HT];
-    __shared__ uint8_t rmax[HT][T];
+    __shared__ dil::Tile<T> dt;
     __shared__ uchar4 rgb[T][T];
     const int n = blockIdx.z, y0 = blockIdx.y * T, x0 = blockIdx.x * T, tid = threadIdx.x;
     const pcb_inpaint_params &p = params[n];
@@ -225,24 +225,16 @@ __global__ void __launch_bounds__(256) inpaint_fused_kernel(const typename K::Sr
             h = mv >= 103 || (strokes && in_stroke(p, gx, gy));                // mask > 0.4 * 255; strokes are drawn at 255
             if (ly >= 5 && ly < 5 + T && lx >= 5 && lx < 5 + T) rgb[ly - 5][lx - 5] = c;
         }
-        hole[ly][lx] = h;
+        dt.hole[ly][lx] = h;
     }
     __syncthreads();
-    for (int q = tid; q < HT * T; q += blockDim.x) {                      // 10-wide row max: columns x-5 .. x+4
-        const int ly = q / T, lx = q - ly * T;
-        uint8_t m = 0;
-#pragma unroll
-        for (int d = 0; d < 10; ++d) m |= hole[ly][lx + d];
-        rmax[ly][lx] = m;
-    }
+    dil::row_max(dt, tid, blockDim.x);                                   // 10-wide row max: columns x-5 .. x+4
     __syncthreads();
     const size_t plane_px = static_cast<size_t>(out) * out;
     for (int q = tid; q < T * T; q += blockDim.x) {                       // 10-high column max, then the per-pixel tail
         const int ly = q / T, lx = q - ly * T, gy = y0 + ly, gx = x0 + lx;
         if (gy >= out || gx >= out) continue;
-        uint8_t m = ok ? 0 : 1;
-#pragma unroll
-        for (int d = 0; d < 10; ++d) m |= rmax[ly + d][lx];
+        const uint8_t m = ok ? dil::col_max(dt, ly, lx) : 1;
         uchar4 c = ok ? rgb[ly][lx] : make_uchar4(0, 0, 0, 0);
         if (p.gray) {
             const unsigned l = (19595u * c.x + 38470u * c.y + 7471u * c.z + 0x8000u) >> 16;

@@ -3,7 +3,8 @@ launch, optional data-parallel gradient all-reduce (NCCL over NVLink) and whole-
 Inference engines (InferStep, SegInferStep): graph-captured eval-mode forward with the BatchNorm + activation passes fused
 into the convolution epilogues.  InpaintEvalStep: held-out evaluation of an inpainting U-Net on a GPU batcher, loss included,
 in one graph that coexists with a captured training step on the same network; SegEvalStep: the same for a segmentation network,
-with its loss and the pixel average precision (metrics.PixelAveragePrecision) in the graph.
+with its loss and the pixel average precision (metrics.PixelAveragePrecision) in the graph.  TextRemovalStep: text removal from
+pages in one graph -- segmentation, the demo's mask, the dilated holes, inpainting and the composite.
 
 The reference has no train script (SURVEY 3): its recipe is prose -- SGD + Nesterov momentum, weight decay,
 cyclic LR (checkpoints/ReadME.md:4).  One step here = forward + loss + backward (+ all-reduce) + SGD update,
@@ -732,21 +733,31 @@ class InferStep:
             self._check_markers()
         torch.cuda.synchronize()
         static_in = tuple(t.clone() if t is not None else None for t in inputs)
-        static_out = torch.empty(tuple(out.shape), dtype=torch.float32, device=out.device)
+        static_out = self._static_out(out)
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
-            static_out.copy_(self._run_forward(*static_in))
+            self._into(static_out, self._run_forward(*static_in))
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            static_out.copy_(self._run_forward(*static_in))
+            self._into(static_out, self._run_forward(*static_in))
         self._check_markers()
         # the captured kernels hold raw pointers to the operand buffers current at capture: keep them (and what rewrites them)
         self._captured_operands += [(c, c.current) for _, _, c in ops.operand_caches(self.net) if c.current is not None]
         torch.cuda.synchronize()
         return graph, static_in, static_out
+
+    def _static_out(self, out):
+        """The buffer run() returns for this shape: a fp32 copy of the forward's output (a subclass whose forward writes a buffer
+        of its own returns that buffer, and nothing is copied)."""
+        return torch.empty(tuple(out.shape), dtype=torch.float32, device=out.device)
+
+    @staticmethod
+    def _into(static_out, out):
+        if out is not static_out:
+            static_out.copy_(out)
 
     def refresh(self):
         """Rewrite the captured operand buffers and BatchNorm coefficients from the current parameters and buffers."""
@@ -793,6 +804,121 @@ class SegInferStep(InferStep):
 
     def _inputs(self, x):
         return (x,)
+
+
+# the segmentation demo's Normalize (Examples/demo_segmentation.py:59-62), the input convention of the published checkpoint
+DEMO_MEAN_STD = ((0.4935, 0.4563, 0.4544), (0.3769, 0.3615, 0.3566))
+
+
+def _round_up(v: int, m: int) -> int:
+    return (v + m - 1) // m * m
+
+
+class _TextRemovalNets(torch.nn.Module):
+    """Both networks of a TextRemovalStep under one module, so InferStep's BatchNorm list, operand caches, fused-output markers
+    and weight refresh cover them together."""
+
+    def __init__(self, seg_net, fill_net):
+        super().__init__()
+        self.seg = seg_net
+        self.fill = fill_net
+
+
+class TextRemovalStep(InferStep):
+    """Text removal from pages in one CUDA graph per page shape, the pipeline the reference's README describes (detect the text
+    and make a mask, white it out, inpaint the hole), each stage as the reference's own code defines it (DESIGN 5.2):
+
+      1. ``Normalize(mean, std)`` of the page and zero padding on the right and bottom to multiples of 8 (EvaluateSet);
+      2. the segmentation network's logits (eval mode, fused BatchNorm + activation epilogues);
+      3. the demo's text mask: ``sigmoid > 0.5``, 3x3 max-pool, unpad (ops.text_mask_postprocess);
+      4. the holes the U-Nets were trained on: the mask as a {0, 255} image, ``> 0.4 * 255``, ``cv2.dilate`` 10x10;
+      5. ``valid = 1 - hole`` and ``page * valid``, padded on the right and bottom to multiples of ``2 ** len(fill_net.decoder)``
+         (the padding is hole);
+      6. the U-Net's fill (eval mode, fused epilogues, the mask chain on its own stream);
+      7. the composite ``valid * page + (1 - valid) * fill`` cropped to the page, not clamped.
+
+    `seg_net`: TextSegament or XceptionTextSegment; `fill_net`: ImageFillOrigin, ImageFillOriginV2 or ImageFill, on the same
+    CUDA device.  `normalize`: (mean, std) of step 1, the demo's by default; None skips it.  The page is segmented at the size it
+    is given: a caller who wants the demo's 600-pixel long side resizes first.
+
+    ``run(page)`` takes fp32 NCHW pages [n, 3, h, w] in [0, 1] (``to_tensor`` of the RGB page) and returns the composite as a
+    static fp32 NCHW buffer that the next call overwrites.  The same call leaves static buffers of its stages:
+    `text_mask` (uint8 [n, 1, h, w], 1 = text: the demo's mask), `valid` (uint8 [n, hu, wu], 1 = kept), `last_logits` and
+    `last_fill` (the two networks' raw outputs).  Counters and weight reloads as InferStep: ``load_state_dict`` on either network
+    is picked up by the next run()."""
+
+    def __init__(self, seg_net: torch.nn.Module, fill_net: torch.nn.Module, normalize=DEMO_MEAN_STD, compute_dtype=torch.bfloat16):
+        from .models.image_inpainting import ImageFill, ImageFillOrigin, ImageFillOriginV2
+        from .models.text_segmentation import TextSegament, XceptionTextSegment
+        if not isinstance(seg_net, (TextSegament, XceptionTextSegment)):
+            raise TypeError(f"TextRemovalStep: seg_net must be a TextSegament or XceptionTextSegment, got {type(seg_net).__name__}")
+        if not isinstance(fill_net, (ImageFillOrigin, ImageFillOriginV2, ImageFill)):
+            raise TypeError(f"TextRemovalStep: fill_net must be an ImageFillOrigin, ImageFillOriginV2 or ImageFill, got "
+                            f"{type(fill_net).__name__}")
+        if compute_dtype not in (torch.bfloat16, torch.float32):
+            raise ValueError("TextRemovalStep: compute_dtype must be torch.bfloat16 or torch.float32")
+        devs = {t.device for net in (seg_net, fill_net) for t in list(net.parameters()) + list(net.buffers())}
+        if len(devs) != 1 or next(iter(devs)).type != "cuda":
+            raise ValueError(f"TextRemovalStep: both networks must be on one CUDA device, found {sorted(str(d) for d in devs)}")
+        self.device = next(iter(devs))
+        self.normalize = None
+        if normalize is not None:
+            mean, std = (tuple(float(v) for v in t) for t in normalize)
+            if len(mean) != 3 or len(std) != 3:
+                raise ValueError("TextRemovalStep: normalize takes (mean, std) with three values each")
+            self.normalize = (mean, std)
+        super().__init__(_TextRemovalNets(seg_net, fill_net), compute_dtype)
+        self.multiple = 2 ** len(fill_net.decoder)        # one nearest x2 per decoder stage
+        self._outs = {}                                   # page shape -> the composite buffer run() returns
+        self._products = {}                               # page shape -> (text_mask, valid, logits, fill) of its graph
+        self._cur = None
+        self.text_mask = self.valid = self.last_logits = self.last_fill = None
+
+    def padded_sizes(self, h: int, w: int):
+        """((hs, ws), (hu, wu)): the segmentation and U-Net grids of an h x w page."""
+        return (_round_up(h, 8), _round_up(w, 8)), (_round_up(h, self.multiple), _round_up(w, self.multiple))
+
+    def _forward(self, page):
+        n, _, h, w = page.shape
+        (hs, ws), (hu, wu) = self.padded_sizes(h, w)
+        x = ops.removal_seg_input(page, self.normalize, hs, ws, self.dtype)
+        logits = self.net.seg(x)
+        text_mask = ops.text_mask_postprocess(logits, (0, ws - w, 0, hs - h), (h, w))
+        corrupted, valid = ops.removal_holes(text_mask, page, hu, wu, self.dtype)
+        # a new view object per call: the layers tag an input plane with the event that made it ready (ops._pconv_launch), and
+        # this plane is rewritten by every call
+        fill = self.net.fill((corrupted, HoleMask.from_plane(valid.view(valid.shape), 3)))
+        key = self._key(page)
+        out = self._outs.get(key)
+        if out is None:                                   # the first eager warm-up: never inside a capture
+            out = self._outs[key] = torch.empty((n, 3, h, w), dtype=torch.float32, device=page.device)
+        ops.removal_composite(fill, page, valid, out=out)
+        self._cur = (text_mask, valid, logits, fill)
+        return out
+
+    def _static_out(self, out):
+        return out                                        # the composite is written straight into the returned buffer
+
+    def _key(self, page):
+        return tuple(page.shape), page.dtype
+
+    def _inputs(self, page):
+        return (page,)
+
+    def _capture(self, inputs):
+        entry = super()._capture(inputs)
+        self._products[self._key(*inputs)] = self._cur   # the captured forward's buffers, rewritten by every replay
+        self._cur = None
+        return entry
+
+    def run(self, page: torch.Tensor) -> torch.Tensor:
+        """Remove the text from a batch of pages (fp32 NCHW [n, 3, h, w]).  Returns the static fp32 NCHW composite."""
+        ops._check_page(page, "TextRemovalStep.run", contiguous=False)
+        if page.device != self.device:
+            raise _lib.PcbError(f"TextRemovalStep.run: the page is on {page.device}, the networks on {self.device}")
+        out = super().run(page.contiguous())
+        self.text_mask, self.valid, self.last_logits, self.last_fill = self._products[self._key(page)]
+        return out
 
 
 class _BatcherEvalStep(InferStep):

@@ -1397,3 +1397,100 @@ def text_mask_postprocess(logits: torch.Tensor, border_pad, out_hw) -> torch.Ten
     _lib.check(_lib.load().pcb_seg_mask_postprocess(x.data_ptr(), _dtype_code(x), n, h, w, nhwc_layout(x), h - bottom, w - right, oh, ow,
                                                     out.data_ptr(), _stream()))
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# text removal: the glue between segmentation, mask and inpainting (csrc/text_removal.cu, engine.TextRemovalStep)
+# ------------------------------------------------------------------------------------------------
+def _check_page(page: torch.Tensor, fn: str, contiguous: bool = True):
+    if not isinstance(page, torch.Tensor) or not page.is_cuda or page.dtype != torch.float32 or page.dim() != 4 or page.shape[1] != 3:
+        shape = tuple(page.shape) if isinstance(page, torch.Tensor) else type(page).__name__
+        raise _lib.PcbError(f"{fn}: expected a 4-D CUDA fp32 page [n, 3, h, w], got {shape}"
+                            + (f" {page.dtype} on {page.device}" if isinstance(page, torch.Tensor) else ""))
+    if contiguous and not page.is_contiguous():
+        raise _lib.PcbError(f"{fn}: the page must be contiguous NCHW")
+    if min(page.shape) < 1:
+        raise _lib.PcbError(f"{fn}: empty page {tuple(page.shape)}")
+
+
+def _check_padded(fn, what, ph, pw, h, w):
+    if int(ph) < h or int(pw) < w:
+        raise _lib.PcbError(f"{fn}: {what} {int(ph)}x{int(pw)} is smaller than the {h}x{w} page")
+
+
+def _compute_code(dtype) -> int:
+    if dtype == torch.bfloat16:
+        return PCB_BF16
+    if dtype == torch.float32:
+        return PCB_F32
+    raise _lib.PcbError(f"unsupported compute dtype {dtype}: the GPU path computes in float32 or bfloat16")
+
+
+def removal_seg_input(page: torch.Tensor, mean_std, hs: int, ws: int, dtype=torch.bfloat16) -> torch.Tensor:
+    """The segmentation network's input in one launch (EvaluateSet, Dataloader.py:271-273, 296-303): ``Normalize(mean, std)``
+    of the fp32 page in torchvision's order, zero padding on the right and bottom to `hs` x `ws`, rounded once to `dtype`.
+    `mean_std`: (mean[3], std[3]), or None to skip the normalization.  Returns the [n, 3, hs, ws] view of a new 8-channel NHWC
+    buffer whose padded pixels and channels are zero."""
+    fn = "removal_seg_input"
+    _check_page(page, fn)
+    n, _, h, w = page.shape
+    _check_padded(fn, "padded size", hs, ws, h, w)
+    norm = None
+    if mean_std is not None:
+        mean, std = (tuple(float(v) for v in t) for t in mean_std)
+        if len(mean) != 3 or len(std) != 3:
+            raise ValueError(f"{fn}: mean_std takes (mean, std) with three values each")
+        norm = (ctypes.c_float * 6)(*mean, *std)
+    code = _compute_code(dtype)
+    buf = torch.empty((n, 8, int(hs), int(ws)), dtype=dtype, device=page.device, memory_format=CL)
+    _lib.check(_lib.load().pcb_removal_seg_input(page.data_ptr(), n, h, w, norm, int(hs), int(ws), buf.data_ptr(), code, _stream()))
+    return buf[:, :3]
+
+
+def removal_holes(text_mask: torch.Tensor, page: torch.Tensor, hu: int, wu: int, dtype=torch.bfloat16):
+    """The inpainting U-Net's input from the demo's text mask in one launch (Dataloader.py:120-121, 128-131): the mask as the
+    {0, 255} image, ``> 0.4 * 255``, ``cv2.dilate`` with a 10x10 kernel, then ``valid = 1 - hole`` and ``page * valid`` on the
+    `hu` x `wu` grid, whose padding on the right and bottom is hole and zero.  `text_mask`: uint8 [n, 1, h, w] (nonzero = text,
+    text_mask_postprocess's output).  Returns (corrupted, valid): the [n, 3, hu, wu] view of a new 8-channel NHWC buffer in
+    `dtype`, and uint8 [n, hu, wu] (1 = valid)."""
+    fn = "removal_holes"
+    _check_page(page, fn)
+    n, _, h, w = page.shape
+    if not isinstance(text_mask, torch.Tensor) or text_mask.dtype != torch.uint8 or tuple(text_mask.shape) != (n, 1, h, w) \
+            or text_mask.device != page.device or not text_mask.is_contiguous():
+        got = (tuple(text_mask.shape), text_mask.dtype, str(text_mask.device)) if isinstance(text_mask, torch.Tensor) else text_mask
+        raise _lib.PcbError(f"{fn}: expected a contiguous uint8 text mask [{n}, 1, {h}, {w}] on {page.device}, got {got}")
+    _check_padded(fn, "padded size", hu, wu, h, w)
+    code = _compute_code(dtype)
+    buf = torch.empty((n, 8, int(hu), int(wu)), dtype=dtype, device=page.device, memory_format=CL)
+    valid = torch.empty((n, int(hu), int(wu)), dtype=torch.uint8, device=page.device)
+    _lib.check(_lib.load().pcb_removal_holes(text_mask.data_ptr(), page.data_ptr(), n, h, w, int(hu), int(wu), valid.data_ptr(),
+                                             buf.data_ptr(), code, _stream()))
+    return buf[:, :3], valid
+
+
+def removal_composite(fill: torch.Tensor, page: torch.Tensor, valid: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The composite ``valid * page + (1 - valid) * fill`` (loss.py:196, comp_img) cropped to the page, as a select: the page
+    where valid, the U-Net output elsewhere.  `fill`: the U-Net output [n, 3, hu, wu] (bf16 or fp32, NHWC, possibly
+    channel-padded); `valid`: uint8 [n, hu, wu] (removal_holes).  Writes fp32 NCHW [n, 3, h, w] into `out` (a new tensor when
+    None) and returns it."""
+    fn = "removal_composite"
+    _check_page(page, fn)
+    n, _, h, w = page.shape
+    if not isinstance(valid, torch.Tensor) or valid.dtype != torch.uint8 or valid.dim() != 3 or valid.shape[0] != n \
+            or valid.device != page.device or not valid.is_contiguous():
+        raise _lib.PcbError(f"{fn}: expected a contiguous uint8 valid plane [{n}, hu, wu] on {page.device}")
+    hu, wu = valid.shape[1:]
+    _check_padded(fn, "valid plane", hu, wu, h, w)
+    if not isinstance(fill, torch.Tensor) or not fill.is_cuda or fill.dim() != 4 or tuple(fill.shape) != (n, 3, hu, wu) \
+            or fill.device != page.device:
+        raise _lib.PcbError(f"{fn}: expected a CUDA U-Net output [{n}, 3, {hu}, {wu}] on {page.device}")
+    if nhwc_layout(fill) is None:
+        fill = fill.contiguous(memory_format=CL)
+    if out is None:
+        out = torch.empty((n, 3, h, w), dtype=torch.float32, device=page.device)
+    elif out.dtype != torch.float32 or tuple(out.shape) != (n, 3, h, w) or not out.is_contiguous() or out.device != page.device:
+        raise _lib.PcbError(f"{fn}: out must be a contiguous fp32 [{n}, 3, {h}, {w}] tensor on {page.device}")
+    _lib.check(_lib.load().pcb_removal_composite(fill.data_ptr(), _dtype_code(fill), nhwc_layout(fill), page.data_ptr(), valid.data_ptr(),
+                                                 n, h, w, hu, wu, out.data_ptr(), _stream()))
+    return out
