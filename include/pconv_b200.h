@@ -273,7 +273,15 @@ int pcb_seg_mask_postprocess(const void *logits, int dtype, int n, int h, int w,
 /* ---- text removal (engine.TextRemovalStep): the glue between segmentation, mask and inpainting ---------------------------
  * `page`: fp32 NCHW [n, 3, h, w], contiguous, device memory.
  *
- * The segmentation input (EvaluateSet, Dataloader.py:271-273, 296-303): per pixel of the [hs, ws] grid (hs >= h, ws >= w),
+ * EvaluateSet's page resize (Dataloader.py:290-291): out fp32 NCHW [n, 3, rh, rw] =
+ * to_tensor(to_pil_image(page[i]).resize((rw, rh), Image.BICUBIC)) per image.  Each byte is mul(255) in fp32, clamped to
+ * [0, 255] (NaN to 0) and truncated, as to_pil_image makes it; then Pillow's two integer passes (horizontal first, clipped
+ * uint8 between them, 22-bit weights) and / 255.  At most a 16x reduction per axis (h <= 16 rh, w <= 16 rw).  `workspace`:
+ * device memory of pcb_page_resize_workspace(n, h, w, rh, rw) bytes (0 for out-of-range sizes), 256-byte aligned; three
+ * launches, no host synchronisation. */
+size_t pcb_page_resize_workspace(int n, int h, int w, int rh, int rw);
+int pcb_page_resize_bicubic(const float *page, int n, int h, int w, int rh, int rw, void *workspace, float *out, pcb_stream_t stream);
+/* The segmentation input (EvaluateSet, Dataloader.py:271-273, 296-303): per pixel of the [hs, ws] grid (hs >= h, ws >= w),
  * (page - mean) / std in fp32 (sub, then div, each rounded; `norm`: HOST pointer to mean[3], std[3], or NULL to skip it),
  * rounded once to `dtype`, zero outside the page.  out: [n, hs, ws, 8] NHWC (channels 3..7 zero), every element written. */
 int pcb_removal_seg_input(const float *page, int n, int h, int w, const float *norm, int hs, int ws, void *out, int dtype,

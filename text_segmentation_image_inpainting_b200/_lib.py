@@ -97,6 +97,8 @@ _SIGS = {
     "pcb_inpaint_pair_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_inpaint_pair_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                          c_void_p, c_void_p]),
+    "pcb_page_resize_workspace": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "pcb_page_resize_bicubic": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_removal_seg_input": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]),
     "pcb_removal_holes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "pcb_removal_composite": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

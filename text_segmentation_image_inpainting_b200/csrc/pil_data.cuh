@@ -10,6 +10,7 @@
 namespace pil {
 
 constexpr int KMAX = 33;      // taps of a bicubic window at scale 8 (2 * ceil(2 * 8) + 1): box / out <= 8
+constexpr int taps_for(int reduction) { return 4 * reduction + 1; }   // the window of a reduction of at most `reduction`
 constexpr int PB = 22;        // Pillow's PRECISION_BITS for 8-bit images
 
 __device__ __forceinline__ double bicubic(double x) {
@@ -21,7 +22,9 @@ __device__ __forceinline__ double bicubic(double x) {
 }
 
 // Pillow's precompute_coeffs + normalize_coeffs_8bpc for output index xx of a box of `insize` input pixels resampled to
-// `outsize`: writes the integer weights to k[0], k[stride], ... and returns the first tap; *count = number of taps.
+// `outsize`: writes the integer weights to k[0], k[stride], ... and returns the first tap; *count = number of taps.  KM bounds
+// the window (taps_for(insize / outsize)), and with it the registers of the weights in double.
+template <int KM = KMAX>
 __device__ inline int pil_coeffs(int xx, int insize, int outsize, int *k, int stride, int *count) {
     const double scale = __ddiv_rn(static_cast<double>(insize), static_cast<double>(outsize));
     const double fs = scale < 1.0 ? 1.0 : scale;
@@ -32,18 +35,18 @@ __device__ inline int pil_coeffs(int xx, int insize, int outsize, int *k, int st
     int xmax = static_cast<int>(__dadd_rn(__dadd_rn(center, support), 0.5));
     if (xmax > insize) xmax = insize;
     xmax -= xmin;
-    if (xmax > KMAX) xmax = KMAX;                    // unreachable for box / out <= 8 (checked on the host)
-    double w[KMAX];
+    if (xmax > KM) xmax = KM;                        // unreachable within the reduction KM was chosen for (checked on the host)
+    double w[KM];
     double ww = 0.0;
 #pragma unroll
-    for (int x = 0; x < KMAX; ++x) {
+    for (int x = 0; x < KM; ++x) {
         if (x < xmax) {
             w[x] = bicubic(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(x + xmin), center), 0.5), ss));
             ww = __dadd_rn(ww, w[x]);
         }
     }
 #pragma unroll
-    for (int x = 0; x < KMAX; ++x) {
+    for (int x = 0; x < KM; ++x) {
         if (x < xmax) {
             const double v = ww != 0.0 ? __ddiv_rn(w[x], ww) : w[x];
             const double s = __dmul_rn(v, static_cast<double>(1 << PB));

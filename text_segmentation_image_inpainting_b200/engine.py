@@ -838,16 +838,23 @@ class TextRemovalStep(InferStep):
       7. the composite ``valid * page + (1 - valid) * fill`` cropped to the page, not clamped.
 
     `seg_net`: TextSegament or XceptionTextSegment; `fill_net`: ImageFillOrigin, ImageFillOriginV2 or ImageFill, on the same
-    CUDA device.  `normalize`: (mean, std) of step 1, the demo's by default; None skips it.  The page is segmented at the size it
-    is given: a caller who wants the demo's 600-pixel long side resizes first.
+    CUDA device.  `normalize`: (mean, std) of step 1, the demo's by default; None skips it.
+
+    `seg_resize`: None segments the page at the size it is given.  An int is EvaluateSet's `resize` (600 in the segmentation
+    demo, the scale the published checkpoint is used at): steps 1-3 then run on the page as EvaluateSet prepares it -- resized
+    with Pillow's bicubic so its long side is about `seg_resize` (ops.evaluate_set_geometry, ops.page_resize_bicubic),
+    normalized and padded on one side to `seg_resize` -- and step 3 brings the mask back to the page's size (EvaluateSet's
+    resize_mask).  Steps 4-7 run at the page's own resolution either way.
 
     ``run(page)`` takes fp32 NCHW pages [n, 3, h, w] in [0, 1] (``to_tensor`` of the RGB page) and returns the composite as a
     static fp32 NCHW buffer that the next call overwrites.  The same call leaves static buffers of its stages:
-    `text_mask` (uint8 [n, 1, h, w], 1 = text: the demo's mask), `valid` (uint8 [n, hu, wu], 1 = kept), `last_logits` and
+    `text_mask` (uint8 [n, 1, h, w], 1 = text: the demo's mask), `valid` (uint8 [n, hu, wu], 1 = kept), `last_resized` (the
+    resized fp32 page, None without `seg_resize`), `last_seg_input` (the segmentation network's input), `last_logits` and
     `last_fill` (the two networks' raw outputs).  Counters and weight reloads as InferStep: ``load_state_dict`` on either network
     is picked up by the next run()."""
 
-    def __init__(self, seg_net: torch.nn.Module, fill_net: torch.nn.Module, normalize=DEMO_MEAN_STD, compute_dtype=torch.bfloat16):
+    def __init__(self, seg_net: torch.nn.Module, fill_net: torch.nn.Module, normalize=DEMO_MEAN_STD, compute_dtype=torch.bfloat16,
+                 seg_resize=None):
         from .models.image_inpainting import ImageFill, ImageFillOrigin, ImageFillOriginV2
         from .models.text_segmentation import TextSegament, XceptionTextSegment
         if not isinstance(seg_net, (TextSegament, XceptionTextSegment)):
@@ -867,23 +874,39 @@ class TextRemovalStep(InferStep):
             if len(mean) != 3 or len(std) != 3:
                 raise ValueError("TextRemovalStep: normalize takes (mean, std) with three values each")
             self.normalize = (mean, std)
+        self.seg_resize = None
+        if seg_resize is not None:
+            if isinstance(seg_resize, bool) or not isinstance(seg_resize, int) or seg_resize <= 0 or seg_resize % 8:
+                raise ValueError(f"TextRemovalStep: seg_resize must be None or a positive multiple of 8, got {seg_resize!r}")
+            self.seg_resize = seg_resize
         super().__init__(_TextRemovalNets(seg_net, fill_net), compute_dtype)
         self.multiple = 2 ** len(fill_net.decoder)        # one nearest x2 per decoder stage
         self._outs = {}                                   # page shape -> the composite buffer run() returns
-        self._products = {}                               # page shape -> (text_mask, valid, logits, fill) of its graph
+        self._products = {}                               # page shape -> the stage buffers of its graph (_PRODUCTS)
         self._cur = None
-        self.text_mask = self.valid = self.last_logits = self.last_fill = None
+        self.text_mask = self.valid = self.last_resized = self.last_seg_input = self.last_logits = self.last_fill = None
+
+    _PRODUCTS = ("text_mask", "valid", "last_resized", "last_seg_input", "last_logits", "last_fill")
+
+    def _seg_geometry(self, h: int, w: int):
+        """((rh, rw), border_pad): the size the page is segmented at and the padding to the segmentation grid."""
+        if self.seg_resize is None:
+            return (h, w), (0, _round_up(w, 8) - w, 0, _round_up(h, 8) - h)
+        return ops.evaluate_set_geometry(h, w, self.seg_resize)
 
     def padded_sizes(self, h: int, w: int):
         """((hs, ws), (hu, wu)): the segmentation and U-Net grids of an h x w page."""
-        return (_round_up(h, 8), _round_up(w, 8)), (_round_up(h, self.multiple), _round_up(w, self.multiple))
+        (rh, rw), (_, right, _, bottom) = self._seg_geometry(h, w)
+        return (rh + bottom, rw + right), (_round_up(h, self.multiple), _round_up(w, self.multiple))
 
     def _forward(self, page):
         n, _, h, w = page.shape
+        (rh, rw), pad = self._seg_geometry(h, w)
         (hs, ws), (hu, wu) = self.padded_sizes(h, w)
-        x = ops.removal_seg_input(page, self.normalize, hs, ws, self.dtype)
+        resized = ops.page_resize_bicubic(page, rh, rw) if self.seg_resize is not None else None
+        x = ops.removal_seg_input(page if resized is None else resized, self.normalize, hs, ws, self.dtype)
         logits = self.net.seg(x)
-        text_mask = ops.text_mask_postprocess(logits, (0, ws - w, 0, hs - h), (h, w))
+        text_mask = ops.text_mask_postprocess(logits, pad, (h, w))
         corrupted, valid = ops.removal_holes(text_mask, page, hu, wu, self.dtype)
         # a new view object per call: the layers tag an input plane with the event that made it ready (ops._pconv_launch), and
         # this plane is rewritten by every call
@@ -893,7 +916,7 @@ class TextRemovalStep(InferStep):
         if out is None:                                   # the first eager warm-up: never inside a capture
             out = self._outs[key] = torch.empty((n, 3, h, w), dtype=torch.float32, device=page.device)
         ops.removal_composite(fill, page, valid, out=out)
-        self._cur = (text_mask, valid, logits, fill)
+        self._cur = (text_mask, valid, resized, x, logits, fill)
         return out
 
     def _static_out(self, out):
@@ -916,8 +939,10 @@ class TextRemovalStep(InferStep):
         ops._check_page(page, "TextRemovalStep.run", contiguous=False)
         if page.device != self.device:
             raise _lib.PcbError(f"TextRemovalStep.run: the page is on {page.device}, the networks on {self.device}")
+        self._seg_geometry(*page.shape[2:])              # refuses a page seg_resize cannot take before anything is launched
         out = super().run(page.contiguous())
-        self.text_mask, self.valid, self.last_logits, self.last_fill = self._products[self._key(page)]
+        for name, t in zip(self._PRODUCTS, self._products[self._key(page)]):
+            setattr(self, name, t)
         return out
 
 

@@ -1426,6 +1426,51 @@ def _compute_code(dtype) -> int:
     raise _lib.PcbError(f"unsupported compute dtype {dtype}: the GPU path computes in float32 or bfloat16")
 
 
+PAGE_RESIZE_MAX_REDUCTION = 16            # page_resize_bicubic's largest reduction per axis (in / out)
+
+
+def evaluate_set_geometry(h: int, w: int, resize: int):
+    """EvaluateSet.resize_pad_tensor's geometry for an h x w page (Dataloader.py:287-303), in Python float arithmetic as written
+    there: ``ratio = resize / max(w, h)``, each side ``int(side * ratio) // 8 * 8``, then the one-sided pad: on the right when the
+    resized width is below `resize`, else at the bottom.  Returns ((rh, rw), border_pad) with border_pad the (left, right, top,
+    bottom) padding, so the segmentation grid is (rh + bottom) x (rw + right).  Raises ValueError for a `resize` that is not a
+    positive multiple of 8, an empty resized side, or a reduction beyond page_resize_bicubic's."""
+    h, w, fix_len = int(h), int(w), int(resize)
+    if fix_len <= 0 or fix_len % 8 != 0:
+        raise ValueError(f"evaluate_set_geometry: resize {resize} is not a positive multiple of 8")
+    if h < 1 or w < 1:
+        raise ValueError(f"evaluate_set_geometry: empty page {h}x{w}")
+    ratio = fix_len / max(w, h)
+    rw, rh = (int(x * ratio) // 8 * 8 for x in (w, h))
+    if rh == 0 or rw == 0:
+        raise ValueError(f"evaluate_set_geometry: a {h}x{w} page resizes to {rh}x{rw} at resize {fix_len}")
+    if h > PAGE_RESIZE_MAX_REDUCTION * rh or w > PAGE_RESIZE_MAX_REDUCTION * rw:
+        raise ValueError(f"evaluate_set_geometry: a {h}x{w} page resizes to {rh}x{rw}, more than a "
+                         f"{PAGE_RESIZE_MAX_REDUCTION}x reduction on an axis")
+    pad = (0, fix_len - rw, 0, 0) if fix_len > rw else (0, 0, 0, fix_len - rh)
+    return (rh, rw), pad
+
+
+def page_resize_bicubic(page: torch.Tensor, rh: int, rw: int) -> torch.Tensor:
+    """EvaluateSet's page resize (Dataloader.py:291) of fp32 NCHW pages [n, 3, h, w] in [0, 1]:
+    ``to_tensor(to_pil_image(page[i]).resize((rw, rh), Image.BICUBIC))`` per image, with Pillow's integer resampler bit for bit.
+    Bytes are recovered as to_pil_image does (``mul(255)``, truncated), clamped to [0, 255] with NaN as 0, so a page made by
+    to_tensor gives back its own bytes.  At most a 16x reduction per axis.  Returns a new fp32 [n, 3, rh, rw] tensor."""
+    fn = "page_resize_bicubic"
+    _check_page(page, fn)
+    n, _, h, w = page.shape
+    rh, rw = int(rh), int(rw)
+    if rh < 1 or rw < 1:
+        raise _lib.PcbError(f"{fn}: empty output size {rh}x{rw}")
+    if h > PAGE_RESIZE_MAX_REDUCTION * rh or w > PAGE_RESIZE_MAX_REDUCTION * rw:
+        raise _lib.PcbError(f"{fn}: {h}x{w} to {rh}x{rw} reduces more than {PAGE_RESIZE_MAX_REDUCTION}x on an axis")
+    lib = _lib.load()
+    ws = torch.empty((lib.pcb_page_resize_workspace(n, h, w, rh, rw),), dtype=torch.uint8, device=page.device)
+    out = torch.empty((n, 3, rh, rw), dtype=torch.float32, device=page.device)
+    _lib.check(lib.pcb_page_resize_bicubic(page.data_ptr(), n, h, w, rh, rw, ws.data_ptr(), out.data_ptr(), _stream()))
+    return out
+
+
 def removal_seg_input(page: torch.Tensor, mean_std, hs: int, ws: int, dtype=torch.bfloat16) -> torch.Tensor:
     """The segmentation network's input in one launch (EvaluateSet, Dataloader.py:271-273, 296-303): ``Normalize(mean, std)``
     of the fp32 page in torchvision's order, zero padding on the right and bottom to `hs` x `ws`, rounded once to `dtype`.
