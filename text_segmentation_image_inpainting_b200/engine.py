@@ -40,10 +40,21 @@ def _flat_view(flat: torch.Tensor, off: int, like: torch.Tensor) -> torch.Tensor
 
 
 class FlatParams:
-    """All trainable parameters of a module re-pointed into one fp32 arena (and their grads into another)."""
+    """All trainable parameters of a module re-pointed into one fp32 arena (and their grads into another).
 
-    def __init__(self, module: torch.nn.Module):
-        self.params: List[torch.nn.Parameter] = [p for p in module.parameters() if p.requires_grad]
+    `retrainable` (a module or parameters of `module`): parameters that get a slot even while frozen, so that their storage moves
+    once, here, and a later `set_trainable()` can train them without moving anything.  `params` lists every slot in
+    `module.parameters()` order; `ranges` the [start, end) arena runs of the slots that are trainable now."""
+
+    def __init__(self, module: torch.nn.Module, retrainable=None):
+        if retrainable is None:
+            self.params: List[torch.nn.Parameter] = [p for p in module.parameters() if p.requires_grad]
+        else:
+            every = list(module.parameters())
+            extra = {id(p) for p in (retrainable.parameters() if isinstance(retrainable, torch.nn.Module) else retrainable)}
+            if not extra <= {id(p) for p in every}:
+                raise ValueError("retrainable: every parameter must belong to the network")
+            self.params = [p for p in every if p.requires_grad or id(p) in extra]
         dev = self.params[0].device
         total = sum(p.numel() for p in self.params)
         # pad every tensor to a multiple of 4 elements so all views stay 16-byte aligned
@@ -63,16 +74,32 @@ class FlatParams:
                 p.data = v
                 p.grad = _flat_view(self.flat_g, o, p.data)
         self.true_numel = total
+        self._sink_made = {}            # slot -> its GradSink, kept across set_trainable() calls
+        self.set_trainable()
+
+    def set_trainable(self):
+        """Gradient sinks and SGD ranges over the slots whose parameter requires a gradient now."""
         # Gradient sinks (ops.GradSink): the weight-gradient kernels (4-D convolution weights) and the BatchNorm backward
         # (1-D scale / shift) write straight into the arena -- no gradient tensor, no autograd accumulation kernel.
         self.sinks = []
         self.sink_of = {}
+        self.ranges = []                # [start, end) arena runs of consecutive trainable slots
         for i, p in enumerate(self.params):
+            if not p.requires_grad:
+                p.__dict__.pop("_pcb_grad_sink", None)
+                continue
+            end = self.offsets[i + 1] if i + 1 < len(self.params) else self.numel
+            if self.ranges and self.ranges[-1][1] == self.offsets[i]:
+                self.ranges[-1][1] = end
+            else:
+                self.ranges.append([self.offsets[i], end])
             ok4 = p.dim() == 4 and p.grad.is_contiguous(memory_format=CL) and (p.grad.data_ptr() % 16) == 0
             ok1 = p.dim() == 1
             if ok4 or ok1:
-                p._pcb_grad_sink = ops.GradSink(p.grad)
-                p._pcb_grad_sink.prezeroed = True        # TrainStep zeroes the whole gradient arena at the start of every step
+                if i not in self._sink_made:
+                    self._sink_made[i] = ops.GradSink(p.grad)
+                    self._sink_made[i].prezeroed = True  # TrainStep zeroes the whole gradient arena at the start of every step
+                p._pcb_grad_sink = self._sink_made[i]
                 self.sinks.append(p._pcb_grad_sink)
                 self.sink_of[i] = p._pcb_grad_sink
 
@@ -129,18 +156,25 @@ class TrainStep:
     `iteration` is the schedule iteration the next update runs, `last_lr` the rate of the last one (device fp64 scalar).
 
     Checkpoints: `state_dict()` / `load_state_dict()` save and restore the parameters, module buffers, momentum, schedule counter
-    and the batcher's generator; see there."""
+    and the batcher's generator; see there.
+
+    Frozen parameters (`requires_grad` False) are never updated: no weight decay, no momentum, as torch.optim.SGD leaves a
+    parameter without a gradient.  Their BatchNorm layers keep training mode and running statistics, and their operand buffers
+    are laid out once instead of at every step.  `retrainable` (a module or parameters of `net`) opts in to training in stages
+    on one step: those parameters get an arena slot even while frozen; after changing `requires_grad` (e.g.
+    ``net.encoder.requires_grad_(True)``), `update_trainable()` switches the step over in place."""
 
     def __init__(self, net: torch.nn.Module, compute_dtype=torch.bfloat16, lr=2e-4, momentum=0.9, weight_decay=1e-4,
                  nesterov=True, process_group=None, use_graph=True, bucket_mb=32, overlap_allreduce=None,
-                 lr_schedule: Optional[CyclicLR] = None):
+                 lr_schedule: Optional[CyclicLR] = None, retrainable=None):
         self.net = net.train()
         self.dtype = compute_dtype
         if lr_schedule is not None and not isinstance(lr_schedule, CyclicLR):
             raise TypeError("lr_schedule must be an engine.CyclicLR")
         self.lr_schedule = lr_schedule
         self._lr, self.momentum, self.wd, self.nesterov = lr, momentum, weight_decay, nesterov
-        self.flat = FlatParams(net)
+        self.retrainable = retrainable is not None
+        self.flat = FlatParams(net, retrainable)
         if lr_schedule is not None:
             dev = self.flat.flat_p.device
             start = lr_schedule.last_batch_iteration + 1
@@ -169,6 +203,7 @@ class TrainStep:
         self.overlap_active = False
         self._comm_stream = torch.cuda.Stream(device=self.flat.flat_p.device) if (self.world > 1 and is_cuda) else None
         self._hooks_installed = False
+        self._hooked = set()            # slots with a post-accumulate hook (a hook cannot be removed, only ignored)
         self._make_buckets()
         if self.pg is not None:
             self._sync_replicas()
@@ -201,10 +236,14 @@ class TrainStep:
         checkpoints cannot silently diverge; every rank then computes the same rate from the same counter.  `momentum`: the
         momentum arena too (after a load; at construction it is zeros on every rank).  BatchNorm batch statistics stay
         rank-local afterwards (the reference has no SyncBN); running statistics therefore drift per rank during training and
-        rank 0's are the ones to checkpoint."""
+        rank 0's are the ones to checkpoint.  Frozen parameters without an arena slot are broadcast one by one."""
         dist = torch.distributed
         src = dist.get_global_rank(self.pg, 0)
         dist.broadcast(self.flat.flat_p, src=src, group=self.pg)
+        slotted = {id(p) for p in self.flat.params}
+        for p in self.net.parameters():
+            if id(p) not in slotted:
+                dist.broadcast(p.data, src=src, group=self.pg)
         if momentum:
             dist.broadcast(self.flat.flat_m, src=src, group=self.pg)
         if self.lr_schedule is not None:
@@ -214,19 +253,67 @@ class TrainStep:
             dist.broadcast(b, src=src, group=self.pg)
         ops.bump_weight_epoch()
 
+    # -- frozen layers -----------------------------------------------------------------------------
+    def _sync_cache_modes(self, refresh_frozen=False):
+        """Give every operand cache of the network the mode of its weight: `frozen` (ops.OperandCache) while the weight requires
+        no gradient, so prefetch_weights() skips it and a captured step has no refresh for it.  A cache that changes mode, and
+        with `refresh_frozen` every frozen one, is rewritten in place once from the weight's current values (the buffers a
+        captured graph reads stay the same); `refresh_frozen` also rewrites every frozen record the captured step holds, in
+        case an eager forward has since given its cache a new one.  Modes change only outside a capture: a refresh captured
+        into the step would run again on every replay (warmup_and_capture() sets the modes before it captures)."""
+        if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+            return
+        done = set()
+        for _, _, cache in ops.operand_caches(self.net):
+            rec = cache.current
+            if rec is None:
+                continue
+            frozen = not rec.weight.requires_grad
+            if frozen != cache.frozen or (frozen and refresh_frozen):
+                cache.frozen = frozen
+                cache.refresh(rec)
+                done.add(id(rec))
+        if refresh_frozen:
+            for rec in self._captured_operands or ():
+                if id(rec) not in done and not rec.weight.requires_grad:
+                    rec.refresh()
+
+    def update_trainable(self):
+        """Switch to the parameters' current `requires_grad` in place, after a stage change such as
+        ``net.encoder.requires_grad_(True)`` or ``net.encoder.freeze_params(k)``: SGD ranges, gradient sinks and all-reduce
+        buckets are rebuilt over the trainable slots, frozen layers' operands are laid out once, and the captured graph is
+        dropped (the next `warmup_and_capture()` recaptures; its warm-up updates count in the schedule).  No parameter moves:
+        a parameter that requires a gradient but has no arena slot (see `retrainable`) is refused before anything changes.
+        Momentum, schedule counter and batcher generator carry over; a slot trained for the first time starts from zeros."""
+        slotted = {id(p) for p in self.flat.params}
+        missing = [n for n, p in self.net.named_parameters() if p.requires_grad and id(p) not in slotted]
+        if missing:
+            raise ValueError(f"update_trainable: {missing[:5]} require a gradient but have no arena slot; construct the step "
+                             "with retrainable= covering them")
+        self.close()
+        self.flat.set_trainable()
+        self._make_buckets()
+        self._hooks_installed = False
+        self._sync_cache_modes(refresh_frozen=True)
+
     # -- gradient exchange ---------------------------------------------------------------------------
     def _make_buckets(self):
         """Buckets of ~bucket_elems consecutive arena elements, cut at parameter boundaries.  Backward produces gradients
-        roughly from the END of the arena (decoder) to its start (encoder), so buckets complete tail first."""
+        roughly from the END of the arena (decoder) to its start (encoder), so buckets complete tail first.  Only trainable
+        slots are exchanged: a bucket never crosses the end of a trainable range."""
         fp = self.flat
         self.buckets = []               # [start, end, [param indices]]
-        start, members = 0, []
-        for i, off in enumerate(fp.offsets):
-            end = fp.offsets[i + 1] if i + 1 < len(fp.offsets) else fp.numel
-            members.append(i)
-            if end - start >= self.bucket_elems or i + 1 == len(fp.offsets):
-                self.buckets.append([start, end, members])
-                start, members = end, []
+        i = 0
+        for rs, re_ in fp.ranges:
+            start, members = rs, []
+            while i < len(fp.offsets) and fp.offsets[i] < re_:
+                end = fp.offsets[i + 1] if i + 1 < len(fp.offsets) else fp.numel
+                if fp.offsets[i] >= rs:
+                    members.append(i)
+                    if end - start >= self.bucket_elems or end == re_:
+                        self.buckets.append([start, end, members])
+                        start, members = end, []
+                i += 1
         self._bucket_of = {}
         for b, (_, _, mem) in enumerate(self.buckets):
             for i in mem:
@@ -240,14 +327,18 @@ class TrainStep:
             return
         self._hooks_installed = True
         for i, p in enumerate(self.flat.params):
+            if not p.requires_grad:
+                continue
             sink = self.flat.sink_of.get(i)
             if sink is not None:
                 sink.on_written = (lambda idx: (lambda: self._param_ready(idx)))(i)
             # parameters whose gradient still arrives through autograd (or a sink that was refused and fell back to it)
-            p.register_post_accumulate_grad_hook((lambda idx: (lambda _p: self._param_ready(idx)))(i))
+            if i not in self._hooked:
+                self._hooked.add(i)
+                p.register_post_accumulate_grad_hook((lambda idx: (lambda _p: self._param_ready(idx)))(i))
 
     def _param_ready(self, idx):
-        if not self._overlap_armed:
+        if not self._overlap_armed or idx not in self._bucket_of:
             return
         b = self._bucket_of[idx]
         if idx in self._pending[b]:
@@ -288,12 +379,13 @@ class TrainStep:
         torch.cuda.current_stream().wait_stream(self._comm_stream)
 
     def _allreduce(self):
-        """Un-overlapped exchange (fallback, and the CPU/gloo path): bucketed SUM all-reduce of the whole arena."""
+        """Un-overlapped exchange (fallback, and the CPU/gloo path): bucketed SUM all-reduce of the trainable ranges."""
         if self.world == 1:
             return
         g = self.flat.flat_g
-        for s in range(0, g.numel(), self.bucket_elems):
-            torch.distributed.all_reduce(g[s:s + self.bucket_elems], group=self.pg)
+        for rs, re_ in self.flat.ranges:
+            for s in range(rs, re_, self.bucket_elems):
+                torch.distributed.all_reduce(g[s:min(s + self.bucket_elems, re_)], group=self.pg)
 
     # -- one eager step ----------------------------------------------------------------------------
     def _prepare(self, x: torch.Tensor, mask: torch.Tensor):
@@ -323,7 +415,8 @@ class TrainStep:
         ops.set_mask_chain_stream(True)
         self._arm_overlap(overlap)
         try:
-            ops.prefetch_weights(self._caches)         # operand re-layout of all layers runs ahead on its own stream
+            self._sync_cache_modes()
+            ops.prefetch_weights(self._caches)         # operand re-layout of all trainable layers runs ahead on its own stream
             loss = self._forward_loss(x, mask)
             loss.backward()
         finally:
@@ -341,14 +434,19 @@ class TrainStep:
         return ops.l1_mean(self.net((xin, hm)))
 
     def _update(self, first_step: bool):
+        """One SGD launch per trainable range (the whole arena unless some slots are frozen): frozen slots keep their
+        parameters and momentum bitwise."""
+        fp = self.flat
         if self.lr_schedule is None:
-            ops.sgd_step(self.flat.flat_p, self.flat.flat_g, self.flat.flat_m, self.lr, self.momentum, self.wd, self.nesterov,
-                         first_step, grad_scale=self.grad_scale)
+            for s, e in fp.ranges:
+                ops.sgd_step(fp.flat_p[s:e], fp.flat_g[s:e], fp.flat_m[s:e], self.lr, self.momentum, self.wd, self.nesterov,
+                             first_step, grad_scale=self.grad_scale)
             return
         s = self.lr_schedule
         ops.lr_cyclic(self._lr_iter, self._lr32, self._lr64, s.base_lr, s.max_lr, s.step_size, CyclicLR.MODES[s.mode], s.gamma)
-        ops.sgd_step_dev(self.flat.flat_p, self.flat.flat_g, self.flat.flat_m, self._lr32, self.momentum, self.wd, self.nesterov,
-                         grad_scale=self.grad_scale)
+        for a, e in fp.ranges:
+            ops.sgd_step_dev(fp.flat_p[a:e], fp.flat_g[a:e], fp.flat_m[a:e], self._lr32, self.momentum, self.wd, self.nesterov,
+                             grad_scale=self.grad_scale)
 
     def _step(self, x, mask, first_step: bool, overlap=None):
         overlap = self.overlap if overlap is None else overlap
@@ -377,6 +475,7 @@ class TrainStep:
         with torch.cuda.stream(side):
             self._step(self.static_x, self.static_m, False)
         torch.cuda.current_stream().wait_stream(side)
+        self._sync_cache_modes()        # caches the step above created (eager_warmup=0) take their mode before the capture
         torch.cuda.synchronize()
         graph = None
         if self.world == 1 or self.overlap:
@@ -440,7 +539,8 @@ class TrainStep:
           * "model": `net.state_dict()` -- the reference's keys, BatchNorm buffers included;
           * "optimizer": in torch.optim.SGD's state_dict format over the trainable parameters (FlatParams order:
             `[p for p in net.parameters() if p.requires_grad]`), each momentum buffer in its parameter's logical shape;
-            `param_groups[0]["lr"]` is the current rate (`last_lr` with a schedule);
+            `param_groups[0]["lr"]` is the current rate (`last_lr` with a schedule).  With `retrainable` it lists all of
+            `net.parameters()` instead, and every slot, frozen or not, carries its buffer, so that it loads at either stage;
           * "last_batch_iteration" (with a schedule): the value that continues the reference's CyclicLR;
           * "batcher_rng" (steps fed by a GPU batcher): the batcher's device generator state.
 
@@ -451,9 +551,14 @@ class TrainStep:
         group = {"lr": float(self._lr64) if sched else float(self.lr), "momentum": self.momentum, "dampening": 0,
                  "weight_decay": self.wd, "nesterov": bool(self.nesterov), "maximize": False, "foreach": None,
                  "differentiable": False, "fused": None, "params": list(range(len(self.flat.params)))}
+        index = list(range(len(self.flat.params)))
+        if self.retrainable:
+            pos = {id(p): j for j, p in enumerate(self.net.parameters())}
+            group["params"] = list(range(len(pos)))
+            index = [pos[id(p)] for p in self.flat.params]
         state = {}
         if self.momentum != 0:
-            state = {i: {"momentum_buffer": cpu(m)} for i, m in enumerate(self._arena_views(self.flat.flat_m))}
+            state = {j: {"momentum_buffer": cpu(m)} for j, m in zip(index, self._arena_views(self.flat.flat_m))}
         sd = {"model": OrderedDict((k, cpu(v)) for k, v in self.net.state_dict().items()),
               "optimizer": {"state": state, "param_groups": [group]}}
         if sched:
@@ -464,8 +569,9 @@ class TrainStep:
         return sd
 
     def _momentum_buffers(self, opt) -> list:
-        """The momentum buffer of every trainable parameter (None: zeros) from a torch.optim.SGD-format state dict, whose one
-        parameter group lists either the trainable parameters or all of `net.parameters()` (frozen ones carry no state)."""
+        """The momentum buffer of every slot (None: zeros) from a torch.optim.SGD-format state dict, whose one parameter group
+        lists the slots, the trainable parameters or all of `net.parameters()`.  Only a frozen parameter without a slot may not
+        carry state (with `retrainable`, a frozen slot keeps its buffer)."""
         groups = opt.get("param_groups")
         if not isinstance(groups, (list, tuple)) or len(groups) != 1:
             raise ValueError("load_state_dict: the optimizer state must have exactly one parameter group")
@@ -479,11 +585,14 @@ class TrainStep:
                                  "would mean something else")
         params = self.flat.params
         every = list(self.net.parameters())
+        trainable = [p for p in params if p.requires_grad]
         ids = list(g.get("params", []))
         if len(ids) == len(params):
             order = params
         elif len(ids) == len(every):
             order = every
+        elif len(ids) == len(trainable):    # a checkpoint of a step without `retrainable` at the current stage
+            order = trainable
         else:
             raise ValueError(f"load_state_dict: the optimizer state lists {len(ids)} parameters; this network has {len(params)} "
                              f"trainable of {len(every)}")
@@ -546,6 +655,7 @@ class TrainStep:
         ops.bump_weight_epoch()
         if self.pg is not None:
             self._sync_replicas(momentum=True)
+        self._sync_cache_modes(refresh_frozen=True)     # frozen layers' operands are not refreshed by the step itself
 
     def close(self):
         """Destroy the captured graphs (the step falls back to eager mode).  REQUIRED before
