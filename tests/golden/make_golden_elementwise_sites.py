@@ -5,10 +5,16 @@ tests/test_gpu_glue_ops.py.
 On a GPU, wrap those attributes of the loaded library with recorders and run what make_golden_conv_dispatch.py --record runs:
   * one eager forward + backward of ImageFillOrigin 512^2 b8, TextSegament 512^2 b8 and XceptionTextSegment 512^2 b16 (bf16),
   * the eager eval forward of XceptionTextSegment at 600^2 b1,
-  * one optimiser step of TrainStep (ImageFillOrigin).
+  * one optimiser step of TrainStep (ImageFillOrigin),
+  * the inference runs (make_golden_conv_dispatch.inference_runs): the eager forward of TextRemovalStep on every page of
+    TEXT_REMOVAL_RUNS (the rows of tools/bench_text_removal.py and tools/bench_text_removal_resize.py, the A4 page segmented at
+    page size, TextSegament + ImageFill at 1700 x 1200 with and without seg_resize=600) and of InferStep(ImageFillOriginV2) at
+    the 1700 x 1200 page's U-Net grid: bilinear resampling at unequal, non-integer ratios, pooling and GAP on odd grids, concat
+    and the unfused residual BatchNorm at page sizes.
 Each call is recorded by its non-pointer arguments, which of its optional pointers were null, whether the two sums of the
-statistics / backward reduction were one [2][c] buffer (one memset instead of two), and the part table of a concat:
-    python tests/golden/make_golden_elementwise_sites.py [out.json]
+statistics / backward reduction were one [2][c] buffer (one memset instead of two), and the part table of a concat.  Sites
+the fixture does not hold yet are appended to it, sorted; the entries already there stay as they are:
+    python tests/golden/make_golden_elementwise_sites.py [fixture.json]
 """
 import json
 import os
@@ -16,7 +22,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), HERE]
 FIXTURE = os.path.join(HERE, "elementwise_sites.json")
 
 # argument names per entry point (include/pconv_b200.h).  "?name": a pointer recorded as null / non-null; "-": a pointer or
@@ -87,6 +93,7 @@ def describe(fn, args):
 def record(path):
     import torch
 
+    from make_golden_conv_dispatch import inference_runs
     from oracle.detfill import det_fill_state_dict, det_tensor
     from text_segmentation_image_inpainting_b200 import _lib
     from text_segmentation_image_inpainting_b200.engine import SegInferStep, SegTrainStep, TrainStep
@@ -124,13 +131,17 @@ def record(path):
         with torch.no_grad():
             SegInferStep(net)._forward(det_tensor("conv_dispatch.x", (1, 3, 600, 600)).to(dev))
         torch.cuda.synchronize()
+        for run in inference_runs(dev):
+            print(run)
     finally:
         for fn, f in originals.items():
             setattr(lib, fn, f)
-    uniq = {json.dumps(s, sort_keys=True) for s in rec}
+    with open(path) as f:
+        known = [json.dumps(s, sort_keys=True) for s in json.load(f)]
+    new = sorted({json.dumps(s, sort_keys=True) for s in rec} - set(known))
     with open(path, "w") as f:
-        f.write("[\n" + ",\n".join(sorted(uniq)) + "\n]\n")
-    print(f"{len(rec)} calls, {len(uniq)} distinct sites -> {path}")
+        f.write("[\n" + ",\n".join(known + new) + "\n]\n")
+    print(f"{len(rec)} calls, {len(new)} new sites appended, {len(known) + len(new)} in all -> {path}")
 
 
 if __name__ == "__main__":

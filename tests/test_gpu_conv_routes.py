@@ -6,7 +6,11 @@ data gradient as four parity classes, the sub-pixel data gradient of a 2x-upsamp
 shape-general kernels (conv_generic.cu).  Three sets of cases:
 
   * one per dense descriptor of tests/golden/conv_dispatch.json (the layers the workloads run), batch capped at 2 -- or the
-    smallest batch above that whose routes (pcb_debug_conv_routes) equal those of the uncapped descriptor;
+    smallest batch above that whose routes (pcb_debug_conv_routes) equal those of the uncapped descriptor.  A descriptor
+    only inference reaches ("forward_only": TextRemovalStep and InferStep at page sizes, up to the 3584 x 2560 U-Net grid) is
+    checked in the forward alone: the forward route of the trace, the forward and its mask pass, the two-call forward, the
+    weight refresh, the fused BatchNorm sums and the eval epilogue; its fp64 references and comparisons run in bands of
+    output rows (input halos included) of at most BAND_BYTES, and its peak device memory must stay below MEMORY_BUDGET;
   * hand cases for what production reaches rarely or never: a stride-1 gather layer, ragged M, two parts (one 2x-upsampled) on
     a non-power-of-two grid, dilation; row-packed layers with cin 1 / 3 / 8 and kw 3 / 5 / 7; stems with holes, no_guard, cout
     32 / 40 and a grid that is not a whole number of tiles; RGB tails with 1 / 3 / 4 image channels, 32 / 64 upsampled channels
@@ -85,6 +89,8 @@ SLOPE = 0.2
 ACTS = (_lib.ACT_NONE, _lib.ACT_RELU, _lib.ACT_LEAKY, _lib.ACT_RELU6)
 DTYPES = {"bf16": (torch.bfloat16, _lib.PCB_BF16), "f32": (torch.float32, _lib.PCB_F32)}
 TC_ROUTES = {"stem", "k2r", "smallco", "tma", "tma_s2", "gather"}
+BAND_BYTES = 2 ** 29         # fp64 working set of one band of output rows (forward-only cases)
+MEMORY_BUDGET = 12 * 2 ** 30  # peak device memory of a forward-only case: page-size cases run on shared GPUs
 
 
 def accumulation_bound(nz, mag, rounds_bf16_intermediate):
@@ -157,13 +163,15 @@ def _fixture_cases():
         n = min(d["n"], 2)
         while _routes(lib, _conv_struct(sp, n)) != full:
             n += 1
-        sp["n"], sp["route"] = n, full
+        sp["n"], sp["route"], sp["forward_only"] = n, full, bool(case.get("forward_only"))
         pstr = "_".join(f"c{p['c']}" + (f"cs{p['xcs']}" if p["xcs"] != p["c"] else "") + ("u" if p["up"] else "")
                         + ("m" + str(p["mup"]) if p["mask"] else "") for p in parts)
         name = (f"fx_{dt}_n{n}_{d['h']}x{d['w']}_{pstr}_o{d['cout']}_k{d['kh']}x{d['kw']}_s{d['stride']}_p{d['pad_h']}x{d['pad_w']}"
                 f"_d{d['dil']}" + (f"_g{d['groups']}" if d["groups"] > 1 else "") + ("_plain" if d["plain"] else "")
                 + ("_same" if d["same_holes"] else "") + ("_noguard" if d["no_guard"] else "")
                 + ("_forcegen" if d["force_generic"] else ""))
+        if sp["forward_only"] and name in out:   # an inference descriptor that caps to a case tested in every direction
+            continue
         out[name] = sp
     return out
 
@@ -307,6 +315,43 @@ def _fl32_sum(t, b):
     return torch.where(tie, toward_e, f)
 
 
+def _int_forward_want(S, s, b, route0, no_guard, dt):
+    """the integer regime's stored forward (module docstring) from the exact sums S, the box sums s and the bias b: (want, alt),
+    alt the other rounding a small-Cout / kernel-to-row route may store (or None)"""
+    empty = s == 0
+    safe = torch.where(empty, torch.ones_like(s), s)
+    inv = (1.0 / safe).float().double()
+    if route0 == "generic":
+        want = ((S / safe).float().double() + b).float()
+        alt = None
+    else:
+        want = _fl32_sum(S * inv, b.expand_as(S))
+        alt = ((S * inv).float().double() + b).float() if route0 in ("smallco", "k2r") else None
+    hole = torch.full_like(want, float("nan") if no_guard else 0.0)
+    want = torch.where(empty, hole, want).to(dt)
+    alt = torch.where(empty, hole, alt).to(dt) if alt is not None else None
+    return want, alt
+
+
+def _gauss_forward_ref(acc, mag, nz, s, b, k2r):
+    """the Gaussian regime's forward reference and its bound (module docstring) from the exact sum acc, the sum of |products|
+    mag, the nonzero-term counts nz and the box sums s: 0 and 0 where s == 0"""
+    empty = s == 0
+    safe = torch.where(empty, torch.ones_like(s), s)
+    e_acc = accumulation_bound(nz, mag, k2r)
+    v_ref = torch.where(empty, torch.zeros_like(acc), acc / safe + b)
+    e_ref = torch.where(empty, torch.zeros_like(acc), e_acc / safe + 2.0 ** -22 * (acc.abs() / safe + v_ref.abs()))
+    return v_ref, e_ref
+
+
+def _check_y_values(name, tag, no_guard, got, v, e, store, live, nan_at_empty=True):
+    """got (fp64 NCHW of a stored forward) within e + the store's rounding of v; under no_guard NaN where the box is empty"""
+    if no_guard:                       # (an activation of NaN is whatever fmaxf / fminf make of it)
+        assert not nan_at_empty or bool(got[~live.expand_as(got)].isnan().all()), f"{name}: {tag}: NaN expected where the box is empty"
+        got = torch.where(live, got, v)
+    assert_within(f"{name}: {tag}", got, v, e + store * (v.abs() + e))
+
+
 def _kernel_routes(records):
     """(forward, data gradient, weight gradient) route names from the kernel records of a trace holding one forward, one data
     gradient and two weight gradients: the route-specific kernels first (a stem or a tail also runs its sub-problem on the
@@ -351,13 +396,16 @@ class _Problem:
                 self.masks.append(None)
                 mfull.append(torch.ones(n, h, w, dtype=torch.float64, device=dev))
         self.mfull = mfull                                                          # per part, [n, h, w]
-        self.M = torch.cat([m[:, None].expand(n, p["c"], h, w) for m, p in zip(mfull, sp["parts"])], 1)   # [n, cin, h, w]
         self.conv = _conv_struct(sp, masks=[m.data_ptr() if m is not None else 0 for m in self.masks])
         self.ho, self.wo = self.conv.ho, self.conv.wo
         self.geo = dict(stride=sp["s"], padding=(sp["ph"], sp["pw"]), dilation=sp["dil"])
         g, cin, cout = sp["groups"], sp["cin"], sp["cout"]
         self.cig, self.cog = cin // g, cout // g
         self.mg = g if (g > 1 and not sp["same_holes"]) else 1
+        if sp.get("forward_only"):             # fp64 operands band by band (band())
+            assert g == 1 and self.mg == 1
+            return
+        self.M = torch.cat([m[:, None].expand(n, p["c"], h, w) for m, p in zip(mfull, sp["parts"])], 1)   # [n, cin, h, w]
         kh, kw = sp["kh"], sp["kw"]
         with torch.backends.cudnn.flags(enabled=False):
             ones = torch.ones(g, self.cig, kh, kw, dtype=torch.float64, device=dev)
@@ -387,11 +435,53 @@ class _Problem:
             v = torch.where(mx[..., None] == 0, torch.full_like(v, HOLE_VALUE), v)
             buf = self.operand(v, p["xcs"])
             self.xbufs.append(buf)
-            xv = nchw(buf, p["c"])
-            xm.append((_up2(xv) if p["up"] else xv) * m[:, None])
+            if not sp.get("forward_only"):
+                xv = nchw(buf, p["c"])
+                xm.append((_up2(xv) if p["up"] else xv) * m[:, None])
         for i, b in enumerate(self.xbufs):
             self.conv.parts[i].x = b.data_ptr()
-        self.XM = torch.cat(xm, 1)
+        self.XM = torch.cat(xm, 1) if xm else None
+
+    def bands(self):
+        """output row ranges whose fp64 working set stays within BAND_BYTES: the reference's im2col columns (cin kh kw values
+        per output pixel), or the eight [n, cout, rows, wo] slabs the Gaussian checks hold at once"""
+        sp = self.sp
+        per_row = 8 * sp["n"] * self.wo * max(sp["cin"] * sp["kh"] * sp["kw"], 8 * sp["cout"])
+        rows = max(1, min(self.ho, BAND_BYTES // per_row))
+        return [(r, min(r + rows, self.ho)) for r in range(0, self.ho, rows)]
+
+    def band(self, r0, r1):
+        """fp64 operands of output rows [r0, r1): x * m over the input rows they read (their halo, zero rows past the image:
+        the convolution then pads only in w), the valid-term counts nz [n, 1, rows, wo] and the box sums s (1 for a plain
+        convolution), for groups == 1"""
+        sp = self.sp
+        a = r0 * sp["s"] - sp["ph"]
+        b = (r1 - 1) * sp["s"] - sp["ph"] + sp["dil"] * (sp["kh"] - 1) + 1
+        lo, hi = max(a, 0), min(b, sp["h"])
+        pad = (0, 0, lo - a, b - hi)
+        xm, boxes = [], []
+        ones = torch.ones(1, 1, sp["kh"], sp["kw"], dtype=torch.float64, device=self.dev)
+        for p, buf, m in zip(sp["parts"], self.xbufs, self.mfull):
+            if p["up"]:
+                xv = _up2(nchw(buf[:, lo // 2:(hi - 1) // 2 + 1], p["c"]))[:, :, lo % 2:lo % 2 + hi - lo]
+            else:
+                xv = nchw(buf[:, lo:hi], p["c"])
+            mm = m[:, None, lo:hi]
+            xm.append(xv * mm)
+            with torch.backends.cudnn.flags(enabled=False):
+                boxes.append(F.conv2d(F.pad(mm, pad), ones, stride=sp["s"], padding=(0, sp["pw"]), dilation=sp["dil"]).round())
+        nz = sum(bx * p["c"] for bx, p in zip(boxes, sp["parts"]))
+        if sp["plain"]:
+            s = torch.ones_like(nz)
+        else:
+            s = boxes[0] * sp["cin"] if sp["same_holes"] else nz
+        return F.pad(torch.cat(xm, 1), pad), nz, s
+
+    def conv_band(self, a, b):
+        """the reference convolution of a band's operands (band()): padding in w only"""
+        sp = self.sp
+        with torch.backends.cudnn.flags(enabled=False):
+            return F.conv2d(a, b, stride=sp["s"], padding=(0, sp["pw"]), dilation=sp["dil"])
 
     def operand(self, vals, cs):
         """vals [..., c] in the storage type, zeros in channels [c, rup(c, 8)), SENTINEL past that"""
@@ -462,6 +552,7 @@ def test_conv_route_vs_fp64(name):
     dgen = torch.Generator(device=dev).manual_seed(sum(map(ord, name)))
     n, cin, cout, kh, kw = sp["n"], sp["cin"], sp["cout"], sp["kh"], sp["kw"]
     P = _Problem(sp, dev, gen)
+    torch.cuda.reset_peak_memory_stats(dev)          # (the peak still counts what is allocated now)
     cref = ctypes.byref(P.conv)
     dt, ho, wo, ycs, dcs = P.dtype, P.ho, P.wo, sp["ycs"], sp["dcs"]
     route = _routes(lib, P.conv)
@@ -516,6 +607,10 @@ def test_conv_route_vs_fp64(name):
             pad = buf[..., p["c"]:c8]
             assert bool(((pad == SENTINEL) | (pad == 0)).all()), f"{name}: {tag} wrote garbage into the channel padding of part {i}"
 
+    if sp.get("forward_only"):
+        _forward_only_checks(name, sp, P, lib, stream, prepare, ints, dgen, ws, route, fuses)
+        return
+
     # ================= integer regime: bit-exact
     ix, iw = sp["ix"], sp["iw"]
     P.set_x([ints(ix, n, sp["h"] >> p["up"], sp["w"] >> p["up"], p["c"]) for p in sp["parts"]])
@@ -555,7 +650,8 @@ def test_conv_route_vs_fp64(name):
         for (k, args), launches in sp.get("tiles", {}).items():
             assert records[(k, args)] == launches, (f"{name}: {k}<{', '.join(args)}> launched {records[(k, args)]} times, the case is "
                                                     f"named for {launches}; kernels: {dict(records)}")
-    traced(name, run, check, state)
+    records = traced(name, run, check, state)
+    print(f"{name}: kernels {sorted(records or {})}")
 
     # mask pass: the fp64 box sums; a plain convolution leaves msum / newmask alone
     s_ref = P.box.permute(1, 0, 2, 3).reshape(mg, N)
@@ -582,18 +678,7 @@ def test_conv_route_vs_fp64(name):
     S = P.conv_ref(P.XM, P.W).round()
     s, b = P.s, bias.double()[None, :, None, None]
     empty = s == 0
-    safe = torch.where(empty, torch.ones_like(s), s)
-    inv = (1.0 / safe).float().double()
-    fused = _fl32_sum(S * inv, b.expand_as(S))
-    if route[0] == "generic":
-        want = ((S / safe).float().double() + b).float()
-        alt = None
-    else:
-        want = fused
-        alt = ((S * inv).float().double() + b).float() if route[0] in ("smallco", "k2r") else None
-    hole = torch.full_like(want, float("nan") if sp["no_guard"] else 0.0)
-    want = torch.where(empty, hole, want).to(dt)
-    alt = torch.where(empty, hole, alt).to(dt) if alt is not None else None
+    want, alt = _int_forward_want(S, s, b, route[0], sp["no_guard"], dt)
     assert_bitwise(f"{name}: forward", nchw(y, cout), want, alt, nan_equal=True)
     assert P.y_padding_ok(y), f"{name}: forward must write zeros into channels [cout, rup(cout, 8)) and nothing past them"
 
@@ -655,22 +740,13 @@ def test_conv_route_vs_fp64(name):
     wf, wd = prepare(P.wm)
     bias = torch.randn(cout, generator=dgen, device=dev) * 0.1
     b = bias.double()[None, :, None, None]
-    acc = P.conv_ref(P.XM, P.W)
-    mag = P.conv_ref(P.XM.abs(), P.W.abs())
-    e_acc = accumulation_bound(P.nz_fwd, mag, route[0] == "k2r")
-    v_ref = torch.where(empty, torch.zeros_like(acc), acc / safe + b)
-    e_ref = torch.where(empty, torch.zeros_like(acc), e_acc / safe + 2.0 ** -22 * (acc.abs() / safe + v_ref.abs()))
-    del acc, mag, e_acc
+    v_ref, e_ref = _gauss_forward_ref(P.conv_ref(P.XM, P.W), P.conv_ref(P.XM.abs(), P.W.abs()), P.nz_fwd, P.s, b, route[0] == "k2r")
     store = 2.0 ** -8 if dt == torch.bfloat16 else 0.0
     live = ~empty if sp["no_guard"] else torch.ones_like(empty)
 
     def check_y(tag, y, v, e, nan_at_empty=True):
         assert P.y_padding_ok(y), f"{name}: {tag} must write zeros into channels [cout, rup(cout, 8)) and nothing past them"
-        got = nchw(y, cout)
-        if sp["no_guard"]:                       # (an activation of NaN is whatever fmaxf / fminf make of it)
-            assert not nan_at_empty or bool(got[~live].isnan().all()), f"{name}: {tag}: NaN expected where the box is empty"
-            got = torch.where(live, got, v)
-        assert_within(f"{name}: {tag}", got, v, e + store * (v.abs() + e))
+        _check_y_values(name, tag, sp["no_guard"], nchw(y, cout), v, e, store, live, nan_at_empty)
 
     y = P.new_y()
     _lib.check(lib.pcb_pconv_forward(cref, wf.data_ptr(), bias.data_ptr(), y.data_ptr(), ycs, msum.data_ptr(), newmask.data_ptr(),
@@ -733,3 +809,140 @@ def test_conv_route_vs_fp64(name):
     wmag = P.wgrad_ref(P.XM.abs(), G.abs())
     werr = accumulation_bound(P.nz_wg, wmag, route[2] == "k2r")
     assert_within(f"{name}: Gaussian weight gradient", dw.double(), wref.permute(0, 2, 3, 1), werr.permute(0, 2, 3, 1))
+
+
+def _forward_only_checks(name, sp, P, lib, stream, prepare, ints, dgen, ws, route, fuses):
+    """the checks of a descriptor only inference reaches: the forward route in the trace; in the integer regime the one-call
+    forward and its mask pass, the two-call forward (mask pass, premasked forward) and the weight refresh; in the Gaussian
+    regime the forward, the fused BatchNorm sums and the eval epilogue at every activation.  Every fp64 reference and
+    comparison runs band by band (P.bands), and nothing page-sized leaves the device."""
+    dev, dt = P.dev, P.dtype
+    n, cout, kh, kw = sp["n"], sp["cout"], sp["kh"], sp["kw"]
+    ho, wo, ycs, N = P.ho, P.wo, sp["ycs"], sp["n"] * P.ho * P.wo
+    cref = ctypes.byref(P.conv)
+    bands = P.bands()
+    ix, iw = sp["ix"], sp["iw"]
+    P.set_x([ints(ix, n, sp["h"] >> p["up"], sp["w"] >> p["up"], p["c"]) for p in sp["parts"]])
+    P.master(ints(iw, cout, kh, kw, P.cig))
+    bias = torch.randint(-16, 17, (cout,), generator=dgen, device=dev).to(torch.float32) / 8
+    b = bias.double()[None, :, None, None]
+    if route[0] == "k2r":
+        cu = max(p["c"] for p in sp["parts"] if p["up"])
+        assert cu * ix * iw <= 256, f"{name}: the tail's bf16 Z rows would round"
+    wf, wd = prepare(P.wm)
+    y = P.new_y()
+    msum = torch.full((1, N), float("nan"), device=dev)
+    newmask = torch.full((1, N), 77, dtype=torch.uint8, device=dev)
+
+    def run():
+        _lib.check(lib.pcb_pconv_forward(cref, wf.data_ptr(), bias.data_ptr(), y.data_ptr(), ycs, msum.data_ptr(), newmask.data_ptr(),
+                                         ws.data_ptr(), stream))
+
+    def check(records):
+        ran, cnt = _kernel_routes(records)
+        assert ran[0] == route[0], f"{name}: the forward ran {ran[0]}, the plan says {route[0]}; kernels: {dict(cnt)}"
+    records = traced(name, run, check, [(y, y.clone()), (msum, float("nan")), (newmask, 77)])
+    print(f"{name}: kernels {sorted(records or {})}")
+
+    msum2 = torch.full((1, N), float("nan"), device=dev)
+    newmask2 = torch.full((1, N), 77, dtype=torch.uint8, device=dev)
+    ws2, y2 = _ws(lib, cref, dev), P.new_y()
+    _lib.check(lib.pcb_pconv_mask_pass(cref, msum2.data_ptr(), newmask2.data_ptr(), ws2.data_ptr(), stream))
+    _lib.check(lib.pcb_pconv_forward_premasked(cref, wf.data_ptr(), bias.data_ptr(), y2.data_ptr(), ycs, msum2.data_ptr(),
+                                               newmask2.data_ptr(), ws2.data_ptr(), stream))
+    torch.cuda.synchronize()
+    assert_bitwise(f"{name}: mask pass + premasked forward vs one-call forward", y2, y, nan_equal=True)
+    del y2, ws2
+    if sp["plain"]:
+        assert bool(msum.isnan().all()) and bool((newmask == 77).all()), f"{name}: a plain convolution must not touch msum / newmask"
+    assert P.y_padding_ok(y), f"{name}: forward must write zeros into channels [cout, rup(cout, 8)) and nothing past them"
+    for r0, r1 in bands:
+        XM, nz, s = P.band(r0, r1)
+        assert float(nz.max()) * ix * iw < 2 ** 24, f"{name}: partial sums could round: not an exact case"
+        if not sp["plain"]:
+            s_ref = s[:, 0].reshape(1, -1)
+            nm_ref = torch.ones_like(s_ref, dtype=torch.uint8) if sp["no_guard"] else (s_ref != 0).to(torch.uint8)
+            for tag, ms, nm in (("", msum, newmask), ("mask pass ", msum2, newmask2)):
+                assert_bitwise(f"{name}: {tag}msum, rows {r0}:{r1}", ms.view(n, ho, wo)[:, r0:r1].reshape(1, -1).double(), s_ref)
+                assert_bitwise(f"{name}: {tag}newmask, rows {r0}:{r1}", nm.view(n, ho, wo)[:, r0:r1].reshape(1, -1), nm_ref)
+        want, alt = _int_forward_want(P.conv_band(XM, P.W).round(), s, b, route[0], sp["no_guard"], dt)
+        assert_bitwise(f"{name}: forward, rows {r0}:{r1}", nchw(y[:, r0:r1], cout), want, alt, nan_equal=True)
+        del XM, want, alt
+
+    wm2 = ints(iw, cout, kh, kw, P.cig)
+    _lib.check(lib.pcb_conv_weight_refresh(cref, wm2.data_ptr(), wf.data_ptr(), wd.data_ptr() if wd is not None else None, stream))
+    wf2, wd2 = prepare(wm2)
+    torch.cuda.synchronize()
+    ib = torch.int16 if wf.dtype == torch.bfloat16 else torch.int32
+    assert torch.equal(wf.view(ib), wf2.view(ib)), f"{name}: refreshed forward operands differ from freshly prepared ones"
+    if wd is not None:
+        assert torch.equal(wd.view(ib), wd2.view(ib)), f"{name}: refreshed data-gradient operands differ from freshly prepared ones"
+    del wf2, wd2
+
+    # Gaussian regime: every output first (forward, BatchNorm sums, eval epilogue per activation), then the bands
+    P.set_x([torch.randn(n, sp["h"] >> p["up"], sp["w"] >> p["up"], p["c"], generator=dgen, device=dev) for p in sp["parts"]])
+    P.master(torch.randn(cout, kh, kw, P.cig, generator=dgen, device=dev).to(dt).float() / 2)
+    wf, wd = prepare(P.wm)
+    bias = torch.randn(cout, generator=dgen, device=dev) * 0.1
+    b = bias.double()[None, :, None, None]
+    scale = torch.rand(cout, generator=dgen, device=dev) + 0.5
+    shift = torch.randn(cout, generator=dgen, device=dev) * 0.1
+    outs = {"forward": P.new_y()}
+    _lib.check(lib.pcb_pconv_forward(cref, wf.data_ptr(), bias.data_ptr(), outs["forward"].data_ptr(), ycs, msum.data_ptr(),
+                                     newmask.data_ptr(), ws.data_ptr(), stream))
+    sums = torch.zeros(2, cout, dtype=torch.float64, device=dev)
+    if fuses:
+        outs["forward with BatchNorm sums"] = P.new_y()
+        _lib.check(lib.pcb_pconv_forward_bn(cref, wf.data_ptr(), bias.data_ptr(), outs["forward with BatchNorm sums"].data_ptr(), ycs,
+                                            msum.data_ptr(), newmask.data_ptr(), ws.data_ptr(), 0, sums.data_ptr(), stream))
+        for act in ACTS:
+            outs[act] = P.new_y()
+            _lib.check(lib.pcb_pconv_forward_affine_act(cref, wf.data_ptr(), bias.data_ptr(), outs[act].data_ptr(), ycs,
+                                                        msum.data_ptr(), newmask.data_ptr(), ws.data_ptr(), 0, scale.data_ptr(),
+                                                        shift.data_ptr(), act, SLOPE, stream))
+    else:
+        yr = P.new_y()
+        rc = lib.pcb_pconv_forward_bn(cref, wf.data_ptr(), bias.data_ptr(), yr.data_ptr(), ycs, msum.data_ptr(), newmask.data_ptr(),
+                                      ws.data_ptr(), 0, sums.data_ptr(), stream)
+        assert rc != 0 and b"does not fuse" in lib.pcb_last_error(), f"{name}: fused BatchNorm sums must be refused"
+        rc = lib.pcb_pconv_forward_affine_act(cref, wf.data_ptr(), bias.data_ptr(), yr.data_ptr(), ycs, msum.data_ptr(),
+                                              newmask.data_ptr(), ws.data_ptr(), 0, scale.data_ptr(), shift.data_ptr(), _lib.ACT_RELU,
+                                              SLOPE, stream)
+        assert rc != 0 and b"does not apply" in lib.pcb_last_error(), f"{name}: fused affine + activation must be refused"
+        torch.cuda.synchronize()
+        assert bool(yr[..., :_rup8(cout)].isnan().all()) and bool((sums == 0).all()), f"{name}: a refused call must not run"
+        del yr
+    torch.cuda.synchronize()
+    for tag, yo in outs.items():
+        assert P.y_padding_ok(yo), f"{name}: {tag} must write zeros into channels [cout, rup(cout, 8)) and nothing past them"
+    store = 2.0 ** -8 if dt == torch.bfloat16 else 0.0
+    sc, sh = scale.double()[None, :, None, None], shift.double()[None, :, None, None]
+    tot = torch.zeros(4, cout, dtype=torch.float64, device=dev)     # sum y, sum y^2, sum |y|, sum y^2 of the stored values
+    for r0, r1 in bands:
+        XM, nz, s = P.band(r0, r1)
+        v_ref, e_ref = _gauss_forward_ref(P.conv_band(XM, P.W), P.conv_band(XM.abs(), P.W.abs()), nz, s, b, route[0] == "k2r")
+        del XM
+        live = s != 0 if sp["no_guard"] else torch.ones_like(s, dtype=torch.bool)
+        rows = f"rows {r0}:{r1}"
+        for tag in ("forward", "forward with BatchNorm sums"):
+            if tag in outs:
+                _check_y_values(name, f"{tag}, {rows}", sp["no_guard"], nchw(outs[tag][:, r0:r1], cout), v_ref, e_ref, store, live)
+        if not fuses:
+            continue
+        if not sp["no_guard"]:
+            yv = outs["forward with BatchNorm sums"][:, r0:r1, :, :cout].double().reshape(-1, cout)
+            tot += torch.stack([yv.sum(0), (yv * yv).sum(0), yv.abs().sum(0), (yv * yv).sum(0)])
+            del yv
+        z = v_ref * sc + sh
+        ez = sc * e_ref + 2.0 ** -23 * (z.abs() + sh.abs())
+        for act in ACTS:
+            va = act_ref(z, act, SLOPE)
+            _check_y_values(name, f"eval epilogue, activation {act}, {rows}", sp["no_guard"], nchw(outs[act][:, r0:r1], cout), va,
+                            ez + 2.0 ** -23 * va.abs(), store, live, act == _lib.ACT_NONE)
+    if fuses and not sp["no_guard"]:
+        for row, what in ((0, "sums"), (1, "squares")):
+            tol = N * 2.0 ** -23 * tot[2 + row]
+            assert bool(((sums[row] - tot[row]).abs() <= tol).all()), f"{name}: BatchNorm {what}"
+    peak = torch.cuda.max_memory_allocated(dev)
+    print(f"{name}: peak device memory {peak / 2 ** 30:.2f} GiB over {len(bands)} band(s)")
+    assert peak < MEMORY_BUDGET, f"{name}: peak device memory {peak / 2 ** 30:.2f} GiB"

@@ -3,7 +3,9 @@ computed on the device (F.conv2d / torch.nn.grad.conv2d_input / conv2d_weight wi
 reference is a direct sum).  Two sets of cases:
 
   * every depthwise descriptor of tests/golden/conv_dispatch.json that the depthwise family accepts (the layers the workloads
-    run: dw4 at dilations up to 29, dw3 at stride 2, the small GPU test cases), batch capped at 2;
+    run: dw4 at dilations up to 29, dw3 at stride 2, the small GPU test cases), batch capped at 2.  A descriptor only
+    inference reaches ("forward_only": the segmentation networks at page sizes) is checked in the forward alone, its fp64
+    references in bands of output rows of at most BAND_BYTES, its peak device memory below MEMORY_BUDGET;
   * hand cases for the paths production does not reach: holes on dw3 (one msum plane or c of them, a half-resolution hole
     plane, large values under the holes), strided channel views, awkward channel counts (8, 40, 296, 2048), dw4 segment,
     x-tile and dilation-phase edges in both storage types, a "valid" 3x3 on dw3, and the depthwise shapes the family leaves to
@@ -53,6 +55,8 @@ INT_RANGE = 4                # |x|, |w|, |dc| <= 4 in the integer regime
 SLOPE = 0.2
 ACTS = (_lib.ACT_NONE, _lib.ACT_RELU, _lib.ACT_LEAKY, _lib.ACT_RELU6)
 DTYPES = {"bf16": (torch.bfloat16, _lib.PCB_BF16), "f32": (torch.float32, _lib.PCB_F32)}
+BAND_BYTES = 2 ** 29         # one fp64 [n, c, rows, wo] slab of a band of output rows (forward-only cases)
+MEMORY_BUDGET = 12 * 2 ** 30  # peak device memory of a forward-only case: page-size cases run on shared GPUs
 
 # the kernels of each route, per direction (forward, data gradient, weight gradient)
 KERNELS = {"dw4": ("dw4_s1_kernel", "dw4_s1_kernel", "dw4_s1_wgrad_kernel"),
@@ -61,7 +65,7 @@ KERNELS = {"dw4": ("dw4_s1_kernel", "dw4_s1_kernel", "dw4_s1_wgrad_kernel"),
 
 
 def _case(n, h, w, c, k=3, s=1, pad=None, dil=1, dtype="bf16", holes=False, mask_up=0, same_holes=False, plain=None,
-          cs=None, route=None):
+          cs=None, route=None, forward_only=False):
     """cs: channel strides (x, y, dc, dx), default c.  route: the kernels of (forward, data gradient, weight gradient);
     default: what the depthwise dispatch documents (dw4 for plain 3x3 stride 1 with padding == dilation, dw3 for other 3x3 at
     a power-of-two stride, the generic kernels otherwise)."""
@@ -76,14 +80,14 @@ def _case(n, h, w, c, k=3, s=1, pad=None, dil=1, dtype="bf16", holes=False, mask
         else:
             route = ("dw3",) * 3
     return dict(n=n, h=h, w=w, c=c, kh=kh, kw=kw, s=s, ph=ph, pw=pw, dil=dil, dtype=dtype, holes=holes, mask_up=mask_up,
-                same_holes=same_holes, plain=plain, cs=tuple(cs) if cs else (c,) * 4, route=route)
+                same_holes=same_holes, plain=plain, cs=tuple(cs) if cs else (c,) * 4, route=route, forward_only=forward_only)
 
 
 def _fixture_cases():
     """one case per distinct depthwise descriptor of the dispatch fixture (the depthwise family's eligibility test, n <= 2)"""
     out = {}
-    for d in (case["conv"] for case in conv_dispatch_cases()):
-        p = d["parts"]
+    for case in conv_dispatch_cases():
+        d, p = case["conv"], case["conv"]["parts"]
         if not (d["groups"] == d["cin"] == d["cout"] > 1 and len(p) == 1):
             continue
         p = p[0]
@@ -93,11 +97,13 @@ def _fixture_cases():
         n = min(d["n"], 2)
         spec = _case(n, d["h"], d["w"], d["cin"], (d["kh"], d["kw"]), d["stride"], (d["pad_h"], d["pad_w"]), d["dil"], dt,
                      holes=bool(p["mask"]), mask_up=p["mask_up"], same_holes=bool(d["same_holes"]), plain=bool(d["plain"]),
-                     cs=(p["x_cstride"],) + (d["cin"],) * 3)
+                     cs=(p["x_cstride"],) + (d["cin"],) * 3, forward_only=bool(case.get("forward_only")))
         name = (f"fx_{dt}_n{n}_{d['h']}x{d['w']}_c{d['cin']}_k{d['kh']}x{d['kw']}_s{d['stride']}_p{d['pad_h']}x{d['pad_w']}"
                 f"_d{d['dil']}" + ("_plain" if d["plain"] else "_renorm") + ("_holes" if p["mask"] else "")
                 + ("_up" if p["mask_up"] else "") + ("_same" if d["same_holes"] else "")
                 + (f"_xcs{p['x_cstride']}" if p["x_cstride"] != d["cin"] else ""))
+        if spec["forward_only"] and name in out:   # an inference descriptor that caps to a case tested in every direction
+            continue
         out[name] = spec
     return out
 
@@ -166,6 +172,7 @@ class _Problem:
             self.mask = None
             m = torch.ones(n, h, w, dtype=torch.float64, device=dev)
         self.M = m[:, None]                                           # [n, 1, h, w]
+        self.ones = torch.ones(1, 1, sp["kh"], sp["kw"], dtype=torch.float64, device=dev)
         cv = _lib.Conv()
         cv.n, cv.h, cv.w, cv.cin, cv.cout, cv.kh, cv.kw = n, h, w, c, c, sp["kh"], sp["kw"]
         cv.stride, cv.pad_h, cv.pad_w, cv.dil, cv.groups, cv.ho, cv.wo = sp["s"], sp["ph"], sp["pw"], sp["dil"], c, self.ho, self.wo
@@ -185,7 +192,25 @@ class _Problem:
             x = torch.where(self.M[:, 0, :, :, None] == 0, torch.full_like(x, HOLE_VALUE), x)
         self.x = strided(x.shape, self.sp["cs"][0], x.to(self.dtype), self.dtype)
         self.conv.parts[0].x = self.x.data_ptr()
-        self.XM = nchw(self.x, self.sp["c"]) * self.M
+        self.XM = None if self.sp["forward_only"] else nchw(self.x, self.sp["c"]) * self.M
+
+    def bands(self):
+        """output row ranges of at most BAND_BYTES in the eight fp64 [n, c, rows, wo] slabs the Gaussian checks hold at once"""
+        rows = max(1, min(self.ho, BAND_BYTES // (8 * 8 * self.sp["n"] * self.wo * self.sp["c"])))
+        return [(r, min(r + rows, self.ho)) for r in range(0, self.ho, rows)]
+
+    def band(self, r0, r1):
+        """x * m over the input rows that output rows [r0, r1) read, zero rows past the image (conv_band pads only in w)"""
+        sp = self.sp
+        a = r0 * sp["s"] - sp["ph"]
+        b = (r1 - 1) * sp["s"] - sp["ph"] + sp["dil"] * (sp["kh"] - 1) + 1
+        lo, hi = max(a, 0), min(b, sp["h"])
+        return F.pad(nchw(self.x[:, lo:hi], sp["c"]) * self.M[:, :, lo:hi], (0, 0, lo - a, b - hi))
+
+    def conv_band(self, a, b):
+        sp = self.sp
+        with torch.backends.cudnn.flags(enabled=False):
+            return F.conv2d(a, b, groups=sp["c"], stride=sp["s"], padding=(0, sp["pw"]), dilation=sp["dil"])
 
     def prepare_weights(self, wm, stream, lib):
         fe, de = ctypes.c_size_t(), ctypes.c_size_t()
@@ -230,6 +255,7 @@ def test_dwconv_vs_fp64(name):
     dgen = torch.Generator(device=dev).manual_seed(sum(map(ord, name)))
     n, h, w, c = sp["n"], sp["h"], sp["w"], sp["c"]
     P = _Problem(sp, dev, gen)
+    torch.cuda.reset_peak_memory_stats(dev)          # (the peak still counts what is allocated now)
     cref = ctypes.byref(P.conv)
     ho, wo, N, dt = P.ho, P.wo, sp["n"] * P.ho * P.wo, P.dtype
     ycs, dcs, dxcs = sp["cs"][1:]
@@ -239,6 +265,10 @@ def test_dwconv_vs_fp64(name):
 
     def ints(*shape):
         return torch.randint(-INT_RANGE, INT_RANGE + 1, shape, generator=dgen, device=dev).to(torch.float32)
+
+    if sp["forward_only"]:
+        _forward_only_checks(name, sp, P, lib, stream, ints, dgen, fuses)
+        return
 
     # ================= integer regime: bit-exact
     P.set_x(ints(n, h, w, c))
@@ -272,7 +302,8 @@ def test_dwconv_vs_fp64(name):
     def check(records):
         ran = {k for k, _ in records if k.startswith(("dw", "generic"))}
         assert ran == want, f"{name}: ran {sorted(ran)}, the case covers {sorted(want)}"
-    traced(name, run, check, state)
+    records = traced(name, run, check, state)
+    print(f"{name}: kernels {sorted(records or {})}")
 
     # mask pass
     if sp["plain"]:
@@ -385,3 +416,128 @@ def test_dwconv_vs_fp64(name):
         wref = P.wgrad_ref(P.XM, G)
         wb = P.wgrad_ref((P.XM != 0).double(), (G != 0).double()) * 2.0 ** -22 * P.wgrad_ref(P.XM.abs(), G.abs())
         assert_within(f"{name}: fp32 weight gradient", dw.double(), wref, wb)
+
+
+def _forward_only_checks(name, sp, P, lib, stream, ints, dgen, fuses):
+    """the checks of a descriptor only inference reaches: the forward kernel in the trace, the mask pass and the forward in
+    the integer regime, the fused BatchNorm sums and the eval epilogue at every activation (or their refusal) in the Gaussian
+    regime, and the fp32 forward; every fp64 reference and comparison runs band by band (P.bands)"""
+    dev, dt = P.dev, P.dtype
+    n, c, ho, wo = sp["n"], sp["c"], P.ho, P.wo
+    N, ycs = n * ho * wo, sp["cs"][1]
+    cref = ctypes.byref(P.conv)
+    bands = P.bands()
+    P.set_x(ints(n, sp["h"], sp["w"], c))
+    P.prepare_weights(ints(c, P.taps), stream, lib)
+    bias = torch.randint(-16, 17, (c,), generator=dgen, device=dev).to(torch.float32) / 8
+    b = bias.double()[None, :, None, None]
+    y = P.new_y()
+    msum = torch.full((P.mg, N), float("nan"), device=dev)
+    newmask = torch.full((P.mg, N), 77, dtype=torch.uint8, device=dev)
+
+    def run():
+        _lib.check(lib.pcb_pconv_forward(cref, P.w_t.data_ptr(), bias.data_ptr(), y.data_ptr(), ycs, msum.data_ptr(),
+                                         newmask.data_ptr(), None, stream))
+
+    def check(records):
+        ran = {k for k, _ in records if k.startswith(("dw", "generic"))}
+        assert ran == {KERNELS[sp["route"][0]][0]}, f"{name}: ran {sorted(ran)}, the case covers {KERNELS[sp['route'][0]][0]}"
+    records = traced(name, run, check, [(y, y.clone()), (msum, float("nan")), (newmask, 77)])
+    print(f"{name}: kernels {sorted(records or {})}")
+
+    def y_tail_kept(y):
+        past = y[..., c:]
+        return bool(((past == SENTINEL) | ((past == 0) & (sp["route"][0] == "generic"))).all())
+
+    if sp["plain"]:
+        assert bool(msum.isnan().all()) and bool((newmask == 77).all()), f"{name}: a plain convolution must not touch msum / newmask"
+    else:
+        s_ref = P.msum[:, 0].reshape(1, N).expand(P.mg, N)
+        assert_bitwise(f"{name}: msum", msum.double(), s_ref)
+        assert_bitwise(f"{name}: newmask", newmask, (s_ref != 0).to(torch.uint8))
+    assert y_tail_kept(y), f"{name}: forward wrote past c"
+    for r0, r1 in bands:
+        S = P.conv_band(P.band(r0, r1), P.W).round()
+        if sp["plain"]:
+            v = (S + b).float()
+        else:
+            s = P.msum[:, :, r0:r1]
+            q = (S / torch.where(s == 0, torch.ones_like(s), s)).float().double()
+            v = torch.where(s == 0, torch.zeros_like(S), q + b).float()
+        assert_bitwise(f"{name}: forward, rows {r0}:{r1}", y[:, r0:r1, :, :c].permute(0, 3, 1, 2), v.to(dt))
+        del S, v
+
+    P.set_x(torch.randn(n, sp["h"], sp["w"], c, generator=dgen, device=dev))
+    P.prepare_weights(torch.randn(c, P.taps, generator=dgen, device=dev) / 3, stream, lib)
+    bias = torch.randn(c, generator=dgen, device=dev) * 0.1
+    b = bias.double()[None, :, None, None]
+    scale = torch.rand(c, generator=dgen, device=dev) + 0.5
+    shift = torch.randn(c, generator=dgen, device=dev) * 0.1
+    outs = {}
+    sums = torch.zeros(2, c, dtype=torch.float64, device=dev)
+    if dt == torch.float32:
+        outs["fp32 forward"] = P.new_y()
+        _lib.check(lib.pcb_pconv_forward(cref, P.w_t.data_ptr(), bias.data_ptr(), outs["fp32 forward"].data_ptr(), ycs, msum.data_ptr(),
+                                         newmask.data_ptr(), None, stream))
+    if fuses:
+        outs["forward with BatchNorm sums"] = P.new_y()
+        _lib.check(lib.pcb_pconv_forward_bn(cref, P.w_t.data_ptr(), bias.data_ptr(), outs["forward with BatchNorm sums"].data_ptr(), ycs,
+                                            msum.data_ptr(), newmask.data_ptr(), None, 0, sums.data_ptr(), stream))
+        for act in ACTS:
+            outs[act] = P.new_y()
+            _lib.check(lib.pcb_pconv_forward_affine_act(cref, P.w_t.data_ptr(), bias.data_ptr(), outs[act].data_ptr(), ycs,
+                                                        msum.data_ptr(), newmask.data_ptr(), None, 0, scale.data_ptr(), shift.data_ptr(),
+                                                        act, SLOPE, stream))
+    else:
+        yr = P.new_y()
+        rc = lib.pcb_pconv_forward_bn(cref, P.w_t.data_ptr(), bias.data_ptr(), yr.data_ptr(), ycs, msum.data_ptr(),
+                                      newmask.data_ptr(), None, 0, sums.data_ptr(), stream)
+        assert rc != 0 and b"does not fuse" in lib.pcb_last_error(), f"{name}: fused BatchNorm sums must be refused"
+        rc = lib.pcb_pconv_forward_affine_act(cref, P.w_t.data_ptr(), bias.data_ptr(), yr.data_ptr(), ycs, msum.data_ptr(),
+                                              newmask.data_ptr(), None, 0, scale.data_ptr(), shift.data_ptr(), _lib.ACT_RELU, SLOPE,
+                                              stream)
+        assert rc != 0 and b"does not apply" in lib.pcb_last_error(), f"{name}: fused affine + activation must be refused"
+        torch.cuda.synchronize()
+        assert bool(yr[..., :c].isnan().all()) and bool((sums == 0).all()), f"{name}: a refused call must not run"
+        del yr
+    torch.cuda.synchronize()
+    for tag, yo in outs.items():
+        assert y_tail_kept(yo), f"{name}: {tag} wrote past c"
+    store = 2.0 ** -8 if dt == torch.bfloat16 else 0.0
+    sc, sh = scale.double()[None, :, None, None], shift.double()[None, :, None, None]
+    tot = torch.zeros(3, c, dtype=torch.float64, device=dev)        # sum y, sum y^2, sum |y| of the stored values
+    for r0, r1 in bands:
+        XM = P.band(r0, r1)
+        acc = P.conv_band(XM, P.W)
+        e_acc = P.conv_band((XM != 0).double(), (P.W != 0).double()) * 2.0 ** -22 * P.conv_band(XM.abs(), P.W.abs())
+        del XM
+        s = P.msum[:, :, r0:r1] if not sp["plain"] else torch.ones_like(P.msum[:, :, r0:r1])
+        empty = (s == 0).expand_as(acc)
+        safe = torch.where(s == 0, torch.ones_like(s), s)
+        v_ref = torch.where(empty, torch.zeros_like(acc), acc / safe + b)
+        e_ref = torch.where(empty, torch.zeros_like(acc), e_acc / safe + 2.0 ** -22 * (acc.abs() / safe + v_ref.abs()))
+        del acc, e_acc, empty
+        rows = f"rows {r0}:{r1}"
+
+        def check_y(tag, v, e):
+            assert_within(f"{name}: {tag}, {rows}", nchw(outs[tag][:, r0:r1], c), v, e + store * (v.abs() + e))
+        for tag in ("fp32 forward", "forward with BatchNorm sums"):
+            if tag in outs:
+                check_y(tag, v_ref, e_ref)
+        if not fuses:
+            continue
+        yv = outs["forward with BatchNorm sums"][:, r0:r1, :, :c].double().reshape(-1, c)
+        tot += torch.stack([yv.sum(0), (yv * yv).sum(0), yv.abs().sum(0)])
+        del yv
+        z = v_ref * sc + sh
+        ez = sc * e_ref + 2.0 ** -23 * (z.abs() + sh.abs())
+        for act in ACTS:
+            va = act_ref(z, act, SLOPE)
+            check_y(act, va, ez + 2.0 ** -23 * va.abs())
+    if fuses:
+        for row, what in ((0, "sums"), (1, "squares")):
+            tol = N * 2.0 ** -23 * tot[2 if row == 0 else 1]
+            assert bool(((sums[row] - tot[row]).abs() <= tol).all()), f"{name}: BatchNorm {what}"
+    peak = torch.cuda.max_memory_allocated(dev)
+    print(f"{name}: peak device memory {peak / 2 ** 30:.2f} GiB over {len(bands)} band(s)")
+    assert peak < MEMORY_BUDGET, f"{name}: peak device memory {peak / 2 ** 30:.2f} GiB"
