@@ -80,7 +80,7 @@ BRANCHES = {
     "conv_plain_passthrough": "plain bias-free convolution backward: dc = gy, no renormalisation pass",
     "conv_renorm_backward": "pcb_pconv_renorm_backward (renormalisation and bias gradient)",
     "bias_grad_sink": "bias gradient written into a gradient sink",
-    "weight_grad_sink_side_stream": "weight gradient written into a sink from the side stream, joined at join_side_streams",
+    "weight_grad_sink_side_stream": "weight gradient written into a sink from the side stream, joined at the training scope's exit",
     "weight_grad_autograd": "weight gradient returned to autograd",
     "weight_used_twice": "a weight used twice in one pass: the second use falls back from the sink to autograd accumulation",
     "rowpacked_dgrad_generic": "row-packed layer whose input needs a gradient: generic data gradient with a per-backward weight cast",
@@ -175,8 +175,8 @@ class Recorder:
 
     def _feature(self, fn, args):
         if fn in self.WGRAD:
-            cur = torch.cuda.current_stream()
-            side = any(cur == st for st in ops.side_streams())
+            scope = ops.current_scope()
+            side = scope is not None and torch.cuda.current_stream() in scope.streams
             if fn == "pcb_pconv_backward_weight_acc" and side:
                 self.features.add("weight_grad_sink_side_stream")
             if fn == "pcb_pconv_backward_weight":
@@ -291,7 +291,8 @@ class Recorder:
             if hint is not None:
                 pend = hint.__dict__.get("_pending_stats")
                 u.facts["bn_sums"] = pend is not None and pend[0] == y.data_ptr()
-                if ops.fused_eval_epilogue_enabled() and not hint[0].training and not hint.__dict__.get("_pcb_residual_site"):
+                scope = ops.current_scope()
+                if scope is not None and not scope.training and not hint[0].training and not hint.__dict__.get("_pcb_residual_site"):
                     fused = hint.__dict__.get("_pcb_fused_out") == (y.data_ptr(), tuple(y.shape))
                     u.facts["epi_offered"], u.facts["epi_fused"] = True, fused
                     if fused:
@@ -301,7 +302,7 @@ class Recorder:
     @staticmethod
     def _coef(bn):
         """host copy of the (scale, shift) the eval epilogue applied (ops.bn_eval_coefficients' cache)"""
-        return None if bn is None else host(bn.__dict__["_pcb_eval_coef"]["buf"])
+        return None if bn is None else host(bn.__dict__["_pcb_bn_coef"]["buf"])
 
     def attach(self, net):
         self.names = {m: (n or type(net).__name__) for n, m in net.named_modules()}
@@ -319,7 +320,7 @@ class Recorder:
         self._unwrap()
 
     def finish(self, sinks=()):
-        """after backward (and join_side_streams): read each handoff and drop every live reference"""
+        """after backward (and the scope's exit): read each handoff and drop every live reference"""
         for u in self.units:
             h = u.live.get("handoff")
             if h is not None:

@@ -124,14 +124,10 @@ def _run_block(block, args):
     with torch.no_grad():
         yu, mu = block(args)
         conv_out, _ = block[0](args)
-        ops.EPILOGUE_SITES.update(fused=0, unfused=0)
-        ops.set_fused_eval_epilogue(True)
-        try:
+        with ops.StepScope(DEV, training=False) as scope:
             yf, mf = block(args)
-        finally:
-            ops.set_fused_eval_epilogue(False)
     torch.cuda.synchronize()
-    return yf, yu, conv_out, mf, mu, dict(ops.EPILOGUE_SITES)
+    return yf, yu, conv_out, mf, mu, {"fused": scope.fused_sites, "unfused": scope.unfused_sites}
 
 
 def _bn_coef(block):
@@ -242,13 +238,9 @@ def test_conv_block_fused_epilogue(case, act, dtype):
     with torch.no_grad():
         yu = seq(x)
         co = seq[0](x)
-        ops.EPILOGUE_SITES.update(fused=0, unfused=0)
-        ops.set_fused_eval_epilogue(True)
-        try:
+        with ops.StepScope(DEV, training=False) as scope:
             yf = seq(x)
-        finally:
-            ops.set_fused_eval_epilogue(False)
-    assert ops.EPILOGUE_SITES == {"fused": 1, "unfused": 0}
+    assert (scope.fused_sites, scope.unfused_sites) == (1, 0)
     assert "_pcb_fused_out" not in seq[1].__dict__
     scale, shift = ops.bn_eval_coefficients(seq[1][0])
     if dtype == torch.float32:
@@ -269,13 +261,9 @@ def test_residual_batchnorm_is_not_fused():
     x = det_tensor("infer.ir", (2, 32, 16, 24)).to(DEV).to(torch.bfloat16).contiguous(memory_format=CL)
     with torch.no_grad():
         yu = blk(x)
-        ops.EPILOGUE_SITES.update(fused=0, unfused=0)
-        ops.set_fused_eval_epilogue(True)
-        try:
+        with ops.StepScope(DEV, training=False) as scope:
             yf = blk(x)
-        finally:
-            ops.set_fused_eval_epilogue(False)
-    assert ops.EPILOGUE_SITES == {"fused": 2, "unfused": 1}
+    assert (scope.fused_sites, scope.unfused_sites) == (2, 1)
     assert float((yf.float() - yu.float()).abs().max()) <= 3e-2 * float(yu.float().abs().max())
 
 

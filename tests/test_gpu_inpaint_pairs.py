@@ -218,14 +218,12 @@ def _eager_eval(net, b, crit):
     from text_segmentation_image_inpainting_b200 import ops
     training = net.training
     net.eval()
-    ops.set_fused_eval_epilogue(True)
     try:
-        with torch.no_grad():
+        with ops.StepScope(b.device, training=False), torch.no_grad():
             xin, hm, clean = b.prepare()
             out = net((xin, hm))
             loss = crit(clean, hm, out, clean) if crit is not None else None
     finally:
-        ops.set_fused_eval_epilogue(False)
         net.train(training)
     torch.cuda.synchronize()
     return out.float(), loss, (crit.last_terms.clone() if crit is not None else None)

@@ -4,9 +4,9 @@ sinks, residuals folded into the BatchNorm pass, LazyCat decoder inputs and Hole
 networks' concatenations, bilinear resampling and residual sums, and the fused eval epilogue.
 
 Runs per network: (a) bf16 training forward + ops.l1_mean backward with autograd gradients; (b) the same with engine.FlatParams
-gradient sinks, parameter gradients read from the arena after ops.join_side_streams(); (c) an eval forward under
-ops.set_fused_eval_epilogue(True) with randomised BatchNorm running statistics, where a convolution and the BatchNorm +
-activation fused into its epilogue are one unit.  Plus fp32 training runs of ImageFillOrigin and TextSegament (generic kernels,
+gradient sinks, parameter gradients read from the arena after the training ops.StepScope exits; (c) an eval forward in an
+inference ops.StepScope with randomised BatchNorm running statistics, where a convolution and the BatchNorm + activation
+fused into its epilogue are one unit.  Plus fp32 training runs of ImageFillOrigin and TextSegament (generic kernels,
 handoffs that are never eligible).  Hand-built module cases reach the glue branches the networks do not reach at these shapes.
 Every case records the branches it reached (module_sites.Recorder.reached); test_branch_coverage runs whatever case has not
 run yet in the session and asserts that the union covers module_sites.BRANCHES."""
@@ -71,17 +71,12 @@ def _run(net, call, dev, dtype, label, sinks=None, train=True):
     rec = Recorder().attach(net)
     rec.with_sinks = sinks is not None
     try:
-        if train:
-            out = call()
-            ops.l1_mean(out).backward()
-            ops.join_side_streams()
-        else:
-            ops.set_fused_eval_epilogue(True)
-            try:
+        with ops.StepScope(dev, training=train):
+            if train:
+                ops.l1_mean(call()).backward()
+            else:
                 with torch.no_grad():
                     call()
-            finally:
-                ops.set_fused_eval_epilogue(False)
         torch.cuda.synchronize()
     finally:
         rec.detach()

@@ -47,10 +47,10 @@ def _update_behind_version(w, seed):
 
 @pytest.fixture
 def inplace():
+    """a training scope: in-place operand refresh and prefetch_weights are on"""
     _, ops = _mods()
-    ops.set_inplace_weight_refresh(True)
-    yield
-    ops.set_inplace_weight_refresh(False)
+    with ops.StepScope(DEV, training=True):
+        yield
 
 
 def test_hit_returns_the_same_buffers_and_launches_nothing():

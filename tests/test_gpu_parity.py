@@ -272,8 +272,8 @@ def test_train_step_engine_graph_matches_eager(dev):
 
 def test_gradient_sink_matches_autograd_accumulation(dev):
     """engine.FlatParams registers in-place gradient sinks on the conv weights (ops.GradSink, written from a side stream and
-    joined by ops.join_side_streams): the arena must hold the gradients autograd would have accumulated (fp32 split-K adds
-    are unordered: compare to 1e-4 of max)."""
+    joined when the training ops.StepScope exits): the arena must hold the gradients autograd would have accumulated (fp32
+    split-K adds are unordered: compare to 1e-4 of max)."""
     from text_segmentation_image_inpainting_b200 import ops
     from text_segmentation_image_inpainting_b200.engine import FlatParams
     from text_segmentation_image_inpainting_b200.masks import HoleMask
@@ -290,9 +290,9 @@ def test_gradient_sink_matches_autograd_accumulation(dev):
         xin = buf[:, :3]
         xin.copy_(x * mask)
         ops.bump_weight_epoch()
-        out = net((xin, HoleMask.from_dense(mask, channel_uniform=True)))
-        ops.l1_mean(out).backward()
-        ops.join_side_streams()
+        with ops.StepScope(dev, training=True):
+            out = net((xin, HoleMask.from_dense(mask, channel_uniform=True)))
+            ops.l1_mean(out).backward()
         torch.cuda.synchronize()
         if with_sinks:
             unused = [i for i, sk in enumerate(flat.sinks) if not sk.used]

@@ -297,15 +297,13 @@ def _eager_eval(net, b, crit, sc):
     from text_segmentation_image_inpainting_b200 import ops
     training = net.training
     net.eval()
-    ops.set_fused_eval_epilogue(True)
     try:
-        with torch.no_grad():
+        with ops.StepScope(b.device, training=False), torch.no_grad():
             x, target = b.prepare()
             out = net(x)
             loss = crit(out, target) if crit is not None else None
             sc.update(out, target)
     finally:
-        ops.set_fused_eval_epilogue(False)
         net.train(training)
     torch.cuda.synchronize()
     return out.float(), loss

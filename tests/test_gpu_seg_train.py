@@ -96,14 +96,17 @@ def test_capture_after_a_partial_convolution_step_in_the_same_process():
     x = torch.rand(2, 3, 256, 256, device="cuda")
     m = torch.ones(2, 3, 256, 256, device="cuda")
     m[:, :, 64:160, 80:176] = 0
-    TrainStep(_small_net().cuda(), lr=1e-3, use_graph=False).step(x, m)
+    pconv = TrainStep(_small_net().cuda(), lr=1e-3, use_graph=False)
+    pconv.step(x, m)
     torch.cuda.synchronize()
-    assert ops._MASK_STREAMS
+    mask_stream = ops._aux_stream("mask", x.device)
+    assert mask_stream in pconv._scope.streams
     b = SegBatcher(2, (512, 512), image_size=128, seed=3)
     b.stage(_sources([(300, 420), (512, 380)], 90))
     ts = SegLossTrainStep(_net()[0].cuda(), b, BinaryFocalLoss(), lr=1e-3, use_graph=True)
     ts.warmup_and_capture(eager_warmup=2)
     assert ts.graph is not None
+    assert mask_stream not in ts._scope.streams          # the scope of the capture
     losses = []
     for _ in range(2):
         b.stage(_sources([(300, 420), (512, 380)], 90))

@@ -195,9 +195,7 @@ class InpaintBatcher(_SourceStager):
                                                self.clean.data_ptr(), st))
         if not capturing:
             self.release()
-        # a new view object per call: the layers tag an input plane with the event that made it ready (ops._pconv_launch), and
-        # this plane is rewritten in place by every call
-        return self.corrupted, HoleMask.from_plane(self.plane.view(self.plane.shape), 3), self.clean
+        return self.corrupted, HoleMask.from_plane(self.plane, 3), self.clean
 
 
 class InpaintPairBatcher(InpaintBatcher):

@@ -183,6 +183,7 @@ class TrainStep:
             # before the first update: the rate that update will use, as the reference's CyclicLR sets it at construction
             self._lr64 = torch.tensor(lr_schedule.rate(start), dtype=torch.float64, device=dev)
         self._caches = [c for _, _, c in ops.operand_caches(net)]
+        self._scope = ops.StepScope(self.flat.flat_g.device, training=True)
         self.pg = process_group
         self.world = torch.distributed.get_world_size(process_group) if process_group is not None else 1
         # data parallel: ranks exchange the SUM of their gradient arenas; the 1/world of the mean is folded into the optimiser
@@ -348,14 +349,15 @@ class TrainStep:
 
     def _launch_bucket(self, b):
         """All-reduce (sum) of bucket b on the communication stream, ordered after everything issued so far on the compute
-        stream (BatchNorm / bias gradients, autograd accumulations) and on the weight-gradient side stream."""
+        stream (BatchNorm / bias gradients, autograd accumulations) and on the auxiliary streams the step has used (the
+        weight-gradient side stream)."""
         if self._launched[b]:
             return
         self._launched[b] = True
         s, e, _ = self.buckets[b]
         comm = self._comm_stream
         comm.wait_stream(torch.cuda.current_stream())
-        for st in ops.side_streams():
+        for st in self._scope.streams:
             comm.wait_stream(st)
         with torch.cuda.stream(comm):
             torch.distributed.all_reduce(self.flat.flat_g[s:e], group=self.pg)
@@ -407,23 +409,15 @@ class TrainStep:
         self.flat.flat_g.zero_()
         for sk in self.flat.sinks:
             sk.used = False
-        ops.begin_step_arena(self.flat.flat_g.device)      # one zero fill for every reduction target of the step
         ops.bump_weight_epoch()
-        # scheduling switches that are only safe inside a loop that joins once per step (scoped to this call):
-        # operand buffers refreshed in place, mask passes running ahead on their own stream
-        ops.set_inplace_weight_refresh(True)
-        ops.set_mask_chain_stream(True)
         self._arm_overlap(overlap)
         try:
-            self._sync_cache_modes()
-            ops.prefetch_weights(self._caches)         # operand re-layout of all trainable layers runs ahead on its own stream
-            loss = self._forward_loss(x, mask)
-            loss.backward()
+            with self._scope:
+                self._sync_cache_modes()
+                ops.prefetch_weights(self._caches)     # operand re-layout of all trainable layers runs ahead on its own stream
+                loss = self._forward_loss(x, mask)
+                loss.backward()
         finally:
-            ops.set_mask_chain_stream(False)
-            ops.set_inplace_weight_refresh(False)
-            ops.end_step_arena(self.flat.flat_g.device)
-            ops.join_side_streams()
             if overlap:
                 self._finish_overlap()
         return loss.detach()
@@ -777,7 +771,7 @@ class InferStep:
     """Graph-captured inference of the partial-conv U-Nets: ``run(x, mask)`` with the reference's inputs (fp32 NCHW image and
     {0, 1} hole mask, prepared like TrainStep._prepare) returns the output as a static fp32 NCHW buffer that the next call
     overwrites.  The net runs in eval mode under no_grad, with the mask chain on its own stream and every eval-mode BatchNorm +
-    activation that directly follows a convolution applied in that convolution's epilogue (ops.set_fused_eval_epilogue).  The
+    activation that directly follows a convolution applied in that convolution's epilogue (an inference ops.StepScope).  The
     first call for an input shape runs the forward eagerly (operand caches, BatchNorm coefficients, counters), then captures it
     in one CUDA graph; later calls copy the inputs in and replay.
 
@@ -792,6 +786,7 @@ class InferStep:
         self.net = net.eval()
         self.dtype = compute_dtype
         self._bns = [m for m in net.modules() if isinstance(m, torch.nn.BatchNorm2d)]
+        self._scope = ops.StepScope(next(net.parameters()).device, training=False)
         self._graphs = {}
         self._captured_operands = []          # (cache, ops.Operands) of every captured convolution
         self._epoch = None
@@ -811,16 +806,8 @@ class InferStep:
         return (x, mask)
 
     def _run_forward(self, *inputs):
-        ops.set_fused_eval_epilogue(True)
-        ops.set_mask_chain_stream(True)
-        try:
-            with torch.no_grad():
-                out = self._forward(*inputs)
-        finally:
-            ops.set_mask_chain_stream(False)
-            ops.set_fused_eval_epilogue(False)
-            ops.join_mask_streams()
-        return out
+        with self._scope, torch.no_grad():
+            return self._forward(*inputs)
 
     def _check_markers(self):
         from .models.BaseModels import B200BNAct
@@ -835,11 +822,10 @@ class InferStep:
 
     def _capture(self, inputs):
         for _ in range(2):                    # eager warm-up: operand caches, coefficients, counters
-            ops.EPILOGUE_SITES.update(fused=0, unfused=0)
             before = _lib.launch_count()
             out = self._run_forward(*inputs)
             self.launches_per_run = _lib.launch_count() - before
-            self.fused_sites, self.unfused_sites = ops.EPILOGUE_SITES["fused"], ops.EPILOGUE_SITES["unfused"]
+            self.fused_sites, self.unfused_sites = self._scope.fused_sites, self._scope.unfused_sites
             self._check_markers()
         torch.cuda.synchronize()
         static_in = tuple(t.clone() if t is not None else None for t in inputs)
@@ -1018,9 +1004,7 @@ class TextRemovalStep(InferStep):
         logits = self.net.seg(x)
         text_mask = ops.text_mask_postprocess(logits, pad, (h, w))
         corrupted, valid = ops.removal_holes(text_mask, page, hu, wu, self.dtype)
-        # a new view object per call: the layers tag an input plane with the event that made it ready (ops._pconv_launch), and
-        # this plane is rewritten by every call
-        fill = self.net.fill((corrupted, HoleMask.from_plane(valid.view(valid.shape), 3)))
+        fill = self.net.fill((corrupted, HoleMask.from_plane(valid, 3)))
         key = self._key(page)
         out = self._outs.get(key)
         if out is None:                                   # the first eager warm-up: never inside a capture

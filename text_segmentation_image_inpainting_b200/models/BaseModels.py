@@ -106,7 +106,7 @@ class B200Conv2d(nn.Conv2d):
         # convolution accumulates the per-channel sum / sum of squares of its output in its own epilogue and parks them on the
         # BatchNorm, which then skips its statistics pass over y (keyed by y's address and shape: any other input is ignored).
         hint = self.__dict__.get("_bn_hint")
-        # Inference (ops.set_fused_eval_epilogue): the eval-mode BatchNorm + activation behind this convolution is applied in its
+        # Inside an inference ops.StepScope: the eval-mode BatchNorm + activation behind this convolution is applied in its
         # epilogue and the output is marked for that BatchNorm, which then passes it through.  Not where the BatchNorm adds a
         # residual (InvertedResidual marks its last BatchNorm `_pcb_residual_site`): the add must follow the BatchNorm, not the activation.
         if hint is not None and x.is_cuda and not hint.__dict__.get("_pcb_residual_site"):

@@ -102,9 +102,9 @@ def partial_convolution_block(in_channels, out_channels, kernel_size, stride=1, 
 class PartialBlock(nn.Sequential):
     """The nn.Sequential of the reference's factory (same children, same state_dict keys).  When it is exactly
     [PartialConv, PartialActivatedBN] the convolution output has a single consumer by construction, so the BatchNorm
-    backward may absorb the convolution's renormalisation backward (ops.RenormHandoff).  For the same reason, under the
-    inference engines' switch (ops.set_fused_eval_epilogue), an eval-mode [PartialConv | PartialConvNoHoles, PartialActivatedBN |
-    PartialActivation] block applies its BatchNorm + activation in the convolution epilogue.  Residual sites never come through
+    backward may absorb the convolution's renormalisation backward (ops.RenormHandoff).  For the same reason, inside an
+    inference ops.StepScope, an eval-mode [PartialConv | PartialConvNoHoles, PartialActivatedBN | PartialActivation] block
+    applies its BatchNorm + activation in the convolution epilogue.  Residual sites never come through
     here: DoublePartialResidual and PartialInvertedResidual call their last convolution and BatchNorm separately."""
 
     def forward(self, args):
@@ -120,7 +120,7 @@ class PartialBlock(nn.Sequential):
 
 
     def _eval_epilogue(self):
-        if len(self) != 2 or type(self[0]) not in (PartialConv, PartialConvNoHoles) or not ops.fused_eval_epilogue_enabled():
+        if len(self) != 2 or type(self[0]) not in (PartialConv, PartialConvNoHoles):
             return None
         tail = self[1]
         if isinstance(tail, PartialActivatedBN):

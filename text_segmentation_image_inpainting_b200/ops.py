@@ -258,43 +258,91 @@ class ConvGeom:
 
 
 # ------------------------------------------------------------------------------------------------
-# per-step zero arena: reduction targets (BatchNorm sums) are slices of ONE buffer that the training engine zeroes once per
-# step, instead of one cudaMemsetAsync per reduction (the step had 106 of them)
+# the execution mode of one engine step
 # ------------------------------------------------------------------------------------------------
-class _ZeroArena:
-    def __init__(self):
-        self.buf, self.off, self.active = None, 0, False
+_SCOPE: Optional["StepScope"] = None
 
 
-_ARENAS = {}
+class StepScope:
+    """The execution mode of one engine step, and the state that lives exactly as long as one entry.  An engine builds one and
+    runs each step (training) or forward (inference) inside ``with scope:``; at most one scope is current at a time.
+
+    Both kinds run every layer's mask pass on the mask stream, ahead of the feature path (its ready events are kept per entry,
+    keyed by mask plane).  A training scope also owns a zero arena, so that reduction targets (BatchNorm sums) are slices of one
+    buffer zeroed once on entry (`zeros_f64`) instead of one memset each.  It lets `OperandCache` rewrite operand buffers in
+    place and `prefetch_weights` refresh them ahead, and lets weight-gradient sinks defer their side stream's join to the exit.  An
+    inference scope applies eval-mode BatchNorm + activation in the convolution epilogues (`eval_epilogue`) and counts the
+    sites: `fused_sites` in an epilogue, `unfused_sites` still run on their own.  Outside any scope every one of these is off.
+
+    Leaving, on an exception too, joins the current stream to the auxiliary streams this entry put work on (`streams`, kept
+    until the next entry) and drops the entry's keep-alive list and ready events."""
+
+    ARENA_BYTES = 1 << 20
+
+    def __init__(self, device, training: bool):
+        self.training = bool(training)
+        self._arena = torch.empty((self.ARENA_BYTES,), dtype=torch.uint8, device=device) if self.training else None
+        self._off = 0
+        self.fused_sites = self.unfused_sites = 0
+        self.streams: List[torch.cuda.Stream] = []
+        self._keep = []
+        self._ready = {}            # mask plane -> the event it is ready at (tensors hash by identity)
+
+    def __enter__(self):
+        global _SCOPE
+        if _SCOPE is not None:
+            raise _lib.PcbError("a StepScope is already current: engine steps do not nest")
+        self._off = self.fused_sites = self.unfused_sites = 0
+        self.streams = []
+        if self._arena is not None:
+            self._arena.zero_()
+        _SCOPE = self
+        return self
+
+    def __exit__(self, *exc):
+        global _SCOPE
+        try:
+            cur = torch.cuda.current_stream()
+            for st in self.streams:
+                cur.wait_stream(st)
+        finally:
+            self._keep, self._ready = [], {}
+            _SCOPE = None
+        return False
+
+    def _use(self, stream, keep=None):
+        """`stream` carries work of this entry (that reads or writes `keep`): join it on exit, keep `keep` alive until then."""
+        if stream not in self.streams:
+            self.streams.append(stream)
+        if keep is not None:
+            self._keep.append(keep)
 
 
-def begin_step_arena(device, nbytes=1 << 20):
-    """Zero the arena of `device` on the current stream and hand out slices of it until end_step_arena()."""
-    key = (device.type, device.index if device.index is not None else torch.cuda.current_device())
-    a = _ARENAS.setdefault(key, _ZeroArena())
-    if a.buf is None or a.buf.numel() < nbytes:
-        a.buf = torch.empty((nbytes,), dtype=torch.uint8, device=device)
-    a.buf.zero_()
-    a.off, a.active = 0, True
-
-
-def end_step_arena(device):
-    key = (device.type, device.index if device.index is not None else torch.cuda.current_device())
-    if key in _ARENAS:
-        _ARENAS[key].active = False
+def current_scope() -> Optional[StepScope]:
+    """The StepScope the current step runs in, or None."""
+    return _SCOPE
 
 
 def zeros_f64(n, device):
-    """n zeroed doubles: a slice of the step arena when one is active (and has room), else a fresh zero tensor."""
-    key = (device.type, device.index if device.index is not None else torch.cuda.current_device())
-    a = _ARENAS.get(key)
+    """n zeroed doubles: a slice of the training scope's arena when it has room, else a fresh zero tensor."""
+    s = _SCOPE
     nbytes = (n * 8 + 255) // 256 * 256
-    if a is not None and a.active and a.off + nbytes <= a.buf.numel():
-        view = a.buf[a.off:a.off + n * 8].view(torch.float64)
-        a.off += nbytes
+    if s is not None and s._arena is not None and device == s._arena.device and s._off + nbytes <= s._arena.numel():
+        view = s._arena[s._off:s._off + n * 8].view(torch.float64)
+        s._off += nbytes
         return view
     return torch.zeros((n,), dtype=torch.float64, device=device)
+
+
+_AUX_STREAMS = {}
+
+
+def _aux_stream(kind: str, device) -> torch.cuda.Stream:
+    """The process-wide auxiliary stream `kind` ("mask", "side": weight gradients, "prefetch": operand refreshes) of `device`."""
+    key = (kind, device.index if device.index is not None else torch.cuda.current_device())
+    if key not in _AUX_STREAMS:
+        _AUX_STREAMS[key] = torch.cuda.Stream(device=device)
+    return _AUX_STREAMS[key]
 
 
 _PROFILE = None     # optional list: (kind, geom, start_event, end_event) appended per conv kernel call
@@ -330,11 +378,11 @@ def _workspace(lib, c, device):
 
 
 def _pconv_launch(lib, geom: ConvGeom, c: Conv, w_fwd, b32, y, bn_sums, epi: Optional["EvalEpilogue"]):
-    """Mask pass + forward of one partial convolution into `y`; returns (msum, newmask).  `bn_sums`: training statistics
-    target (pcb_pconv_forward_bn); `epi`: eval-mode BatchNorm + activation applied in the epilogue (pcb_pconv_forward_affine_act)."""
-    global _LAST_MASK_EVENT
-    _LAST_MASK_EVENT = None
+    """Mask pass + forward of one partial convolution into `y`; returns (msum, newmask, the event newmask is ready at on the
+    mask stream or None).  `bn_sums`: training statistics target (pcb_pconv_forward_bn); `epi`: eval-mode BatchNorm +
+    activation applied in the epilogue (pcb_pconv_forward_affine_act)."""
     dev = y.device
+    scope = _SCOPE
 
     def forward(mask_pass_done, msum, newmask, ws):
         if epi is None:
@@ -345,19 +393,19 @@ def _pconv_launch(lib, geom: ConvGeom, c: Conv, w_fwd, b32, y, bn_sums, epi: Opt
                                                 newmask.data_ptr(), ws.data_ptr(), mask_pass_done, _ptr(scale), _ptr(shift), epi.code,
                                                 epi.slope, _stream())
 
-    if _MASK_CHAIN_STREAM and _PROFILE is None and not geom.plain:
+    if scope is not None and _PROFILE is None and not geom.plain:
         # Mask updates never depend on features (partial_convolution.py:59-77): the mask pass of this layer runs on the
         # mask stream, ordered only after the passes that produced its input planes, i.e. ahead of the feature path.
-        # Its buffers are allocated on that stream and kept alive until join_side_streams() (engine, once per step).
-        main, ms = torch.cuda.current_stream(), _mask_stream(dev)
+        # Its buffers are allocated on that stream and kept alive until the scope's exit joins it.
+        main, ms = torch.cuda.current_stream(), _aux_stream("mask", dev)
         for (_, _, _, pl, _) in geom.parts:
             if pl is None:
                 continue
-            ev_in = getattr(pl, "_pcb_ev", None)
+            ev_in = scope._ready.get(pl)
             if ev_in is None:                        # a plane written on the main stream (the network's input mask): mark it
                 ev_in = torch.cuda.Event()           # ready from here on, so later consumers (the tail) need not wait for main
                 ev_in.record(main)
-                pl._pcb_ev = ev_in
+                scope._ready[pl] = ev_in
             ms.wait_event(ev_in)
         with torch.cuda.stream(ms):
             msum = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.float32, device=dev)
@@ -367,36 +415,23 @@ def _pconv_launch(lib, geom: ConvGeom, c: Conv, w_fwd, b32, y, bn_sums, epi: Opt
             ev = torch.cuda.Event()
             ev.record()
         main.wait_event(ev)
-        _DEFERRED.append((msum, newmask, ws))
-        _LAST_MASK_EVENT = ev
+        scope._use(ms, (msum, newmask, ws))
         _lib.check(forward(1, msum, newmask, ws))
     else:
         msum = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.float32, device=dev)
         newmask = torch.empty((geom.mg, geom.n, geom.ho, geom.wo), dtype=torch.uint8, device=dev)
         ws = _workspace(lib, c, dev)
+        ev = None
         with _Timed("fwd", geom):
             _lib.check(forward(0, msum, newmask, ws))
-    return msum, newmask
+    return msum, newmask, ev
 
 
 # ------------------------------------------------------------------------------------------------
 # inference: eval-mode BatchNorm + activation fused into the convolution epilogue
 # ------------------------------------------------------------------------------------------------
-_FUSED_EVAL_EPILOGUE = False
-# sites seen while the switch is on: "fused" = BatchNorm/activation passes applied in a convolution epilogue, "unfused" =
-# BatchNorm/activation passes that still ran on their own (bn_act / activation_only)
-EPILOGUE_SITES = {"fused": 0, "unfused": 0}
-
-
-def set_fused_eval_epilogue(enabled: bool):
-    """Let the convolution blocks apply their eval-mode BatchNorm + activation in the convolution epilogue (the inference
-    engines set this for the duration of their forward).  Off by default: a plain ``net.eval(); net(x)`` runs the two-pass path."""
-    global _FUSED_EVAL_EPILOGUE
-    _FUSED_EVAL_EPILOGUE = bool(enabled)
-
-
-def fused_eval_epilogue_enabled() -> bool:
-    return _FUSED_EVAL_EPILOGUE
+def _inference_scope() -> Optional[StepScope]:
+    return _SCOPE if _SCOPE is not None and not _SCOPE.training else None
 
 
 def bn_eval_coefficients(bn) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -405,7 +440,7 @@ def bn_eval_coefficients(bn) -> Tuple[torch.Tensor, torch.Tensor]:
     changes, so a captured graph that reads them sees the new values.  Not recomputed during a graph capture."""
     key = (_WEIGHT_EPOCH, bn.weight._version, bn.bias._version, bn.running_mean._version, bn.running_var._version,
            bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr())
-    cache = bn.__dict__.setdefault("_pcb_eval_coef", {})
+    cache = bn.__dict__.setdefault("_pcb_bn_coef", {})
     if cache.get("key") != key:
         if torch.cuda.is_current_stream_capturing():
             raise _lib.PcbError("BatchNorm eval coefficients are stale inside a graph capture: refresh them before capturing")
@@ -436,9 +471,10 @@ class EvalEpilogue:
 
 
 def eval_epilogue(bn, act) -> Optional[EvalEpilogue]:
-    """The epilogue for a convolution whose ONLY consumer is `act(bn(.))`, or None when the switch is off, the BatchNorm is in
-    training mode / has no running statistics or affine parameters, or the activation has no kernel."""
-    if not _FUSED_EVAL_EPILOGUE:
+    """The epilogue for a convolution whose ONLY consumer is `act(bn(.))`, or None outside an inference StepScope, when the
+    BatchNorm is in training mode / has no running statistics or affine parameters, or when the activation has no kernel.
+    A plain ``net.eval(); net(x)`` therefore runs the two-pass path."""
+    if _inference_scope() is None:
         return None
     if bn is not None and (bn.training or bn.running_mean is None or bn.weight is None or bn.bias is None):
         return None
@@ -461,14 +497,16 @@ def _partial_conv_fused_eval(geom: ConvGeom, wprep, bias, xs, epi: EvalEpilogue)
     else:
         y = torch.empty((geom.n, geom.cout, geom.ho, geom.wo), dtype=xs[0].dtype, device=dev, memory_format=CL)
     b32 = bias.detach().float().contiguous() if bias is not None else None
-    msum, newmask = _pconv_launch(lib, geom, c, wprep.w_fwd, b32, y, None, epi)
+    out = _pconv_launch(lib, geom, c, wprep.w_fwd, b32, y, None, epi)
     epi.fused = True
-    EPILOGUE_SITES["fused"] += 1
-    return y, msum, newmask
+    if _SCOPE is not None:
+        _SCOPE.fused_sites += 1
+    return (y, *out)
 
 
 class PartialConvFn(torch.autograd.Function):
-    """y, msum, newmask = pconv(cat(up?(x_i)), W, b | mask)   (models/partial_convolution.py:49-80 / :121-137)."""
+    """y, msum, newmask = pconv(cat(up?(x_i)), W, b | mask)   (models/partial_convolution.py:49-80 / :121-137), and the event
+    newmask is ready at when the mask pass ran on the mask stream (else None)."""
 
     @staticmethod
     def forward(ctx, geom: ConvGeom, wprep, weight, bias, handoff, *xs):
@@ -487,7 +525,7 @@ class PartialConvFn(torch.autograd.Function):
                 and nhwc_layout(y) == geom.cout:
             bn_sums = zeros_f64(2 * geom.cout, dev)
             handoff.bn_sums = bn_sums
-        msum, newmask = _pconv_launch(lib, geom, c, w_fwd, b32, y, bn_sums, None)
+        msum, newmask, mask_ready = _pconv_launch(lib, geom, c, w_fwd, b32, y, bn_sums, None)
         ctx.geom, ctx.wprep, ctx.has_bias, ctx.weight_ref, ctx.bias_ref = geom, wprep, bias is not None, weight, bias
         ctx.handoff = handoff
         if handoff is not None:
@@ -498,10 +536,10 @@ class PartialConvFn(torch.autograd.Function):
         ctx.mark_non_differentiable(msum, newmask)
         # without this autograd zero-fills a gradient tensor for msum and newmask on every backward (two fill kernels per layer)
         ctx.set_materialize_grads(False)
-        return y, msum, newmask
+        return y, msum, newmask, mask_ready
 
     @staticmethod
-    def backward(ctx, gy, _gmsum, _gnewmask):
+    def backward(ctx, gy, _gmsum, _gnewmask, _gready):
         if gy is None:
             return (None,) * (5 + len(ctx.saved_tensors) - 1)
         lib = _lib.load()
@@ -545,9 +583,9 @@ class PartialConvFn(torch.autograd.Function):
         if ctx.needs_input_grad[2]:
             # A training engine may register a gradient sink on the parameter (engine.FlatParams: a view of its flat fp32
             # gradient arena with the weight's physical layout).  The kernel then writes the gradient in place (it overwrites:
-            # no accumulation pass) and autograd gets no tensor; with the side stream below the join can then wait until
-            # the engine calls join_side_streams(), so the weight gradient also overlaps the element-wise backward kernels
-            # of the layers that follow.  A second use of the same weight in one pass falls back to autograd accumulation.
+            # no accumulation pass) and autograd gets no tensor; inside a training StepScope the side stream below then joins
+            # at the scope's exit, so the weight gradient also overlaps the element-wise backward kernels of the layers that
+            # follow.  A second use of the same weight in one pass falls back to autograd accumulation.
             sink = getattr(ctx.weight_ref, "_pcb_grad_sink", None)
             wgrad_fn = lib.pcb_pconv_backward_weight
             shape = (geom.cout, geom.cin // geom.groups, geom.kh, geom.kw)
@@ -564,20 +602,18 @@ class PartialConvFn(torch.autograd.Function):
             # kernels of a low-resolution layer (far fewer tiles than SMs each) fill the GPU together.  Buffers are
             # allocated on the main stream before the fork and the streams re-join before this function returns.
             if (any(need) or sink is not None) and _PROFILE is None:
-                side = _side_stream(dev)
+                side = _aux_stream("side", dev)
                 side.wait_stream(torch.cuda.current_stream())
+                deferred = sink is not None and _SCOPE is not None and _SCOPE.training
+                if deferred:
+                    _SCOPE._use(side, (dc, ws, xs))            # keep the side stream's operands alive until the join
                 with torch.cuda.stream(side):
                     _lib.check(wgrad_fn(ctypes.byref(c), dc.data_ptr(), dcs, dw_buf.data_ptr(), ws.data_ptr(), _stream()))
-                if sink is not None:
-                    deferred = True
-                    _DEFERRED.append((dc, ws, xs))            # keep the side stream's operands alive until the join
-                    if sink.on_written is not None:
-                        sink.on_written()
             else:
                 with _Timed("wgrad", geom):
                     _lib.check(wgrad_fn(ctypes.byref(c), dc.data_ptr(), dcs, dw_buf.data_ptr(), ws.data_ptr(), _stream()))
-                if sink is not None and sink.on_written is not None:
-                    sink.on_written()
+            if sink is not None and sink.on_written is not None:
+                sink.on_written()
         gxs: List[Optional[torch.Tensor]] = [None] * len(xs)
         if any(need):
             # gradient buffer per source tensor; parts write their channel slices.  Full resolution -- except on the sub-pixel
@@ -631,15 +667,11 @@ def bump_weight_epoch():
     _WEIGHT_EPOCH += 1
 
 
-_INPLACE_WEIGHT_REFRESH = False
-
-
-def set_inplace_weight_refresh(enabled: bool):
-    """Training engines that update the masters once per step (after every backward of that step has run) may let an
-    `OperandCache` rewrite its operand buffers in place instead of allocating + zero-filling new ones each step.
-    Off by default: a backward that runs after a later weight update would otherwise read the new weights."""
-    global _INPLACE_WEIGHT_REFRESH
-    _INPLACE_WEIGHT_REFRESH = bool(enabled)
+def _inplace_weight_refresh() -> bool:
+    """Inside a training StepScope an `OperandCache` may rewrite its operand buffers in place instead of allocating + zero-filling
+    new ones: the engine updates the masters once per step, after every backward of that step has run.  Outside one, a backward
+    that runs after a later weight update would read the new weights."""
+    return _SCOPE is not None and _SCOPE.training
 
 
 def _operand_key(weight: torch.Tensor, geom: ConvGeom, frozen: bool):
@@ -689,8 +721,8 @@ class Operands:
 
 class OperandCache:
     """A module's operands of one convolution weight, kept from one call to the next.  `get(weight, geom)` returns the current
-    record while its key (`_operand_key`) matches, else the current record rewritten in place when set_inplace_weight_refresh()
-    is on and the layout is unchanged, else a new record: the buffers of a record a captured graph keeps are never freed.
+    record while its key (`_operand_key`) matches, else the current record rewritten in place inside a training StepScope when
+    the layout is unchanged, else a new record: the buffers of a record a captured graph keeps are never freed.
 
     `frozen` (weights no optimiser updates, the VGG loss): the key leaves out the weight epoch, so the operands are laid out again
     only when the weight itself changes, never in place and never inside a graph capture.  `derive`: see Operands."""
@@ -710,7 +742,7 @@ class OperandCache:
             return rec
         if self.frozen and torch.cuda.is_current_stream_capturing():
             raise _lib.PcbError("VGG operands are stale inside a graph capture: run the loss once before capturing")
-        if (_INPLACE_WEIGHT_REFRESH and not self.frozen and rec is not None and rec.geom.signature == geom.signature
+        if (_inplace_weight_refresh() and not self.frozen and rec is not None and rec.geom.signature == geom.signature
                 and rec.w_fwd.device == weight.device
                 and Operands.sizes(geom.struct(None)) == (rec.w_fwd.numel(), rec.w_dg.numel() if rec.w_dg is not None else 0)):
             rec.weight, rec.geom = weight, geom
@@ -732,22 +764,17 @@ def operand_caches(*roots: torch.nn.Module):
     return [(m, name, c) for r in roots for m in r.modules() for name, c in vars(m).items() if isinstance(c, OperandCache)]
 
 
-_PREFETCH_STREAMS = {}
-
-
 def prefetch_weights(caches):
     """Re-lay-out the weights behind `caches` (OperandCache; frozen and empty ones are skipped) on a prefetch stream, ahead of the
-    layers' forward calls (training engines call this right after the optimiser step / epoch bump; requires the in-place refresh
-    mode).  Each layer's forward then only waits on its own event, so the re-layout of layer k overlaps the layers before it."""
+    layers' forward calls (training engines call this right after the optimiser step / epoch bump; only inside a training
+    StepScope).  Each layer's forward then only waits on its own event, so the re-layout of layer k overlaps the layers before it."""
     caches = [c for c in caches if c.current is not None and not c.frozen]
-    if not _INPLACE_WEIGHT_REFRESH or not caches:
+    if not _inplace_weight_refresh() or not caches:
         return
     dev = caches[0].current.weight.device
-    key_dev = (dev.type, dev.index if dev.index is not None else torch.cuda.current_device())
-    if key_dev not in _PREFETCH_STREAMS:
-        _PREFETCH_STREAMS[key_dev] = torch.cuda.Stream(device=dev)
-    ps = _PREFETCH_STREAMS[key_dev]
+    ps = _aux_stream("prefetch", dev)
     ps.wait_stream(torch.cuda.current_stream())           # after the optimiser step, and after every reader of the old buffers
+    _SCOPE._use(ps)
     with torch.cuda.stream(ps):
         for cache in caches:
             rec = cache.current
@@ -758,77 +785,15 @@ def prefetch_weights(caches):
             cache.ready.record()
 
 
-_MASK_CHAIN_STREAM = False
-_LAST_MASK_EVENT = None
-_SIDE_STREAMS = {}
-_MASK_STREAMS = {}
-_DEFERRED = []
-
-
-def set_mask_chain_stream(enabled: bool):
-    """Run every layer's mask pass (mask box sums, new mask, tap-validity words) on a dedicated stream ahead of the feature
-    path.  Only for callers that call join_side_streams() once per step (the buffers of the pass live until then)."""
-    global _MASK_CHAIN_STREAM
-    _MASK_CHAIN_STREAM = bool(enabled)
-
-
-def _mask_stream(dev):
-    key = (dev.type, dev.index if dev.index is not None else torch.cuda.current_device())
-    if key not in _MASK_STREAMS:
-        _MASK_STREAMS[key] = torch.cuda.Stream(device=dev)
-    return _MASK_STREAMS[key]
-
-
 class GradSink:
     """In-place destination for a convolution weight gradient (see PartialConvFn.backward).  The owner resets `used` before
-    every backward pass and calls join_side_streams() after it."""
+    every backward pass; inside a training StepScope the gradient is complete on the scope's exit, outside one when the
+    backward returns."""
 
     def __init__(self, view: torch.Tensor):
         self.view, self.used = view, False
         self.prezeroed = False        # the owner guarantees `view` is zero when the backward pass starts (skip the kernel's memset)
         self.on_written = None        # optional callback: the kernel that writes `view` has just been launched
-
-
-def side_streams():
-    """The weight-gradient side streams created so far (a training engine orders its gradient exchange after them)."""
-    return list(_SIDE_STREAMS.values())
-
-
-def _in_capture(st) -> bool:
-    """True when `st` takes part in the capture of the current stream (it waited on captured work and holds captured work)."""
-    with torch.cuda.stream(st):
-        return torch.cuda.is_current_stream_capturing()
-
-
-def join_side_streams():
-    """Make the current stream wait for every weight gradient still running on a side stream (gradient sinks only).
-
-    Inside a graph capture only the streams this capture forked are joined: a stream the captured step never used (the mask
-    stream of an earlier partial-convolution network, during the capture of a segmentation step) holds no captured work, and
-    waiting on it would end the capture with cudaErrorStreamCaptureIsolation."""
-    cur = torch.cuda.current_stream()
-    capturing = torch.cuda.is_current_stream_capturing()
-    for st in list(_SIDE_STREAMS.values()) + list(_MASK_STREAMS.values()) + list(_PREFETCH_STREAMS.values()):
-        if capturing and not _in_capture(st):
-            continue
-        cur.wait_stream(st)
-    _DEFERRED.clear()
-
-
-def join_mask_streams():
-    """Make the current stream wait for the mask passes issued on the mask stream since the last join (inference: a forward
-    without side streams).  Waits only when there were any, so a graph capture never depends on a stream it did not use."""
-    if _DEFERRED:
-        for st in _MASK_STREAMS.values():
-            torch.cuda.current_stream().wait_stream(st)
-    _DEFERRED.clear()
-
-
-def _side_stream(dev):
-    key = (dev.type, dev.index if dev.index is not None else torch.cuda.current_device())
-    if key not in _SIDE_STREAMS:
-        _SIDE_STREAMS[key] = torch.cuda.Stream(device=dev)
-    return _SIDE_STREAMS[key]
 
 
 class RenormHandoff:
@@ -876,11 +841,11 @@ def partial_conv(x, mask, weight, bias, stride, padding, dilation, groups, same_
         return _partial_conv_dense_masks(x, hm, weight, bias, stride, padding, dilation, groups, same_holes, no_guard, cache)
     wprep = (cache if cache is not None else OperandCache()).get(weight, geom)
     out = _partial_conv_fused_eval(geom, wprep, bias, xs, epilogue) if epilogue is not None else None
-    y, msum, newmask = out if out is not None else PartialConvFn.apply(geom, wprep, weight, bias, handoff, *xs)
+    y, msum, newmask, mask_ready = out if out is not None else PartialConvFn.apply(geom, wprep, weight, bias, handoff, *xs)
     planes = [newmask[g] for g in range(geom.mg)]
-    if _LAST_MASK_EVENT is not None:                      # written on the mask stream: consumers there wait on this event
+    if mask_ready is not None:                            # written on the mask stream: consumers there wait on this event
         for pl in planes:
-            pl._pcb_ev = _LAST_MASK_EVENT
+            _SCOPE._ready[pl] = mask_ready
     if geom.mg == 1:
         new = HoleMask.from_plane(planes[0], cout, 0)
     else:
@@ -1074,8 +1039,9 @@ def bn_act(x, bn, act, residual=None, handoff=None, pre_sums=None):
     convolution whose output `x` is, when this call is that output's only consumer."""
     x = as_feature(x)
     code, slope = act_code(act)
-    if _FUSED_EVAL_EPILOGUE:
-        EPILOGUE_SITES["unfused"] += 1
+    scope = _inference_scope()
+    if scope is not None:
+        scope.unfused_sites += 1
     if residual is not None:
         residual = as_feature(residual)
     if bn is None:
@@ -1096,8 +1062,9 @@ def bn_act(x, bn, act, residual=None, handoff=None, pre_sums=None):
 def activation_only(x, act, residual=None):
     x = as_feature(x)
     code, slope = act_code(act)
-    if _FUSED_EVAL_EPILOGUE:
-        EPILOGUE_SITES["unfused"] += 1
+    scope = _inference_scope()
+    if scope is not None:
+        scope.unfused_sites += 1
     return BNActFn.apply(x, None, None, residual, None, None, None, False, 0.0, 0.0, code, slope)
 
 

@@ -111,18 +111,17 @@ def main():
         ev = InpaintEvalStep(n, b, extractor)
         ev.warmup_and_capture()
         crit = InpaintingLoss(extractor) if extractor is not None else None
+        scope = ops.StepScope(dev, training=False)
 
         def eager():
             n.eval()
-            ops.set_fused_eval_epilogue(True)
             try:
-                with torch.no_grad():
+                with scope, torch.no_grad():
                     xin, hm, clean = b.prepare()
                     out = n((xin, hm))
                     if crit is not None:
                         crit(clean, hm, out, clean)
             finally:
-                ops.set_fused_eval_epilogue(False)
                 n.train()
         eager()
         graph_ms, eager_ms = [], []
