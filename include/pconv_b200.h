@@ -297,6 +297,16 @@ int pcb_removal_holes(const uint8_t *text_mask, const float *page, int n, int h,
  * plane pcb_removal_holes wrote. */
 int pcb_removal_composite(const void *fill, int dtype, int cstride, const float *page, const uint8_t *valid, int n, int h, int w,
                           int hu, int wu, float *out, pcb_stream_t stream);
+/* The segmentation demo's region image (Examples/demo_segmentation.py:17-25, 40-45, draw_bounding_box(page, mask, threshold)):
+ * out uint8 [n, h, w, 3] = np.array(to_pil_image(page[i])) with the convex hull of every outer contour of the text mask (uint8
+ * [n, 1, h, w], nonzero = text) whose cv2.contourArea exceeds `area_threshold` filled as cv2.drawContours(..., -1) fills it,
+ * in RGB (50, 128, 30).  Computed from the regions of the mask (DESIGN 4.14): union-find labelling, windowed areas, hulls of
+ * the row extents, fillPoly's LINE_8 spans.  `workspace`: device memory of pcb_text_regions_workspace(n, h, w) bytes (0 for
+ * out-of-range sizes: (h + 1) * (w + 1) < 2^31, n <= 65535), 256-byte aligned; eleven launches whose grids depend on (n, h, w)
+ * only, no host synchronisation (capturable).  Every output byte is written. */
+size_t pcb_text_regions_workspace(int n, int h, int w);
+int pcb_text_region_hulls(const uint8_t *text_mask, const float *page, int n, int h, int w, double area_threshold, void *workspace,
+                          uint8_t *out, pcb_stream_t stream);
 
 /* ---- inpainting training data (ImageInpaintingData.process_images, Dataloader.py:110-162) -------------------------------
  * One decoded source per image: RGB uint8 [h][rgb_stride] (3 bytes per pixel) and the text mask uint8 [h][mask_stride]. */

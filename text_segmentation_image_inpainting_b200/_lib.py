@@ -102,6 +102,8 @@ _SIGS = {
     "pcb_removal_seg_input": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]),
     "pcb_removal_holes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "pcb_removal_composite": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pcb_text_regions_workspace": (c_size_t, [c_int, c_int, c_int]),
+    "pcb_text_region_hulls": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p]),
     "pcb_seg_validate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int]),
     "pcb_seg_sample": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "pcb_seg_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,

@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpconv_b200.so")
 STAMP = os.path.join(HERE, "libpconv_b200.stamp")     # fingerprint of the sources the .so was built from (travels with it)
-SOURCES = ["api.cu", "conv_tc.cu", "conv_smallco.cu", "conv_k2r.cu", "conv_stem.cu", "conv_generic.cu", "elementwise.cu", "dwconv.cu", "seg_ops.cu", "inpaint_data.cu", "inpaint_loss.cu", "seg_data.cu", "seg_loss.cu", "text_removal.cu"]
+SOURCES = ["api.cu", "conv_tc.cu", "conv_smallco.cu", "conv_k2r.cu", "conv_stem.cu", "conv_generic.cu", "elementwise.cu", "dwconv.cu", "seg_ops.cu", "inpaint_data.cu", "inpaint_loss.cu", "seg_data.cu", "seg_loss.cu", "text_removal.cu", "text_regions.cu"]
 HEADERS = ["pcb_common.cuh", "pcb_ptx.cuh", "pcb_tc_epi.cuh", "pil_data.cuh", "pcb_dilate.cuh", os.path.join("..", "..", "include", "pconv_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",

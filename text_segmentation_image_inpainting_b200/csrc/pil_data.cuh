@@ -1,4 +1,5 @@
 // pil_data.cuh -- pieces shared by the GPU data paths (inpaint_data.cu, seg_data.cu):
+//   * to_pil_image's byte of a fp32 page value (text_removal.cu, text_regions.cu);
 //   * Pillow's bicubic resampling coefficients (precompute_coeffs + normalize_coeffs_8bpc) and its 8-bit clip, bit for bit:
 //     the weights are computed in double with explicitly rounded operations (no FMA contraction, which Pillow's x86-64 build
 //     does not do either);
@@ -60,6 +61,12 @@ __device__ inline int pil_coeffs(int xx, int insize, int outsize, int *k, int st
 __device__ __forceinline__ int clip8(int acc) {
     acc >>= PB;
     return acc < 0 ? 0 : (acc > 255 ? 255 : acc);
+}
+
+// torchvision's to_pil_image byte of a fp32 page value: pic.mul(255).byte(), clamped to [0, 255], NaN to 0
+__device__ __forceinline__ int page_byte(float p) {
+    const float v = __fmul_rn(p, 255.f);
+    return v >= 255.f ? 255 : (v > 0.f ? static_cast<int>(v) : 0);
 }
 
 __device__ __forceinline__ uint4 philox(uint4 c, uint32_t k0, uint32_t k1) {

@@ -49,12 +49,6 @@ size_t resize_ws_bytes(int n, int h, int rh, int rw) {
     return align256(ks * KP * sizeof(int)) + align256(ks * sizeof(int2)) + static_cast<size_t>(n) * h * rw * sizeof(uchar4);
 }
 
-// torchvision's to_pil_image byte: pic.mul(255).byte(), clamped to [0, 255], NaN to 0
-__device__ __forceinline__ int page_byte(float p) {
-    const float v = __fmul_rn(p, 255.f);
-    return v >= 255.f ? 255 : (v > 0.f ? static_cast<int>(v) : 0);
-}
-
 // One thread per output column (i < rw, over the page width) or output row (i >= rw, over its height).
 __global__ void __launch_bounds__(HX) page_coeffs_kernel(int h, int w, int rh, int rw, int *__restrict__ k, int2 *__restrict__ bounds) {
     const int i = blockIdx.x * HX + threadIdx.x, ks = rw + rh;
@@ -82,9 +76,9 @@ __global__ void __launch_bounds__(HX) page_hpass_kernel(const float *__restrict_
         int a0 = 1 << (pil::PB - 1), a1 = a0, a2 = a0;
         for (int t = 0; t < bd.y; ++t) {
             const int kt = kk[t * HX + threadIdx.x];
-            a0 += page_byte(__ldg(p + t)) * kt;
-            a1 += page_byte(__ldg(p + plane + t)) * kt;
-            a2 += page_byte(__ldg(p + 2 * plane + t)) * kt;
+            a0 += pil::page_byte(__ldg(p + t)) * kt;
+            a1 += pil::page_byte(__ldg(p + plane + t)) * kt;
+            a2 += pil::page_byte(__ldg(p + 2 * plane + t)) * kt;
         }
         tmp[(static_cast<size_t>(b) * h + r) * rw + x] =
             make_uchar4(static_cast<uint8_t>(pil::clip8(a0)), static_cast<uint8_t>(pil::clip8(a1)), static_cast<uint8_t>(pil::clip8(a2)), 0);

@@ -942,15 +942,21 @@ class TextRemovalStep(InferStep):
     normalized and padded on one side to `seg_resize` -- and step 3 brings the mask back to the page's size (EvaluateSet's
     resize_mask).  Steps 4-7 run at the page's own resolution either way.
 
+    `region_hulls`: None leaves the step as above.  A number is the segmentation demo's area threshold (500 in its call): the
+    graph then also draws the demo's ``_contour`` image from the step's own text mask and page (ops.text_region_hulls: the
+    convex hull of every outer text contour with contourArea above the threshold, filled in RGB (50, 128, 30) on the page's
+    bytes), so with ``seg_resize=600`` one run() gives both of the demo's images and the text-removed page.
+
     ``run(page)`` takes fp32 NCHW pages [n, 3, h, w] in [0, 1] (``to_tensor`` of the RGB page) and returns the composite as a
     static fp32 NCHW buffer that the next call overwrites.  The same call leaves static buffers of its stages:
     `text_mask` (uint8 [n, 1, h, w], 1 = text: the demo's mask), `valid` (uint8 [n, hu, wu], 1 = kept), `last_resized` (the
     resized fp32 page, None without `seg_resize`), `last_seg_input` (the segmentation network's input), `last_logits` and
-    `last_fill` (the two networks' raw outputs).  Counters and weight reloads as InferStep: ``load_state_dict`` on either network
+    `last_fill` (the two networks' raw outputs), and `text_regions` (uint8 [n, h, w, 3], the demo's region image; None without
+    `region_hulls`).  Counters and weight reloads as InferStep: ``load_state_dict`` on either network
     is picked up by the next run()."""
 
     def __init__(self, seg_net: torch.nn.Module, fill_net: torch.nn.Module, normalize=DEMO_MEAN_STD, compute_dtype=torch.bfloat16,
-                 seg_resize=None):
+                 seg_resize=None, region_hulls=None):
         from .models.image_inpainting import ImageFill, ImageFillOrigin, ImageFillOriginV2
         from .models.text_segmentation import TextSegament, XceptionTextSegment
         if not isinstance(seg_net, (TextSegament, XceptionTextSegment)):
@@ -975,14 +981,21 @@ class TextRemovalStep(InferStep):
             if isinstance(seg_resize, bool) or not isinstance(seg_resize, int) or seg_resize <= 0 or seg_resize % 8:
                 raise ValueError(f"TextRemovalStep: seg_resize must be None or a positive multiple of 8, got {seg_resize!r}")
             self.seg_resize = seg_resize
+        self.region_hulls = None
+        if region_hulls is not None:
+            if isinstance(region_hulls, bool) or not isinstance(region_hulls, (int, float)) \
+                    or not float("-inf") < float(region_hulls) < float("inf"):
+                raise ValueError(f"TextRemovalStep: region_hulls must be None or a finite area threshold, got {region_hulls!r}")
+            self.region_hulls = region_hulls
         super().__init__(_TextRemovalNets(seg_net, fill_net), compute_dtype)
         self.multiple = 2 ** len(fill_net.decoder)        # one nearest x2 per decoder stage
         self._outs = {}                                   # page shape -> the composite buffer run() returns
         self._products = {}                               # page shape -> the stage buffers of its graph (_PRODUCTS)
         self._cur = None
         self.text_mask = self.valid = self.last_resized = self.last_seg_input = self.last_logits = self.last_fill = None
+        self.text_regions = None
 
-    _PRODUCTS = ("text_mask", "valid", "last_resized", "last_seg_input", "last_logits", "last_fill")
+    _PRODUCTS = ("text_mask", "valid", "last_resized", "last_seg_input", "last_logits", "last_fill", "text_regions")
 
     def _seg_geometry(self, h: int, w: int):
         """((rh, rw), border_pad): the size the page is segmented at and the padding to the segmentation grid."""
@@ -1010,7 +1023,8 @@ class TextRemovalStep(InferStep):
         if out is None:                                   # the first eager warm-up: never inside a capture
             out = self._outs[key] = torch.empty((n, 3, h, w), dtype=torch.float32, device=page.device)
         ops.removal_composite(fill, page, valid, out=out)
-        self._cur = (text_mask, valid, resized, x, logits, fill)
+        regions = ops.text_region_hulls(text_mask, page, self.region_hulls) if self.region_hulls is not None else None
+        self._cur = (text_mask, valid, resized, x, logits, fill, regions)
         return out
 
     def _static_out(self, out):

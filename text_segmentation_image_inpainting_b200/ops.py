@@ -1506,3 +1506,44 @@ def removal_composite(fill: torch.Tensor, page: torch.Tensor, valid: torch.Tenso
     _lib.check(_lib.load().pcb_removal_composite(fill.data_ptr(), _dtype_code(fill), nhwc_layout(fill), page.data_ptr(), valid.data_ptr(),
                                                  n, h, w, hu, wu, out.data_ptr(), _stream()))
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# the segmentation demo's region image (csrc/text_regions.cu)
+# ------------------------------------------------------------------------------------------------
+TEXT_REGION_COLOR = (50, 128, 30)         # draw_bounding_box's fill (Examples/demo_segmentation.py:24)
+TEXT_REGION_LAUNCHES = 11                 # kernels per text_region_hulls call
+
+
+def text_region_hulls(text_mask: torch.Tensor, page: torch.Tensor, area_threshold=500, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The segmentation demo's ``_contour`` image before JPEG encoding (Examples/demo_segmentation.py:17-25, 40-45):
+    ``draw_bounding_box(np.array(to_pil_image(page[i])), mask image, area_threshold)`` per page, bit for bit -- every outer
+    contour of the mask (findContours RETR_TREE) whose contourArea exceeds `area_threshold` gets its convex hull filled
+    (drawContours, thickness -1) in RGB (50, 128, 30) over the page's bytes.  500 is the demo's call.  Computed on the GPU from
+    the mask's regions (DESIGN 4.14), eleven launches, no host synchronisation (capturable).
+
+    `text_mask`: uint8 [n, 1, h, w], nonzero = text (text_mask_postprocess's output); `page`: fp32 NCHW [n, 3, h, w] in [0, 1],
+    its bytes recovered as to_pil_image does (``mul(255)``, truncated, clamped, NaN as 0).  Writes uint8 [n, h, w, 3] into
+    `out` (a new tensor when None) and returns it."""
+    fn = "text_region_hulls"
+    _check_page(page, fn)
+    n, _, h, w = page.shape
+    if not isinstance(text_mask, torch.Tensor) or text_mask.dtype != torch.uint8 or tuple(text_mask.shape) != (n, 1, h, w) \
+            or text_mask.device != page.device or not text_mask.is_contiguous():
+        got = (tuple(text_mask.shape), text_mask.dtype, str(text_mask.device)) if isinstance(text_mask, torch.Tensor) else text_mask
+        raise _lib.PcbError(f"{fn}: expected a contiguous uint8 text mask [{n}, 1, {h}, {w}] on {page.device}, got {got}")
+    if isinstance(area_threshold, bool) or not isinstance(area_threshold, (int, float)) or not float("-inf") < float(area_threshold) < float("inf"):
+        raise _lib.PcbError(f"{fn}: area_threshold must be a finite number, got {area_threshold!r}")
+    if out is None:
+        out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=page.device)
+    elif not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or not out.is_contiguous() \
+            or out.device != page.device:
+        raise _lib.PcbError(f"{fn}: out must be a contiguous uint8 [{n}, {h}, {w}, 3] tensor on {page.device}")
+    lib = _lib.load()
+    size = lib.pcb_text_regions_workspace(n, h, w)
+    if size == 0:
+        raise _lib.PcbError(f"{fn}: a {n}x{h}x{w} page batch is out of range ((h + 1) * (w + 1) < 2^31, at most 65535 pages)")
+    ws = torch.empty((size,), dtype=torch.uint8, device=page.device)
+    _lib.check(lib.pcb_text_region_hulls(text_mask.data_ptr(), page.data_ptr(), n, h, w, float(area_threshold), ws.data_ptr(),
+                                         out.data_ptr(), _stream()))
+    return out

@@ -55,3 +55,34 @@ def random_hole_masks(n, h, w, seed=0, channels=3):
     rng = np.random.Generator(np.random.PCG64(seed))
     planes = np.stack([random_hole_plane(h, w, rng) for _ in range(n)]).astype(np.float32)
     return np.repeat(planes[:, None], channels, axis=1)
+
+
+def manga_text_mask(h, w, seed=0):
+    """uint8 [h, w] text mask (1 = text) of a manga-like page: speech-bubble rings (ellipse outlines a few pixels thick),
+    each holding columns of glyph-sized blobs (small filled rectangles, some with a hole, some split in two); bubbles cut by
+    the page border leave their glyphs as regions of their own."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    m = np.zeros((h, w), np.uint8)
+    s = max(1.0, min(h, w) / 1200.0)
+    yy, xx = np.ogrid[0:h, 0:w]
+    for _ in range(int(12 * s * s)):
+        ay, ax = int(rng.integers(90, 200) * s), int(rng.integers(60, 140) * s)
+        cy, cx = int(rng.integers(0, h)), int(rng.integers(0, w))
+        y0, y1, x0, x1 = max(cy - ay - 4, 0), min(cy + ay + 5, h), max(cx - ax - 4, 0), min(cx + ax + 5, w)
+        if y0 >= y1 or x0 >= x1:
+            continue
+        r = ((yy[y0:y1] - cy) / ay) ** 2 + ((xx[:, x0:x1] - cx) / ax) ** 2
+        m[y0:y1, x0:x1][(r <= 1.0) & (r >= (1 - 3.0 / min(ax, ay)) ** 2)] = 1              # the bubble's ring
+        g = int(rng.integers(9, 15) * s)                                                   # glyph pitch
+        for col in range(cx + ax // 2 - g, cx - ax // 2, -g - 2):
+            for row in range(cy - ay // 2, cy + ay // 2 - g, g + 1):
+                if not (0 <= row and row + g <= h and 0 <= col and col + g <= w) or rng.random() < 0.15:
+                    continue
+                gh, gw = int(rng.integers(g // 2, g)), int(rng.integers(g // 2, g))
+                m[row:row + gh, col:col + gw] = 1
+                kind = rng.random()
+                if kind < 0.3 and gh > 4 and gw > 4:
+                    m[row + 2:row + gh - 2, col + 2:col + gw - 2] = 0                      # a glyph with a hole
+                elif kind < 0.5 and gw > 3:
+                    m[row:row + gh, col + gw // 2] = 0                                     # a glyph in two strokes
+    return m
